@@ -21,13 +21,15 @@ generator.  Workloads (BASELINE.json configs):
             copy-engine pull ("ce") or NCCL all-gather ("nccl") overlapped with the next rollout's steps; the ranks'
             clocks are aligned on the device before the warm-up steps.
   flush_protocol  the round-1 protocol kept for comparison: per-step events with a 256 MiB L2-flush fill between steps, and
-            the same measurement around an EMPTY kernel (the floor of that protocol: ~6 us on B200).
+            the same measurement around an EMPTY kernel (the floor of that protocol).
   e2e       same metric through the public ManagerBasedRLEnv.step_host() with HOST (pinned) buffers: H2D of the actions and
             D2H of observations + reward + done masks inside the timed region, every step, stream-synchronised.
   roofline  algorithmic bytes of the step kernel(s) / average step duration in the timed region vs the measured HBM peak.
   cpu_baseline  the CPU oracle (oracle/wl_oracle.c, "port") timed on this box's host cores.
 --impl reference times that same CPU implementation (all physical cores) as the reference arm: the reference's own PhysX
-pipeline is a closed binary that is not in /root/reference (DESIGN.md).  It does not import the product package.
+pipeline is a closed binary that is not part of the reference sources (DESIGN.md).  It does not import the product package.
+--dump-outputs DIR writes what the last timed step returned (bench.dump_outputs) so that two builds can be compared output
+for output: the inputs depend only on the arguments (seeded tasks, counter-based actions).
 """
 from __future__ import annotations
 
@@ -53,16 +55,17 @@ UNIT = "env-steps/s"
 BYTES_PER_ENV_STEP = (13 * 16 + 8) + (9 * 16 + 56 + 4 + 2)
 WORKLOADS = {
     "drift": {"task": "drift", "envs": 4096, "bytes": BYTES_PER_ENV_STEP, "obs_dim": 14, "blob": "drift.bin",
-              "label": "RSS_DRIFT_CONFIG MushrDriftRL, dt 5ms x4, DR+push+noise on", "kernel": "wl_step_duo_kernel (Drift family, 8 envs per CTA)",
-              "traffic_profile": "profiles/r02_ncu_step_drift_4096.txt"},
+              "label": "RSS_DRIFT_CONFIG MushrDriftRL, dt 5ms x4, DR+push+noise on", "kernel": "wl_step_duo_kernel (Drift family, 8 envs per CTA)"},
     "elev": {"task": "elevation", "envs": 4096, "bytes": (15 * 16 + 8) + (11 * 16 + 689 * 4 + 4 + 2), "obs_dim": 689, "blob": "elevation.bin",
              "label": "RSS_ELEV_CONFIG MushrElevationRL, dt 10ms x10 (5 ms sub-steps), reference terrain raster + 676-ray height scan",
-             "kernel": "wl_step_quad_kernel<ELEVATION> + wl_scan_kernel<TMA>", "traffic_profile": "profiles/r02_ncu_step_elev_4096.txt"},
+             "kernel": "wl_step_quad_kernel<ELEVATION> + wl_scan_kernel<TMA>"},
     "hound4wd": {"task": "hound_4wd", "envs": 8192, "bytes": BYTES_PER_ENV_STEP, "obs_dim": 14, "blob": "hound_4wd.bin",
                  "label": "HOUND 4WD: MuSHR + HOUND_SUS_ACTUATOR_CFG (4 driven wheels) + Mushr4WDActionCfg, mass/friction DR, dt 5ms x4",
-                 "kernel": "wl_step_duo_kernel (4WD action map)", "traffic_profile": "profiles/r02_ncu_step_hound_8192.txt"},
+                 "kernel": "wl_step_duo_kernel (4WD action map)"},
 }
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024                                    # H100 SXM
+NUM_SMS = 132
+DUMP_MAX_BYTES = 64 * 1024 * 1024
 
 
 def _peaks():
@@ -72,21 +75,27 @@ def _peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
-def _traffic(path):
-    """dram bytes per launch recorded in the committed `ncu --set full` summary of this workload (or None)."""
-    p = ROOT / path
-    if not p.exists():
-        return None
-    tot = 0.0
-    for line in p.read_text().splitlines():
-        for key in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            if line.strip().startswith(key + " ="):
-                val, unit = line.split("=")[1].split()[:2]
-                tot += float(val) * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(unit, 1)
-    return tot or None
+def dump_outputs(out_dir, obs, rew, terminated, truncated, seed=0):
+    """Write what one step returned to its caller as float32 .npy files.  Above DUMP_MAX_BYTES the rows of a fixed, seeded
+    sample of envs are written instead, with their indices in env_index.npy."""
+    import numpy as np
+    import torch
+    arrays = {"obs": obs, "reward": rew, "terminated": terminated, "truncated": truncated}
+    n = obs.shape[0]
+    row_bytes = sum(a[0].numel() * 4 for a in arrays.values())
+    out_dir = Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    if n * row_bytes > DUMP_MAX_BYTES:
+        keep = max(1, DUMP_MAX_BYTES // (row_bytes + 8))
+        idx = np.sort(np.random.default_rng(seed).choice(n, size=keep, replace=False))
+        np.save(out_dir / "env_index.npy", idx.astype(np.float64))
+        ti = torch.as_tensor(idx, device=obs.device)
+        arrays = {k: a[ti] for k, a in arrays.items()}
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a.float().cpu().numpy())
 
 
 class ClockSampler:
@@ -327,7 +336,7 @@ def run_ours(args):
     sims = [sim0] + [wl.WheeledSim(mk(1000 * m), dev) for m in range(1, M)]
     for s in sims:
         s.startup(); s.reset(None, 0)
-    # rollout length: rsl_rl num_steps_per_env is 128 (rsl_rl_ppo_cfg.py:6), shortened so that the driver's short runs still hold
+    # rollout length: rsl_rl num_steps_per_env is 128 (rsl_rl_ppo_cfg.py:6), shortened so that short runs still hold
     # exchanges inside the K steps.  The run is continuous: step k (warm-up steps included) fills row k % T_ROLL of slab
     # (k // T_ROLL) % 2 and an exchange follows every T_ROLL-th step, so a window of K steps holds ~K / T_ROLL of them
     fam = w["task"] in ("drift", "hound_4wd")
@@ -418,9 +427,9 @@ def run_ours(args):
             else:
                 slabs[i_s].all_gather()
     # Both the W warm-up steps and the K timed steps are captured into CUDA graphs (how a rollout is meant to be driven: the
-    # Python + driver launch path costs ~8 us per step here, more than the kernel), instantiated and uploaded at set-up.  On the
+    # Python + driver launch path of one step can cost more than the kernel), instantiated and uploaded at set-up.  On the
     # device the sequence is  [spin][rank alignment][W warm-up steps] e0 [K steps] e1 : the warm-up runs IMMEDIATELY before the
-    # clock starts (caches, clocks and -- N > 1 -- the NVLink lanes are in their steady state: idle lanes take ~0.1 ms to wake),
+    # clock starts (caches, clocks and -- N > 1 -- the NVLink lanes are in their steady state: idle lanes take time to wake),
     # and the spin keeps the GPU busy while the host enqueues everything, so e0..e1 holds no host launch latency.
     sim_x = wl.WheeledSim(mk(777), dev); sim_x.startup(); sim_x.reset(None, 0)        # loads the step kernels' module before capture
     sim_x.bind_step(acts[0], RolloutSlab(1, E, sim0.obs_dim, 2, dev).step_outputs(0))(0)
@@ -474,6 +483,9 @@ def run_ours(args):
     e1.record()
     barrier()
     tot_ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:                       # what the last timed step returned, before anything reuses the slabs
+        k_last = W + K - 1
+        dump_outputs(args.dump_outputs, *slabs[(k_last // T_ROLL) % n_slabs].step_outputs(k_last % T_ROLL), seed=args.seed)
     launches = (sum(s.launch_count for s in sims) - l0) if graph is None else K
     n_exchanges = len(gev)
     # duration of one exchange on its own (eager, outside the timed region): all-gather ms / barrier ms
@@ -676,12 +688,11 @@ def run_ours(args):
                            "stream sync, every step.  zero_copy_obs_on_device (round 1's figure: obs left on the GPU) is listed for comparison"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": _traffic(w["traffic_profile"]) if E == w["envs"] else None, "traffic_unit": "bytes/launch (dram read + write, ncu --set full)",
-                         "traffic_source": w["traffic_profile"], "peak_source": peak_src, "kernel": w["kernel"],
+                         "peak_source": peak_src, "kernel": w["kernel"],
                          "bytes_per_env_step": w["bytes"], "avg_step_us": kern_s * 1e6,
-                         "kernel_variant": ("duo (8 envs per 64-thread CTA: env warp 4 lanes/env + aux warp)" if (fam and E <= 37888)
-                                            else "quad (4 lanes/env)" if E <= 148 * 4 * 32 * 2 else "thread-per-env"),
-                         "note": f"{E} envs move {w['bytes'] * E / 1e6:.1f} MB per launch: latency-bound at this size, see profiles/ for the N sweep"},
+                         "kernel_variant": ("duo (8 envs per 64-thread CTA: env warp 4 lanes/env + aux warp)" if (fam and E <= NUM_SMS * 4 * 32 * 2)
+                                            else "quad (4 lanes/env)" if E <= NUM_SMS * 4 * 32 * 2 else "thread-per-env"),
+                         "note": f"{E} envs move {w['bytes'] * E / 1e6:.1f} MB per launch: latency-bound at this size"},
             "cpu_baseline": cpu,
             "flush_protocol": {"step_us_median": statistics.median(flush_us), "step_us_mean": statistics.mean(flush_us),
                                "value": total_envs / (statistics.mean(flush_us) * 1e-6) if world == 1 else None,
@@ -729,6 +740,9 @@ def main():
     ap.add_argument("--cpu-budget", type=float, default=12.0)
     ap.add_argument("--no-extras", action="store_true", help="skip the supplementary figures (policy-in-loop, fused rollout)")
     ap.add_argument("--eager", action="store_true", help="time eager stream launches instead of one CUDA graph of the K steps")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one returned (obs, reward, terminated, truncated) as "
+                         "DIR/<name>.npy in float32, at most 64 MB (rank 0's envs; a seeded sample of rows above that)")
     ap.add_argument("--gather", default="auto", choices=["auto", "nccl", "ce", "fanout", "mcast"],
                     help="N > 1 slab exchange: fused into the step kernel as NVSwitch-multicast stores (mcast; auto for the Drift family, "
                          "falling back to per-peer stores = fanout, then to NCCL), copy-engine pull over symmetric memory (ce; auto "

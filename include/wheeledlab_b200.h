@@ -1,5 +1,5 @@
 /*
- * wheeledlab_b200.h -- C-ABI of the B200-native vectorised wheeled-robot step.
+ * wheeledlab_b200.h -- C-ABI of the H100-native vectorised wheeled-robot step.
  *
  * This is the drop-in boundary for ONE path of UWRobotLearning/WheeledLab: the
  * object `gym.make(<id>, cfg=env_cfg)` returns (isaaclab.envs:ManagerBasedRLEnv,
@@ -394,7 +394,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
               wl_sim** out);
 int wl_destroy(wl_sim* sim);
 const char* wl_last_error(void);
-/* compiled-for architecture string, e.g. "sm_100a" */
+/* compiled-for architecture string, e.g. "sm_90a" */
 const char* wl_build_info(void);
 
 /* ---- hot path -------------------------------------------------------------- */
@@ -527,7 +527,7 @@ int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, con
                     float beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream);
 
 /* A caller that drives wl_step through a CUDA graph of K steps (how a rollout is meant to be issued: one launch per K steps)
- * pays the upload of the instantiated graph to the device on its FIRST launch (~10 us for 20 kernel nodes); this moves that
+ * pays the upload of the instantiated graph to the device on its FIRST launch; this moves that
  * upload to set-up time.  graph_exec = cudaGraphExec_t (torch: CUDAGraph.raw_cuda_graph_exec()). */
 int wl_graph_upload(void* graph_exec, void* stream);
 

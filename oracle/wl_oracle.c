@@ -12,7 +12,7 @@
  *     golden vectors generated from the reference's own Python
  *     (tests/golden/, tests/golden/make_golden.py).
  *   - The rigid-body / tyre / actuator integrator stands in for PhysX-5 (closed
- *     binary, absent from /root/reference and from this image): PARITY UNPINNED at
+ *     binary, absent from the reference sources and not installable offline): PARITY UNPINNED at
  *     the PhysX boundary.  The model is builder-defined (DESIGN.md "Physics model").
  *   - Visual task camera: the post-processing (crop, ColorJitter, GaussianBlur, Grayscale, Normalize) is PINNED by
  *     golden vectors from the reference's own torchvision functions; the renderer that feeds it stands in for the RTX

@@ -5,4 +5,4 @@ from . import rendering  # noqa: F401
 
 class RecordVideo(Wrapper):
     def __init__(self, env, *a, **k):
-        raise NotImplementedError("video recording needs the reference's RTX viewport (out of scope for the B200 env: render() is None)")
+        raise NotImplementedError("video recording needs the reference's RTX viewport (out of scope for the fused-step env: render() is None)")

@@ -4,4 +4,4 @@ from ..core import Wrapper
 
 class RecordVideo(Wrapper):
     def __init__(self, env, *a, **k):
-        raise NotImplementedError("video recording needs the reference's RTX viewport (out of scope for the B200 env: render() is None)")
+        raise NotImplementedError("video recording needs the reference's RTX viewport (out of scope for the fused-step env: render() is None)")

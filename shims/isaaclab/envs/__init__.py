@@ -62,7 +62,7 @@ class ManagerBasedEnv(metaclass=_LazyEnvMeta):
 
 class ManagerBasedRLEnv(ManagerBasedEnv):
     """gym entry point 'isaaclab.envs:ManagerBasedRLEnv' (wheeledlab_tasks/__init__.py:16): construct the
-    B200-native env from the reference's own cfg object."""
+    fused-step env from the reference's own cfg object."""
 
     def __new__(cls, cfg=None, render_mode=None, **kwargs):
         from wheeledlab_b200.compat import env_from_reference_cfg

@@ -73,4 +73,4 @@ def root_height_below_minimum(env, minimum_height: float, asset_cfg: SceneEntity
 
 
 def image(env, sensor_cfg=None, data_type="rgb", convert_perspective_to_orthogonal=False, normalize=True):
-    raise NotImplementedError("camera observations are out of scope for the B200 hot path (SURVEY 8f-4)")
+    raise NotImplementedError("camera observations are out of scope for the fused hot path (SURVEY 8f-4)")

@@ -1,4 +1,4 @@
-"""Event functions: markers only.  The B200 env lowers them by name onto wl_startup / the fused step
+"""Event functions: markers only.  The fused-step env lowers them by name onto wl_startup / the fused step
 (a13, a14 in SURVEY 8a); calling them directly is not supported."""
 
 

@@ -1,6 +1,6 @@
 """Stand-in for `pxr` (OpenUSD) as far as the UNMODIFIED reference touches it at import time:
 wheeledlab_tasks/visual/utils/__init__.py:154-186 (create_geometry) builds a Usd.Stage with the 2-colour plane mesh and saves it
-for the RTX scene.  The B200 env renders that plane from the traversability map itself (wl_camera_kernel), so the stage
+for the RTX scene.  The fused-step env renders that plane from the traversability map itself (wl_camera_kernel), so the stage
 calls are absorbed: every attribute access / call returns an inert object and nothing is written to disk."""
 
 

@@ -4,7 +4,7 @@
 Two producers must agree byte for byte (tests/test_compat_cpu.py, tests/test_gpu_parity.py):
   * the package's own restatement of the reference configuration (wheeledlab_b200.tasks.make_task), and
   * the lowering of the REFERENCE'S OWN cfg objects (wheeledlab_b200.compat.spec_from_reference_cfg), imported from
-    /root/reference in the authoring container (this script records them as <name>.ref.bin when the tree is present).
+    the reference's source/ directory when its path is given as the first argument (recorded as <name>.ref.bin).
 The blobs also let non-Python hosts (examples/c_host) and bench.py's reference arm build a task without importing the package.
 num_envs = 4096, seed = 42, env_id_offset = 0 in every blob (the first fields of wl_config; consumers patch them).
 """
@@ -25,13 +25,13 @@ def blob(cfg) -> bytes:
     return C.string_at(C.addressof(cfg), C.sizeof(cfg))
 
 
-def import_reference_tasks():
-    """Import the UNMODIFIED wheeledlab_tasks package of /root/reference against the stand-ins in shims/ (gymnasium, isaaclab,
+def import_reference_tasks(ref: Path):
+    """Import the UNMODIFIED wheeledlab_tasks package of the reference's source/ directory `ref` against the stand-ins in shims/ (gymnasium, isaaclab,
     pxr, matplotlib).  Importing it registers the four gym ids (wheeledlab_tasks/__init__.py:14-63) and -- quirk Q10 -- builds the
     Visual traversability map and tries to create <assets>/data/rgb_maps: the reference tree is read-only here, so that one
     makedirs is skipped."""
     import os
-    ref = Path("/root/reference/source")
+    ref = Path(ref)
     sys.path[:0] = [str(ROOT / "shims"), str(ref / "wheeledlab"), str(ref / "wheeledlab_assets"), str(ref / "wheeledlab_tasks")]
     real = os.makedirs
 
@@ -61,9 +61,9 @@ def main():
         spec = wl.make_task(tid, num_envs=4096, seed=42)
         (OUT / f"{name}.bin").write_bytes(blob(spec.cfg))
         print(name, C.sizeof(spec.cfg), "bytes")
-    if Path("/root/reference/source").exists():          # authoring container: lower the reference's own cfg objects
+    if len(sys.argv) > 1:                                # the reference's source/ directory: lower its own cfg objects
         from wheeledlab_b200.compat import spec_from_reference_cfg
-        gym = import_reference_tasks()
+        gym = import_reference_tasks(Path(sys.argv[1]))
         for gid in gym.registry:
             for key, suffix in (("env_cfg_entry_point", "ref"), ("play_env_cfg_entry_point", "play.ref")):
                 cls = gym.spec(gid).kwargs.get(key)

@@ -1,9 +1,8 @@
 #!/usr/bin/env python
-"""Generate golden input/output vectors by EXECUTING THE REFERENCE'S OWN PYTHON (read-only tree at
-/root/reference) on CPU torch tensors, against the IsaacLab stand-in in shims/ (config carriers + trivial
-state accessors only).  Run in the authoring container:
+"""Generate golden input/output vectors by EXECUTING THE REFERENCE'S OWN PYTHON on CPU torch tensors,
+against the IsaacLab stand-in in shims/ (config carriers + trivial state accessors only):
 
-    python tests/golden/make_golden.py          # writes tests/golden/*.npz
+    python tests/golden/make_golden.py <the reference's source/ directory>     # writes tests/golden/*.npz
 
 Two kinds of fixture (DESIGN.md 5): values produced by the REFERENCE'S OWN functions (action terms, drift / elevation /
 visual term functions, reset_root_state_along_track, the curriculum term, the camera post-processing), and values that pass
@@ -11,8 +10,8 @@ through an IsaacLab function restated in shims/ ([UPSTREAM-RECALL]: is_terminate
 quat_from_euler_xyz) -- the latter pin the oracle to the restatement, not to IsaacLab.
 The vectors pin the oracle's restatement of: the action terms (ackermann_actions.py, rc_car_actions.py), the
 drift reward/termination terms (mushr_drift_env_cfg.py:160-240,343-348), reset_root_state_along_track
-(drifting/mdp/events.py), increase_reward_weight_over_time (curriculums.py), root_euler_xyz.  They cannot
-travel as code (/root/reference does not exist on the GPU box), hence the committed .npz fixtures.
+(drifting/mdp/events.py), increase_reward_weight_over_time (curriculums.py), root_euler_xyz.  The reference is
+not part of this repository, hence the committed .npz fixtures.
 """
 import sys
 import types
@@ -23,7 +22,9 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference/source")
+if len(sys.argv) != 2:
+    sys.exit("usage: python tests/golden/make_golden.py <the reference's source/ directory>")
+REF = Path(sys.argv[1])
 sys.path[:0] = [str(ROOT / "shims"), str(REF / "wheeledlab"), str(REF / "wheeledlab_assets")]
 pkg = types.ModuleType("wheeledlab_tasks")          # skip wheeledlab_tasks/__init__.py (gymnasium/pxr import chain)
 pkg.__path__ = [str(REF / "wheeledlab_tasks" / "wheeledlab_tasks")]

@@ -1,8 +1,12 @@
 """ctypes wrapper of the CPU oracle (oracle/wl_oracle.c).  TEST INFRASTRUCTURE ONLY."""
 from __future__ import annotations
 
+import atexit
 import ctypes as C
+import os
+import shutil
 import subprocess
+import tempfile
 from pathlib import Path
 
 import numpy as np
@@ -12,12 +16,20 @@ ODIR = ROOT / "oracle"
 
 
 def _ensure_built(native=False):
-    targets = ["libwl_oracle.so", "libwl_oracle_f64.so"] + (["libwl_oracle_native.so"] if native else [])
-    subprocess.run(["make", "-C", str(ODIR), *targets], check=True, stdout=subprocess.DEVNULL)
+    in_tree = [ODIR / "libwl_oracle.so", ODIR / "libwl_oracle_f64.so"]
+    if not (all(p.exists() for p in in_tree) and not os.access(ODIR, os.W_OK)):     # a read-only tree is used as built
+        subprocess.run(["make", "-C", str(ODIR), *(p.name for p in in_tree)], check=True, stdout=subprocess.DEVNULL)
+    if not native:
+        return None
+    # the host-tuned build is made for the host that runs it, outside the (possibly read-only) source tree
+    out = Path(tempfile.mkdtemp(prefix="wl_oracle_native_"))
+    atexit.register(shutil.rmtree, out, True)
+    subprocess.run(["make", "-C", str(ODIR), f"NATIVE_DIR={out}", str(out / "libwl_oracle_native.so")], check=True, stdout=subprocess.DEVNULL)
+    return out
 
 
-def _load(name):
-    lib = C.CDLL(str(ODIR / name))
+def _load(path):
+    lib = C.CDLL(str(path))
     vp, i32, i64, u32, u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64
     lib.wlo_create.restype = vp
     lib.wlo_create.argtypes = [vp, vp]
@@ -54,8 +66,8 @@ _libs = {}
 
 def get_lib(kind="f32"):
     if kind not in _libs:
-        _ensure_built(native=(kind == "native"))
-        _libs[kind] = _load({"f32": "libwl_oracle.so", "f64": "libwl_oracle_f64.so", "native": "libwl_oracle_native.so"}[kind])
+        ndir = _ensure_built(native=(kind == "native"))
+        _libs[kind] = _load(ndir / "libwl_oracle_native.so" if kind == "native" else ODIR / {"f32": "libwl_oracle.so", "f64": "libwl_oracle_f64.so"}[kind])
     return _libs[kind]
 
 

@@ -37,12 +37,12 @@ def test_state_bytes_and_alignment():
         assert wl.lib.wl_state_bytes(n) >= off + 160
 
 
-def test_build_targets_sm100a():
+def test_build_targets_sm90a():
     import subprocess
     import wheeledlab_b200 as wl
-    assert b"sm_100a" in wl.lib.wl_build_info()
+    assert b"sm_90a" in wl.lib.wl_build_info()
     out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-lelf", str(wl.LIB_PATH)], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
 
 
 def test_no_cuda_device_fails_loudly():

@@ -1,27 +1,26 @@
-"""The reference's own env-cfg objects (imported from /root/reference when present -- authoring container only)
-lower to exactly the restated TaskSpec; skipped on the GPU box where the reference tree does not exist."""
+"""The reference's own env-cfg objects lower to exactly the restated TaskSpec.  The objects are rebuilt from the record of
+the unmodified reference package in tests/golden/ref_cfgs.json.gz (tests/golden/make_ref_cfgs.py, tests/recorded_cfgs.py)."""
 import sys
-import types
 from pathlib import Path
 
 import pytest
 
-REF = Path("/root/reference/source")
 ROOT = Path(__file__).resolve().parent.parent
 
 
 @pytest.fixture(scope="module")
-def ref_cfgs():
-    if not REF.exists():
-        pytest.skip("/root/reference not present (GPU box)")
-    sys.path[:0] = [str(ROOT / "shims"), str(REF / "wheeledlab"), str(REF / "wheeledlab_assets")]
-    pkg = types.ModuleType("wheeledlab_tasks")
-    pkg.__path__ = [str(REF / "wheeledlab_tasks" / "wheeledlab_tasks")]
-    sys.modules.setdefault("wheeledlab_tasks", pkg)
-    from wheeledlab_tasks.drifting import mushr_drift_env_cfg as D
-    from wheeledlab_tasks.drifting import f1tenth_drift_env_cfg as F
-    from wheeledlab_tasks.elevation import mushr_elevation_env_cfg as E
-    return D, F, E
+def ref_registry():
+    if str(ROOT / "shims") not in sys.path:
+        sys.path.insert(0, str(ROOT / "shims"))          # isaaclab.managers: the term cfgs the tests add to a recorded cfg
+    import recorded_cfgs
+    return recorded_cfgs.load()
+
+
+@pytest.fixture(scope="module")
+def ref_cfgs(ref_registry):
+    """Factories of the reference's MushrDriftRLEnvCfg, F1TenthDriftRLEnvCfg and MushrElevationRLEnvCfg."""
+    return tuple(ref_registry[gid]["cfgs"]["env_cfg_entry_point"]
+                 for gid in ("Isaac-MushrDriftRL-v0", "Isaac-F1TenthDriftRL-v0", "Isaac-MushrElevationRL-v0"))
 
 
 def _cfg_dict(c):
@@ -36,7 +35,7 @@ def test_drift_cfg_lowers_to_restated_spec(ref_cfgs):
     D, _, _ = ref_cfgs
     import wheeledlab_b200 as wl
     from wheeledlab_b200.compat import spec_from_reference_cfg
-    cfg = D.MushrDriftRLEnvCfg()
+    cfg = D()
     cfg.scene.num_envs = 64
     got = spec_from_reference_cfg(cfg)
     exp = wl.drift_task(num_envs=64, seed=42)
@@ -52,10 +51,10 @@ def test_drift_cfg_lowers_to_restated_spec(ref_cfgs):
 def test_f1tenth_and_elevation_cfgs_lower(ref_cfgs):
     _, F, E = ref_cfgs
     from wheeledlab_b200.compat import spec_from_reference_cfg
-    f = F.F1TenthDriftRLEnvCfg(); f.scene.num_envs = 8
+    f = F(); f.scene.num_envs = 8
     s = spec_from_reference_cfg(f)
     assert s.cfg.action_kind == 2 and abs(s.cfg.base_length - 0.365) < 1e-6 and abs(s.cfg.base_width - 0.284) < 1e-6
-    e = E.MushrElevationRLEnvCfg(); e.scene.num_envs = 8
+    e = E(); e.scene.num_envs = 8
     s = spec_from_reference_cfg(e)
     assert s.cfg.task == 1 and s.cfg.max_episode_length == 200 and s.cfg.decimation == 10 and s.cfg.substeps == 2
     assert s.reward_names == ["vel_towards_goal", "height_z", "falling_penalty", "termination_penalty"]
@@ -66,7 +65,7 @@ def test_unknown_term_fails_loudly(ref_cfgs):
     D, _, _ = ref_cfgs
     from wheeledlab_b200.compat import spec_from_reference_cfg
     from isaaclab.managers import RewardTermCfg
-    cfg = D.MushrDriftRLEnvCfg()
+    cfg = D()
     cfg.rewards.side_slip = RewardTermCfg(func=lambda env: 0, weight=1.0)
     with pytest.raises(NotImplementedError):
         spec_from_reference_cfg(cfg)
@@ -77,7 +76,7 @@ def test_unknown_term_becomes_host_side_term_when_allowed(ref_cfgs):
     D, _, _ = ref_cfgs
     from wheeledlab_b200.compat import spec_from_reference_cfg
     from isaaclab.managers import RewardTermCfg, TerminationTermCfg
-    cfg = D.MushrDriftRLEnvCfg()
+    cfg = D()
     f = lambda env, k=1.0: 0
     g = lambda env: 0
     cfg.rewards.my_bonus = RewardTermCfg(func=f, weight=3.0, params={"k": 2.0})
@@ -92,34 +91,27 @@ def test_unknown_term_becomes_host_side_term_when_allowed(ref_cfgs):
     assert "my_bonus" not in s.reward_names and len(s.reward_names) == 7      # built-in slots untouched
 
 
-# ---- the registration path: UNMODIFIED wheeledlab_tasks/__init__.py against shims/ (gymnasium, isaaclab, pxr, matplotlib) ----
+# ---- the registration path: the four ids UNMODIFIED wheeledlab_tasks/__init__.py registers against shims/ (as recorded) ----
 def _cfg_blob(c):
     import ctypes as C
     return C.string_at(C.addressof(c), C.sizeof(c))
 
 
-def test_unmodified_registration_and_all_cfgs_lower_to_the_committed_blobs():
-    """`import wheeledlab_tasks` (reference source, untouched) registers the four gym ids through the gymnasium stand-in; every
-    train and play cfg lowers through compat.spec_from_reference_cfg to exactly the committed fixture, and the train cfgs equal
-    make_task(id) byte for byte."""
-    if not REF.exists():
-        pytest.skip("/root/reference not present (GPU box)")
-    import importlib.util
+def test_unmodified_registration_and_all_cfgs_lower_to_the_committed_blobs(ref_registry):
+    """`import wheeledlab_tasks` (reference source, untouched) registered the four gym ids through the gymnasium stand-in
+    (recorded with their cfg objects); every train and play cfg lowers through compat.spec_from_reference_cfg to exactly
+    the committed fixture, and the train cfgs equal make_task(id) byte for byte."""
     import numpy as np
     import wheeledlab_b200 as wl
     from wheeledlab_b200.compat import spec_from_reference_cfg
-    spec = importlib.util.spec_from_file_location("make_cfg_blobs", ROOT / "tests" / "golden" / "make_cfg_blobs.py")
-    mk = importlib.util.module_from_spec(spec); spec.loader.exec_module(mk)
-    gym = mk.import_reference_tasks()
-    assert sorted(gym.registry) == sorted(wl.GYM_IDS)
-    for gid in gym.registry:
-        s = gym.spec(gid)
-        assert s.entry_point == "isaaclab.envs:ManagerBasedRLEnv" and s.kwargs["rsl_rl_cfg_entry_point"].count(":") == 1
+    assert sorted(ref_registry) == sorted(wl.GYM_IDS)
+    for gid, s in ref_registry.items():
+        assert s["entry_point"] == "isaaclab.envs:ManagerBasedRLEnv" and s["kwargs"]["rsl_rl_cfg_entry_point"].count(":") == 1
         for key, suffix in (("env_cfg_entry_point", "ref"), ("play_env_cfg_entry_point", "play.ref")):
-            cls = s.kwargs.get(key)
-            if cls is None:
+            make_cfg = s["cfgs"].get(key)
+            if make_cfg is None:
                 continue
-            cfg = cls(); cfg.scene.num_envs = 4096
+            cfg = make_cfg(); cfg.scene.num_envs = 4096
             got = spec_from_reference_cfg(cfg)
             fixture = (ROOT / "tests" / "golden" / "cfg_blobs" / f"{gid}.{suffix}.bin").read_bytes()
             if "Visual" in gid:                      # the reference draws a new random traversability map at every import (quirk Q10)
@@ -130,15 +122,15 @@ def test_unmodified_registration_and_all_cfgs_lower_to_the_committed_blobs():
                 if "Elevation" not in gid:
                     assert got.cfg.curr_n == 0 and not any(got.cfg.rew_weight)
     # a modified observation group is rejected, not silently replaced by the built-in one (ADVICE r1)
-    bad = gym.spec("Isaac-MushrDriftRL-v0").kwargs["env_cfg_entry_point"]()
+    bad = ref_registry["Isaac-MushrDriftRL-v0"]["cfgs"]["env_cfg_entry_point"]()
     bad.observations.policy.base_lin_vel_term = None
     with pytest.raises(NotImplementedError):
         spec_from_reference_cfg(bad)
 
 
 def test_make_task_reproduces_the_lowered_reference_cfgs():
-    """Runs everywhere (also on the GPU box, where /root/reference does not exist): the package's own restatement of the four
-    registered tasks equals the blobs lowered from the reference's cfg objects, byte for byte."""
+    """The package's own restatement of the four registered tasks equals the blobs lowered from the reference's cfg
+    objects, byte for byte."""
     import numpy as np
     import wheeledlab_b200 as wl
     blobs = ROOT / "tests" / "golden" / "cfg_blobs"

@@ -1,5 +1,5 @@
 """The oracle against GOLDEN VECTORS produced by executing the reference's own Python
-(tests/golden/make_golden.py, run where /root/reference exists; fixtures committed as .npz).
+(tests/golden/make_golden.py, run against the reference's sources; fixtures committed as .npz).
 fp32 tolerance: the reference evaluates with torch/libm, the oracle with its deterministic polynomials
 (|err| <= ~3e-7 relative, test_oracle_cpu.py) -> rtol 2e-6 / atol 2e-6; masks must match exactly away
 from float ties."""

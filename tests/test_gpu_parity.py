@@ -815,7 +815,7 @@ def test_c_host_example_matches_python_path(tmp_path):
         obs, rew, term, trunc = sim.step(sim.synth_actions(t), t)
         obs_sum += int(obs.cpu().numpy().view(np.uint32).astype(np.uint64).sum()); rew_sum += int(rew.cpu().numpy().view(np.uint32).astype(np.uint64).sum())
         n_term += int(term.sum()); n_trunc += int(trunc.sum())
-    assert got["envs"] == n and got["steps"] == steps and "sm_100a" in got["build"]
+    assert got["envs"] == n and got["steps"] == steps and "sm_90a" in got["build"]
     assert (got["obs_bits_sum"], got["rew_bits_sum"], got["terminated"], got["truncated"]) == (obs_sum, rew_sum, n_term, n_trunc)
     assert n_trunc > 0 and n_term > 0                              # the run crossed the 250-step time-out and saw off-track resets
 
@@ -968,7 +968,7 @@ def test_two_process_nccl_gather_equals_single_rank(tmp_path, mode):
 
 def test_gym_make_through_the_registry_and_the_reference_smoke_loop():
     """wheeledlab_tasks/__init__.py:14-63 registers `entry_point="isaaclab.envs:ManagerBasedRLEnv"`; with shims/ on the path
-    gym.make(id, cfg=...) resolves to the B200 env.  The loop is the reference's own smoke test
+    gym.make(id, cfg=...) resolves to the fused-step env.  The loop is the reference's own smoke test
     (wheeledlab_tasks/test/create_and_step_env.py:26-44): reset, then sample-and-step under inference_mode."""
     _need_gpu()
     import sys
@@ -1072,7 +1072,7 @@ def test_fused_adam_matches_torch_adam_single_rank():
 
 def test_two_process_fused_allreduce_adam(tmp_path):
     """DP learner step (SURVEY 8f-2): gradient all-reduce fused into the Adam kernel over symmetric memory, 2 ranks, vs
-    torch.optim.Adam on the NCCL-averaged gradient; replicas stay bit-identical (skipped on a single-GPU box)."""
+    torch.optim.Adam on the NCCL-averaged gradient; replicas stay bit-identical (skipped on a single-GPU machine)."""
     _need_gpu()
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")

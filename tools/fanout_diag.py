@@ -1,6 +1,6 @@
 """Where does the time of the N>1 slab exchange go?  torchrun --nproc-per-node N tools/fanout_diag.py
 Graphs of T env steps (Drift, 4096 envs/rank) in the exchange forms, each replayed several times (first replay = first touch
-of the peer mappings); prints per-replay microseconds, max over ranks.  Diagnostic only (profiles/r02_fanout_diag_*.json)."""
+of the peer mappings); prints per-replay microseconds, max over ranks.  Diagnostic only."""
 import json, os, sys
 import torch, torch.distributed as dist
 

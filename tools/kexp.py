@@ -2,7 +2,7 @@
 """Kernel A/B experiments with the bench protocol (L2 flushed between steps, CUDA events around each step launch).
 
     python tools/kexp.py build                 # here (nvcc cross-compiles): build_ab/libwl_<name>.so for every variant
-    python tools/kexp.py run [--envs 4096]     # on the GPU box: one subprocess per variant, one JSON line each
+    python tools/kexp.py run [--envs 4096]     # on the GPU: one subprocess per variant, one JSON line each
 Variants are sets of -D macros of csrc/wl_api.cu (experiment switches, never part of the shipped library)."""
 import json
 import os

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Text summary of an `ncu --set full` report (the format bench.py's roofline.traffic reads):
+"""Text summary of an `ncu --set full` report (DRAM bytes, duration, occupancy, stall samples per launch):
 
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep "capture command / context" > profiles/r02_ncu_step_drift_4096.txt
+    python tools/ncu_summary.py step.ncu-rep "capture command / context" > ncu_step_summary.txt
 """
 import csv
 import io

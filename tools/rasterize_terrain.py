@@ -1,9 +1,13 @@
 #!/usr/bin/env python
 """Rasterise the TOP surface of the reference's elevation terrain (Terrains/huge_compact.usd: 363 388 vertices,
-726 900 triangles, +-20.5 m, z in [0, 2]) onto the regular height-field the B200 elevation path consumes: for every raster
+726 900 triangles, +-20.5 m, z in [0, 2]) onto the regular height-field the elevation path consumes: for every raster
 sample, z = max over the triangles covering (x, y) of the barycentric height -- what the reference's vertical ray from
-z + 20 m hits (SURVEY.md Appendix C).  Authoring-container tool (needs /root/reference); the result is committed as a
-data file (wheeledlab_b200/data/terrain_huge_compact_0p1m.npz, 58 KB) because the reference tree does not exist on the GPU box.
+z + 20 m hits (SURVEY.md Appendix C).  Needs the reference's assets:
+
+    python tools/rasterize_terrain.py <the reference's source/ directory>
+
+The result is committed as a data file (wheeledlab_b200/data/terrain_huge_compact_0p1m.npz, 58 KB) because the reference
+is not part of this repository.
 """
 import subprocess
 import sys
@@ -53,7 +57,7 @@ int main(int argc, char** argv) {
 """
 
 
-def main(usd="/root/reference/source/wheeledlab_assets/data/Terrains/huge_compact.usd", cell=0.1, half=20.5,
+def main(usd, cell=0.1, half=20.5,
          out=HERE.parent / "wheeledlab_b200" / "data" / "terrain_huge_compact_0p1m.npz"):
     crate = Crate(usd)
     pts_field = [f for f in crate.array_fields("default") if f[0] == 24]          # vec3f arrays: extent, normals, points
@@ -82,7 +86,7 @@ def main(usd="/root/reference/source/wheeledlab_assets/data/Terrains/huge_compac
 
 
 if __name__ == "__main__":
-    H = main()
+    H = main(Path(sys.argv[1]) / "wheeledlab_assets" / "data" / "Terrains" / "huge_compact.usd")
     # SURVEY 8c spot heights (decoded independently there): top surface z at (x, y)
     def at(x, y):
         return H[int(round((y + 20.5) / 0.1)), int(round((x + 20.5) / 0.1))]

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""profiles/rNN_sass_tma.txt: per kernel of the built library, the static instruction count and the SASS mnemonics that prove
+"""Per kernel of the built library, the static instruction count and the SASS mnemonics that prove
 which hardware paths are used (TMA, bulk copies, mbarriers, named barriers, fire-and-forget atomics, IEEE slow paths).
 
-    python tools/sass_evidence.py > profiles/r02_sass_tma.txt
+    python tools/sass_evidence.py > sass_evidence.txt
 """
 import collections
 import re
@@ -32,12 +32,12 @@ def main():
                 rows[name][k] += 1
         if "UTMALDG" in m.group(2) or "UBLKCP" in m.group(2) or ("STG" in m.group(2) and "STRONG.SYS" in m.group(2)):
             proofs.append(f"{name}: /*{m.group(1)}*/ {m.group(2).strip()}")
-    print("# cuobjdump -sass wheeledlab_b200/libwheeledlab_b200.so (sm_100a): static instruction count per kernel and the mnemonics that prove the")
+    print("# cuobjdump -sass wheeledlab_b200/libwheeledlab_b200.so (sm_90a): static instruction count per kernel and the mnemonics that prove the")
     print("# hardware paths used.  UTMALDG.2D = cp.async.bulk.tensor.2d (TMA tile of the height-field, wl_scan_kernel<true>); UBLKCP = cp.async.bulk")
     print("# 1-D (policy weight blob, wl_act_step_quad_kernel); SYNCS = mbarrier arrive / expect_tx / try_wait; BAR.ARV + BAR.SYNC = named barriers")
     print("# of the env-warp / aux-warp hand-off (wl_step_duo_kernel); REDG = fire-and-forget reductions of the episode log (no ticket, no fence);")
     print("# ATOMG = the K-step rollout's last-CTA ticket; FCHK = range check of an IEEE division with slow-path call (the integrator sub-step uses")
-    print("# fdiv_norm / fsqrt_norm instead).  No tcgen05 / TMEM anywhere: there is no dense contraction on this path (tensor cores unused by design).")
+    print("# fdiv_norm / fsqrt_norm instead).  No wgmma anywhere: there is no dense contraction on this path (tensor cores unused by design).")
     print("# STG...STRONG.SYS = multimem.st.relaxed.sys (wl_step_duo_kernel: output rows stored once to the NVSwitch multicast alias of the symmetric")
     print("# rollout buffers, replicated by the switch into every rank's copy; wl_set_multicast_fanout); in the other kernels STRONG.SYS marks the")
     print("# system-scope loads/stores of the peer-memory all-reduce (wl_dp_adam_kernel) and of the flag protocols.")

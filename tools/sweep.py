@@ -2,7 +2,7 @@
 """N-sweep of the fused step kernel: per-launch duration (CUDA events) and achieved algorithmic HBM GB/s.
 
     python tools/sweep.py [--sizes 4096,65536,...] [--steps 30] [--task drift]
-Prints one JSON object; run under gpurun and copy the result into profiles/.
+Prints one JSON object.
 """
 import argparse, json, statistics, sys
 from pathlib import Path

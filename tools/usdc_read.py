@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Minimal pure-Python reader for USDC ("PXR-USDC" crate) files -- just enough to pull array attributes such as a Mesh's
 `points` / `faceVertexIndices` out of the reference's binary assets without `pxr` (not installed here).
-Format notes: SURVEY.md Appendix C.  Authoring-container tool (the assets live under /root/reference).
+Format notes: SURVEY.md Appendix C.  Used on the reference's assets, which are not part of this repository.
 """
 from __future__ import annotations
 

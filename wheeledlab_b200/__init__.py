@@ -1,6 +1,6 @@
-"""wheeledlab_b200 -- B200-native fused step for the WheeledLab Drift / Elevation / Visual tasks.
+"""wheeledlab_b200 -- H100-native fused step for the WheeledLab Drift / Elevation / Visual tasks.
 
-Importing the package loads ``libwheeledlab_b200.so`` (hand-written sm_100a kernels behind a C ABI);
+Importing the package loads ``libwheeledlab_b200.so`` (hand-written sm_90a kernels behind a C ABI);
 it raises if the library has not been built -- there is no CPU or eager-PyTorch fallback.
 """
 from ._lib import LIB_PATH, WlConfig, WlError, lib  # noqa: F401

@@ -22,7 +22,7 @@ class NativeLibraryMissing(ImportError):
 def _load() -> C.CDLL:
     if not LIB_PATH.exists():
         raise NativeLibraryMissing(
-            f"{LIB_PATH} not found. wheeledlab_b200 has no CPU fallback: build the sm_100a extension first "
+            f"{LIB_PATH} not found. wheeledlab_b200 has no CPU fallback: build the sm_90a extension first "
             f"(python -c 'import __graft_entry__ as g; g.build()' from the repo root)."
         )
     return C.CDLL(str(LIB_PATH), mode=os.RTLD_GLOBAL if hasattr(os, "RTLD_GLOBAL") else C.DEFAULT_MODE)

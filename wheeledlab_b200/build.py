@@ -12,7 +12,7 @@ LIB = PKG / "libwheeledlab_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",                    # bit-exact parity with the oracle (DESIGN.md "Determinism")
     "-Xcompiler", "-fPIC", "-shared",
 ]

@@ -1,5 +1,5 @@
 // wl_api.cu -- kernels + the extern "C" ABI declared in include/wheeledlab_b200.h.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false -lineinfo -O3 (see build.py).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false -lineinfo -O3 (see build.py).
 #include <cstdio>
 #include <cstdlib>
 #include <cmath>
@@ -39,8 +39,10 @@ struct wl_sim {
     int scan_mode;          // ray-cast tile staging: 1 one TMA tile per CTA (default), 2 TMA producer/consumer pipeline, 0 plain loads (A/B)
 };
 
-// below this many envs one thread/env cannot fill 148 SMs x 4 schedulers; use 4 lanes per env
-#define WL_QUAD_MAX_ENVS (148 * 4 * 32 * 2)
+// SMs of the H100 SXM the launch geometry is sized for
+#define WL_NUM_SMS 132
+// below this many envs one thread/env cannot fill the SMs x 4 schedulers; use 4 lanes per env
+#define WL_QUAD_MAX_ENVS (WL_NUM_SMS * 4 * 32 * 2)
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) { g_err = msg; return code; }
@@ -146,7 +148,7 @@ __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool con
 
 // One thread per env.  TASK selects the MDP + terrain at compile time.
 #ifndef WL_STEP_MIN_BLOCKS
-#define WL_STEP_MIN_BLOCKS 4      // 4 CTAs x 128 threads / SM (<= 128 registers); see profiles/ for the occupancy A/B
+#define WL_STEP_MIN_BLOCKS 4      // 4 CTAs x 128 threads / SM (<= 128 registers); overridable for occupancy A/B builds
 #endif
 // STAGE 0: the whole env.step.  STAGE 1 / 2: the same code cut after section E (wl_step_stage_a / wl_step_stage_b), so that
 // host-side (Python) reward and termination terms can run between "rewards" and "reset" exactly where the reference's
@@ -457,7 +459,7 @@ __device__ __forceinline__ void bar_arrive(int id) { asm volatile("bar.arrive %0
 __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
 
 // FAN = 0: no peer: the fan-out / multicast / packed-row code is not in the kernel at all (the dependent stream of one warp per
-// scheduler also pays for instruction fetch: 770 static instructions fewer on the single-GPU path, 0.4 us per step).
+// scheduler also pays for instruction fetch: several hundred static instructions fewer on the single-GPU path).
 // FAN = 2: multicast only -- the host has checked that num_envs is a multiple of 8 and the output rows are aligned, so every row
 // is a full wide store: local copy + ONE multimem.st, no per-peer loops, no element-wise fallback in the instruction stream.
 // FAN = 1: the general fan-out (per-peer stores; multicast for the rows that qualify).
@@ -560,7 +562,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             done = tmask != 0u;
             // fan-out active, full CTA, aligned rows: 32 + 8 + 8 contiguous bytes leave as four wide stores (one NVLink /
             // multicast write each instead of 24 small ones); otherwise element by element (without peers the staging round
-            // trip sits at the kernel's tail and costs 0.17 us per step, profiles/r02_kexp_pack.txt)
+            // trip would sit at the kernel's tail for nothing)
             const bool packed = (FAN == 2) || ((FAN == 1) && ((pf.n | pf.mc) != 0) && (env0 + WL_DUO_ENVS <= n) && ((reinterpret_cast<uintptr_t>(rew + env0) & 15u) == 0) &&
                                 (((reinterpret_cast<uintptr_t>(terminated_o + env0) | reinterpret_cast<uintptr_t>(truncated_o + env0)) & 7u) == 0));
             const uint8_t tb = (uint8_t)((tmask & ~1u) ? 1 : 0), ub = (uint8_t)((tmask & 1u) ? 1 : 0);
@@ -1074,9 +1076,8 @@ wl_scan_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUte
 }
 
 // ---------------------------------------------------------------------------------------
-// The same ray-caster as a TMA producer / consumer PIPELINE (wl_set_scan_tma(2); measured 13.2 us vs 12.4 us for one tile per
-// CTA at 4096 envs, 150 vs 135 us at 65536 -- 16 resident one-tile CTAs per SM already hide the set-up + TMA latency, and the
-// ray loop is issue-bound -- so it is NOT the default; profiles/r02_scan_ab.jsonl): persistent CTAs (a few per SM) walk the envs; warp 4 is
+// The same ray-caster as a TMA producer / consumer PIPELINE (wl_set_scan_tma(2); NOT the default: resident one-tile CTAs per
+// SM already hide the set-up + TMA latency, and the ray loop is issue-bound): persistent CTAs (a few per SM) walk the envs; warp 4 is
 // the producer -- it reads the next env's pose, forms the per-env constants and issues the cp.async.bulk.tensor.2d of that
 // env's window into the other shared-memory stage -- while warps 0..3 take the 676 rays of the current env out of the stage
 // that has landed.  full[s] (TMA transaction bytes) and empty[s] (one arrival per consumer warp) are mbarriers; the pose load,
@@ -1597,15 +1598,15 @@ wl_camera_kernel(const __grid_constant__ wl_config c, const float4* __restrict__
 }
 
 // ---------------------------------------------------------------------------------------
-// launch geometry: spread small N over all 148 SMs, use fatter CTAs once the chip is full
+// launch geometry: spread small N over all SMs, use fatter CTAs once the chip is full
 // ---------------------------------------------------------------------------------------
 // launch with (or without) the programmatic-dependent-launch attribute
-// (measured on B200, 4096-env Drift step, back-to-back launches: 9.0 us/step with the attribute vs 6.65 us without --
-// profiles/r02_kexp_c_pdl.jsonl -- the dependent grid's early-resident CTAs cost more than the launch gap they hide; the
-// attribute is therefore OFF unless WL_PDL=1)
+// (OFF unless WL_PDL=1; DESIGN.md 6e.  A kernel launched with it must wait (griddepcontrol.wait) before its first read of
+// anything a previous launch may have written: the thread, quad and act-step kernels do.  wl_step_duo_kernel does not --
+// a wait on its dependent chain costs more than PDL saves -- so it is always launched without the attribute.)
 static bool g_pdl = (getenv("WL_PDL") != nullptr) && (atoi(getenv("WL_PDL")) != 0);
 template <typename... KArgs, typename... Args>
-static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t cs, const Args&... args) {
+static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t cs, bool pdl, const Args&... args) {
     static_assert(sizeof...(KArgs) == sizeof...(Args), "argument count");
     cudaLaunchConfig_t lc;
     memset(&lc, 0, sizeof lc);
@@ -1613,7 +1614,7 @@ static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem,
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = attr; lc.numAttrs = g_pdl ? 1 : 0;
+    lc.attrs = attr; lc.numAttrs = pdl ? 1 : 0;
     // parameters by address: the 1.5 KB wl_config is read in place by the runtime, not copied through a by-value call chain.
     // (each argument must already have exactly the kernel's parameter type: checked below)
     static_assert((std::is_same<typename std::decay<KArgs>::type, typename std::decay<Args>::type>::value && ...), "argument types must match the kernel's");
@@ -1622,8 +1623,8 @@ static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem,
 }
 
 static inline int pick_block(int n) {
-    if (n >= 148 * 128 * 4) return 128;
-    if (n >= 148 * 64 * 2) return 64;
+    if (n >= WL_NUM_SMS * 128 * 4) return 128;
+    if (n >= WL_NUM_SMS * 64 * 2) return 64;
     return 32;
 }
 
@@ -1631,7 +1632,7 @@ static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
     const int n = sim->cfg.num_envs;
     if (sim->scan_mode == 2 && sim->has_tmap) {              // TMA producer/consumer pipeline, persistent CTAs
         static const int per_sm = [] { const char* e = getenv("WL_SCAN_CTAS_PER_SM"); int v = e ? atoi(e) : 6; return v < 1 ? 1 : (v > 12 ? 12 : v); }();
-        const int grid = n < 148 * per_sm ? n : 148 * per_sm;    // (WL_SCAN_CTAS_PER_SM: tuning experiments only)
+        const int grid = n < WL_NUM_SMS * per_sm ? n : WL_NUM_SMS * per_sm;    // (WL_SCAN_CTAS_PER_SM: tuning experiments only)
         wl_scan_pipe_kernel<<<grid, WL_SCAN_THREADS + 32, 0, cs>>>(sim->cfg, sim->tmap, sim->state, d_obs);
     } else if (sim->scan_mode >= 1 && sim->has_tmap)
         wl_scan_kernel<true><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->state, sim->hf, d_obs);
@@ -1653,7 +1654,7 @@ static int launch_camera(wl_sim* sim, float* d_obs, uint32_t t, uint32_t stream_
 extern "C" {
 
 const char* wl_last_error(void) { return g_err.c_str(); }
-const char* wl_build_info(void) { return "wheeledlab_b200 abi=2 arch=sm_100a fmad=false"; }
+const char* wl_build_info(void) { return "wheeledlab_b200 abi=2 arch=sm_90a fmad=false"; }
 size_t wl_config_sizeof(void) { return sizeof(wl_config); }
 
 const char* wl_config_describe(void) {
@@ -1938,11 +1939,11 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
         const bool rows_ok = (n % WL_DUO_ENVS) == 0 && (((uintptr_t)d_obs | (uintptr_t)d_rew) & 15u) == 0 &&
                              (((uintptr_t)d_terminated | (uintptr_t)d_truncated) & 7u) == 0;
         if (sim->fan.mc && rows_ok)
-            launch_k(wl_step_duo_kernel<2>, grid, 64, 0, cs, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<2>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else if (sim->fan.n > 0 || sim->fan.mc)
-            launch_k(wl_step_duo_kernel<1>, grid, 64, 0, cs, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<1>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else
-            launch_k(wl_step_duo_kernel<0>, grid, 64, 0, cs, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<0>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
     } else if (sim->fan.n > 0) {
         return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
     } else if (variant == 4) {
@@ -1950,14 +1951,14 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
 #define WL_QUAD_BS 32
 #endif
         const int bs = WL_QUAD_BS, threads = 4 * n, grid = (threads + bs - 1) / bs + 1;      // + the janitor CTA
-        if (elev) launch_k(wl_step_quad_kernel<WL_TASK_ELEVATION>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
-        else if (vis) launch_k(wl_step_quad_kernel<WL_TASK_VISUAL>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
-        else launch_k(wl_step_quad_kernel<WL_TASK_DRIFT>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
+        if (elev) launch_k(wl_step_quad_kernel<WL_TASK_ELEVATION>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
+        else if (vis) launch_k(wl_step_quad_kernel<WL_TASK_VISUAL>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
+        else launch_k(wl_step_quad_kernel<WL_TASK_DRIFT>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
     } else {
         const int bs = pick_block(n), grid = (n + bs - 1) / bs + 1;
-        if (elev) launch_k(wl_step_kernel<WL_TASK_ELEVATION, 0>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
-        else if (vis) launch_k(wl_step_kernel<WL_TASK_VISUAL, 0>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
-        else launch_k(wl_step_kernel<WL_TASK_DRIFT, 0>, grid, bs, 0, cs, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
+        if (elev) launch_k(wl_step_kernel<WL_TASK_ELEVATION, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
+        else if (vis) launch_k(wl_step_kernel<WL_TASK_VISUAL, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
+        else launch_k(wl_step_kernel<WL_TASK_DRIFT, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
     }
     WL_LAUNCH_CHECK(sim, "wl_step_kernel");
     if (elev) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
@@ -2062,7 +2063,7 @@ int wl_step_host(wl_sim* sim, const float* h_action, float* d_action, float* d_o
     return cuda_check(cudaStreamSynchronize(cs), "wl_step_host: stream synchronize");
 }
 
-// device alias of a pinned host block (cudaHostGetDevicePointer costs ~0.5 us per call: resolved once per block and cached)
+// device alias of a pinned host block (cudaHostGetDevicePointer is a driver call: resolved once per block and cached)
 static void* host_alias(wl_sim* sim, const void* h) {
     for (int k = 0; k < sim->hp_n; ++k) if (sim->hp_host[k] == h) return sim->hp_dev[k];
     void* d = nullptr;
@@ -2177,9 +2178,9 @@ int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, 
         attr_set[sim->device] = true;
     }
     if (sim->cfg.task == WL_TASK_VISUAL)
-        launch_k(wl_act_step_quad_kernel<WL_TASK_VISUAL>, grid, WL_ACT_THREADS, smem, cs, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
+        launch_k(wl_act_step_quad_kernel<WL_TASK_VISUAL>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
     else
-        launch_k(wl_act_step_quad_kernel<WL_TASK_DRIFT>, grid, WL_ACT_THREADS, smem, cs, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
+        launch_k(wl_act_step_quad_kernel<WL_TASK_DRIFT>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
     WL_LAUNCH_CHECK(sim, "wl_act_step_quad_kernel");
     return post_step(sim, step_counter, cs);
 }

@@ -4,7 +4,7 @@
 // One env's whole step lives in registers; HBM is touched once per group on the way in
 // and once on the way out (DESIGN.md "Kernels").
 //
-// Reference behaviour restated here (file:line under /root/reference/source):
+// Reference behaviour restated here (file:line under the reference's source/ directory):
 //   action term     wheeledlab/wheeledlab/envs/mdp/actions/ackermann_actions.py:119-145,150-201
 //                   wheeledlab/wheeledlab/envs/mdp/actions/rc_car_actions.py:12-29,36-64
 //   actuators       wheeledlab_assets/wheeledlab_assets/hound.py:4-52

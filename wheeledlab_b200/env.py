@@ -265,7 +265,7 @@ class ManagerBasedRLEnv:
     _RING = 512      # step() / step_host() output buffers are reused after this many steps (fewer when rows are wide, see _ring_len)
     _HOST_OBS_RING = 4   # pinned host observation buffers of step_host(host_obs=True)
 
-    metadata = {"render_modes": [None, "human", "rgb_array"], "isaac_sim_version": "b200-native"}
+    metadata = {"render_modes": [None, "human", "rgb_array"], "isaac_sim_version": "h100-native"}
 
     def __init__(self, cfg: TaskSpec | str = "Isaac-MushrDriftRL-v0", render_mode=None, device="cuda:0", **task_kw):
         self._task_spec: TaskSpec = make_task(cfg, **task_kw) if isinstance(cfg, str) else cfg

@@ -1,7 +1,7 @@
 """WheeledSim: thin, allocation-owning wrapper over the C-ABI (one handle = one GPU's env shard).
 
 torch is used for device memory and streams only; every computation is a launch of the
-hand-written sm_100a kernels in ``csrc/`` through ``libwheeledlab_b200.so``.
+hand-written sm_90a kernels in ``csrc/`` through ``libwheeledlab_b200.so``.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ G_PMASS, G_PMU_D, G_PMU_C, G_PKD, G_CMD, G_CMDB, G_PIW = 9, 10, 11, 12, 13, 14, 
 NUM_GROUPS = 16
 
 
-_raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)     # cudaStream_t as an int, ~0.3 us (Stream object: ~2 us)
+_raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)     # cudaStream_t as an int, cheaper than building a Stream object
 
 
 def _stream_ptr(device) -> C.c_void_p:

@@ -1,7 +1,7 @@
 """Task descriptions lowered to the POD ``wl_config`` the kernels consume.
 
 Every number below restates a value from the reference configuration (file:line under
-``/root/reference/source``); nothing is imported from the reference at run time.
+the reference's ``source/`` directory); nothing is imported from the reference at run time.
 
   gym ids            wheeledlab_tasks/wheeledlab_tasks/__init__.py:14-63
   Drift env          wheeledlab_tasks/wheeledlab_tasks/drifting/mushr_drift_env_cfg.py

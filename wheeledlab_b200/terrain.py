@@ -2,7 +2,7 @@
 
 The reference loads ``Terrains/huge_compact.usd`` (a 726 900-triangle mesh: a slab with top at z = 0.2 over
 +-20.5 m carrying ramps/boxes up to z = 2.0, slopes mostly 15-25 deg; SURVEY Appendix A.4/C) and collides /
-ray-casts against the triangles.  The B200 path works on a regular raster of the TOP surface (what a vertical
+ray-casts against the triangles.  The fused path works on a regular raster of the TOP surface (what a vertical
 ray from z+20 hits): ``procedural_heightfield`` synthesises a terrain with the same envelope (BASELINE config 3
 says "procedural terrain"); a raster of the real mesh can be passed instead (same array contract).
 
