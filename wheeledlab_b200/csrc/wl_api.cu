@@ -51,6 +51,18 @@ static int cuda_check(cudaError_t e, const char* what) {
     return fail(WL_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 
+// every kernel launch made through a handle is counted (wl_launch_count) and checked here
+static int launched(wl_sim* sim, const char* what, int count = 1) {
+    sim->launches += count;
+    return cuda_check(cudaGetLastError(), what);
+}
+// f(std::integral_constant<int, T>{}) for the first listed task T equal to `task`, else for WL_TASK_DRIFT: a caller
+// instantiates its kernel for the tasks it lists only
+template <int... TASKS, typename F>
+static void with_task(int task, F&& f) {
+    if (!((task == TASKS && (f(std::integral_constant<int, TASKS>{}), true)) || ...)) f(std::integral_constant<int, WL_TASK_DRIFT>{});
+}
+
 static inline void ensure_device(const wl_sim* sim) {
     int cur = -1;
     if (cudaGetDevice(&cur) == cudaSuccess && cur != sim->device) cudaSetDevice(sim->device);   // launches go to the handle's device
@@ -119,6 +131,17 @@ __device__ __forceinline__ void janitor(const wl_config& c, wl_globals* __restri
     if (lane < WL_MAX_REW_TERMS) gl->rew_weight[t & 1u][lane] = w;     // W(t), read by step t+1
     if (lane == 0) gl->log_ptr[t % 3u] = d_log;
 }
+// true in the janitor CTA, whose first warp has then run the janitor.  wts: W(t) when the caller has already loaded it.
+__device__ __forceinline__ bool janitor_cta(const wl_config& c, wl_globals* __restrict__ gl, uint32_t t, float* __restrict__ d_log,
+                                            const float* wts = nullptr) {
+    if (blockIdx.x != gridDim.x - 1) return false;
+    if (threadIdx.x < 32) {
+        float wj[WL_MAX_REW_TERMS];
+        if (wts == nullptr) { load_weights(c, gl, t, wj); wts = wj; }
+        janitor(c, gl, t, wts, d_log);
+    }
+    return true;
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -172,18 +195,16 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
     EnvState e;
     float wts[WL_MAX_REW_TERMS];            // W(t): issued with the state loads so the latency hides behind the integrator
     load_weights(c, gl, t, wts);
-    if (STAGE != 1 && blockIdx.x == gridDim.x - 1) {          // the janitor CTA (appended to the grid, owns no envs)
-        if (threadIdx.x < 32) janitor(c, gl, t, wts, d_log);
-        return;
-    }
+    if (STAGE != 1 && janitor_cta(c, gl, t, d_log, wts)) return;
     if (STAGE == 2) {
         if (i < n) {
             load_env(st, n, i, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
             tmask = sio.tmask[i];
             if (sio.extra_truncated && sio.extra_truncated[i]) tmask |= 1u;            // host-side time-out style term
             if (sio.extra_terminated && sio.extra_terminated[i]) tmask |= 0x80u;       // host-side termination term
-            terminated_o[i] = (tmask & ~1u) ? 1 : 0;
-            truncated_o[i] = (tmask & 1u) ? 1 : 0;
+            const DoneBytes db = done_bytes(tmask);
+            terminated_o[i] = db.terminated;
+            truncated_o[i] = db.truncated;
             done = tmask != 0u;
         }
     } else if (i < n) {
@@ -195,25 +216,11 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
         float wheel_target[4], steer_target[2];
         process_action(c, a.x, a.y, wheel_target, steer_target);
         // B. decimation x (actuators -> integrator)
-        Chassis b;
-        M3 R = rotmat(e.qw, e.qx, e.qy, e.qz);
-        V3 cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-        b.pc = V3{e.p.x + cw.x, e.p.y + cw.y, e.p.z + cw.z};
-        b.v = e.v; b.qw = e.qw; b.qx = e.qx; b.qy = e.qy; b.qz = e.qz;
-        b.wb = rotT(R, e.w);
+        Chassis b = chassis_from_env(c, e);
         StepConsts kc = make_step_consts<4>(c, e);
-        for (int d = 0; d < c.decimation; ++d) {
-            float lo[4], hi[4];
-#pragma unroll
-            for (int w = 0; w < 4; ++w) dc_limits(c, c.dc_effort[w], e.omega[w], lo[w], hi[w]);
-            for (int j = 0; j < c.substeps; ++j) physics_substep<TASK, 1>(c, T, e, b, wheel_target, lo, hi, steer_target, kc);
-        }
-        R = rotmat(b.qw, b.qx, b.qy, b.qz);
-        cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-        e.p = V3{b.pc.x - cw.x, b.pc.y - cw.y, b.pc.z - cw.z};
-        e.v = b.v; e.qw = b.qw; e.qx = b.qx; e.qy = b.qy; e.qz = b.qz;
-        e.w = rot(R, b.wb);
-        // C. counters   D. terminations   E. rewards (value = f*w*dt, skipped when w == 0)
+        run_substeps<TASK, 1>(c, T, e, b, wheel_target, c.dc_effort, steer_target, kc);
+        const M3 R = env_from_chassis(c, e, b);
+        // C. counters   D. terminations   E. rewards
         e.ep_len += 1;
         const bool time_out = e.ep_len >= c.max_episode_length;
         float f[WL_MAX_REW_TERMS];
@@ -225,25 +232,18 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
         } else {
             const bool oob = drift_off_track(c, e.p.x, e.p.y);
             drift_reward_terms(c, e.steer[0], e.steer[1], det_atan2(vb.y, vb.x), e.p, vb, b.wb, e.w.z, oob, time_out, f);
-            tmask = (time_out ? 1u : 0u) | (oob ? 2u : 0u);
+            tmask = drift_term_mask(time_out, oob);
         }
         tmask &= (uint32_t)c.term_enable;
-        float total = 0.0f;
-#pragma unroll
-        for (int k = 0; k < WL_MAX_REW_TERMS; ++k) {
-            if (k < c.num_rew_terms) {
-                float w = wts[k];
-                if (w != 0.0f) { float val = f[k] * w * c.d_step_dt; total += val; e.sums[k] += val; }
-            }
-        }
-        rew[i] = total;
+        rew[i] = weigh_rewards(c, wts, f, e.sums);
         if (STAGE == 1) {                    // cut: state (with this step's episode sums) back to HBM, term bits for stage 2
             sio.tmask[i] = (uint8_t)tmask;
             store_env(st, n, i, e, ELEV);
             return;
         }
-        terminated_o[i] = (tmask & ~1u) ? 1 : 0;
-        truncated_o[i] = (tmask & 1u) ? 1 : 0;
+        const DoneBytes db = done_bytes(tmask);
+        terminated_o[i] = db.terminated;
+        truncated_o[i] = db.truncated;
         if (STAGE == 0 && sio.tmask != nullptr) sio.tmask[i] = (uint8_t)tmask;      // per-term masks (wl_set_term_bits)
         done = tmask != 0u;
     }
@@ -252,9 +252,7 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
     log_accumulate(gl->acc[t % 3u], done, tmask, e.sums);
     if (i < n) {
         const uint32_t gid = (uint32_t)(c.env_id_offset + i);
-        if (done) {
-            if (ELEV) elev_reset_env(c, e, gid, t); else if (VIS) visual_reset_env(c, vm, e, gid, t); else drift_reset_env(c, e, gid, t);
-        }
+        if (done) reset_env(c, TASK, vm, e, gid, t);
         // G. commands   H. interval events (post-reset state)   I. observations
         if (VIS) {
             float o[8]; visual_proprio(c, e, o);
@@ -290,13 +288,26 @@ __device__ __forceinline__ float euler_lane(float qw, float qx, float qy, float 
     return wrap_2pi(ang);
 }
 
+// lane w of the quad of env i (n = c.num_envs).  A whole quad is live or not; a dead quad shadows the last env (ii, gid; it
+// stores nothing) so that the quad shuffles stay convergent.  base = the quad's first lane in the warp.
+struct QuadLane { int i, w; bool live; int ii; uint32_t gid; unsigned base; };
+__device__ __forceinline__ QuadLane quad_lane(const wl_config& c, int n, int i, int w) {
+    const bool live = i < n;
+    const int ii = live ? i : n - 1;
+    return QuadLane{i, w, live, ii, (uint32_t)(c.env_id_offset + ii), (threadIdx.x & 31u) & ~3u};
+}
+
 template <int TASK>
 __device__ __forceinline__ void quad_env_step(const wl_config& c, const Terrain& T, const VisualMap& vm, float* __restrict__ acc_row,
-                                              const float wts[WL_MAX_REW_TERMS], EnvState& e, int i, int w, bool live, uint32_t gid,
-                                              unsigned base, uint32_t t, float2 a, const float znoise[4], float* __restrict__ obs_row,
-                                              float* __restrict__ rew, uint8_t* __restrict__ terminated_o,
-                                              uint8_t* __restrict__ truncated_o, uint8_t* __restrict__ term_bits = nullptr) {
+                                              const float wts[WL_MAX_REW_TERMS], EnvState& e, const QuadLane& L, uint32_t t, float2 a,
+                                              const float znoise[4], float* __restrict__ obs_row, float* __restrict__ rew,
+                                              uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o,
+                                              uint8_t* __restrict__ term_bits = nullptr) {
     constexpr bool ELEV = (TASK == WL_TASK_ELEVATION), VIS = (TASK == WL_TASK_VISUAL);
+    const int i = L.i, w = L.w;
+    const bool live = L.live;
+    const uint32_t gid = L.gid;
+    const unsigned base = L.base;
     // A. action manager (redundant in the 4 lanes)
     e.prev_action[0] = e.action[0]; e.prev_action[1] = e.action[1];
     e.action[0] = a.x; e.action[1] = a.y;
@@ -306,24 +317,11 @@ __device__ __forceinline__ void quad_env_step(const wl_config& c, const Terrain&
     const float my_effort = (w == 0) ? c.dc_effort[0] : (w == 1) ? c.dc_effort[1] : (w == 2) ? c.dc_effort[2] : c.dc_effort[3];
     float my_steer_target[2] = {(w == 3) ? steer_target[1] : steer_target[0], 0.0f};
     // B. decimation x (actuators -> integrator)
-    Chassis b;
-    M3 R = rotmat(e.qw, e.qx, e.qy, e.qz);
-    V3 cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-    b.pc = V3{e.p.x + cw.x, e.p.y + cw.y, e.p.z + cw.z};
-    b.v = e.v; b.qw = e.qw; b.qx = e.qx; b.qy = e.qy; b.qz = e.qz;
-    b.wb = rotT(R, e.w);
+    Chassis b = chassis_from_env(c, e);
     StepConsts kc = make_step_consts<1>(c, e);
-    const float my_targets[4] = {my_target, 0.0f, 0.0f, 0.0f};
-    for (int d = 0; d < c.decimation; ++d) {
-        float lo[4], hi[4];
-        dc_limits(c, my_effort, e.omega[0], lo[0], hi[0]);
-        for (int j = 0; j < c.substeps; ++j) physics_substep<TASK, 4>(c, T, e, b, my_targets, lo, hi, my_steer_target, kc);
-    }
-    R = rotmat(b.qw, b.qx, b.qy, b.qz);
-    cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-    e.p = V3{b.pc.x - cw.x, b.pc.y - cw.y, b.pc.z - cw.z};
-    e.v = b.v; e.qw = b.qw; e.qx = b.qx; e.qy = b.qy; e.qz = b.qz;
-    e.w = rot(R, b.wb);
+    const float my_targets[4] = {my_target, 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
+    run_substeps<TASK, 4>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc);
+    M3 R = env_from_chassis(c, e, b);
     // C./D./E. counters, terminations, rewards (redundant in the 4 lanes)
     e.ep_len += 1;
     const bool time_out = e.ep_len >= c.max_episode_length;
@@ -340,7 +338,7 @@ __device__ __forceinline__ void quad_env_step(const wl_config& c, const Terrain&
         const float steer_l = __shfl_sync(0xffffffffu, e.steer[0], base + 2), steer_r = __shfl_sync(0xffffffffu, e.steer[0], base + 3);
         const bool oob = drift_off_track(c, e.p.x, e.p.y);
         drift_reward_terms(c, steer_l, steer_r, det_atan2(vb.y, vb.x), e.p, vb, b.wb, e.w.z, oob, time_out, f);
-        tmask = (time_out ? 1u : 0u) | (oob ? 2u : 0u);
+        tmask = drift_term_mask(time_out, oob);
     }
     // I'. observation inputs from the post-physics state, formed HERE so that this lane's euler atan2 overlaps the reward
     // terms' atan2 / sqrt chains in one basic block; an env that resets (or gets pushed) redoes them below -- the rare path
@@ -349,23 +347,17 @@ __device__ __forceinline__ void quad_env_step(const wl_config& c, const Terrain&
     if (!VIS) eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
     if (!VIS && !ELEV) wbo = rotT(R, e.w);                        // (R^T of the WORLD rate, as the oracle forms it: not b.wb bit for bit)
     tmask &= (uint32_t)c.term_enable;
-    float total = 0.0f;
-#pragma unroll
-    for (int k = 0; k < WL_MAX_REW_TERMS; ++k) {
-        if (k < c.num_rew_terms) {
-            float wgt = wts[k];
-            if (wgt != 0.0f) { float val = f[k] * wgt * c.d_step_dt; total += val; e.sums[k] += val; }
-        }
-    }
+    const float total = weigh_rewards(c, wts, f, e.sums);
     const bool done = tmask != 0u;
     if (live && w == 0) {
-        rew[i] = total; terminated_o[i] = (tmask & ~1u) ? 1 : 0; truncated_o[i] = (tmask & 1u) ? 1 : 0;
+        const DoneBytes db = done_bytes(tmask);
+        rew[i] = total; terminated_o[i] = db.terminated; truncated_o[i] = db.truncated;
         if (term_bits != nullptr) term_bits[i] = (uint8_t)tmask;      // per-term masks for TerminationManager.get_term
     }
     // F. per-step episode log: one contribution per env (lane 0 of each live quad), then auto-reset
     log_accumulate(acc_row, done && live && (w == 0), tmask, e.sums);
     if (done) {
-        if (ELEV) elev_reset_env(c, e, gid, t); else if (VIS) visual_reset_env(c, vm, e, gid, t); else drift_reset_env(c, e, gid, t);
+        reset_env(c, TASK, vm, e, gid, t);
         if (!VIS) eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
         if (!VIS && !ELEV) { R = rotmat(e.qw, e.qx, e.qy, e.qz); vb = rotT(R, e.v); wbo = rotT(R, e.w); }   // (the oracle's own operations: signed zeros)
     }
@@ -408,31 +400,23 @@ wl_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st
     const VisualMap vm = VIS ? visual_map(c, T.hf) : VisualMap{nullptr, nullptr};
     const int n = c.num_envs;
     const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-    const int i = tid >> 2, w = tid & 3;
-    const bool live = i < n;                 // a whole quad is live or not (blockDim is a multiple of 4)
-    const int ii = live ? i : n - 1;         // dead quads shadow the last env (no stores) so shuffles stay convergent
-    const uint32_t gid = (uint32_t)(c.env_id_offset + ii);
-    const unsigned base = (threadIdx.x & 31u) & ~3u;
+    const QuadLane L = quad_lane(c, n, tid >> 2, tid & 3);      // (blockDim is a multiple of 4)
     pdl_wait();
     const uint32_t t = decode_step(gl, t_arg);
-    float wts[WL_MAX_REW_TERMS];
-    if (blockIdx.x == gridDim.x - 1) {       // the janitor CTA (appended to the grid, owns no envs)
-        if (threadIdx.x < 32) { load_weights(c, gl, t, wts); janitor(c, gl, t, wts, d_log); }
-        return;
-    }
+    if (janitor_cta(c, gl, t, d_log)) return;
     EnvState e;
     QuadRaw raw;
-    quad_issue_loads(st, n, ii, w, raw, ELEV, c.dr_wheel_mass_enable != 0);
-    const float2 a = action[ii];
+    quad_issue_loads(st, n, L.ii, L.w, raw, ELEV, c.dr_wheel_mass_enable != 0);
+    const float2 a = action[L.ii];
+    float wts[WL_MAX_REW_TERMS];
     load_weights(c, gl, t, wts);
     // the observation noise depends on (env id, step) only: drawn here, while the state loads are in flight (nothing above
     // has consumed a loaded value yet)
     float zn[4];
-    if (!ELEV && !VIS) quad_obs_noise(c, w, gid, t, RNG_OBS, 0u, zn); else zn[0] = zn[1] = zn[2] = zn[3] = 0.0f;
-    quad_unpack(raw, w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
-    const int od = ELEV ? WL_OBS_DIM_ELEV : VIS ? WL_OBS_DIM_VISUAL + vis_cam_floats(c) : WL_OBS_DIM_BLIND;
-    quad_env_step<TASK>(c, T, vm, gl->acc[t % 3u], wts, e, i, w, live, gid, base, t, a, zn, obs + (size_t)od * ii, rew, terminated_o, truncated_o, term_bits);
-    if (live) store_env_quad(st, n, i, w, e, ELEV);
+    if (!ELEV && !VIS) quad_obs_noise(c, L.w, L.gid, t, RNG_OBS, 0u, zn); else zn[0] = zn[1] = zn[2] = zn[3] = 0.0f;
+    quad_unpack(raw, L.w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
+    quad_env_step<TASK>(c, T, vm, gl->acc[t % 3u], wts, e, L, t, a, zn, obs + (size_t)obs_row_floats(c, TASK) * L.ii, rew, terminated_o, truncated_o, term_bits);
+    if (L.live) store_env_quad(st, n, L.i, L.w, e, ELEV);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -473,10 +457,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     const int n = c.num_envs;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t t = decode_step(gl, t_arg);
-    if (blockIdx.x == gridDim.x - 1) {       // the janitor CTA (appended to the grid, owns no envs)
-        if (threadIdx.x < 32) { float wj[WL_MAX_REW_TERMS]; load_weights(c, gl, t, wj); janitor(c, gl, t, wj, d_log); }
-        return;
-    }
+    if (janitor_cta(c, gl, t, d_log)) return;
     const int env0 = blockIdx.x * WL_DUO_ENVS;
     const Terrain T{nullptr};
     if (warp == 1) {
@@ -551,21 +532,14 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             float f[WL_MAX_REW_TERMS];
             drift_reward_terms(c, fi[10], fi[11], det_atan2(vb.y, vb.x), p, vb, wb, fi[9], oob, time_out, f);
             tmask = raw & (uint32_t)c.term_enable;
-            float total = 0.0f;
-#pragma unroll
-            for (int k = 0; k < WL_MAX_REW_TERMS; ++k) {
-                if (k < c.num_rew_terms) {
-                    float wgt = wts[k];
-                    if (wgt != 0.0f) { float val = f[k] * wgt * c.d_step_dt; total += val; sums[k] += val; }
-                }
-            }
+            const float total = weigh_rewards(c, wts, f, sums);
             done = tmask != 0u;
             // fan-out active, full CTA, aligned rows: 32 + 8 + 8 contiguous bytes leave as four wide stores (one NVLink /
             // multicast write each instead of 24 small ones); otherwise element by element (without peers the staging round
             // trip would sit at the kernel's tail for nothing)
             const bool packed = (FAN == 2) || ((FAN == 1) && ((pf.n | pf.mc) != 0) && (env0 + WL_DUO_ENVS <= n) && ((reinterpret_cast<uintptr_t>(rew + env0) & 15u) == 0) &&
                                 (((reinterpret_cast<uintptr_t>(terminated_o + env0) | reinterpret_cast<uintptr_t>(truncated_o + env0)) & 7u) == 0));
-            const uint8_t tb = (uint8_t)((tmask & ~1u) ? 1 : 0), ub = (uint8_t)((tmask & 1u) ? 1 : 0);
+            const auto [tb, ub] = done_bytes(tmask);
             if (packed) {
                 sh.rewrow[lane] = total; sh.maskrow[0][lane] = tb; sh.maskrow[1][lane] = ub;
                 __syncwarp(0xffu);
@@ -590,12 +564,10 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         return;
     }
     // ================= env warp: the quad (lane = wheel), 8 envs =================
-    const int q = lane >> 2, w = lane & 3;
-    const int i = env0 + q;
-    const bool live = i < n;
-    const int ii = live ? i : n - 1;
-    const uint32_t gid = (uint32_t)(c.env_id_offset + ii);
-    const unsigned base = (unsigned)lane & ~3u;
+    const int q = lane >> 2;
+    const QuadLane L = quad_lane(c, n, env0 + q, lane & 3);
+    const int i = L.i, w = L.w, ii = L.ii;
+    const bool live = L.live;
     const bool wm = c.dr_wheel_mass_enable != 0;
     EnvState e;
     QuadRaw raw;
@@ -607,33 +579,20 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     e.action[0] = a.x; e.action[1] = a.y;
     const float my_effort = (w == 0) ? c.dc_effort[0] : (w == 1) ? c.dc_effort[1] : (w == 2) ? c.dc_effort[2] : c.dc_effort[3];
     // B. decimation x (actuators -> integrator)
-    Chassis b;
-    M3 R = rotmat(e.qw, e.qx, e.qy, e.qz);
-    V3 cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-    b.pc = V3{e.p.x + cw.x, e.p.y + cw.y, e.p.z + cw.z};
-    b.v = e.v; b.qw = e.qw; b.qx = e.qx; b.qy = e.qy; b.qz = e.qz;
-    b.wb = rotT(R, e.w);
+    Chassis b = chassis_from_env(c, e);
     StepConsts kc = make_step_consts<1>(c, e);
     bar_sync(1);
-    const float my_targets[4] = {sh.tgt[q][w], 0.0f, 0.0f, 0.0f};
+    const float my_targets[4] = {sh.tgt[q][w], 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
     const float my_steer_target[2] = {sh.tgt[q][(w == 3) ? 5 : 4], 0.0f};
-    for (int d = 0; d < c.decimation; ++d) {
-        float lo[4], hi[4];
-        dc_limits(c, my_effort, e.omega[0], lo[0], hi[0]);
-        for (int jj = 0; jj < c.substeps; ++jj) physics_substep<WL_TASK_DRIFT, 4>(c, T, e, b, my_targets, lo, hi, my_steer_target, kc);
-    }
-    R = rotmat(b.qw, b.qx, b.qy, b.qz);
-    cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
-    e.p = V3{b.pc.x - cw.x, b.pc.y - cw.y, b.pc.z - cw.z};
-    e.v = b.v; e.qw = b.qw; e.qx = b.qx; e.qy = b.qy; e.qz = b.qz;
-    e.w = rot(R, b.wb);
+    run_substeps<WL_TASK_DRIFT, 4>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc);
+    M3 R = env_from_chassis(c, e, b);
     // C./D. counters, terminations (the env warp needs `done` for the reset; the reward side lives in the aux warp)
     e.ep_len += 1;
     const bool time_out = e.ep_len >= c.max_episode_length;
     V3 vb = rotT(R, e.v);
-    const float steer_l = __shfl_sync(0xffffffffu, e.steer[0], base + 2), steer_r = __shfl_sync(0xffffffffu, e.steer[0], base + 3);
+    const float steer_l = __shfl_sync(0xffffffffu, e.steer[0], L.base + 2), steer_r = __shfl_sync(0xffffffffu, e.steer[0], L.base + 3);
     const bool oob = drift_off_track(c, e.p.x, e.p.y);
-    const uint32_t raw_mask = (time_out ? 1u : 0u) | (oob ? 2u : 0u);
+    const uint32_t raw_mask = drift_term_mask(time_out, oob);
     if (w == 0) {
         float* fo = sh.fin[q];
         fo[0] = e.p.x; fo[1] = e.p.y; fo[2] = e.p.z; fo[3] = vb.x; fo[4] = vb.y; fo[5] = vb.z;
@@ -647,7 +606,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     const bool done = (raw_mask & (uint32_t)c.term_enable) != 0u;
     // F. auto-reset (sums and log: aux warp)
     if (done) {
-        drift_reset_env(c, e, gid, t);
+        drift_reset_env(c, e, L.gid, t);
         eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
         R = rotmat(e.qw, e.qx, e.qy, e.qz); vb = rotT(R, e.v); wbo = rotT(R, e.w);
     }
@@ -712,20 +671,32 @@ static int policy_offsets(int obs_dim, int32_t off[13]) {
     return p;
 }
 
-__device__ __forceinline__ void mbar_init(uint64_t* b) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(b))); }
+// ---- shared-memory mbarriers and TMA copies that complete on them (one definition of each PTX form) --------------------
+// mbar_init_fence makes the initialised barriers visible to the async proxy before any copy names them
+__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count));
+}
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void mbar_expect(uint64_t* b, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* b) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* b) {       // phase 0 (each barrier is used once per launch)
+__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory"); }
+__device__ __forceinline__ void mbar_wait_parity(uint64_t* b, uint32_t parity) {
     const uint32_t mb = smem_u32(b);
     uint32_t ok = 0;
     while (!ok)
         asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(mb), "r"(0u) : "memory");
+                     : "=r"(ok) : "r"(mb), "r"(parity) : "memory");
+}
+// 1-D bulk copy global -> shared
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* b) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(b)) : "memory");
+}
+// the box of the 2-D tensor map at element (x, y) -> shared
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tmap, int x, int y, uint64_t* b) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(smem_u32(dst)), "l"(tmap), "r"(x), "r"(y), "r"(smem_u32(b)) : "memory");
 }
 __device__ __forceinline__ float elu(float x) { return x > 0.0f ? x : __expf(x) - 1.0f; }
 
@@ -779,7 +750,7 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     __shared__ __align__(8) uint64_t mbar[2];
     pdl_trigger();
     pdl_wait();
-    if (blockIdx.x == gridDim.x - 1) {                       // the janitor CTA (appended to the grid, owns no envs)
+    if (blockIdx.x == gridDim.x - 1) {                       // the janitor CTA; the step is decoded in its branch only
         if (threadIdx.x < 32) {
             const uint32_t tj = decode_step(gl, t_arg);
             float wj[WL_MAX_REW_TERMS];
@@ -793,8 +764,8 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     // ---- bulk async copies (TMA, 1-D) bring the blob from L2 into shared memory while the env state loads fly: the two
     // first-layer blocks (7.5 KB) complete on mbar[0], everything else (34 KB) on mbar[1] and lands during layer 1
     if (threadIdx.x == 0) {
-        mbar_init(&mbar[0]); mbar_init(&mbar[1]);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
+        mbar_init_fence();
         const int a0 = po_off.o[0], a1 = po_off.o[2], c0 = po_off.o[6], c1 = po_off.o[8];
         mbar_expect(&mbar[0], (uint32_t)((a1 - a0) + (c1 - c0)) * 4u);
         bulk_g2s(sw + a0, blob + a0, (uint32_t)(a1 - a0) * 4u, &mbar[0]);
@@ -807,16 +778,12 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     const VisualMap vm = VIS ? visual_map(c, T.hf) : VisualMap{nullptr, nullptr};
     const int n = c.num_envs;
     const bool stepper = threadIdx.x < 4 * WL_ACT_ENVS;      // warps 0..3 own the env quads; warps 4..7 only help with the MLPs
-    const int q = (threadIdx.x >> 2) & (WL_ACT_ENVS - 1), w = threadIdx.x & 3;
-    const int i = blockIdx.x * WL_ACT_ENVS + q;
-    const bool live = i < n;
-    const int ii = live ? i : n - 1;
-    const uint32_t gid = (uint32_t)(c.env_id_offset + ii);
-    const unsigned base = (threadIdx.x & 31u) & ~3u;
+    const int q = (threadIdx.x >> 2) & (WL_ACT_ENVS - 1);
+    const QuadLane L = quad_lane(c, n, blockIdx.x * WL_ACT_ENVS + q, threadIdx.x & 3);
     EnvState e;
     float wts[WL_MAX_REW_TERMS];
     if (stepper) {
-        load_env_quad(st, n, ii, w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
+        load_env_quad(st, n, L.ii, L.w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
         load_weights(c, gl, t, wts);
     }
     for (int k = threadIdx.x; k < WL_ACT_ENVS * 16; k += WL_ACT_THREADS) {
@@ -826,12 +793,12 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     // the policy noise does not depend on the weights: draw it while the copies are in flight
     float z0 = 0.0f, z1 = 0.0f, zn[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     if (stepper) {
-        const uint4 r = philox4x32(c.seed, gid, t, RNG_POLICY, 0u);
+        const uint4 r = philox4x32(c.seed, L.gid, t, RNG_POLICY, 0u);
         box_muller(r.x, r.y, z0, z1);
-        if (!ELEV && !VIS) quad_obs_noise(c, w, gid, t, RNG_OBS, 0u, zn);
+        if (!ELEV && !VIS) quad_obs_noise(c, L.w, L.gid, t, RNG_OBS, 0u, zn);
     }
     __syncthreads();                                         // mbarrier init visible to every waiter; obs rows written
-    mbar_wait(&mbar[0]);
+    mbar_wait_parity(&mbar[0], 0);
     // ---- MLPs: warp k takes envs 4k..4k+3 of the CTA; its 32 lanes tile the 128 (actor | critic) hidden columns 4 at a
     // time, so a lane holds 4 units x 4 envs in registers.  Layer exchanges stay warp-local (__syncwarp).  W1t has obs_dim
     // rows; rows obs_dim..nin1-1 read whatever follows in the blob and meet the zero padding of x.
@@ -846,7 +813,7 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
         mlp_tile_layer(sw + oW1 + ucol, sw + oB1 + ucol, sx + env0 * WL_ACT_XS, WL_ACT_XS, nin1, acc);
         mlp_tile_store_elu(h0 + ucol, WL_ACT_HS, acc);
         __syncwarp();
-        mbar_wait(&mbar[1]);                                 // layer-2 / head weights have landed (copy overlapped layer 1)
+        mbar_wait_parity(&mbar[1], 0);                          // layer-2 / head weights have landed (copy overlapped layer 1)
         mlp_tile_layer(sw + oW2 + ucol, sw + oB2 + ucol, h0, WL_ACT_HS, WL_HID, acc);
         __syncwarp();                                        // every lane has finished reading layer-1 activations
         mlp_tile_store_elu(h0 + ucol, WL_ACT_HS, acc);
@@ -859,7 +826,7 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
         float m0 = 0.0f, m1 = 0.0f, vv = 0.0f;
 #pragma unroll
         for (int u = 0; u < 16; ++u) {
-            const int j = 16 * w + u;
+            const int j = 16 * L.w + u;
             const float xa = hrow[j], xc = hrow[WL_HID + j];
             m0 = fmaf(w3a[2 * j], xa, m0); m1 = fmaf(w3a[2 * j + 1], xa, m1);
             vv = fmaf(w3c[j], xc, vv);
@@ -871,16 +838,15 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
         // Gaussian head: a = mean + std * z (rsl_rl ActorCritic.act), log-prob summed over the action dims
         const float s0 = sw[po_off.o[12]], s1 = sw[po_off.o[12] + 1];
         const float2 a = make_float2(fmaf(s0, z0, m0), fmaf(s1, z1, m1));
-        if (live && w == 0) {
-            reinterpret_cast<float2*>(po.actions)[i] = a;
-            reinterpret_cast<float2*>(po.mean)[i] = make_float2(m0, m1);
-            po.log_prob[i] = -0.5f * (z0 * z0 + z1 * z1) - __logf(s0) - __logf(s1) - 1.8378770664093453f;   // 2 * 0.5 log(2 pi)
-            po.value[i] = vv;
+        if (L.live && L.w == 0) {
+            reinterpret_cast<float2*>(po.actions)[L.i] = a;
+            reinterpret_cast<float2*>(po.mean)[L.i] = make_float2(m0, m1);
+            po.log_prob[L.i] = -0.5f * (z0 * z0 + z1 * z1) - __logf(s0) - __logf(s1) - 1.8378770664093453f;   // 2 * 0.5 log(2 pi)
+            po.value[L.i] = vv;
         }
         // ---- the env step on the sampled action
-        const int od = ELEV ? WL_OBS_DIM_ELEV : VIS ? WL_OBS_DIM_VISUAL + vis_cam_floats(c) : WL_OBS_DIM_BLIND;
-        quad_env_step<TASK>(c, T, vm, gl->acc[t % 3u], wts, e, i, w, live, gid, base, t, a, zn, obs + (size_t)od * ii, rew, terminated_o, truncated_o);
-        if (live) store_env_quad(st, n, i, w, e, ELEV);
+        quad_env_step<TASK>(c, T, vm, gl->acc[t % 3u], wts, e, L, t, a, zn, obs + (size_t)obs_row_floats(c, TASK) * L.ii, rew, terminated_o, truncated_o);
+        if (L.live) store_env_quad(st, n, L.i, L.w, e, ELEV);
     }
 }
 
@@ -900,33 +866,28 @@ wl_rollout_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__
     const VisualMap vm = VIS ? visual_map(c, T.hf) : VisualMap{nullptr, nullptr};
     const int n = c.num_envs;
     const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-    const int i = tid >> 2, w = tid & 3;
-    const bool live = i < n;
-    const int ii = live ? i : n - 1;
-    const uint32_t gid = (uint32_t)(c.env_id_offset + ii);
-    const unsigned base = (threadIdx.x & 31u) & ~3u;
+    const QuadLane L = quad_lane(c, n, tid >> 2, tid & 3);
     EnvState e;
-    load_env_quad(st, n, ii, w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
+    load_env_quad(st, n, L.ii, L.w, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
     float wts[WL_MAX_REW_TERMS];             // W(t0) holds for the whole window (it never crosses an episode boundary)
     load_weights(c, gl, t0, wts);
     if (blockIdx.x == 0 && threadIdx.x < 32) janitor(c, gl, t0, wts, nullptr);      // flushes step t0-1's log row
-    const int od = ELEV ? WL_OBS_DIM_ELEV : VIS ? WL_OBS_DIM_VISUAL + vis_cam_floats(c) : WL_OBS_DIM_BLIND;
+    const int od = obs_row_floats(c, TASK);
     for (int k = 0; k < K; ++k) {
         const uint32_t t = t0 + (uint32_t)k;
         float2 a;
-        if (action != nullptr) a = action[(size_t)k * n + ii];
+        if (action != nullptr) a = action[(size_t)k * n + L.ii];
         else {
-            uint4 r = philox4x32(c.seed, gid, t, RNG_ACTION, 0u);
+            uint4 r = philox4x32(c.seed, L.gid, t, RNG_ACTION, 0u);
             a = make_float2(2.0f * u01(r.x) - 1.0f, 2.0f * u01(r.y) - 1.0f);
         }
-        if (act_out != nullptr && live && w == 0) act_out[(size_t)k * n + i] = a;
+        if (act_out != nullptr && L.live && L.w == 0) act_out[(size_t)k * n + L.i] = a;
         float zn[4];
-        if (!ELEV && !VIS) quad_obs_noise(c, w, gid, t, RNG_OBS, 0u, zn); else zn[0] = zn[1] = zn[2] = zn[3] = 0.0f;
-        quad_env_step<TASK>(c, T, vm, d_log + (size_t)k * WL_LOG_FLOATS, wts, e, i, w, live, gid, base, t, a, zn,
-                            obs + ((size_t)k * n + ii) * od, rew + (size_t)k * n, terminated_o + (size_t)k * n,
-                            truncated_o + (size_t)k * n);
+        if (!ELEV && !VIS) quad_obs_noise(c, L.w, L.gid, t, RNG_OBS, 0u, zn); else zn[0] = zn[1] = zn[2] = zn[3] = 0.0f;
+        quad_env_step<TASK>(c, T, vm, d_log + (size_t)k * WL_LOG_FLOATS, wts, e, L, t, a, zn, obs + ((size_t)k * n + L.ii) * od,
+                            rew + (size_t)k * n, terminated_o + (size_t)k * n, truncated_o + (size_t)k * n);
     }
-    if (live) store_env_quad(st, n, i, w, e, ELEV);
+    if (L.live) store_env_quad(st, n, L.i, L.w, e, ELEV);
     // last CTA (ticket, amortised over the K steps of the launch): turn the K accumulator rows into means and leave the
     // globals as K single steps would have: W of the last step in its slot, its reset count where the next launch looks for
     // it (the curriculum boundary at t0 + K is evaluated there), nothing pending for the log, the next row re-armed
@@ -975,6 +936,22 @@ wl_rollout_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__
 // the tile, the miss value selected at the end) and fully unrolled so that the compiler interleaves them: the loop is bound by
 // instruction latency (F2I, LDS, dependent FFMAs), not by bytes.  Per-ray arithmetic unchanged (bit-identical outputs).
 struct ScanPose { float bx, by, bz, cy, sy, pz; int ox, oy; };
+// the scan constants of env i: ray-caster parent = base_link (root + R (0,0,base_link_z)), yaw of the yaw-aligned rays
+// (attach_yaw_only), and the window origin (in samples), which covers base +- (half*sqrt2 + 1 cell)
+__device__ __forceinline__ ScanPose scan_pose(const wl_config& c, const float4* __restrict__ st, int n, int i) {
+    const float inv = c.d_inv_hf_cell;
+    float4 g0 = ldg4(st, WL_G_POS, n, i), g1 = ldg4(st, WL_G_QUAT, n, i);
+    EnvState e0; e0.p = V3{g0.x, g0.y, g0.z}; e0.qw = g1.x; e0.qx = g1.y; e0.qy = g1.z; e0.qz = g1.w;
+    M3 R = rotmat(e0.qw, e0.qx, e0.qy, e0.qz);
+    ScanPose q;
+    q.bx = fm(c.base_link_z, R.r[2], e0.p.x); q.by = fm(c.base_link_z, R.r[5], e0.p.y); q.bz = fm(c.base_link_z, R.r[8], e0.p.z);
+    yaw_cs(e0, q.cy, q.sy);
+    q.pz = e0.p.z;
+    const float reach = c.scan_half * 1.41421356237f + c.hf_cell;
+    q.ox = ((int)floorf((q.bx - reach - c.hf_x0) * inv)) & ~3;      // two's complement: rounds toward -inf
+    q.oy = (int)floorf((q.by - reach - c.hf_y0) * inv);
+    return q;
+}
 __device__ __forceinline__ void scan_rays(const wl_config& c, const float* __restrict__ tl, const ScanPose& q, float* __restrict__ row, int tid) {
     constexpr int ITER = (WL_SCAN_RAYS + WL_SCAN_THREADS - 1) / WL_SCAN_THREADS;
     const float inv = c.d_inv_hf_cell;
@@ -1027,52 +1004,31 @@ __global__ void __launch_bounds__(WL_SCAN_THREADS, 8)
 wl_scan_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const float4* __restrict__ st,
                const float* __restrict__ hf, float* __restrict__ obs) {
     __shared__ __align__(128) float tile[WL_TILE_W * WL_TILE_H];
-    __shared__ __align__(8) unsigned long long mbar;
-    __shared__ float sp[8];                  // per-env constants of the scan, formed ONCE by thread 0: bx by bz cy sy pz ox oy
-    const int n = c.num_envs;
+    __shared__ __align__(8) uint64_t mbar;
+    __shared__ ScanPose sp;                  // per-env constants of the scan, formed ONCE by thread 0
     const int i = blockIdx.x;
-    const float inv = c.d_inv_hf_cell;
     if (threadIdx.x == 0) {
-        float4 g0 = ldg4(st, WL_G_POS, n, i), g1 = ldg4(st, WL_G_QUAT, n, i);
-        EnvState e0; e0.p = V3{g0.x, g0.y, g0.z}; e0.qw = g1.x; e0.qx = g1.y; e0.qy = g1.z; e0.qz = g1.w;
-        M3 R = rotmat(e0.qw, e0.qx, e0.qy, e0.qz);
-        // ray-caster parent = base_link (root + R (0,0,base_link_z)); rays are yaw-aligned (attach_yaw_only)
-        const float bx0 = fm(c.base_link_z, R.r[2], e0.p.x), by0 = fm(c.base_link_z, R.r[5], e0.p.y), bz0 = fm(c.base_link_z, R.r[8], e0.p.z);
-        float cy0, sy0; yaw_cs(e0, cy0, sy0);
-        // window origin (in samples): covers base +- (half*sqrt2 + 1 cell)
-        const float reach = c.scan_half * 1.41421356237f + c.hf_cell;
-        const int ox0 = ((int)floorf((bx0 - reach - c.hf_x0) * inv)) & ~3;      // two's complement: rounds toward -inf
-        const int oy0 = (int)floorf((by0 - reach - c.hf_y0) * inv);
-        sp[0] = bx0; sp[1] = by0; sp[2] = bz0; sp[3] = cy0; sp[4] = sy0; sp[5] = e0.p.z; sp[6] = __int_as_float(ox0); sp[7] = __int_as_float(oy0);
+        const ScanPose p = scan_pose(c, st, c.num_envs, i);
+        sp = p;
         if (USE_TMA) {
-            const uint32_t mb = smem_u32(&mbar), dst = smem_u32(tile);
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mb));
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"((uint32_t)(WL_TILE_W * WL_TILE_H * 4)) : "memory");
-            asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                         ::"r"(dst), "l"(&tmap), "r"(ox0), "r"(oy0), "r"(mb) : "memory");
+            mbar_init(&mbar, 1);
+            mbar_init_fence();
+            mbar_expect(&mbar, WL_TILE_W * WL_TILE_H * 4);
+            tma_load_2d(tile, &tmap, p.ox, p.oy, &mbar);
         }
     }
     __syncthreads();                         // constants + mbarrier visible to everyone
-    const float bx = sp[0], by = sp[1], bz = sp[2], cy = sp[3], sy = sp[4], pz = sp[5];
-    const int ox = __float_as_int(sp[6]), oy = __float_as_int(sp[7]);
+    const ScanPose q = sp;
     if (USE_TMA) {
-        const uint32_t mb = smem_u32(&mbar);     // all threads wait for the bytes (phase 0)
-        uint32_t ok = 0;
-        while (!ok) {
-            asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                         : "=r"(ok) : "r"(mb), "r"(0u) : "memory");
-        }
+        mbar_wait_parity(&mbar, 0);          // all threads wait for the bytes
     } else {
         for (int k = threadIdx.x; k < WL_TILE_W * WL_TILE_H; k += WL_SCAN_THREADS) {
-            int tx = k % WL_TILE_W, ty = k / WL_TILE_W, gx = ox + tx, gy = oy + ty;
+            int tx = k % WL_TILE_W, ty = k / WL_TILE_W, gx = q.ox + tx, gy = q.oy + ty;
             tile[k] = (gx >= 0 && gy >= 0 && gx < c.hf_nx && gy < c.hf_ny) ? __ldg(hf + (size_t)gy * c.hf_pitch + gx) : 0.0f;
         }
         __syncthreads();
     }
-    float* row = obs + (size_t)WL_OBS_DIM_ELEV * i + 13;
-    ScanPose q{bx, by, bz, cy, sy, pz, ox, oy};
-    scan_rays(c, tile, q, row, threadIdx.x);
+    scan_rays(c, tile, q, obs + (size_t)WL_OBS_DIM_ELEV * i + 13, threadIdx.x);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1085,29 +1041,20 @@ wl_scan_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUte
 // Rays are taken in linear order (r = thread + 128 j: all 32 lanes busy, fully coalesced stores).  Same arithmetic.
 // ---------------------------------------------------------------------------------------
 #define WL_SCAN_STAGES 2
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory"); }
-__device__ __forceinline__ void mbar_wait_parity(uint64_t* b, uint32_t parity) {
-    const uint32_t mb = smem_u32(b);
-    uint32_t ok = 0;
-    while (!ok)
-        asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                     : "=r"(ok) : "r"(mb), "r"(parity) : "memory");
-}
 __global__ void __launch_bounds__(WL_SCAN_THREADS + 32)
 wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const float4* __restrict__ st,
                     float* __restrict__ obs) {
     __shared__ __align__(128) float tile[WL_SCAN_STAGES][WL_TILE_W * WL_TILE_H];
     __shared__ __align__(8) uint64_t full[WL_SCAN_STAGES], empty[WL_SCAN_STAGES];
-    __shared__ float sp[WL_SCAN_STAGES][8];                  // bx by bz cy sy pz ox oy of the env in the stage
+    __shared__ ScanPose sp[WL_SCAN_STAGES];                  // the scan constants of the env in the stage
     const int n = c.num_envs;
-    const float inv = c.d_inv_hf_cell;
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int s = 0; s < WL_SCAN_STAGES; ++s) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&full[s])));
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(&empty[s])), "r"(WL_SCAN_THREADS / 32));
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], WL_SCAN_THREADS / 32);
         }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1119,20 +1066,10 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
             const int s = k % WL_SCAN_STAGES;
             const uint32_t ph = (uint32_t)(k / WL_SCAN_STAGES) & 1u;
             mbar_wait_parity(&empty[s], ph ^ 1u);                        // stage free (passes at once on its first use)
-            float4 g0 = ldg4(st, WL_G_POS, n, i), g1 = ldg4(st, WL_G_QUAT, n, i);
-            EnvState e0; e0.p = V3{g0.x, g0.y, g0.z}; e0.qw = g1.x; e0.qx = g1.y; e0.qy = g1.z; e0.qz = g1.w;
-            M3 R = rotmat(e0.qw, e0.qx, e0.qy, e0.qz);
-            const float bx0 = fm(c.base_link_z, R.r[2], e0.p.x), by0 = fm(c.base_link_z, R.r[5], e0.p.y), bz0 = fm(c.base_link_z, R.r[8], e0.p.z);
-            float cy0, sy0; yaw_cs(e0, cy0, sy0);
-            const float reach = c.scan_half * 1.41421356237f + c.hf_cell;
-            const int ox0 = ((int)floorf((bx0 - reach - c.hf_x0) * inv)) & ~3;
-            const int oy0 = (int)floorf((by0 - reach - c.hf_y0) * inv);
-            float* p = sp[s];
-            p[0] = bx0; p[1] = by0; p[2] = bz0; p[3] = cy0; p[4] = sy0; p[5] = e0.p.z; p[6] = __int_as_float(ox0); p[7] = __int_as_float(oy0);
-            const uint32_t mb = smem_u32(&full[s]), dst = smem_u32(tile[s]);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"((uint32_t)(WL_TILE_W * WL_TILE_H * 4)) : "memory");
-            asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                         ::"r"(dst), "l"(&tmap), "r"(ox0), "r"(oy0), "r"(mb) : "memory");
+            const ScanPose p = scan_pose(c, st, n, i);
+            sp[s] = p;
+            mbar_expect(&full[s], WL_TILE_W * WL_TILE_H * 4);
+            tma_load_2d(tile[s], &tmap, p.ox, p.oy, &full[s]);
         }
         return;
     }
@@ -1142,12 +1079,8 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
         const int s = k % WL_SCAN_STAGES;
         const uint32_t ph = (uint32_t)(k / WL_SCAN_STAGES) & 1u;
         mbar_wait_parity(&full[s], ph);
-        const float bx = sp[s][0], by = sp[s][1], bz = sp[s][2], cy = sp[s][3], sy = sp[s][4], pz = sp[s][5];
-        const int ox = __float_as_int(sp[s][6]), oy = __float_as_int(sp[s][7]);
-        const float* tl = tile[s];
-        float* row = obs + (size_t)WL_OBS_DIM_ELEV * i + 13;
-        ScanPose q{bx, by, bz, cy, sy, pz, ox, oy};
-        scan_rays(c, tl, q, row, threadIdx.x);
+        const ScanPose q = sp[s];
+        scan_rays(c, tile[s], q, obs + (size_t)WL_OBS_DIM_ELEV * i + 13, threadIdx.x);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);                           // this warp is done with the stage
     }
@@ -1213,9 +1146,7 @@ __global__ void wl_reset_kernel(const __grid_constant__ wl_config c, float4* __r
     EnvState e;
     const bool elev = c.task == WL_TASK_ELEVATION;
     load_env(st, n, i, e, elev);
-    if (elev) elev_reset_env(c, e, (uint32_t)(c.env_id_offset + i), t);      // command b-frame vector is NOT refreshed by reset()
-    else if (c.task == WL_TASK_VISUAL) visual_reset_env(c, visual_map(c, aux), e, (uint32_t)(c.env_id_offset + i), t);
-    else drift_reset_env(c, e, (uint32_t)(c.env_id_offset + i), t);
+    reset_env(c, c.task, visual_map(c, aux), e, (uint32_t)(c.env_id_offset + i), t);      // (elevation: the command b-frame vector is NOT refreshed by reset())
     store_env(st, n, i, e, elev);
 }
 
@@ -1638,8 +1569,7 @@ static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
         wl_scan_kernel<true><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->state, sim->hf, d_obs);
     else
         wl_scan_kernel<false><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->state, sim->hf, d_obs);
-    sim->launches++;
-    return cuda_check(cudaGetLastError(), "wl_scan_kernel");
+    return launched(sim, "wl_scan_kernel");
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1647,8 +1577,7 @@ static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
 // ---------------------------------------------------------------------------------------
 static int launch_camera(wl_sim* sim, float* d_obs, uint32_t t, uint32_t stream_id, uint32_t sub, const float* d_aug, cudaStream_t cs) {
     wl_camera_kernel<<<sim->cfg.num_envs, WL_CAM_THREADS, 0, cs>>>(sim->cfg, sim->state, sim->globals, sim->hf, d_obs, t, stream_id, sub, d_aug);
-    sim->launches++;
-    return cuda_check(cudaGetLastError(), "wl_camera_kernel");
+    return launched(sim, "wl_camera_kernel");
 }
 
 extern "C" {
@@ -1675,6 +1604,7 @@ const char* wl_config_describe(void) {
 
 int wl_set_step_counter(wl_sim* sim, int64_t value, void* stream) {
     if (!sim) return fail(WL_EINVAL, "wl_set_step_counter: null handle");
+    ensure_device(sim);
     const uint32_t v = (uint32_t)value;
     sim->base_host = value;
     return cuda_check(cudaMemcpyAsync(&sim->globals->step_base, &v, sizeof v, cudaMemcpyHostToDevice, (cudaStream_t)stream),
@@ -1684,9 +1614,8 @@ int wl_advance_counter(wl_sim* sim, int32_t K, void* stream) {
     if (!sim || K < 0) return fail(WL_EINVAL, "wl_advance_counter: bad argument");
     ensure_device(sim);
     wl_advance_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(sim->globals, (uint32_t)K);
-    sim->launches++;
     sim->base_host += K;
-    return cuda_check(cudaGetLastError(), "wl_advance_kernel");
+    return launched(sim, "wl_advance_kernel");
 }
 int wl_note_device_counter(wl_sim* sim, int64_t value) {
     if (!sim) return fail(WL_EINVAL, "wl_note_device_counter: null handle");
@@ -1699,8 +1628,7 @@ int wl_log_flush(wl_sim* sim, void* stream) {
     ensure_device(sim);
     if (sim->last_t < 0) return WL_OK;
     wl_flush_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(sim->cfg, sim->globals, (uint32_t)(sim->last_t + 1));
-    sim->launches++;
-    return cuda_check(cudaGetLastError(), "wl_flush_kernel");
+    return launched(sim, "wl_flush_kernel");
 }
 float* wl_reward_weights(wl_sim* sim) { return sim ? sim->globals->rew_weight[(uint32_t)sim->last_t & 1u] : nullptr; }
 
@@ -1836,7 +1764,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
         if (cr != CUDA_SUCCESS) { delete s; return fail(WL_ECUDA, "cuTensorMapEncodeTiled failed (code " + std::to_string((int)cr) + ")"); }
         s->has_tmap = true;
     }
-    s->obs_dim = (cfg->task == WL_TASK_ELEVATION) ? WL_OBS_DIM_ELEV : (cfg->task == WL_TASK_VISUAL) ? WL_OBS_DIM_VISUAL + (cfg->vis_cam ? cfg->vis_cam_w * (cfg->vis_cam_h - cfg->vis_cam_row0) : 0) : WL_OBS_DIM_BLIND;
+    s->obs_dim = obs_row_floats(*cfg, cfg->task);
     // live reward weights
     for (int slot = 0; slot < 2; ++slot)
         if (int rc = cuda_check(cudaMemcpy(s->globals->rew_weight[slot], cfg->rew_weight, sizeof(float) * WL_MAX_REW_TERMS,
@@ -1866,12 +1794,6 @@ int wl_set_kernel_variant(wl_sim* sim, int32_t lanes_per_env) {
 }
 int64_t wl_launch_count(const wl_sim* sim) { return sim ? sim->launches : 0; }
 
-#define WL_LAUNCH_CHECK(sim, what)                                                     \
-    do {                                                                               \
-        (sim)->launches++;                                                             \
-        if (int rc_ = cuda_check(cudaGetLastError(), what)) return rc_;                \
-    } while (0)
-
 }   // extern "C"
 // Steps are issued with consecutive counters (the janitor protocol, see wl_globals).  Resolve this launch's counter on the host
 // mirror; on a jump publish the pending log row, carry the weights to the slot the step will read and clear the rows.
@@ -1882,8 +1804,7 @@ static int prep_step(wl_sim* sim, int64_t step_counter, int32_t n_steps, cudaStr
     if (t != sim->last_t + 1) {
         if (sim->last_t >= 0) wl_flush_kernel<<<1, 32, 0, cs>>>(sim->cfg, sim->globals, (uint32_t)(sim->last_t + 1));
         wl_rearm_kernel<<<1, 32, 0, cs>>>(sim->globals, (uint32_t)sim->last_t & 1u, (uint32_t)(t - 1) & 1u);
-        sim->launches += 2;
-        if (int rc = cuda_check(cudaGetLastError(), "wl_rearm_kernel")) return rc;
+        if (int rc = launched(sim, "wl_rearm_kernel", 2)) return rc;
     }
     sim->last_t = t + n_steps - 1;
     return WL_OK;
@@ -1894,8 +1815,7 @@ static int post_step(wl_sim* sim, int64_t step_counter, cudaStream_t cs) {
     const int64_t t_next = sim->last_t + 1;
     if (t_next % sim->cfg.max_episode_length != 0) return WL_OK;
     wl_boundary_kernel<<<1, 32, 0, cs>>>(sim->cfg, sim->globals, (uint32_t)t_next);
-    sim->launches++;
-    return cuda_check(cudaGetLastError(), "wl_boundary_kernel");
+    return launched(sim, "wl_boundary_kernel");
 }
 extern "C" {
 
@@ -1904,8 +1824,7 @@ int wl_startup(wl_sim* sim, void* stream) {
     ensure_device(sim);
     const int n = sim->cfg.num_envs, bs = 128;
     wl_startup_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state);
-    WL_LAUNCH_CHECK(sim, "wl_startup_kernel");
-    return WL_OK;
+    return launched(sim, "wl_startup_kernel");
 }
 
 int wl_reset(wl_sim* sim, const int64_t* d_env_ids, int32_t n_ids, int64_t step_counter, void* stream) {
@@ -1915,8 +1834,7 @@ int wl_reset(wl_sim* sim, const int64_t* d_env_ids, int32_t n_ids, int64_t step_
     if (n <= 0) return WL_OK;
     const int bs = 128;
     wl_reset_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, sim->hf, d_env_ids, n, (uint32_t)step_counter);
-    WL_LAUNCH_CHECK(sim, "wl_reset_kernel");
-    return WL_OK;
+    return launched(sim, "wl_reset_kernel");
 }
 
 int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated,
@@ -1951,16 +1869,16 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
 #define WL_QUAD_BS 32
 #endif
         const int bs = WL_QUAD_BS, threads = 4 * n, grid = (threads + bs - 1) / bs + 1;      // + the janitor CTA
-        if (elev) launch_k(wl_step_quad_kernel<WL_TASK_ELEVATION>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
-        else if (vis) launch_k(wl_step_quad_kernel<WL_TASK_VISUAL>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
-        else launch_k(wl_step_quad_kernel<WL_TASK_DRIFT>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
+        with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
+            launch_k(wl_step_quad_kernel<task>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
+        });
     } else {
         const int bs = pick_block(n), grid = (n + bs - 1) / bs + 1;
-        if (elev) launch_k(wl_step_kernel<WL_TASK_ELEVATION, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
-        else if (vis) launch_k(wl_step_kernel<WL_TASK_VISUAL, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
-        else launch_k(wl_step_kernel<WL_TASK_DRIFT, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
+        with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
+            launch_k(wl_step_kernel<task, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
+        });
     }
-    WL_LAUNCH_CHECK(sim, "wl_step_kernel");
+    if (int rc = launched(sim, "wl_step_kernel")) return rc;
     if (elev) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
     if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
     return post_step(sim, step_counter, cs);
@@ -1973,18 +1891,10 @@ static int launch_stage(wl_sim* sim, const float2* act, float* d_obs, float* d_r
                         float* d_log, uint32_t t, StageIO sio, cudaStream_t cs) {
     const int n = sim->cfg.num_envs, bs = pick_block(n), grid = (n + bs - 1) / bs + (STAGE == 2 ? 1 : 0);   // stage b: + the janitor CTA
     Terrain T{sim->hf};
-    switch (sim->cfg.task) {
-    case WL_TASK_ELEVATION:
-        wl_step_kernel<WL_TASK_ELEVATION, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
-        break;
-    case WL_TASK_VISUAL:
-        wl_step_kernel<WL_TASK_VISUAL, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
-        break;
-    default:
-        wl_step_kernel<WL_TASK_DRIFT, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
-    }
-    WL_LAUNCH_CHECK(sim, STAGE == 1 ? "wl_step_kernel<stage a>" : "wl_step_kernel<stage b>");
-    return WL_OK;
+    with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
+        wl_step_kernel<task, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
+    });
+    return launched(sim, STAGE == 1 ? "wl_step_kernel<stage a>" : "wl_step_kernel<stage b>");
 }
 extern "C" {
 
@@ -2032,15 +1942,15 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
     Terrain T{sim->hf};
     const int bs = 32, threads = 4 * n, grid = (threads + bs - 1) / bs;
     cudaStream_t cs = (cudaStream_t)stream;
+    ensure_device(sim);
     if (int rc = cuda_check(cudaMemsetAsync(d_log, 0, (size_t)K * WL_LOG_FLOATS * sizeof(float), cs), "wl_rollout: clear log rows")) return rc;
     if (int rc = prep_step(sim, step_counter, K, cs)) return rc;
     const float2* act = reinterpret_cast<const float2*>(d_actions);
     float2* aout = reinterpret_cast<float2*>(d_actions_out);
-    if (sim->cfg.task == WL_TASK_VISUAL)
-        wl_rollout_quad_kernel<WL_TASK_VISUAL><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, aout, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, K, &sim->globals->ticket);
-    else
-        wl_rollout_quad_kernel<WL_TASK_DRIFT><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, aout, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, K, &sim->globals->ticket);
-    WL_LAUNCH_CHECK(sim, "wl_rollout_quad_kernel");
+    with_task<WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
+        wl_rollout_quad_kernel<task><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, aout, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, K, &sim->globals->ticket);
+    });
+    if (int rc = launched(sim, "wl_rollout_quad_kernel")) return rc;
     return post_step(sim, step_counter, cs);
 }
 
@@ -2051,6 +1961,7 @@ int wl_step_host(wl_sim* sim, const float* h_action, float* d_action, float* d_o
     if (!sim || !h_action || !d_action || !d_obs || !d_result || !h_result) return fail(WL_EINVAL, "wl_step_host: null argument");
     const size_t n = (size_t)sim->cfg.num_envs;
     cudaStream_t cs = (cudaStream_t)stream;
+    ensure_device(sim);
     if (int rc = cuda_check(cudaMemcpyAsync(d_action, h_action, n * 2 * sizeof(float), cudaMemcpyHostToDevice, cs), "H2D actions")) return rc;
     float* d_rew = reinterpret_cast<float*>(d_result);
     uint8_t* d_term = reinterpret_cast<uint8_t*>(d_result) + n * 4;
@@ -2093,7 +2004,7 @@ int wl_observe(wl_sim* sim, float* d_obs, int64_t step_counter, int32_t call_idx
     const int n = sim->cfg.num_envs, bs = 128;
     wl_observe_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, d_obs, (uint32_t)step_counter,
                                                                          (uint32_t)call_idx);
-    WL_LAUNCH_CHECK(sim, "wl_observe_kernel");
+    if (int rc = launched(sim, "wl_observe_kernel")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return launch_scan(sim, d_obs, (cudaStream_t)stream);
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         return launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM_EXTRA, (uint32_t)call_idx, nullptr, (cudaStream_t)stream);
@@ -2122,8 +2033,7 @@ int wl_curriculum(wl_sim* sim, int32_t n_terms, const int32_t* slots, const floa
         a.slots[t] = slots[t]; a.inc[t] = increases[t];
     }
     wl_curriculum_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(sim->globals, a);
-    WL_LAUNCH_CHECK(sim, "wl_curriculum_kernel");
-    return WL_OK;
+    return launched(sim, "wl_curriculum_kernel");
 }
 
 int wl_synth_actions(wl_sim* sim, float* d_action, int64_t step_counter, int32_t dist, void* stream) {
@@ -2132,8 +2042,7 @@ int wl_synth_actions(wl_sim* sim, float* d_action, int64_t step_counter, int32_t
     const int n = sim->cfg.num_envs, bs = 128;
     wl_synth_actions_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->globals, reinterpret_cast<float2*>(d_action),
                                                                                (uint32_t)step_counter, dist);
-    WL_LAUNCH_CHECK(sim, "wl_synth_actions_kernel");
-    return WL_OK;
+    return launched(sim, "wl_synth_actions_kernel");
 }
 
 int wl_derive_suspension(wl_sim* sim, float* d_susp_pos, float* d_susp_vel, void* stream) {
@@ -2142,12 +2051,10 @@ int wl_derive_suspension(wl_sim* sim, float* d_susp_pos, float* d_susp_vel, void
     if (((uintptr_t)d_susp_pos & 15u) || ((uintptr_t)d_susp_vel & 15u)) return fail(WL_EINVAL, "wl_derive_suspension: outputs must be 16-byte aligned");
     const int n = sim->cfg.num_envs, bs = 128;
     Terrain T{sim->hf};
-    if (sim->cfg.task == WL_TASK_ELEVATION)
-        wl_suspension_kernel<WL_TASK_ELEVATION><<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, T, (float4*)d_susp_pos, (float4*)d_susp_vel);
-    else
-        wl_suspension_kernel<WL_TASK_DRIFT><<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, T, (float4*)d_susp_pos, (float4*)d_susp_vel);
-    WL_LAUNCH_CHECK(sim, "wl_suspension_kernel");
-    return WL_OK;
+    with_task<WL_TASK_ELEVATION>(sim->cfg.task, [&](auto task) {
+        wl_suspension_kernel<task><<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, T, (float4*)d_susp_pos, (float4*)d_susp_vel);
+    });
+    return launched(sim, "wl_suspension_kernel");
 }
 
 int32_t wl_policy_blob_floats(int32_t obs_dim, int32_t offsets[13]) {
@@ -2177,11 +2084,10 @@ int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, 
         cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         attr_set[sim->device] = true;
     }
-    if (sim->cfg.task == WL_TASK_VISUAL)
-        launch_k(wl_act_step_quad_kernel<WL_TASK_VISUAL>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
-    else
-        launch_k(wl_act_step_quad_kernel<WL_TASK_DRIFT>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
-    WL_LAUNCH_CHECK(sim, "wl_act_step_quad_kernel");
+    with_task<WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
+        launch_k(wl_act_step_quad_kernel<task>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
+    });
+    if (int rc = launched(sim, "wl_act_step_quad_kernel")) return rc;
     return post_step(sim, step_counter, cs);
 }
 

@@ -395,6 +395,38 @@ __device__ __forceinline__ void physics_substep(const wl_config& c, const Terrai
     chassis_integrate(c, k, R, b, Fb, Tb, e.inv_mass);
 }
 
+// ---- B. decimation x (actuators -> integrator) on the chassis at the centre of mass ------------------------------------
+__device__ __forceinline__ Chassis chassis_from_env(const wl_config& c, const EnvState& e) {
+    const M3 R = rotmat(e.qw, e.qx, e.qy, e.qz);
+    const V3 cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
+    Chassis b;
+    b.pc = V3{e.p.x + cw.x, e.p.y + cw.y, e.p.z + cw.z};
+    b.v = e.v; b.qw = e.qw; b.qx = e.qx; b.qy = e.qy; b.qz = e.qz;
+    b.wb = rotT(R, e.w);
+    return b;
+}
+// effort: the DC-motor effort limit per wheel (LANES == 4: slot 0 = this lane's wheel); the speed-dependent limits are
+// formed once per physics step
+template <int TASK, int LANES>
+__device__ __forceinline__ void run_substeps(const wl_config& c, const Terrain& T, EnvState& e, Chassis& b, const float target[4],
+                                             const float effort[4], const float steer_target[2], const StepConsts& kc) {
+    for (int d = 0; d < c.decimation; ++d) {
+        float lo[4], hi[4];
+#pragma unroll
+        for (int w = 0; w < 4 / LANES; ++w) dc_limits(c, effort[w], e.omega[w], lo[w], hi[w]);
+        for (int j = 0; j < c.substeps; ++j) physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
+    }
+}
+// back to the root frame: writes e.p / v / q / w, returns the rotation of the new attitude
+__device__ __forceinline__ M3 env_from_chassis(const wl_config& c, EnvState& e, const Chassis& b) {
+    const M3 R = rotmat(b.qw, b.qx, b.qy, b.qz);
+    const V3 cw = rot(R, V3{c.com[0], c.com[1], c.com[2]});
+    e.p = V3{b.pc.x - cw.x, b.pc.y - cw.y, b.pc.z - cw.z};
+    e.v = b.v; e.qw = b.qw; e.qx = b.qx; e.qy = b.qy; e.qz = b.qz;
+    e.w = rot(R, b.wb);
+    return R;
+}
+
 // ---- drift terminations / rewards -----------------------------------------------------
 __device__ __forceinline__ bool drift_off_track(const wl_config& c, float x, float y) {
     float st = c.trk_straight, ro = c.trk_corner_out, ri = c.trk_corner_in;
@@ -430,6 +462,8 @@ __device__ __forceinline__ void drift_reward_terms(const wl_config& c, float ste
     f[WL_DR_TERM_PENS] = (out_of_bounds && !time_out) ? 1.0f : 0.0f;
     f[7] = 0.0f;
 }
+// drift termination mask: bit 0 time_out, bit 1 out of bounds
+__device__ __forceinline__ uint32_t drift_term_mask(bool time_out, bool oob) { return (time_out ? 1u : 0u) | (oob ? 2u : 0u); }
 
 // ---- elevation task (elevation/mushr_elevation_env_cfg.py) -------------------------------------------------
 // terminations :339-376 -> mask bits [0 time_out, 1 cart_out_of_bounds, 2 stuck, 3 rollover, 4 at_goal]; rewards :155-305
@@ -517,7 +551,11 @@ __device__ __forceinline__ VisualMap visual_map(const wl_config& c, const float*
 // map lookup = TraversabilityHashmapUtil.get_map_id (utils/traversability_utils.py:83-88: +spacing/2, truncation,
 // clamp, indexed [y_idx, x_idx]; quirk Q14)
 // ---- visual task, camera term (software pinhole camera over the 2-colour plane mesh; restated in oracle/wl_oracle.c) ----
-__device__ __forceinline__ int vis_cam_floats(const wl_config& c) { return c.vis_cam ? c.vis_cam_w * (c.vis_cam_h - c.vis_cam_row0) : 0; }
+__host__ __device__ __forceinline__ int vis_cam_floats(const wl_config& c) { return c.vis_cam ? c.vis_cam_w * (c.vis_cam_h - c.vis_cam_row0) : 0; }
+// floats per observation row of the task (the visual row is the camera floats followed by the proprioceptive ones)
+__host__ __device__ __forceinline__ int obs_row_floats(const wl_config& c, int task) {
+    return task == WL_TASK_ELEVATION ? WL_OBS_DIM_ELEV : task == WL_TASK_VISUAL ? WL_OBS_DIM_VISUAL + vis_cam_floats(c) : WL_OBS_DIM_BLIND;
+}
 // torchvision rgb_to_grayscale of a grey pixel (r = g = b = v): the weights sum to 0.9999, not 1
 __device__ __forceinline__ float cam_gray(float v) { return fm(0.114f, v, fm(0.587f, v, 0.2989f * v)); }
 __device__ __forceinline__ float cam_clamp01(float v) { return r_min(r_max(v, 0.0f), 1.0f); }
@@ -599,6 +637,24 @@ __device__ __forceinline__ void visual_proprio(const wl_config& c, const EnvStat
     o[6] = r_clamp(e.action[0], -1.0f, 1.0f); o[7] = r_clamp(e.action[1], -1.0f, 1.0f);
 }
 
+// ---- E. reward weighting and done flags ----------------------------------------------------
+// value = f * w * dt per term, terms with w == 0 skipped; adds each value to the episode sums, returns the step reward
+__device__ __forceinline__ float weigh_rewards(const wl_config& c, const float wts[WL_MAX_REW_TERMS], const float f[WL_MAX_REW_TERMS],
+                                               float sums[WL_MAX_REW_TERMS]) {
+    float total = 0.0f;
+#pragma unroll
+    for (int k = 0; k < WL_MAX_REW_TERMS; ++k) {
+        if (k < c.num_rew_terms) {
+            float w = wts[k];
+            if (w != 0.0f) { float val = f[k] * w * c.d_step_dt; total += val; sums[k] += val; }
+        }
+    }
+    return total;
+}
+// terminated / truncated bytes of a termination mask: bit 0 (time_out) truncates, every other bit terminates
+struct DoneBytes { uint8_t terminated, truncated; };
+__device__ __forceinline__ DoneBytes done_bytes(uint32_t tmask) { return DoneBytes{(uint8_t)((tmask & ~1u) ? 1 : 0), (uint8_t)((tmask & 1u) ? 1 : 0)}; }
+
 // ---- reset / pushes / observations -----------------------------------------------------
 __device__ __forceinline__ void sample_interval_timers(const wl_config& c, EnvState& e, uint32_t a, uint32_t b) {
     e.t_hf = uniform(a, c.push_hf_interval[0], c.push_hf_interval[1]);
@@ -623,6 +679,12 @@ __device__ __forceinline__ void drift_reset_env(const wl_config& c, EnvState& e,
     e.action[0] = e.action[1] = e.prev_action[0] = e.prev_action[1] = 0.0f;
     uint4 r2 = philox4x32(c.seed, gid, t, RNG_RESET, 1u);
     sample_interval_timers(c, e, r2.x, r2.y);
+}
+// the task's reset; vm is read by the visual task only
+__device__ __forceinline__ void reset_env(const wl_config& c, int task, const VisualMap& vm, EnvState& e, uint32_t gid, uint32_t t) {
+    if (task == WL_TASK_ELEVATION) elev_reset_env(c, e, gid, t);
+    else if (task == WL_TASK_VISUAL) visual_reset_env(c, vm, e, gid, t);
+    else drift_reset_env(c, e, gid, t);
 }
 // returns true when a push changed the velocities
 __device__ __forceinline__ bool interval_pushes(const wl_config& c, EnvState& e, uint32_t gid, uint32_t t, float step_dt) {
