@@ -37,6 +37,9 @@ struct wl_sim {
     CUtensorMap tmap;       // 2-D tensor map over the height-field (elevation task)
     bool has_tmap;
     int scan_mode;          // ray-cast tile staging: 1 one TMA tile per CTA (default), 2 TMA producer/consumer pipeline, 0 plain loads (A/B)
+    uint32_t spec;          // spec_key(step_spec(cfg)): picks the duo kernel's instantiation (see with_spec)
+    const void* duo_kernel; // the duo kernel duo_threads was sized for (see duo_block)
+    int duo_threads;
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -61,6 +64,17 @@ static int launched(wl_sim* sim, const char* what, int count = 1) {
 template <int... TASKS, typename F>
 static void with_task(int task, F&& f) {
     if (!((task == TASKS && (f(std::integral_constant<int, TASKS>{}), true)) || ...)) f(std::integral_constant<int, WL_TASK_DRIFT>{});
+}
+
+// The step specs of the shipped Drift-family configs (make_task("drift") / "hound_4wd" / "f1tenth_drift" and the lowered Drift
+// and F1Tenth train / play cfgs): RWD or 4WD action map, clip bounding, no reverse, pushes and observation noise on, no
+// wheel-mass DR, decimation 4 x 1 sub-step.  The duo kernel is instantiated for these; every other config runs its generic body.
+static constexpr uint32_t SPEC_DRIFT_RWD = spec_key(StepSpec{WL_ACT_RWD, WL_BOUND_CLIP, 1, 1, 1, 0, 4, 1});
+static constexpr uint32_t SPEC_DRIFT_4WD = spec_key(StepSpec{WL_ACT_4WD, WL_BOUND_CLIP, 1, 1, 1, 0, 4, 1});
+// f(std::integral_constant<uint32_t, K>{}) for the listed spec key K equal to `spec`, else for K = 0 (the generic instantiation)
+template <uint32_t... KS, typename F>
+static void with_spec(uint32_t spec, F&& f) {
+    if (!((spec == KS && (f(std::integral_constant<uint32_t, KS>{}), true)) || ...)) f(std::integral_constant<uint32_t, 0u>{});
 }
 
 static inline void ensure_device(const wl_sim* sim) {
@@ -430,6 +444,12 @@ wl_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st
 // wl_step_quad_kernel, operation for operation.
 // ---------------------------------------------------------------------------------------
 #define WL_DUO_ENVS 8
+// A CTA is the env warp, the aux warp and, when the whole grid is resident at once with it (duo_block), a third "spacer" warp
+// that exits at once.  The warps of an SM's CTAs take consecutive scheduler (sub-partition) slots: with 2-warp CTAs the
+// env warps of the ~4 CTAs per SM at 4096 envs sat two per scheduler on two of the four schedulers; with 3 slots per CTA
+// each env warp has a scheduler of its own (measured with %warpid on H100, DESIGN.md 6e).  The spacer warp holds
+// registers, so at 8192 envs it would leave CTAs waiting for a second wave: there the CTA stays at 2 warps.
+#define WL_DUO_THREADS 96
 struct DuoShared {
     float tgt[WL_DUO_ENVS][8];      // wheel_target[4], steer_target[2]
     float noise[WL_DUO_ENVS][12];   // observation noise normals (Philox blocks 0..2)
@@ -447,13 +467,18 @@ __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64
 // FAN = 2: multicast only -- the host has checked that num_envs is a multiple of 8 and the output rows are aligned, so every row
 // is a full wide store: local copy + ONE multimem.st, no per-peer loops, no element-wise fallback in the instruction stream.
 // FAN = 1: the general fan-out (per-peer stores; multicast for the rows that qualify).
-template <int FAN>
-__global__ void __launch_bounds__(64)
+// K: the step spec key (wl_step.cuh, Spec).  The single-GPU path (FAN = 0) is instantiated for the shipped Drift-family specs
+// (with_spec): their action map, bounding, push and noise branches are folded and the sub-step trip counts are constants;
+// K = 0 reads the config at run time (every other config, and FAN = 1 / 2).
+template <int FAN, uint32_t K>
+__global__ void __launch_bounds__(WL_DUO_THREADS)
 wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
                    const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
                    uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
                    uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf) {
+    using S = Spec<K>;
     __shared__ DuoShared sh;
+    if (threadIdx.x >= 64) return;                              // the spacer warp
     const int n = c.num_envs;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t t = decode_step(gl, t_arg);
@@ -481,7 +506,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         // A. action map -> targets of the whole env step
         if (lane < 8) {
             float wt[4], stt[2];
-            process_action(c, a.x, a.y, wt, stt);
+            process_action<K>(c, a.x, a.y, wt, stt);
             sh.tgt[j][0] = wt[0]; sh.tgt[j][1] = wt[1]; sh.tgt[j][2] = wt[2]; sh.tgt[j][3] = wt[3];
             sh.tgt[j][4] = stt[0]; sh.tgt[j][5] = stt[1];
         }
@@ -491,13 +516,13 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             const int jn = lane / 3, k = lane - 3 * jn;
             const int in_ = (env0 + jn < n) ? env0 + jn : n - 1;
             float z[4];
-            quad_obs_noise(c, k, (uint32_t)(c.env_id_offset + in_), t, RNG_OBS, 0u, z);
+            quad_obs_noise<K>(c, k, (uint32_t)(c.env_id_offset + in_), t, RNG_OBS, 0u, z);
             sh.noise[jn][4 * k + 0] = z[0]; sh.noise[jn][4 * k + 1] = z[1]; sh.noise[jn][4 * k + 2] = z[2]; sh.noise[jn][4 * k + 3] = z[3];
         }
         // P. interval pushes of an env that does NOT reset this step (the env warp ignores them otherwise)
         if (lane < 8) {
             float hf = 0.0f, dvx = 0.0f, dvy = 0.0f, dwh = 0.0f, lf = 0.0f, dwl = 0.0f;
-            if (c.push_enable) {
+            if (S::push_enable(c)) {
                 t_hf = t_hf - c.d_step_dt;
                 if (t_hf < 1.0e-6f) {
                     uint4 r = philox4x32(c.seed, gid, t, RNG_PUSH_HF, 0u);
@@ -568,7 +593,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     const QuadLane L = quad_lane(c, n, env0 + q, lane & 3);
     const int i = L.i, w = L.w, ii = L.ii;
     const bool live = L.live;
-    const bool wm = c.dr_wheel_mass_enable != 0;
+    const bool wm = S::wheel_mass(c);
     EnvState e;
     QuadRaw raw;
     quad_issue_loads(st, n, ii, w, raw, false, wm, false);
@@ -580,11 +605,11 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     const float my_effort = (w == 0) ? c.dc_effort[0] : (w == 1) ? c.dc_effort[1] : (w == 2) ? c.dc_effort[2] : c.dc_effort[3];
     // B. decimation x (actuators -> integrator)
     Chassis b = chassis_from_env(c, e);
-    StepConsts kc = make_step_consts<1>(c, e);
+    StepConsts kc = make_step_consts<1, K>(c, e);
     bar_sync(1);
     const float my_targets[4] = {sh.tgt[q][w], 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
     const float my_steer_target[2] = {sh.tgt[q][(w == 3) ? 5 : 4], 0.0f};
-    run_substeps<WL_TASK_DRIFT, 4>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc);
+    run_substeps<WL_TASK_DRIFT, 4, K>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc);
     M3 R = env_from_chassis(c, e, b);
     // C./D. counters, terminations (the env warp needs `done` for the reset; the reward side lives in the aux warp)
     e.ep_len += 1;
@@ -612,7 +637,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     }
     // H. interval pushes + noise, drawn by the aux warp
     bar_sync(3);
-    if (c.push_enable) {
+    if (S::push_enable(c)) {
         if (done) { e.t_hf = e.t_hf - c.d_step_dt; e.t_lf = e.t_lf - c.d_step_dt; }       // fresh timers exceed step_dt: no push on a reset step
         else {
             const float* pu = sh.push[q];
@@ -1559,6 +1584,20 @@ static inline int pick_block(int n) {
     return 32;
 }
 
+// block size of a duo-kernel launch of `grid` CTAs: with the spacer warp when every CTA is resident at once with it, else 64
+template <typename KF>
+static int duo_block(wl_sim* sim, KF kernel, int grid) {
+    const void* kp = reinterpret_cast<const void*>(kernel);
+    if (sim->duo_kernel != kp) {
+        int per_sm = 0, sms = 0;
+        const bool ok = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, WL_DUO_THREADS, 0) == cudaSuccess &&
+                        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, sim->device) == cudaSuccess;
+        sim->duo_threads = (ok && grid <= per_sm * sms) ? WL_DUO_THREADS : 64;
+        sim->duo_kernel = kp;
+    }
+    return sim->duo_threads;
+}
+
 static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
     const int n = sim->cfg.num_envs;
     if (sim->scan_mode == 2 && sim->has_tmap) {              // TMA producer/consumer pipeline, persistent CTAs
@@ -1746,6 +1785,9 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     s->variant = 0;
     s->has_tmap = false;
     s->scan_mode = 1;
+    s->spec = spec_key(step_spec(s->cfg));
+    s->duo_kernel = nullptr;
+    s->duo_threads = 64;
     if (cfg->task == WL_TASK_ELEVATION) {
         typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -1857,11 +1899,13 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
         const bool rows_ok = (n % WL_DUO_ENVS) == 0 && (((uintptr_t)d_obs | (uintptr_t)d_rew) & 15u) == 0 &&
                              (((uintptr_t)d_terminated | (uintptr_t)d_truncated) & 7u) == 0;
         if (sim->fan.mc && rows_ok)
-            launch_k(wl_step_duo_kernel<2>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<2, 0u>, grid, duo_block(sim, wl_step_duo_kernel<2, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else if (sim->fan.n > 0 || sim->fan.mc)
-            launch_k(wl_step_duo_kernel<1>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else
-            launch_k(wl_step_duo_kernel<0>, grid, 64, 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
+                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            });
     } else if (sim->fan.n > 0) {
         return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
     } else if (variant == 4) {

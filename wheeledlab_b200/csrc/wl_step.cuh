@@ -145,16 +145,49 @@ __device__ __forceinline__ void store_env_quad(float4* __restrict__ st, int n, i
     }
 }
 
+// ---- step spec: the config fields that pick a branch or set a trip count in the Drift-family step ----------------------
+// A kernel templated on a packed spec key K != 0 reads these fields as constants, so the branches it does not take and the
+// sub-step loop's trip count are resolved at compile time.  K == 0 is the generic instantiation: every field is read from
+// the config at run time.
+struct StepSpec { int32_t action_kind, bounding, no_reverse, push_enable, noise, wheel_mass, decimation, substeps; };
+
+__host__ __device__ constexpr StepSpec step_spec(const wl_config& c) {
+    return StepSpec{c.action_kind, c.bounding, c.no_reverse != 0, c.push_enable != 0, c.enable_corruption != 0,
+                    c.dr_wheel_mass_enable != 0, c.decimation, c.substeps};
+}
+// bit 31 set, [0,2) action kind, [2,4) bounding, 4..7 the flags, [8,16) decimation, [16,24) substeps; 0 if a field does not fit
+__host__ __device__ constexpr uint32_t spec_key(const StepSpec& s) {
+    return (s.action_kind < 0 || s.action_kind > 3 || s.bounding < 0 || s.bounding > 3 || s.decimation < 1 || s.decimation > 255 ||
+            s.substeps < 1 || s.substeps > 255) ? 0u
+         : 0x80000000u | (uint32_t)s.action_kind | ((uint32_t)s.bounding << 2) | ((uint32_t)s.no_reverse << 4) |
+           ((uint32_t)s.push_enable << 5) | ((uint32_t)s.noise << 6) | ((uint32_t)s.wheel_mass << 7) |
+           ((uint32_t)s.decimation << 8) | ((uint32_t)s.substeps << 16);
+}
+template <uint32_t K>
+struct Spec {
+    static constexpr bool fixed = K != 0u;
+    __device__ __forceinline__ static int action_kind(const wl_config& c) { return fixed ? (int)(K & 3u) : c.action_kind; }
+    __device__ __forceinline__ static int bounding(const wl_config& c) { return fixed ? (int)((K >> 2) & 3u) : c.bounding; }
+    __device__ __forceinline__ static bool no_reverse(const wl_config& c) { return fixed ? ((K >> 4) & 1u) != 0u : c.no_reverse != 0; }
+    __device__ __forceinline__ static bool push_enable(const wl_config& c) { return fixed ? ((K >> 5) & 1u) != 0u : c.push_enable != 0; }
+    __device__ __forceinline__ static bool noise(const wl_config& c) { return fixed ? ((K >> 6) & 1u) != 0u : c.enable_corruption != 0; }
+    __device__ __forceinline__ static bool wheel_mass(const wl_config& c) { return fixed ? ((K >> 7) & 1u) != 0u : c.dr_wheel_mass_enable != 0; }
+    __device__ __forceinline__ static int decimation(const wl_config& c) { return fixed ? (int)((K >> 8) & 0xFFu) : c.decimation; }
+    __device__ __forceinline__ static int substeps(const wl_config& c) { return fixed ? (int)((K >> 16) & 0xFFu) : c.substeps; }
+};
+
 // ---- A. action term ---------------------------------------------------------------
+template <uint32_t K = 0>
 __device__ __forceinline__ void process_action(const wl_config& c, float a0, float a1, float wheel_target[4], float steer_target[2]) {
-    if (c.bounding == WL_BOUND_CLIP) { a0 = r_clamp(a0, -1.0f, 1.0f); a1 = r_clamp(a1, -1.0f, 1.0f); }
-    else if (c.bounding == WL_BOUND_TANH) { a0 = det_tanh(a0); a1 = det_tanh(a1); }      // ackermann_actions.py:126-127
+    using S = Spec<K>;
+    if (S::bounding(c) == WL_BOUND_CLIP) { a0 = r_clamp(a0, -1.0f, 1.0f); a1 = r_clamp(a1, -1.0f, 1.0f); }
+    else if (S::bounding(c) == WL_BOUND_TANH) { a0 = det_tanh(a0); a1 = det_tanh(a1); }      // ackermann_actions.py:126-127
     float v = a0 * c.act_scale[0] + c.act_offset[0];
     float delta = a1 * c.act_scale[1] + c.act_offset[1];
-    if (c.no_reverse) v = r_max(v, 0.0f);
+    if (S::no_reverse(c)) v = r_max(v, 0.0f);
     float tan_d = det_tan(delta);
     float L = c.base_length, W = c.base_width, r = c.wheel_radius_cfg;
-    if (c.action_kind == WL_ACT_RWD) {
+    if (S::action_kind(c) == WL_ACT_RWD) {
         float wt = v * c.d_inv_wheel_radius_cfg;
         wheel_target[WL_BL] = wt; wheel_target[WL_BR] = wt; wheel_target[WL_FL] = 0.0f; wheel_target[WL_FR] = 0.0f;
         steer_target[0] = tan_d; steer_target[1] = tan_d;      // quirk Q1
@@ -169,7 +202,7 @@ __device__ __forceinline__ void process_action(const wl_config& c, float a0, flo
     wheel_target[WL_FR] = v * fabsf(Rrr * rden);
     wheel_target[WL_BL] = v * fabsf(Rl * rden);
     wheel_target[WL_BR] = v * fabsf(Rr * rden);
-    if (c.action_kind == WL_ACT_4WD) { steer_target[0] = tan_d; steer_target[1] = tan_d; }
+    if (S::action_kind(c) == WL_ACT_4WD) { steer_target[0] = tan_d; steer_target[1] = tan_d; }
     else { steer_target[0] = det_atan(L / Rl); steer_target[1] = det_atan(L / Rr); }
 }
 
@@ -232,16 +265,16 @@ struct Chassis { V3 pc; float qw, qx, qy, qz; V3 v; V3 wb; };
 // wheel), h / I_w and 1 / (1 + h kd / I_w) of the implicit DC-motor damper
 struct StepConsts { float I[3], invI[3]; float hI[4], idk[4], fxk[4]; };
 
-template <int NW>
+template <int NW, uint32_t K = 0>
 __device__ __forceinline__ StepConsts make_step_consts(const wl_config& c, const EnvState& e) {
     StepConsts k;
     const float mass = e.mass, inv_mass = e.inv_mass;
 #pragma unroll
     for (int i = 0; i < NW; ++i) {
-        k.hI[i] = c.dr_wheel_mass_enable ? c.d_h * e.inv_Iw[i] : c.d_hI;
+        k.hI[i] = Spec<K>::wheel_mass(c) ? c.d_h * e.inv_Iw[i] : c.d_hI;
         k.idk[i] = 1.0f / fm(k.hI[i], e.kd[i], 1.0f);
         // longitudinal stick cap (tire_mx / h) with this wheel's own spin inertia
-        k.fxk[i] = c.dr_wheel_mass_enable ? c.d_inv_h / fm(c.wheel_radius * c.wheel_radius, e.inv_Iw[i], c.tire_mx_rest) : c.d_fxk;
+        k.fxk[i] = Spec<K>::wheel_mass(c) ? c.d_inv_h / fm(c.wheel_radius * c.wheel_radius, e.inv_Iw[i], c.tire_mx_rest) : c.d_fxk;
     }
     float ms = mass * c.d_inv_mass_nominal;          // inertia scales with the DR mass ratio (a14)
     float ms_inv = c.mass_nominal * inv_mass;
@@ -406,15 +439,17 @@ __device__ __forceinline__ Chassis chassis_from_env(const wl_config& c, const En
     return b;
 }
 // effort: the DC-motor effort limit per wheel (LANES == 4: slot 0 = this lane's wheel); the speed-dependent limits are
-// formed once per physics step
-template <int TASK, int LANES>
+// formed once per physics step.  With a fixed spec (K != 0) the trip counts are constants but the loops stay rolled: fully
+// unrolled, the 4 x 1 Drift sub-steps were no faster on H100 (DESIGN.md 6e) and cost ~900 more static instructions
+template <int TASK, int LANES, uint32_t K = 0>
 __device__ __forceinline__ void run_substeps(const wl_config& c, const Terrain& T, EnvState& e, Chassis& b, const float target[4],
                                              const float effort[4], const float steer_target[2], const StepConsts& kc) {
-    for (int d = 0; d < c.decimation; ++d) {
+    using S = Spec<K>;
+    for (int d = 0; d < S::decimation(c); ++d) {
         float lo[4], hi[4];
 #pragma unroll
         for (int w = 0; w < 4 / LANES; ++w) dc_limits(c, effort[w], e.omega[w], lo[w], hi[w]);
-        for (int j = 0; j < c.substeps; ++j) physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
+        for (int j = 0; j < S::substeps(c); ++j) physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
     }
 }
 // back to the root frame: writes e.p / v / q / w, returns the rotation of the new attitude
@@ -774,9 +809,10 @@ __device__ __forceinline__ void fan_store8(const PeerFan& pf, float2* p, float2 
 // quad version: lane k in {0,1,2} owns Philox block k (4 normals, drawn by quad_obs_noise at the TOP of the kernel, under
 // the shadow of the state loads) and writes obs[4k..4k+3]; lane 3 writes the last action.  `eu_k` = this lane's euler angle
 // (lane0 roll, lane1 pitch, lane2 yaw), already wrapped.
+template <uint32_t K = 0>
 __device__ __forceinline__ void quad_obs_noise(const wl_config& c, int w, uint32_t gid, uint32_t t, uint32_t stream, uint32_t sub0, float z[4]) {
     z[0] = z[1] = z[2] = z[3] = 0.0f;
-    if (c.enable_corruption) {
+    if (Spec<K>::noise(c)) {
         uint4 r = philox4x32(c.seed, gid, t, stream, sub0 + (uint32_t)(w < 3 ? w : 0));
         box_muller(r.x, r.y, z[0], z[1]);
         box_muller(r.z, r.w, z[2], z[3]);
