@@ -455,6 +455,7 @@ struct DuoShared {
     float noise[WL_DUO_ENVS][12];   // observation noise normals (Philox blocks 0..2)
     float push[WL_DUO_ENVS][8];     // hf fired, dvx, dvy, dwz_hf, t_hf_new, lf fired, dwz_lf, t_lf_new
     float fin[WL_DUO_ENVS][16];     // post-physics: p(3) vb(3) wb(3) wz_world steer_l steer_r raw-tmask(bits)
+    __align__(16) float rst[WL_DUO_ENVS][16];   // reset outcome: px py qw qz t_hf t_lf (DriftReset, timers after this step) vb(3) wbo(3) euler[wheel lane]
     __align__(16) float obs[WL_DUO_ENVS * WL_OBS_DIM_BLIND];   // the 8 observation rows of the CTA, staged for 128-bit stores
     __align__(16) float rewrow[WL_DUO_ENVS];                    // the CTA's 8 rewards and 2 x 8 done bytes, staged the same way
     __align__(8) uint8_t maskrow[2][WL_DUO_ENVS];
@@ -470,8 +471,10 @@ __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64
 // K: the step spec key (wl_step.cuh, Spec).  The single-GPU path (FAN = 0) is instantiated for the shipped Drift-family specs
 // (with_spec): their action map, bounding, push and noise branches are folded and the sub-step trip counts are constants;
 // K = 0 reads the config at run time (every other config, and FAN = 1 / 2).
+// Launch bounds: 4 CTAs per SM hold the 4096-env grid with the spacer warp (duo_block); without the minimum, ptxas traded
+// a register spill in the env warp for an occupancy no launch here needs.
 template <int FAN, uint32_t K>
-__global__ void __launch_bounds__(WL_DUO_THREADS)
+__global__ void __launch_bounds__(WL_DUO_THREADS, 4)
 wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
                    const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
                    uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
@@ -542,6 +545,26 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             }
             sh.push[j][0] = hf; sh.push[j][1] = dvx; sh.push[j][2] = dvy; sh.push[j][3] = dwh; sh.push[j][4] = t_hf;
             sh.push[j][5] = lf; sh.push[j][6] = dwl; sh.push[j][7] = t_lf;
+        }
+        // Z. the auto-reset outcome of every env, whether it resets or not: lane = (env, wheel) as in the env warp, which
+        // only selects it after bar.sync 3.  A reset env is not pushed: its fresh timers exceed step_dt and only count down.
+        // (Drawn before the action map, in the shadow of the loads, it delayed bar.arrive 1 and the step took longer.)
+        {
+            const QuadLane Lz = quad_lane(c, n, env0 + (lane >> 2), lane & 3);
+            DriftReset d = drift_reset_draw(c, Lz.gid, t);
+            EnvState z;
+            drift_reset_apply(d, z);
+            const float eu = euler_lane(z.qw, z.qx, z.qy, z.qz, Lz.w);
+            const M3 R = rotmat(z.qw, z.qx, z.qy, z.qz);
+            const V3 vb = rotT(R, z.v), wbo = rotT(R, z.w);
+            if (S::push_enable(c)) { d.t_hf = d.t_hf - c.d_step_dt; d.t_lf = d.t_lf - c.d_step_dt; }
+            float* ro = sh.rst[lane >> 2];
+            if (Lz.w == 0) {
+                reinterpret_cast<float4*>(ro)[0] = make_float4(d.px, d.py, d.qw, d.qz);
+                reinterpret_cast<float4*>(ro)[1] = make_float4(d.t_hf, d.t_lf, vb.x, vb.y);
+                reinterpret_cast<float4*>(ro)[2] = make_float4(vb.z, wbo.x, wbo.y, wbo.z);
+            }
+            ro[12 + Lz.w] = eu;
         }
         bar_arrive(3);
         // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
@@ -625,29 +648,26 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         fo[12] = __uint_as_float(raw_mask);
     }
     bar_arrive(2);
-    // I'. observation inputs from the post-physics state (an env that resets / gets pushed redoes them below)
+    // I'. observation inputs from the post-physics state (an env that resets / gets pushed takes others below)
     float eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
     V3 wbo = rotT(R, e.w);
     const bool done = (raw_mask & (uint32_t)c.term_enable) != 0u;
-    // F. auto-reset (sums and log: aux warp)
-    if (done) {
-        drift_reset_env(c, e, L.gid, t);
-        eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
-        R = rotmat(e.qw, e.qx, e.qy, e.qz); vb = rotT(R, e.v); wbo = rotT(R, e.w);
-    }
-    // H. interval pushes + noise, drawn by the aux warp
+    // F. auto-reset and H. interval pushes: the reset outcome, the push draws and the noise come from the aux warp
     bar_sync(3);
-    if (S::push_enable(c)) {
-        if (done) { e.t_hf = e.t_hf - c.d_step_dt; e.t_lf = e.t_lf - c.d_step_dt; }       // fresh timers exceed step_dt: no push on a reset step
-        else {
-            const float* pu = sh.push[q];
-            bool fired = false;
-            if (pu[0] != 0.0f) { e.v.x = e.v.x + pu[1]; e.v.y = e.v.y + pu[2]; e.w.z = e.w.z + pu[3]; fired = true; }
-            e.t_hf = pu[4];
-            if (pu[5] != 0.0f) { e.w.z = e.w.z + pu[6]; fired = true; }
-            e.t_lf = pu[7];
-            if (fired) { vb = rotT(R, e.v); wbo = rotT(R, e.w); }
-        }
+    if (done) {                                                 // (sums and log: aux warp)
+        const float4* ro = reinterpret_cast<const float4*>(sh.rst[q]);
+        const float4 r0 = ro[0], r1 = ro[1], r2 = ro[2];
+        drift_reset_apply(DriftReset{r0.x, r0.y, r0.z, r0.w, r1.x, r1.y}, e);
+        vb = V3{r1.z, r1.w, r2.x}; wbo = V3{r2.y, r2.z, r2.w};
+        eu_k = sh.rst[q][12 + w];
+    } else if (S::push_enable(c)) {
+        const float* pu = sh.push[q];
+        bool fired = false;
+        if (pu[0] != 0.0f) { e.v.x = e.v.x + pu[1]; e.v.y = e.v.y + pu[2]; e.w.z = e.w.z + pu[3]; fired = true; }
+        e.t_hf = pu[4];
+        if (pu[5] != 0.0f) { e.w.z = e.w.z + pu[6]; fired = true; }
+        e.t_lf = pu[7];
+        if (fired) { vb = rotT(R, e.v); wbo = rotT(R, e.w); }
     }
     const int k4 = (w < 3) ? 4 * w : 0;
     const float zn[4] = {sh.noise[q][k4], sh.noise[q][k4 + 1], sh.noise[q][k4 + 2], sh.noise[q][k4 + 3]};

@@ -691,29 +691,35 @@ struct DoneBytes { uint8_t terminated, truncated; };
 __device__ __forceinline__ DoneBytes done_bytes(uint32_t tmask) { return DoneBytes{(uint8_t)((tmask & ~1u) ? 1 : 0), (uint8_t)((tmask & 1u) ? 1 : 0)}; }
 
 // ---- reset / pushes / observations -----------------------------------------------------
-__device__ __forceinline__ void sample_interval_timers(const wl_config& c, EnvState& e, uint32_t a, uint32_t b) {
-    e.t_hf = uniform(a, c.push_hf_interval[0], c.push_hf_interval[1]);
-    e.t_lf = uniform(b, c.push_lf_interval[0], c.push_lf_interval[1]);
-}
-__device__ __forceinline__ void drift_reset_env(const wl_config& c, EnvState& e, uint32_t gid, uint32_t t) {
+// The drift reset in two parts: the draw (a function of (seed, env id, step) and the config only, never of the state) and
+// its application to the state.  The duo kernel draws in its aux warp and applies in its env warp.
+struct DriftReset { float px, py, qw, qz, t_hf, t_lf; };
+__device__ __forceinline__ DriftReset drift_reset_draw(const wl_config& c, uint32_t gid, uint32_t t) {
     uint4 r = philox4x32(c.seed, gid, t, RNG_RESET, 0u);
     uint32_t idx = __umulhi(r.x, (uint32_t)c.num_ref_poses);
     float nx = (2.0f * u01(r.y) - 1.0f) * c.reset_pos_noise;
     float ny = (2.0f * u01(r.z) - 1.0f) * c.reset_pos_noise;
     float nyaw = (2.0f * u01(r.w) - 1.0f) * c.reset_yaw_noise;
-    e.p.x = c.ref_poses[3 * idx + 0] + nx;
-    e.p.y = c.ref_poses[3 * idx + 1] + ny;
-    e.p.z = 0.0f;
+    float px = c.ref_poses[3 * idx + 0] + nx;
+    float py = c.ref_poses[3 * idx + 1] + ny;
     float yaw = c.ref_poses[3 * idx + 2] * 0.017453292519943295f + nyaw;
     float sh, ch; det_sincos(yaw * 0.5f, sh, ch);
-    e.qw = ch; e.qx = 0.0f; e.qy = 0.0f; e.qz = sh;
+    uint4 r2 = philox4x32(c.seed, gid, t, RNG_RESET, 1u);
+    return DriftReset{px, py, ch, sh, uniform(r2.x, c.push_hf_interval[0], c.push_hf_interval[1]),
+                      uniform(r2.y, c.push_lf_interval[0], c.push_lf_interval[1])};
+}
+__device__ __forceinline__ void drift_reset_apply(const DriftReset& d, EnvState& e) {
+    e.p.x = d.px; e.p.y = d.py; e.p.z = 0.0f;
+    e.qw = d.qw; e.qx = 0.0f; e.qy = 0.0f; e.qz = d.qz;
     e.v = V3{0.0f, 0.0f, 0.0f}; e.w = V3{0.0f, 0.0f, 0.0f};
     e.ep_len = 0;
 #pragma unroll
     for (int k = 0; k < WL_MAX_REW_TERMS; ++k) e.sums[k] = 0.0f;
     e.action[0] = e.action[1] = e.prev_action[0] = e.prev_action[1] = 0.0f;
-    uint4 r2 = philox4x32(c.seed, gid, t, RNG_RESET, 1u);
-    sample_interval_timers(c, e, r2.x, r2.y);
+    e.t_hf = d.t_hf; e.t_lf = d.t_lf;
+}
+__device__ __forceinline__ void drift_reset_env(const wl_config& c, EnvState& e, uint32_t gid, uint32_t t) {
+    drift_reset_apply(drift_reset_draw(c, gid, t), e);
 }
 // the task's reset; vm is read by the visual task only
 __device__ __forceinline__ void reset_env(const wl_config& c, int task, const VisualMap& vm, EnvState& e, uint32_t gid, uint32_t t) {
