@@ -1,0 +1,188 @@
+#!/usr/bin/env python
+"""Phase trace of wl_step_duo_kernel: when each warp reaches each hand-off of one Drift step, and where it ran.
+
+    python tools/duo_trace.py build [--out DIR]                    # compile the traced library (-DWL_DUO_TRACE) into DIR
+    python tools/duo_trace.py run --lib DIR/libwl_trace.so [--tag T] [--envs 4096] [--task drift] [--json OUT]
+
+`run` steps M independent env sets round-robin inside one CUDA graph, as bench.py does, so that the working set is larger
+than L2 and every launch starts cold.  Every warp that owns envs stamps %globaltimer at its hand-offs and records %smid and
+%warpid (csrc/wl_api.cu, WL_DUO_TRACE).  Times are ns after the launch's first warp entry, median over launches of the
+per-launch median warp, except where a row says otherwise.  The traced build is a diagnostic build: its stamps and
+records cost time of their own, so compare traces with traces, and bench.py figures with bench.py figures."""
+import argparse
+import json
+import math
+import os
+import subprocess
+import sys
+import tempfile
+from pathlib import Path
+
+ROOT = Path(__file__).resolve().parent.parent
+
+# DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64
+TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
+     [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3"]
+
+
+def build(out: Path, defines):
+    sys.path.insert(0, str(ROOT))
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("_wl_build", ROOT / "wheeledlab_b200" / "build.py")
+    b = importlib.util.module_from_spec(spec); spec.loader.exec_module(b)
+    out.mkdir(parents=True, exist_ok=True)
+    lib = out / "libwl_trace.so"
+    cmd = [b.NVCC, *b.NVCC_FLAGS, "-DWL_DUO_TRACE", *[f"-D{d}" for d in defines], "-o", str(lib), str(b.CSRC / "wl_api.cu")]
+    subprocess.run(cmd, check=True, cwd=str(ROOT))
+    print(lib)
+
+
+def _median(xs):
+    xs = sorted(xs)
+    return xs[len(xs) // 2] if xs else None
+
+
+def summarize(recs, tag, n_launch_expected):
+    import numpy as np
+    launches = {}                                              # one launch = (env set, step counter)
+    for idx, kk in enumerate(zip(recs["st"].tolist(), recs["t"].tolist())):
+        launches.setdefault(kk, []).append(idx)
+    L = sorted(launches.values(), key=lambda ix: int(recs["ts"][ix, 0].min()))
+    rows = {name: [] for name in TR}
+    aux_rows = {"aux: state loads landed": 3, "aux: bar.arrive 1": 4, "aux: bar.arrive 3": 15, "aux: bar.sync 2": 13, "aux: last store": 14}
+    aux = {k: [] for k in aux_rows}
+    launch_last, gap_med_last, starts, ends, shared, own, late_cta, last_is_late = [], [], [], [], [], [], [], []
+    prev_end = None
+    for ix in L:
+        ix = np.asarray(ix)
+        ts = recs["ts"][ix].astype(np.int64)
+        role = recs["role"][ix]
+        t0 = int(ts[:, 0].min())
+        env = ts[role == 0]
+        for c, name in enumerate(TR):
+            col = env[:, c]
+            col = col[col > 0]
+            if len(col):
+                rows[name].append(float(np.median(col - t0)))
+        ax = ts[role == 1]
+        for name, c in aux_rows.items():
+            col = ax[:, c]; col = col[col > 0]
+            if len(col):
+                aux[name].append(float(np.median(col - t0)))
+        last = int(ts[:, 14].max())
+        launch_last.append(last - t0)
+        gap_med_last.append(last - float(np.median(env[:, 14])))
+        starts.append(t0); ends.append(last)
+        # scheduler placement of the env warps: (SM, %warpid % 4)
+        ew = ix[role == 0]
+        sched = [(int(s), int(w) % 4) for s, w in zip(recs["smid"][ew], recs["warpid"][ew])]
+        cnt = {}
+        for p in sched:
+            cnt[p] = cnt.get(p, 0) + 1
+        own.append(sum(1 for p in sched if cnt[p] == 1) / max(1, len(sched)))
+        shared.append(sum(1 for v in cnt.values() if v > 1))
+        if prev_end is not None:
+            # CTAs of this launch whose env warp entered only after the previous launch's last store (a second wave)
+            late = env[:, 0] > prev_end
+            late_cta.append(int(late.sum()))
+            last_is_late.append(bool(late[int(np.argmax(env[:, 14]))]))
+        prev_end = last
+    period = [b - a for a, b in zip(starts, starts[1:])]
+    gap = [s - e for e, s in zip(ends, starts[1:])]
+    out = {"tag": tag, "launches": len(L), "launches expected": n_launch_expected, "records": int(len(recs))}
+    for name in TR[:-1]:
+        if rows[name]:
+            out[name] = _median(rows[name])
+    out.update({k: _median(v) for k, v in aux.items()})
+    out.update({
+        "launch last store": _median(launch_last),
+        "launch last store - median env-warp last store": _median(gap_med_last),
+        "period: first entry to next launch's first entry": _median(period),
+        "next launch's first entry - this launch's last store (negative: overlap)": _median(gap),
+        "env warps with a scheduler of their own (fraction, median)": _median(own),
+        "(SM, scheduler) pairs holding >1 env warp of the launch (median)": _median(shared),
+        "env warps entering after the previous launch's last store (median)": _median(late_cta),
+        "launches whose last env-warp store is from such a late warp": int(sum(last_is_late)),
+    })
+    return out
+
+
+def run(args):
+    import numpy as np
+    import torch
+    import wheeledlab_b200 as wl
+    from wheeledlab_b200._lib import lib
+    import ctypes as C
+    dev = "cuda:0"
+    E = args.envs
+    mk = lambda s: wl.make_task(args.task, num_envs=E, seed=42 + s)
+    sim0 = wl.WheeledSim(mk(0), dev)
+    L2 = torch.cuda.get_device_properties(0).L2_cache_size
+    M = max(4, math.ceil(2.2 * L2 / (sim0._buf.numel() * 4)))
+    sims = [sim0] + [wl.WheeledSim(mk(1000 * m), dev) for m in range(1, M)]
+    for s in sims:
+        s.startup(); s.reset(None, 0)
+    acts = torch.stack([sim0.synth_actions(t) for t in range(64)])
+    outs = [(torch.empty((E, sim0.obs_dim), device=dev), torch.empty(E, device=dev), torch.empty(E, dtype=torch.uint8, device=dev),
+             torch.empty(E, dtype=torch.uint8, device=dev)) for _ in range(M)]
+    R = args.rounds * M
+    bound = [sims[k % M].bind_step(acts[k % 64], outs[k % M]) for k in range(R)]
+    tc = [0] * M
+
+    def steps():
+        for k in range(R):
+            bound[k](tc[k % M]); tc[k % M] += 1
+    steps(); torch.cuda.synchronize()                          # untraced warm-up (module load, first touches)
+    g, cs = torch.cuda.CUDAGraph(), torch.cuda.Stream()
+    cs.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(cs):
+        with torch.cuda.graph(g, stream=cs):
+            steps()
+    torch.cuda.current_stream().wait_stream(cs)
+    g.replay(); torch.cuda.synchronize()
+    per_launch = 2 * ((E + 7) // 8)
+    dtype = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
+                      ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR))])
+    assert dtype.itemsize == 168
+    cap = per_launch * R
+    buf = torch.zeros(cap * dtype.itemsize, dtype=torch.uint8, device=dev)
+    lib.wl_duo_trace_arm.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wl_duo_trace_arm.restype = C.c_int
+    assert lib.wl_duo_trace_arm(C.c_void_p(buf.data_ptr()), cap) >= 0
+    torch.cuda._sleep(200_000)
+    g.replay(); torch.cuda.synchronize()
+    n = lib.wl_duo_trace_arm(None, 0)
+    recs = np.frombuffer(buf.cpu().numpy().tobytes(), dtype=dtype)[:min(n, cap)]
+    out = summarize(recs, args.tag, R)
+    out.update({"task": args.task, "envs": E, "env sets": M, "gpu": torch.cuda.get_device_name(0)})
+    s = json.dumps(out, indent=1)
+    print(s)
+    if args.json:
+        Path(args.json).parent.mkdir(parents=True, exist_ok=True)
+        Path(args.json).write_text(s + "\n")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("cmd", choices=["build", "run"])
+    ap.add_argument("--out", default=None, help="build: output directory (default: a new temporary directory)")
+    ap.add_argument("-D", dest="defines", action="append", default=[], help="build: extra macro")
+    ap.add_argument("--lib", help="run: the traced library")
+    ap.add_argument("--tag", default="trace")
+    ap.add_argument("--envs", type=int, default=4096)
+    ap.add_argument("--task", default="drift")
+    ap.add_argument("--rounds", type=int, default=2, help="run: graph of rounds x M steps")
+    ap.add_argument("--json", default=None)
+    args = ap.parse_args()
+    if args.cmd == "build":
+        build(Path(args.out) if args.out else Path(tempfile.mkdtemp(prefix="wl_trace_")), args.defines)
+    elif os.environ.get("WHEELEDLAB_B200_LIB") != str(Path(args.lib).resolve()):
+        env = dict(os.environ, WHEELEDLAB_B200_LIB=str(Path(args.lib).resolve()))
+        sys.exit(subprocess.run([sys.executable, __file__, *sys.argv[1:]], env=env).returncode)
+    else:
+        sys.path.insert(0, str(ROOT))
+        run(args)
+
+
+if __name__ == "__main__":
+    main()

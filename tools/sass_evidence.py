@@ -12,7 +12,8 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 LIB = ROOT / "wheeledlab_b200" / "libwheeledlab_b200.so"
-KEYS = ["INSTR", "UTMALDG", "UBLKCP", "SYNCS", "BAR.ARV", "BAR.SYNC", "REDG", "ATOMG", "MUFU.RCP", "MUFU.RSQ", "FCHK", "SHFL", "STRONG.SYS"]
+KEYS = ["INSTR", "UTMALDG", "UBLKCP", "SYNCS", "BAR.ARV", "BAR.SYNC", "REDG", "ATOMG", "MUFU.RCP", "MUFU.RSQ", "FCHK", "SHFL", "STRONG.SYS",
+        "PREEXIT", "ACQBULK", "CCTL.E.PF2"]
 
 
 def main():
@@ -41,6 +42,8 @@ def main():
     print("# STG...STRONG.SYS = multimem.st.relaxed.sys (wl_step_duo_kernel: output rows stored once to the NVSwitch multicast alias of the symmetric")
     print("# rollout buffers, replicated by the switch into every rank's copy; wl_set_multicast_fanout); in the other kernels STRONG.SYS marks the")
     print("# system-scope loads/stores of the peer-memory all-reduce (wl_dp_adam_kernel) and of the flag protocols.")
+    print("# PREEXIT = griddepcontrol.launch_dependents and ACQBULK = griddepcontrol.wait (programmatic dependent launch); CCTL.E.PF2 =")
+    print("# prefetch.global.L2 (wl_step_duo_kernel: the lines of its first loads, requested before the wait).")
     print("kernel | " + " | ".join(KEYS))
     for n in sorted(rows):
         print(n[:64] + " | " + " | ".join(str(rows[n].get(k, 0)) for k in KEYS))

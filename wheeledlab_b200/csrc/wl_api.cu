@@ -463,6 +463,59 @@ struct DuoShared {
 __device__ __forceinline__ void bar_arrive(int id) { asm volatile("bar.arrive %0, 64;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
 
+// ---- phase trace of the duo kernel (diagnostic build only: -DWL_DUO_TRACE, tools/duo_trace.py; without the macro the
+// kernel's machine code is unchanged).  Every warp that owns envs stamps %globaltimer at its hand-offs and appends one
+// record.  A stamp takes a value as `dep` and is predicated on it, so it is issued only once that value has arrived.
+#ifdef WL_DUO_TRACE
+// (the aux warp stamps TR_BAR1 at its bar.arrive 1 and TR_ARRIVE2 once it passes bar.sync 2)
+enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 = TR_PASS0 + 8, TR_LAST, TR_AUX_ARRIVE3, TR_N };
+struct DuoTraceRec {
+    unsigned long long st;          // the env set (state buffer) of the launch
+    uint32_t t, cta, smid, warpid;  // step counter, blockIdx.x, %smid, %warpid
+    uint32_t role, passes, pad[2];  // 0 env warp, 1 aux warp; sub-step passes stamped
+    unsigned long long ts[TR_N];    // %globaltimer, ns (0: not stamped)
+};
+__device__ DuoTraceRec* g_duo_trace;
+__device__ unsigned int g_duo_trace_cap, g_duo_trace_n;
+__device__ __forceinline__ unsigned long long tr_now(uint32_t dep) {
+    unsigned long long ts;
+    asm volatile("{\n .reg .pred p;\n setp.ne.u32 p, %1, 0x7fc00001;\n mov.u64 %0, 0;\n @p mov.u64 %0, %%globaltimer;\n}"
+                 : "=l"(ts) : "r"(dep) : "memory");
+    return ts;
+}
+#define TR_DECL unsigned long long tr_[TR_N] = {}; uint32_t tr_pass_ = 0
+#define TR(k, dep) (tr_[k] = tr_now((uint32_t)(dep)))
+#define TR_PASS_HOOK , [&](const EnvState& es) { if (tr_pass_ < 8) tr_[TR_PASS0 + tr_pass_] = tr_now(__float_as_uint(es.omega[0])); ++tr_pass_; }
+__device__ __forceinline__ void tr_commit(const unsigned long long* ts, uint32_t passes, const float4* st, uint32_t t, uint32_t role) {
+    if ((threadIdx.x & 31) != 0 || g_duo_trace == nullptr) return;
+    const unsigned int k = atomicAdd(&g_duo_trace_n, 1u);
+    if (k >= g_duo_trace_cap) return;
+    DuoTraceRec& r = g_duo_trace[k];
+    uint32_t smid, warpid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    asm volatile("mov.u32 %0, %%warpid;" : "=r"(warpid));
+    r.st = reinterpret_cast<unsigned long long>(st); r.t = t; r.cta = blockIdx.x; r.smid = smid; r.warpid = warpid;
+    r.role = role; r.passes = passes;
+    for (int i = 0; i < TR_N; ++i) r.ts[i] = ts[i];
+}
+#define TR_COMMIT(role) tr_commit(tr_, tr_pass_, st, t, role)
+#else
+#define TR_DECL
+#define TR(k, dep)
+#define TR_PASS_HOOK
+#define TR_COMMIT(role)
+#endif
+
+// lane g < 13: the line of state group g holding envs env0..env0+7 (8 x 16 bytes); lane 13: their actions; lane 14: the
+// wheel-inertia group when the wheel-mass DR reads it.  An L2 prefetch is safe before griddepcontrol.wait: L2 is the
+// point of coherence, so a line the previous kernel writes afterwards is not left stale there.
+__device__ __forceinline__ void duo_prefetch_l2(const float4* st, const float2* action, int n, int env0, int lane, bool wm) {
+    const void* p = (lane < 13) ? static_cast<const void*>(st + (size_t)lane * n + env0)
+                  : (lane == 13) ? static_cast<const void*>(action + env0)
+                  : (lane == 14 && wm) ? static_cast<const void*>(st + (size_t)WL_G_PIW * n + env0) : nullptr;
+    if (p != nullptr) asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+
 // FAN = 0: no peer: the fan-out / multicast / packed-row code is not in the kernel at all (the dependent stream of one warp per
 // scheduler also pays for instruction fetch: several hundred static instructions fewer on the single-GPU path).
 // FAN = 2: multicast only -- the host has checked that num_envs is a multiple of 8 and the output rows are aligned, so every row
@@ -481,12 +534,20 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
                    uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf) {
     using S = Spec<K>;
     __shared__ DuoShared sh;
+    TR_DECL;
+    TR(TR_ENTRY, 0);
     if (threadIdx.x >= 64) return;                              // the spacer warp
     const int n = c.num_envs;
+    TR(TR_PARAMS, n);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int env0 = blockIdx.x * WL_DUO_ENVS;
+    // Launched with PDL, this prologue runs while the previous step's tail is still running: up to the wait it reads only
+    // kernel parameters and requests into L2 the lines both warps load first (the janitor CTA owns no envs).
+    if (warp == 0 && env0 < n) duo_prefetch_l2(st, action, n, env0, lane, S::wheel_mass(c));
+    pdl_wait();
+    TR(TR_WAITED, n);
     const uint32_t t = decode_step(gl, t_arg);
     if (janitor_cta(c, gl, t, d_log)) return;
-    const int env0 = blockIdx.x * WL_DUO_ENVS;
     const Terrain T{nullptr};
     if (warp == 1) {
         // ================= aux warp: lane j < 8 <-> env env0 + j =================
@@ -506,6 +567,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         }
         float wts[WL_MAX_REW_TERMS];
         load_weights(c, gl, t, wts);
+        TR(TR_LOADS, __float_as_uint(a.x) ^ __float_as_uint(s1.w) ^ __float_as_uint(t_lf));
         // A. action map -> targets of the whole env step
         if (lane < 8) {
             float wt[4], stt[2];
@@ -514,6 +576,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             sh.tgt[j][4] = stt[0]; sh.tgt[j][5] = stt[1];
         }
         bar_arrive(1);
+        TR(TR_BAR1, __float_as_uint(sh.tgt[j][0]));
         // N. observation noise: lane = (env, Philox block)
         if (lane < 24) {
             const int jn = lane / 3, k = lane - 3 * jn;
@@ -565,10 +628,13 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
                 reinterpret_cast<float4*>(ro)[2] = make_float4(vb.z, wbo.x, wbo.y, wbo.z);
             }
             ro[12 + Lz.w] = eu;
+            TR(TR_AUX_ARRIVE3, __float_as_uint(eu));
         }
         bar_arrive(3);
         // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
         bar_sync(2);
+        TR(TR_ARRIVE2, __float_as_uint(sh.fin[j][0]));
+        pdl_trigger();                                          // (see the env warp's trigger)
         uint32_t tmask = 0u;
         float sums[WL_MAX_REW_TERMS] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
         bool done = false;
@@ -609,6 +675,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             stg4(st, WL_G_SUM0, n, i, make_float4(sums[0], sums[1], sums[2], sums[3]));
             stg4(st, WL_G_SUM1, n, i, make_float4(sums[4], sums[5], sums[6], sums[7]));
         }
+        TR(TR_LAST, __float_as_uint(sums[7]));
+        TR_COMMIT(1);
         return;
     }
     // ================= env warp: the quad (lane = wheel), 8 envs =================
@@ -621,6 +689,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     QuadRaw raw;
     quad_issue_loads(st, n, ii, w, raw, false, wm, false);
     const float2 a = action[ii];
+    TR(TR_LOADS, __float_as_uint(raw.pos.x) ^ __float_as_uint(raw.kd) ^ __float_as_uint(a.y));
     quad_unpack(raw, w, e, false, wm, c.d_inv_Iw);
     // A. action manager: only the bookkeeping; the map itself comes from the aux warp
     e.prev_action[0] = e.action[0]; e.prev_action[1] = e.action[1];
@@ -632,7 +701,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     bar_sync(1);
     const float my_targets[4] = {sh.tgt[q][w], 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
     const float my_steer_target[2] = {sh.tgt[q][(w == 3) ? 5 : 4], 0.0f};
-    run_substeps<WL_TASK_DRIFT, 4, K>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc);
+    TR(TR_BAR1, __float_as_uint(my_targets[0]));
+    run_substeps<WL_TASK_DRIFT, 4, K>(c, T, e, b, my_targets, my_efforts, my_steer_target, kc TR_PASS_HOOK);
     M3 R = env_from_chassis(c, e, b);
     // C./D. counters, terminations (the env warp needs `done` for the reset; the reward side lives in the aux warp)
     e.ep_len += 1;
@@ -648,6 +718,11 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         fo[12] = __uint_as_float(raw_mask);
     }
     bar_arrive(2);
+    TR(TR_ARRIVE2, raw_mask);
+    // The next step's launch may begin once every CTA is here (the aux warp triggers after bar.sync 2; the spacer warp and
+    // the janitor CTA have exited).  Triggering at entry instead let each grid launch the next while only partly resident,
+    // and triggering after the last store was slower on H100 (DESIGN.md 6e).
+    pdl_trigger();
     // I'. observation inputs from the post-physics state (an env that resets / gets pushed takes others below)
     float eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
     V3 wbo = rotT(R, e.w);
@@ -690,6 +765,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         else blind_obs_quad(c, e, w, eu_k, vb, wbo, zn, obs + (size_t)WL_OBS_DIM_BLIND * ii, live);
     }
     if (live) store_env_quad(st, n, i, w, e, false, false);
+    TR(TR_LAST, __float_as_uint(e.omega[0]));
+    TR_COMMIT(0);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1577,9 +1654,9 @@ wl_camera_kernel(const __grid_constant__ wl_config c, const float4* __restrict__
 // launch geometry: spread small N over all SMs, use fatter CTAs once the chip is full
 // ---------------------------------------------------------------------------------------
 // launch with (or without) the programmatic-dependent-launch attribute
-// (OFF unless WL_PDL=1; DESIGN.md 6e.  A kernel launched with it must wait (griddepcontrol.wait) before its first read of
-// anything a previous launch may have written: the thread, quad and act-step kernels do.  wl_step_duo_kernel does not --
-// a wait on its dependent chain costs more than PDL saves -- so it is always launched without the attribute.)
+// (A kernel launched with it must wait (griddepcontrol.wait) before its first read of anything a previous launch may have
+// written.  The single-GPU duo kernel is always launched with it (DESIGN.md 6e); the fan-out forms of the duo kernel share
+// its code but are launched without it; the thread, quad and act-step kernels use it only with WL_PDL=1.)
 static bool g_pdl = (getenv("WL_PDL") != nullptr) && (atoi(getenv("WL_PDL")) != 0);
 template <typename... KArgs, typename... Args>
 static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t cs, bool pdl, const Args&... args) {
@@ -1924,7 +2001,7 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
             launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
-                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
             });
     } else if (sim->fan.n > 0) {
         return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
@@ -1947,6 +2024,18 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
     return post_step(sim, step_counter, cs);
 }
+
+#ifdef WL_DUO_TRACE
+// phase-trace build only (tools/duo_trace.py): duo-kernel warps append records to `buf` (capacity `cap`) from the next
+// launch on; returns the number appended since the last call
+int wl_duo_trace_arm(void* buf, uint32_t cap) {
+    unsigned int n = 0, zero = 0;
+    if (cudaMemcpyFromSymbol(&n, g_duo_trace_n, sizeof n) != cudaSuccess) return -1;
+    if (cudaMemcpyToSymbol(g_duo_trace, &buf, sizeof buf) != cudaSuccess || cudaMemcpyToSymbol(g_duo_trace_cap, &cap, sizeof cap) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_duo_trace_n, &zero, sizeof zero) != cudaSuccess) return -1;
+    return (int)n;
+}
+#endif
 
 // ---- env.step cut in two (host-side reward / termination terms run in between) ----------------------------------------
 }   // extern "C" (templates have C++ linkage)

@@ -441,15 +441,21 @@ __device__ __forceinline__ Chassis chassis_from_env(const wl_config& c, const En
 // effort: the DC-motor effort limit per wheel (LANES == 4: slot 0 = this lane's wheel); the speed-dependent limits are
 // formed once per physics step.  With a fixed spec (K != 0) the trip counts are constants but the loops stay rolled: fully
 // unrolled, the 4 x 1 Drift sub-steps were no faster on H100 (DESIGN.md 6e) and cost ~900 more static instructions
-template <int TASK, int LANES, uint32_t K = 0>
+// `pass_done` is called after every sub-step (the duo kernel's phase trace, WL_DUO_TRACE; empty otherwise).
+struct NoPassHook { __device__ __forceinline__ void operator()(const EnvState&) const {} };
+template <int TASK, int LANES, uint32_t K = 0, typename PassHook = NoPassHook>
 __device__ __forceinline__ void run_substeps(const wl_config& c, const Terrain& T, EnvState& e, Chassis& b, const float target[4],
-                                             const float effort[4], const float steer_target[2], const StepConsts& kc) {
+                                             const float effort[4], const float steer_target[2], const StepConsts& kc,
+                                             PassHook pass_done = {}) {
     using S = Spec<K>;
     for (int d = 0; d < S::decimation(c); ++d) {
         float lo[4], hi[4];
 #pragma unroll
         for (int w = 0; w < 4 / LANES; ++w) dc_limits(c, effort[w], e.omega[w], lo[w], hi[w]);
-        for (int j = 0; j < S::substeps(c); ++j) physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
+        for (int j = 0; j < S::substeps(c); ++j) {
+            physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
+            pass_done(e);
+        }
     }
 }
 // back to the root frame: writes e.p / v / q / w, returns the rotation of the new attitude
