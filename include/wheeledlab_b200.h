@@ -468,6 +468,11 @@ int wl_set_scan_tma(wl_sim* sim, int32_t use_tma);
 int32_t wl_obs_dim(const wl_sim* sim);
 /* number of kernel launches issued through this handle since creation */
 int64_t wl_launch_count(const wl_sim* sim);
+/* what the most recent wl_step on this handle launched (read-only; launches nothing): the kernel variant actually used (1, 4
+ * or 8 after the automatic choice; 0 before the first wl_step), the handle's step-spec key, whether the Drift-family duo
+ * kernel (variant 8) ran an instantiation specialised on that key (1) or its generic body (0), and the threads per CTA of the
+ * launch (duo kernel: 96 with the spacer warp, 64 without).  Any output pointer may be NULL. */
+int wl_step_launch_info(const wl_sim* sim, int32_t* variant, uint32_t* spec_key, int32_t* specialised, int32_t* threads_per_cta);
 
 /* Visual task camera term alone (wl_step / wl_observe launch it themselves when cfg.vis_cam != 0): fills the first
  * vis_cam_w * (vis_cam_h - vis_cam_row0) floats of every observation row from the current state.  d_aug = NULL draws the

@@ -21,6 +21,14 @@ def test_library_loads_and_exports_all_header_symbols():
     assert declared == set(EXPORTED_SYMBOLS)
 
 
+def test_step_launch_info_rejects_a_null_handle():
+    import wheeledlab_b200 as wl
+    v, k, s, th = C.c_int32(-7), C.c_uint32(7), C.c_int32(-7), C.c_int32(-7)
+    assert wl.lib.wl_step_launch_info(None, C.byref(v), C.byref(k), C.byref(s), C.byref(th)) < 0
+    assert b"wl_step_launch_info" in wl.lib.wl_last_error()
+    assert (v.value, k.value, s.value, th.value) == (-7, 7, -7, -7), "outputs written on failure"
+
+
 def test_config_layout_matches_oracle_header():
     import wheeledlab_b200 as wl
     from oracle_lib import get_lib

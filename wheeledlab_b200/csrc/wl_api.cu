@@ -40,6 +40,9 @@ struct wl_sim {
     uint32_t spec;          // spec_key(step_spec(cfg)): picks the duo kernel's instantiation (see with_spec)
     const void* duo_kernel; // the duo kernel duo_threads was sized for (see duo_block)
     int duo_threads;
+    int step_variant;       // what the most recent wl_step launched (wl_step_launch_info): variant after the automatic choice
+    int step_specialised;   // (the duo kernel ran a spec instantiation, not its generic body)
+    int step_threads;       // (threads per CTA)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1011,18 +1014,21 @@ wl_rollout_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__
     }
     if (L.live) store_env_quad(st, n, L.i, L.w, e, ELEV);
     // last CTA (ticket, amortised over the K steps of the launch): turn the K accumulator rows into means and leave the
-    // globals as K single steps would have: W of the last step in its slot, its reset count where the next launch looks for
-    // it (the curriculum boundary at t0 + K is evaluated there), nothing pending for the log, the next row re-armed
+    // globals as K single steps would have: W of the last step in its slot, its raw accumulator row where the next launch
+    // looks for it (the curriculum boundary at t0 + K reads its reset count; the next janitor re-publishes it to last_log,
+    // which must not then lose the episode sums), nothing pending for the log, the next row re-armed
     if ((threadIdx.x & 31) == 0) __threadfence();
     __syncthreads();
     if (threadIdx.x != 0) return;
     const unsigned tk = atomicAdd(ticket, 1u);
     if (tk != gridDim.x - 1) return;
     __threadfence();
-    float last_cnt = 0.0f;
+    float last_raw[16];
     for (int k = 0; k < K; ++k) {
         float* row = d_log + (size_t)k * WL_LOG_FLOATS;
         const float cnt = __ldcg(&row[8]);
+        if (k == K - 1)
+            for (int q = 0; q < 16; ++q) last_raw[q] = __ldcg(&row[q]);
         if (cnt > 0.0f) {
             const float denom = cnt * c.episode_length_s;
             for (int q = 0; q < WL_MAX_REW_TERMS; ++q) row[q] = __ldcg(&row[q]) / denom;
@@ -1030,11 +1036,10 @@ wl_rollout_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__
         } else {
             for (int q = 0; q < 16; ++q) row[q] = gl->last_log[q];         // no reset in this step: the previous row persists
         }
-        last_cnt = cnt;
     }
     const uint32_t tl = t0 + (uint32_t)K - 1u;
     for (int q = 0; q < WL_MAX_REW_TERMS; ++q) gl->rew_weight[tl & 1u][q] = wts[q];
-    for (int q = 0; q < 16; ++q) { gl->acc[tl % 3u][q] = (q == 8) ? last_cnt : 0.0f; gl->acc[(tl + 1u) % 3u][q] = 0.0f; }
+    for (int q = 0; q < 16; ++q) { gl->acc[tl % 3u][q] = last_raw[q]; gl->acc[(tl + 1u) % 3u][q] = 0.0f; }
     gl->log_ptr[tl % 3u] = nullptr;
     *ticket = 0u;
 }
@@ -1885,6 +1890,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     s->spec = spec_key(step_spec(s->cfg));
     s->duo_kernel = nullptr;
     s->duo_threads = 64;
+    s->step_variant = s->step_specialised = s->step_threads = 0;
     if (cfg->task == WL_TASK_ELEVATION) {
         typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -1932,6 +1938,14 @@ int wl_set_kernel_variant(wl_sim* sim, int32_t lanes_per_env) {
     return WL_OK;
 }
 int64_t wl_launch_count(const wl_sim* sim) { return sim ? sim->launches : 0; }
+int wl_step_launch_info(const wl_sim* sim, int32_t* variant, uint32_t* spec_key, int32_t* specialised, int32_t* threads_per_cta) {
+    if (!sim) return fail(WL_EINVAL, "wl_step_launch_info: null handle");
+    if (variant) *variant = sim->step_variant;
+    if (spec_key) *spec_key = sim->spec;
+    if (specialised) *specialised = sim->step_specialised;
+    if (threads_per_cta) *threads_per_cta = sim->step_threads;
+    return WL_OK;
+}
 
 }   // extern "C"
 // Steps are issued with consecutive counters (the janitor protocol, see wl_globals).  Resolve this launch's counter on the host
@@ -1991,6 +2005,7 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     if (int rc = prep_step(sim, step_counter, 1, cs)) return rc;
     const bool elev = sim->cfg.task == WL_TASK_ELEVATION, vis = sim->cfg.task == WL_TASK_VISUAL;
     StageIO sio0{sim->term_bits, nullptr, nullptr};
+    int specialised = 0, cta_threads = 0;
     if (variant == 8) {
         const int grid = (n + WL_DUO_ENVS - 1) / WL_DUO_ENVS + 1;                            // + the janitor CTA
         const bool rows_ok = (n % WL_DUO_ENVS) == 0 && (((uintptr_t)d_obs | (uintptr_t)d_rew) & 15u) == 0 &&
@@ -2001,8 +2016,10 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
             launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
+                specialised = k.value != 0u;
                 launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
             });
+        cta_threads = sim->duo_threads;
     } else if (sim->fan.n > 0) {
         return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
     } else if (variant == 4) {
@@ -2013,12 +2030,15 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
         with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
             launch_k(wl_step_quad_kernel<task>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits);
         });
+        cta_threads = bs;
     } else {
         const int bs = pick_block(n), grid = (n + bs - 1) / bs + 1;
         with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
             launch_k(wl_step_kernel<task, 0>, grid, bs, 0, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio0);
         });
+        cta_threads = bs;
     }
+    sim->step_variant = variant; sim->step_specialised = specialised; sim->step_threads = cta_threads;
     if (int rc = launched(sim, "wl_step_kernel")) return rc;
     if (elev) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
     if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
