@@ -531,6 +531,56 @@ int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_va
 int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, float beta1,
                     float beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream);
 
+/* ---- the learner: rsl_rl PPO.update() for the Drift-family actor-critic, trained in the act-step blob in place -------
+ * rsl_rl PPO.update() (modified_rsl_rl_runner.py:118; rsl-rl-lib >= 2.3.0) [UPSTREAM-RECALL] on the network wl_act_step
+ * runs (obs_dim <= 16, [64, 64] ELU actor and critic, 2 actions, learned per-action std), with the weights, gradients
+ * and Adam moments all in the blob layout above.  One call enqueues the whole update (epochs x mini-batches), never
+ * syncs the host and is graph-capturable:
+ *   advantages normalised once over the batch ((A - mean) / (unbiased std + 1e-8), computed on the fly; the caller's
+ *   tensor is not modified); old sigma = the blob's std when the update starts; per mini-batch i (rows
+ *   perm[i*B .. (i+1)*B), B = batch / num_mini_batches, the same permutation every epoch): clipped surrogate +
+ *   value_loss_coef * (clipped) value loss - entropy_coef * entropy, gradient (torch autograd semantics at max / clamp
+ *   edges), KL-adaptive learning rate, clip_grad_norm_(max_grad_norm), Adam (0.9, 0.999, 1e-8).
+ * The reduction order depends only on (batch, the device's SM count): results are bit-identical run to run. */
+typedef struct wl_ppo_params {
+    int32_t obs_dim;
+    int32_t batch;                  /* T * N rows of the slab */
+    int32_t num_learning_epochs;
+    int32_t num_mini_batches;
+    float clip_param;
+    float value_loss_coef;
+    float entropy_coef;
+    float max_grad_norm;
+    float desired_kl;
+    int32_t adaptive;               /* 1: schedule "adaptive" (the KL rule moves the device lr); 0: "fixed" */
+    int32_t use_clipped_value_loss;
+    int32_t _pad;
+} wl_ppo_params;
+typedef struct wl_ppo_batch {      /* device arrays over the [T*N] rows, slab order (row = t*N + n) */
+    const float* obs;               /* [batch, obs_dim] the observations the actions were drawn from */
+    const float* actions;           /* [batch, 2] */
+    const float* values;            /* [batch] values at collection time (the value-clip anchor) */
+    const float* log_prob;          /* [batch] log-probabilities at collection time */
+    const float* mean;              /* [batch, 2] action means at collection time */
+    const float* returns;           /* [batch] */
+    const float* advantages;        /* [batch] un-normalised */
+    const int64_t* perm;            /* [batch] a permutation of 0..batch-1 (torch.randperm) */
+} wl_ppo_batch;
+/* the device state d_state[wl_ppo_state_floats()] (fp32; the caller zero-fills it and sets [0] = initial learning rate):
+ *   [0] learning rate  [1] Adam step count  [2..3] old std  [4] advantage mean  [5] advantage std
+ *   [6] sum of surrogate losses  [7] sum of value losses  [8] sum of entropies (over this update's mini-batches)
+ *   [9] the last mini-batch's KL  [10..] per mini-batch (KL, learning rate used) pairs of the last update, up to
+ *   WL_PPO_MAX_UPDATES mini-batches */
+#define WL_PPO_MAX_UPDATES 256
+int32_t wl_ppo_state_floats(void);
+/* workspace for wl_ppo_update on the current device (it holds one gradient row per CTA; 0 and wl_last_error() on error) */
+size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches);
+/* d_blob / d_adam_m / d_adam_v: wl_policy_blob_floats(obs_dim) floats each, 16-byte aligned; the moments start zero.
+ * Padding rows and columns of the blob stay exactly zero.  The workspace's first blob-sized row holds the last
+ * mini-batch's reduced gradient (before clipping) after the call. */
+int wl_ppo_update(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
+                  float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* A caller that drives wl_step through a CUDA graph of K steps (how a rollout is meant to be issued: one launch per K steps)
  * pays the upload of the instantiated graph to the device on its FIRST launch; this moves that
  * upload to set-up time.  graph_exec = cudaGraphExec_t (torch: CUDAGraph.raw_cuda_graph_exec()). */

@@ -1486,6 +1486,16 @@ wl_gae_seg_kernel(const float* __restrict__ rew, const float* __restrict__ val, 
 // Adam to its own replica of the parameters.  10.5 K parameters = 42 KB per rank: one launch instead of NCCL all-reduce +
 // optimizer kernels.  The caller brackets the launch with barriers (gradients complete / safe to overwrite).
 struct GradPeers { int32_t n; int32_t pad; const float* g[WL_MAX_PEERS]; };
+// torch.optim.Adam's update of one parameter (bias corrections bc = 1 - beta^t, complements cb = 1 - beta); shared by every
+// optimiser kernel
+__device__ __forceinline__ void adam_update(float* param, float* m, float* v, int i, float g, float lr, float beta1, float cb1,
+                                            float beta2, float cb2, float eps, float bc1, float bc2) {
+    const float p = param[i];
+    const float mi = fmaf(beta1, m[i], cb1 * g);
+    const float vi = fmaf(beta2, v[i], cb2 * g * g);
+    m[i] = mi; v[i] = vi;
+    param[i] = p - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
+}
 __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__ m, float* __restrict__ v, const __grid_constant__ GradPeers gp,
                                   float lr, float beta1, float beta2, float eps, float weight_decay, float bc1, float bc2, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1493,13 +1503,11 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
     float g = 0.0f;
     for (int r = 0; r < gp.n; ++r) g += __ldcg(gp.g[r] + i);           // (L2-coherent loads: peers have just written)
     g = g / (float)gp.n;
-    float p = param[i];
-    if (weight_decay != 0.0f) g = fmaf(weight_decay, p, g);
-    const float mi = fmaf(beta1, m[i], (1.0f - beta1) * g);
-    const float vi = fmaf(beta2, v[i], (1.0f - beta2) * g * g);
-    m[i] = mi; v[i] = vi;
-    param[i] = p - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);          // torch.optim.Adam's update (bias corrections bc = 1 - beta^t)
+    if (weight_decay != 0.0f) g = fmaf(weight_decay, param[i], g);
+    adam_update(param, m, v, i, g, lr, beta1, 1.0f - beta1, beta2, 1.0f - beta2, eps, bc1, bc2);
 }
+
+#include "wl_ppo.cuh"
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2289,6 +2297,90 @@ int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, con
     const float bc1 = 1.0f - powf(beta1, (float)step), bc2 = 1.0f - powf(beta2, (float)step);
     wl_dp_adam_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(d_param, d_m, d_v, gp, lr, beta1, beta2, eps, weight_decay, bc1, bc2, n);
     return cuda_check(cudaGetLastError(), "wl_dp_adam_kernel");
+}
+
+// workspace of wl_ppo_update: [reduced row][fp64 block sums of squares][one gradient row per CTA], each 256-byte aligned
+struct PpoWorkspace { int blob_floats, rowlen, ctas, norm_parts; size_t norm_off, rows_off, bytes; };
+static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
+    if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
+    if (obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
+    int dev = 0, sms = 0;
+    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
+    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
+    int32_t off[13];
+    w.blob_floats = policy_offsets(obs_dim, off);
+    w.rowlen = (w.blob_floats + WL_PPO_STATS + 3) & ~3;
+    const int tiles = (batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE;
+    w.ctas = tiles < sms ? tiles : sms;
+    w.norm_parts = (w.rowlen + 255) / 256;
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    w.norm_off = al(sizeof(float) * w.rowlen);
+    w.rows_off = al(w.norm_off + sizeof(double) * w.norm_parts);
+    w.bytes = w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas;
+    return WL_OK;
+}
+
+int32_t wl_ppo_state_floats(void) { return 10 + 2 * WL_PPO_MAX_UPDATES; }
+
+size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches) {
+    PpoWorkspace w;
+    return ppo_workspace("wl_ppo_workspace_bytes", obs_dim, batch, num_mini_batches, w) ? 0 : w.bytes;
+}
+
+int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
+                  void* d_workspace, size_t workspace_bytes, void* stream) {
+    if (!p || !b) return fail(WL_EINVAL, "wl_ppo_update: null params / batch");
+    if (!b->obs || !b->actions || !b->values || !b->log_prob || !b->mean || !b->returns || !b->advantages || !b->perm)
+        return fail(WL_EINVAL, "wl_ppo_update: null array in batch");
+    if (!d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
+        return fail(WL_EINVAL, "wl_ppo_update: null d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
+    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, "wl_ppo_update: num_learning_epochs must be >= 1");
+    PpoWorkspace w;
+    if (int rc = ppo_workspace("wl_ppo_update", p->obs_dim, p->batch, p->num_mini_batches, w)) return rc;
+    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
+        return fail(WL_EINVAL, "wl_ppo_update: d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
+    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
+        return fail(WL_EINVAL, "wl_ppo_update: d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
+    if (workspace_bytes < w.bytes)
+        return fail(WL_EINVAL, "wl_ppo_update: workspace_bytes too small (wl_ppo_workspace_bytes gives " + std::to_string(w.bytes) + ")");
+    PolicyOffsets po;
+    policy_offsets(p->obs_dim, po.o);
+    const int B = p->batch / p->num_mini_batches;
+    const size_t smem = sizeof(float) * ((size_t)w.blob_floats + 2 * WL_HID * WL_HID + WL_HID + WL_PPO_TILE * WL_PPO_XS +
+                                         4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
+    int dev = 0;
+    cudaGetDevice(&dev);
+    static bool attr_set[64] = {false};                      // the attribute is per device
+    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_ppo_update"))
+            return rc;
+        attr_set[dev] = true;
+    }
+    cudaStream_t cs = (cudaStream_t)stream;
+    char* ws = (char*)d_workspace;
+    float* red = (float*)ws;
+    double* norm_part = (double*)(ws + w.norm_off);
+    float* rows = (float*)(ws + w.rows_off);
+    wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
+    if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
+    PpoArgs a;
+    a.b = *b; a.obs_dim = p->obs_dim; a.B = B; a.tiles = (B + WL_PPO_TILE - 1) / WL_PPO_TILE;
+    a.clip = p->clip_param; a.vcoef = p->value_loss_coef; a.inv_B = 1.0f / (float)B; a.clipped_value = p->use_clipped_value_loss != 0;
+    PpoStepArgs sa{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
+    for (int e = 0; e < p->num_learning_epochs; ++e) {
+        for (int i = 0; i < p->num_mini_batches; ++i) {
+            a.row0 = (int64_t)i * B;
+            sa.update_index = e * p->num_mini_batches + i;
+            wl_ppo_grad_kernel<<<w.ctas, WL_PPO_THREADS, smem, cs>>>(d_blob, w.blob_floats, po, a, d_state, rows, w.rowlen);
+            wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
+                                                               p->entropy_coef, red, norm_part);
+            wl_ppo_step_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                 w.blob_floats, po, p->obs_dim, sa);
+            if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel")) return rc;
+        }
+    }
+    return WL_OK;
 }
 
 int wl_test_detmath(int32_t op, const float* d_in, const float* d_in2, float* d_out, int32_t n, void* stream) {

@@ -53,6 +53,60 @@ def pack_actor_critic(actor, critic, std: torch.Tensor, obs_dim: int, device, ou
     return blob
 
 
+def _blob_layers(blob: torch.Tensor, obs_dim: int):
+    """Zero-copy views of the blob: per net, three (W [in, out] input-major, b [out]) pairs; plus std [2]."""
+    off, _ = blob_layout(obs_dim)
+    nets = []
+    for net_i, nout in enumerate((2, 1)):
+        o = off[net_i * 6:net_i * 6 + 6]
+        nets.append([(blob[o[0]:o[0] + obs_dim * HIDDEN].view(obs_dim, HIDDEN), blob[o[1]:o[1] + HIDDEN]),
+                     (blob[o[2]:o[2] + HIDDEN * HIDDEN].view(HIDDEN, HIDDEN), blob[o[3]:o[3] + HIDDEN]),
+                     (blob[o[4]:o[4] + HIDDEN * nout].view(HIDDEN, nout), blob[o[5]:o[5] + nout])])
+    return nets[0], nets[1], blob[off[12]:off[12] + 2]
+
+
+def actor_critic_state_dict(blob: torch.Tensor, obs_dim: int) -> dict:
+    """The blob as an rsl_rl ActorCritic state dict (actor.0/2/4.weight|bias, critic.0/2/4.weight|bias, std) [UPSTREAM-RECALL]:
+    the ``model_state_dict`` of the checkpoints rsl_rl's runner saves and ``play_policy.py`` loads.  Tensors are copies."""
+    actor, critic, std = _blob_layers(blob, obs_dim)
+    sd = {}
+    for name, layers in (("actor", actor), ("critic", critic)):
+        for k, (w, b) in enumerate(layers):
+            sd[f"{name}.{2 * k}.weight"] = w.t().contiguous()
+            sd[f"{name}.{2 * k}.bias"] = b.clone()
+    sd["std"] = std.clone()
+    return sd
+
+
+def load_actor_critic_state_dict(sd: dict, obs_dim: int, out: torch.Tensor | None = None, device=None) -> torch.Tensor:
+    """Inverse of actor_critic_state_dict: fills `out` (or a new zeroed blob) from an rsl_rl ActorCritic state dict."""
+    if out is None:
+        out = torch.zeros(blob_layout(obs_dim)[1], dtype=torch.float32, device=device or sd["std"].device)
+    actor, critic, std = _blob_layers(out, obs_dim)
+    with torch.no_grad():
+        for name, layers in (("actor", actor), ("critic", critic)):
+            for k, (w, b) in enumerate(layers):
+                wt, bt = sd[f"{name}.{2 * k}.weight"], sd[f"{name}.{2 * k}.bias"]
+                if tuple(wt.shape) != (w.shape[1], w.shape[0]) or tuple(bt.shape) != tuple(b.shape):
+                    raise ValueError(f"{name}.{2 * k}: shape {tuple(wt.shape)} does not match the [64, 64] ELU network of obs_dim {obs_dim}")
+                w.copy_(wt.t())
+                b.copy_(bt)
+        std.copy_(sd["std"])
+    return out
+
+
+def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor) -> torch.Tensor:
+    """V(obs) [N] in torch from zero-copy views of the blob (the bootstrap value of compute_returns): a CUDA graph that
+    captures it reads the weights the last update left in the blob."""
+    _, critic, _ = _blob_layers(blob, obs_dim)
+    x = obs
+    for k, (w, b) in enumerate(critic):
+        x = torch.addmm(b, x, w)
+        if k < 2:
+            x = torch.nn.functional.elu(x)
+    return x.squeeze(-1)
+
+
 class PolicyBuffers:
     """[T, N] storage of what alg.act() records per step (rsl_rl RolloutStorage fields)."""
 
