@@ -2299,6 +2299,13 @@ int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, con
     return cuda_check(cudaGetLastError(), "wl_dp_adam_kernel");
 }
 
+// dynamic shared memory of wl_ppo_grad_kernel: the blob (grows with obs_dim), W2 transposed, the tile's rows
+static size_t ppo_grad_smem(int obs_dim) {
+    int32_t off[13];
+    return sizeof(float) * ((size_t)policy_offsets(obs_dim, off) + 2 * WL_HID * WL_HID + WL_HID + WL_PPO_TILE * WL_PPO_XS +
+                            4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
+}
+
 // workspace of wl_ppo_update: [reduced row][fp64 block sums of squares][one gradient row per CTA], each 256-byte aligned
 struct PpoWorkspace { int blob_floats, rowlen, ctas, norm_parts; size_t norm_off, rows_off, bytes; };
 static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
@@ -2308,6 +2315,15 @@ static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t
     int dev = 0, sms = 0;
     if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
     if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
+    // the grad kernel's shared-memory limit is a per-device attribute: raised once to what the widest obs_dim needs, so
+    // updates of any obs_dim share it in one process.  The workspace query reaches here before the first update, so
+    // callers that query outside a graph capture (FusedPPO, PPOIteration.start) never set it inside one.
+    static bool attr_set[64] = {false};
+    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_grad_smem(16)), fn))
+            return rc;
+        attr_set[dev] = true;
+    }
     int32_t off[13];
     w.blob_floats = policy_offsets(obs_dim, off);
     w.rowlen = (w.blob_floats + WL_PPO_STATS + 3) & ~3;
@@ -2347,16 +2363,7 @@ int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, 
     PolicyOffsets po;
     policy_offsets(p->obs_dim, po.o);
     const int B = p->batch / p->num_mini_batches;
-    const size_t smem = sizeof(float) * ((size_t)w.blob_floats + 2 * WL_HID * WL_HID + WL_HID + WL_PPO_TILE * WL_PPO_XS +
-                                         4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {false};                      // the attribute is per device
-    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_ppo_update"))
-            return rc;
-        attr_set[dev] = true;
-    }
+    const size_t smem = ppo_grad_smem(p->obs_dim);
     cudaStream_t cs = (cudaStream_t)stream;
     char* ws = (char*)d_workspace;
     float* red = (float*)ws;
