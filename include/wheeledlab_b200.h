@@ -581,6 +581,25 @@ size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_b
 int wl_ppo_update(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
                   float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the wide actor-critic: the Elevation / Visual policy and its PPO update -------------------------------------------
+ * The same network and blob layout as above with ReLU instead of ELU between the layers (the reference's Elevation and
+ * Visual agent cfgs, activation="relu"), for any obs_dim in 1..4096.  FP32 FFMA throughout; layer 1 runs as a K-chunked
+ * SGEMM, since W1t no longer fits in shared memory.
+ * wl_policy_act: for every env of `sim`, the actor mean, critic value, sampled action and log-prob of d_obs_in [N, obs_dim]
+ * into `out`.  The noise is wl_act_step's (seed, env_id_offset + env, decoded step_counter -- device-relative counters
+ * included), so a = mean + std * z matches it bit for bit for the same mean.  One launch; it does not step the env:
+ * follow it with wl_step(out.actions, ..., the same step_counter). */
+int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter,
+                  void* stream);
+/* rsl_rl PPO.update() on that network: the semantics, structs and d_state layout of wl_ppo_update (relu'(z) = (h > 0), 0
+ * at z == 0 as torch's threshold_backward).  Per mini-batch: the gathered layer-1 forward, layers 2-3 and the loss with
+ * back-propagation to layer 1's pre-activation, the gathered split-K dW1, then wl_ppo_update's reduce and Adam step.
+ * No float atomics: results are bit-identical run to run for a given (batch, SM count).  The workspace also holds the
+ * mini-batch's layer-1 activations and their gradients (2 x batch / num_mini_batches x 128 floats). */
+size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches);
+int wl_ppo_update_wide(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
+                       float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* A caller that drives wl_step through a CUDA graph of K steps (how a rollout is meant to be issued: one launch per K steps)
  * pays the upload of the instantiated graph to the device on its FIRST launch; this moves that
  * upload to set-up time.  graph_exec = cudaGraphExec_t (torch: CUDAGraph.raw_cuda_graph_exec()). */

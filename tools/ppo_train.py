@@ -1,10 +1,11 @@
-"""A whole Drift PPO training loop on one GPU: FusedPolicyRollout -> bootstrap value -> compute_returns -> FusedPPO.update,
-one CUDA graph per iteration (learner.PPOIteration), with rsl_rl's default Drift settings (learner.PPOConfig).
+"""A whole PPO training loop on one GPU (Drift, or Elevation with ``--task elevation``): FusedPolicyRollout -> bootstrap value -> compute_returns -> FusedPPO.update,
+one CUDA graph per iteration (learner.PPOIteration), with rsl_rl's default Drift settings (learner.PPOConfig) and the
+task's network: [64, 64] ELU for Drift, ReLU for Elevation (its agent cfg, activation="relu").
 
 Prints, per iteration, the mean return of the episodes that ended during it, the learning rate and the losses; the
 statistics are read back once per iteration, after the graph replay.
 
-    python tools/ppo_train.py --envs 4096 --iters 50 [--eager] [--out results.txt]
+    python tools/ppo_train.py [--task elevation] --envs 4096 --iters 50 [--eager] [--out results.txt]
 """
 from __future__ import annotations
 
@@ -20,6 +21,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--task", choices=["drift", "elevation"], default="drift")
     ap.add_argument("--envs", type=int, default=4096)
     ap.add_argument("--steps", type=int, default=128, help="rollout length T (num_steps_per_env)")
     ap.add_argument("--iters", type=int, default=50)
@@ -32,14 +34,16 @@ def main():
     from wheeledlab_b200.policy import pack_actor_critic
     dev = "cuda:0"
     torch.manual_seed(a.seed)
-    sim = wl.WheeledSim(wl.drift_task(num_envs=a.envs, seed=a.seed), dev)
+    make, activation, name = (wl.drift_task, "elu", "Drift") if a.task == "drift" else (wl.elevation_task, "relu", "Elevation")
+    sim = wl.WheeledSim(make(num_envs=a.envs, seed=a.seed), dev)
     sim.startup(); sim.reset(None, 0)
     D = sim.obs_dim
-    mk = lambda out: torch.nn.Sequential(torch.nn.Linear(D, 64), torch.nn.ELU(), torch.nn.Linear(64, 64), torch.nn.ELU(), torch.nn.Linear(64, out))
+    act = torch.nn.ELU if activation == "elu" else torch.nn.ReLU
+    mk = lambda out: torch.nn.Sequential(torch.nn.Linear(D, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
     blob = pack_actor_critic(mk(2), mk(1), torch.ones(2), D, dev)           # init_noise_std = 1.0 (rsl_rl_ppo_cfg.py:13)
-    it = PPOIteration(sim, blob, PPOConfig(), a.steps).start(0, capture=not a.eager)
+    it = PPOIteration(sim, blob, PPOConfig(), a.steps, activation=activation).start(0, capture=not a.eager)
     cur = torch.zeros(a.envs, device=dev)
-    lines = [f"# Drift PPO, {a.envs} envs x {a.steps} steps, PPOConfig() defaults, seed {a.seed}, "
+    lines = [f"# {name} PPO (obs_dim {D}, {activation}), {a.envs} envs x {a.steps} steps, PPOConfig() defaults, seed {a.seed}, "
              f"{'eager update' if a.eager else 'one graph per iteration'}, {torch.cuda.get_device_name(0)}",
              "iter  mean_episode_reward  episodes  learning_rate  value_loss  surrogate  entropy  ms"]
     print(lines[0]); print(lines[1])

@@ -123,6 +123,7 @@ class WlPolicyOut(C.Structure):
 lib.wl_policy_blob_floats.restype = _i32
 lib.wl_policy_blob_floats.argtypes = [_i32, C.POINTER(_i32)]
 lib.wl_act_step.argtypes = [_vp, _vp, _vp, WlPolicyOut, _vp, _vp, _vp, _vp, _vp, _i64, _vp]
+lib.wl_policy_act.argtypes = [_vp, _vp, _vp, WlPolicyOut, _i64, _vp]
 lib.wl_camera.argtypes = [_vp, _vp, _i64, _vp, _vp]
 lib.wl_step_stage_a.argtypes = [_vp, _vp, _vp, _vp, _i64, _vp]
 lib.wl_step_stage_b.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]
@@ -147,6 +148,9 @@ lib.wl_ppo_state_floats.argtypes = []
 lib.wl_ppo_workspace_bytes.restype = _sz
 lib.wl_ppo_workspace_bytes.argtypes = [_i32, _i32, _i32]
 lib.wl_ppo_update.argtypes = [C.POINTER(WlPpoParams), C.POINTER(WlPpoBatch), _vp, _vp, _vp, _vp, _vp, _sz, _vp]
+lib.wl_ppo_wide_workspace_bytes.restype = _sz
+lib.wl_ppo_wide_workspace_bytes.argtypes = [_i32, _i32, _i32]
+lib.wl_ppo_update_wide.argtypes = [C.POINTER(WlPpoParams), C.POINTER(WlPpoBatch), _vp, _vp, _vp, _vp, _vp, _sz, _vp]
 lib.wl_test_detmath.argtypes = [_i32, _vp, _vp, _vp, _i32, _vp]
 lib.wl_test_philox.argtypes = [_u64, _u32, _u32, _u32, _u32, _vp, _i32, _vp]
 lib.wl_test_null.argtypes = [_i32, _i32, _vp]
@@ -156,7 +160,7 @@ lib.wl_graph_upload.argtypes = [_vp, _vp]
 EXPORTED_SYMBOLS = [
     "wl_config_describe", "wl_config_sizeof", "wl_config_finalize", "wl_set_step_counter", "wl_advance_counter", "wl_note_device_counter", "wl_log_flush", "wl_reward_weights", "wl_set_seed", "wl_set_term_bits", "wl_set_peer_fanout", "wl_set_multicast_fanout", "wl_state_bytes", "wl_globals_offset", "wl_create", "wl_destroy",
     "wl_last_error", "wl_build_info", "wl_startup", "wl_reset", "wl_step", "wl_step_host", "wl_step_host_zero_copy", "wl_rollout", "wl_result_bytes", "wl_observe", "wl_curriculum",
-    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_null", "wl_test_null_cfg",
+    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_policy_act", "wl_ppo_wide_workspace_bytes", "wl_ppo_update_wide", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_null", "wl_test_null_cfg",
 ]
 
 

@@ -827,11 +827,9 @@ __device__ __forceinline__ float elu(float x) { return x > 0.0f ? x : __expf(x) 
 
 // one hidden layer for a register tile of 4 units x 4 envs: per 4 inputs, 4 LDS.128 of activations (one per env, a pure
 // broadcast: the whole warp shares the env tile) and 4 LDS.128 of input-major weights (conflict-free: the 16 lanes of a
-// net read 256 contiguous bytes) feed 64 FMAs; accumulation order per output = bias, then inputs ascending
-__device__ __forceinline__ void mlp_tile_layer(const float* W, const float* bias, const float* x0, int xstride, int nin, float acc[4][4]) {
-    const float4 b0 = *reinterpret_cast<const float4*>(bias);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) { acc[e][0] = b0.x; acc[e][1] = b0.y; acc[e][2] = b0.z; acc[e][3] = b0.w; }
+// net read 256 contiguous bytes) feed 64 FMAs; accumulation order per output = bias, then inputs ascending.
+// mlp_tile_accum adds inputs 0..nin-1 to acc (nin a multiple of 4), so a layer can also be run in K chunks.
+__device__ __forceinline__ void mlp_tile_accum(const float* W, const float* x0, int xstride, int nin, float acc[4][4]) {
 #pragma unroll 4
     for (int j = 0; j < nin; j += 4) {
         float xs[4][4];
@@ -851,6 +849,24 @@ __device__ __forceinline__ void mlp_tile_layer(const float* W, const float* bias
             }
         }
     }
+}
+__device__ __forceinline__ void mlp_tile_layer(const float* W, const float* bias, const float* x0, int xstride, int nin, float acc[4][4]) {
+    const float4 b0 = *reinterpret_cast<const float4*>(bias);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { acc[e][0] = b0.x; acc[e][1] = b0.y; acc[e][2] = b0.z; acc[e][3] = b0.w; }
+    mlp_tile_accum(W, x0, xstride, nin, acc);
+}
+
+// the policy's Gaussian head (rsl_rl ActorCritic.act): z ~ N(0,1)^2 from the generator's policy stream for (global env,
+// step), a = mean + std * z, log-prob summed over the two action dims.  wl_act_step and wl_policy_act share it, so their
+// samples agree bit for bit.
+__device__ __forceinline__ void policy_noise(uint64_t seed, uint32_t gid, uint32_t t, float& z0, float& z1) {
+    const uint4 r = philox4x32(seed, gid, t, RNG_POLICY, 0u);
+    box_muller(r.x, r.y, z0, z1);
+}
+__device__ __forceinline__ void gaussian_head(float m0, float m1, float s0, float s1, float z0, float z1, float2& a, float& lp) {
+    a = make_float2(fmaf(s0, z0, m0), fmaf(s1, z1, m1));
+    lp = -0.5f * (z0 * z0 + z1 * z1) - __logf(s0) - __logf(s1) - 1.8378770664093453f;   // 2 * 0.5 log(2 pi)
 }
 
 __device__ __forceinline__ void mlp_tile_store_elu(float* h0, int hstride, const float acc[4][4]) {
@@ -918,8 +934,7 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     // the policy noise does not depend on the weights: draw it while the copies are in flight
     float z0 = 0.0f, z1 = 0.0f, zn[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     if (stepper) {
-        const uint4 r = philox4x32(c.seed, L.gid, t, RNG_POLICY, 0u);
-        box_muller(r.x, r.y, z0, z1);
+        policy_noise(c.seed, L.gid, t, z0, z1);
         if (!ELEV && !VIS) quad_obs_noise(c, L.w, L.gid, t, RNG_OBS, 0u, zn);
     }
     __syncthreads();                                         // mbarrier init visible to every waiter; obs rows written
@@ -960,13 +975,13 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
         m1 += __shfl_xor_sync(0xffffffffu, m1, 1); m1 += __shfl_xor_sync(0xffffffffu, m1, 2);
         vv += __shfl_xor_sync(0xffffffffu, vv, 1); vv += __shfl_xor_sync(0xffffffffu, vv, 2);
         m0 += sw[po_off.o[5]]; m1 += sw[po_off.o[5] + 1]; vv += sw[po_off.o[11]];
-        // Gaussian head: a = mean + std * z (rsl_rl ActorCritic.act), log-prob summed over the action dims
-        const float s0 = sw[po_off.o[12]], s1 = sw[po_off.o[12] + 1];
-        const float2 a = make_float2(fmaf(s0, z0, m0), fmaf(s1, z1, m1));
+        float2 a;
+        float lp;
+        gaussian_head(m0, m1, sw[po_off.o[12]], sw[po_off.o[12] + 1], z0, z1, a, lp);
         if (L.live && L.w == 0) {
             reinterpret_cast<float2*>(po.actions)[L.i] = a;
             reinterpret_cast<float2*>(po.mean)[L.i] = make_float2(m0, m1);
-            po.log_prob[L.i] = -0.5f * (z0 * z0 + z1 * z1) - __logf(s0) - __logf(s1) - 1.8378770664093453f;   // 2 * 0.5 log(2 pi)
+            po.log_prob[L.i] = lp;
             po.value[L.i] = vv;
         }
         // ---- the env step on the sampled action
@@ -1508,6 +1523,7 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 }
 
 #include "wl_ppo.cuh"
+#include "wl_wide.cuh"
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2308,6 +2324,17 @@ static size_t ppo_grad_smem(int obs_dim) {
 
 // workspace of wl_ppo_update: [reduced row][fp64 block sums of squares][one gradient row per CTA], each 256-byte aligned
 struct PpoWorkspace { int blob_floats, rowlen, ctas, norm_parts; size_t norm_off, rows_off, bytes; };
+static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_batches, int sms, PpoWorkspace& w) {
+    int32_t off[13];
+    w.blob_floats = policy_offsets(obs_dim, off);
+    w.rowlen = (w.blob_floats + WL_PPO_STATS + 3) & ~3;
+    const int tiles = (batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE;
+    w.ctas = tiles < sms ? tiles : sms;
+    w.norm_parts = (w.rowlen + 255) / 256;
+    w.norm_off = align256(sizeof(float) * w.rowlen);
+    w.rows_off = align256(w.norm_off + sizeof(double) * w.norm_parts);
+    w.bytes = w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas;
+}
 static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
     if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
     if (obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
@@ -2324,16 +2351,7 @@ static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t
             return rc;
         attr_set[dev] = true;
     }
-    int32_t off[13];
-    w.blob_floats = policy_offsets(obs_dim, off);
-    w.rowlen = (w.blob_floats + WL_PPO_STATS + 3) & ~3;
-    const int tiles = (batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE;
-    w.ctas = tiles < sms ? tiles : sms;
-    w.norm_parts = (w.rowlen + 255) / 256;
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    w.norm_off = al(sizeof(float) * w.rowlen);
-    w.rows_off = al(w.norm_off + sizeof(double) * w.norm_parts);
-    w.bytes = w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas;
+    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, w);
     return WL_OK;
 }
 
@@ -2385,6 +2403,128 @@ int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, 
             wl_ppo_step_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
                                                                  w.blob_floats, po, p->obs_dim, sa);
             if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel")) return rc;
+        }
+    }
+    return WL_OK;
+}
+
+// ---- the wide (ReLU) actor-critic: wl_policy_act and wl_ppo_update_wide (DESIGN 6g) ----------------------------------
+// offsets inside the copy of the blob without its W1t blocks ([o1, o6) | [o7, end)) the wide kernels keep in shared
+// memory; returns its float count (the same for every obs_dim)
+static int wide_compact_offsets(const PolicyOffsets& po, int blob_floats, PolicyOffsets& pc) {
+    const int na = po.o[6] - po.o[1];
+    for (int k = 0; k < 13; ++k) pc.o[k] = (k == 0 || k == 6) ? -1 : (k < 6 ? po.o[k] - po.o[1] : na + po.o[k] - po.o[7]);
+    return na + blob_floats - po.o[7];
+}
+static size_t wide_compact_bytes() {
+    PolicyOffsets po, pc;
+    return sizeof(float) * (size_t)wide_compact_offsets(po, policy_offsets(1, po.o), pc);
+}
+static size_t policy_act_smem() { return sizeof(float) * (2 * WL_WIDE_STAGE + WL_WIDE_ROWS * WL_PPO_HS) + wide_compact_bytes(); }
+static size_t ppo_wide_grad_smem() {
+    return wide_compact_bytes() + sizeof(float) * (2 * WL_HID * WL_HID + WL_HID + 4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
+}
+static size_t ppo_wide_dw1_smem() { return sizeof(float) * 2 * WL_PPO_TILE * (WL_DW1_K + 2 * WL_HID); }
+
+// the dynamic shared-memory limits of the wide kernels, raised once per device (the sizes do not depend on obs_dim)
+static int wide_attributes(int dev, const char* fn) {
+    static bool attr_set[64] = {false};
+    if (dev < 0 || dev >= 64 || attr_set[dev]) return WL_OK;
+    if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)policy_act_smem()), fn)) return rc;
+    if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_wide_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_wide_grad_smem()), fn)) return rc;
+    if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_wide_dw1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_wide_dw1_smem()), fn)) return rc;
+    attr_set[dev] = true;
+    return WL_OK;
+}
+
+int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
+        return fail(WL_EINVAL, "wl_policy_act: null argument");
+    const int D = sim->obs_dim, n = sim->cfg.num_envs;
+    if (D < 1 || D > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, "wl_policy_act: obs_dim must be in 1..4096");
+    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))
+        return fail(WL_EINVAL, "wl_policy_act: policy blob must be 16-byte aligned, actions/mean 8-byte aligned");
+    ensure_device(sim);
+    if (int rc = wide_attributes(sim->device, "wl_policy_act")) return rc;
+    PolicyOffsets po, pc;
+    const int blob_floats = policy_offsets(D, po.o);
+    wide_compact_offsets(po, blob_floats, pc);
+    wl_policy_act_kernel<<<(n + WL_WIDE_ROWS - 1) / WL_WIDE_ROWS, WL_WIDE_THREADS, policy_act_smem(), (cudaStream_t)stream>>>(
+        d_obs_in, n, D, d_policy_blob, blob_floats, po, pc, out, sim->globals, sim->cfg.seed, sim->cfg.env_id_offset, (uint32_t)step_counter);
+    return launched(sim, "wl_policy_act_kernel");
+}
+
+// workspace of wl_ppo_update_wide: wl_ppo_update's, then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
+struct PpoWideWorkspace { PpoWorkspace w; size_t h1_off, dz_off, bytes; };
+static int ppo_wide_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWideWorkspace& x) {
+    if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
+    if (obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
+    if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
+    int dev = 0, sms = 0;
+    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
+    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
+    if (int rc = wide_attributes(dev, fn)) return rc;       // (the workspace query comes first, outside any graph capture)
+    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, x.w);
+    const size_t hb = sizeof(float) * 2 * WL_HID * (size_t)WL_PPO_TILE * ((batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE);
+    x.h1_off = align256(x.w.bytes);
+    x.dz_off = align256(x.h1_off + hb);
+    x.bytes = x.dz_off + hb;
+    return WL_OK;
+}
+
+size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches) {
+    PpoWideWorkspace x;
+    return ppo_wide_workspace("wl_ppo_wide_workspace_bytes", obs_dim, batch, num_mini_batches, x) ? 0 : x.bytes;
+}
+
+int wl_ppo_update_wide(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
+                       void* d_workspace, size_t workspace_bytes, void* stream) {
+    if (!p || !b) return fail(WL_EINVAL, "wl_ppo_update_wide: null params / batch");
+    if (!b->obs || !b->actions || !b->values || !b->log_prob || !b->mean || !b->returns || !b->advantages || !b->perm)
+        return fail(WL_EINVAL, "wl_ppo_update_wide: null array in batch");
+    if (!d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
+        return fail(WL_EINVAL, "wl_ppo_update_wide: null d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
+    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, "wl_ppo_update_wide: num_learning_epochs must be >= 1");
+    PpoWideWorkspace x;
+    if (int rc = ppo_wide_workspace("wl_ppo_update_wide", p->obs_dim, p->batch, p->num_mini_batches, x)) return rc;
+    const PpoWorkspace& w = x.w;
+    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
+        return fail(WL_EINVAL, "wl_ppo_update_wide: d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
+    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
+        return fail(WL_EINVAL, "wl_ppo_update_wide: d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
+    if (workspace_bytes < x.bytes)
+        return fail(WL_EINVAL, "wl_ppo_update_wide: workspace_bytes too small (wl_ppo_wide_workspace_bytes gives " + std::to_string(x.bytes) + ")");
+    PolicyOffsets po, pc;
+    policy_offsets(p->obs_dim, po.o);
+    wide_compact_offsets(po, w.blob_floats, pc);
+    const int B = p->batch / p->num_mini_batches;
+    cudaStream_t cs = (cudaStream_t)stream;
+    char* ws = (char*)d_workspace;
+    float* red = (float*)ws;
+    double* norm_part = (double*)(ws + w.norm_off);
+    float* rows = (float*)(ws + w.rows_off);
+    float* H1 = (float*)(ws + x.h1_off);
+    float* dZ1 = (float*)(ws + x.dz_off);
+    wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
+    if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
+    PpoArgs a;
+    a.b = *b; a.obs_dim = p->obs_dim; a.B = B; a.tiles = (B + WL_PPO_TILE - 1) / WL_PPO_TILE;
+    a.clip = p->clip_param; a.vcoef = p->value_loss_coef; a.inv_B = 1.0f / (float)B; a.clipped_value = p->use_clipped_value_loss != 0;
+    PpoStepArgs sa{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
+    const dim3 dw1_grid((unsigned)((p->obs_dim + WL_DW1_K - 1) / WL_DW1_K), (unsigned)w.ctas);
+    for (int e = 0; e < p->num_learning_epochs; ++e) {
+        for (int i = 0; i < p->num_mini_batches; ++i) {
+            a.row0 = (int64_t)i * B;
+            sa.update_index = e * p->num_mini_batches + i;
+            wl_ppo_wide_fwd_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE, cs>>>(d_blob, po, a, H1);
+            wl_ppo_wide_grad_kernel<<<w.ctas, WL_PPO_THREADS, ppo_wide_grad_smem(), cs>>>(d_blob, w.blob_floats, po, pc, a, d_state, H1, dZ1,
+                                                                                         rows, w.rowlen);
+            wl_ppo_wide_dw1_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
+            wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
+                                                               p->entropy_coef, red, norm_part);
+            wl_ppo_step_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                 w.blob_floats, po, p->obs_dim, sa);
+            if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_update_wide kernels")) return rc;
         }
     }
     return WL_OK;

@@ -39,6 +39,49 @@ __device__ __forceinline__ bool ppo_is_param(int c, const PolicyOffsets& po, int
     return p;
 }
 
+// the loss terms of mini-batch row `row` (< B) with the network outputs (mu0, mu1, V) = (m0, m1, vv): d[0..4] = dL/dmu0,
+// dL/dmu1, dL/dV, dL/dsigma0, dL/dsigma1 (the log-prob part), d[5..7] = surrogate, value loss, KL
+__device__ __forceinline__ void ppo_sample_derivs(const PpoArgs& a, int row, float m0, float m1, float vv, float sg_0, float sg_1,
+                                                  float so0, float so1, float adv_mean, float adv_den, float* d) {
+    const int64_t g = a.b.perm[a.row0 + row];
+    const float2 act = reinterpret_cast<const float2*>(a.b.actions)[g];
+    const float2 mo = reinterpret_cast<const float2*>(a.b.mean)[g];
+    const float A = (a.b.advantages[g] - adv_mean) / adv_den;
+    const float R = a.b.returns[g], vo = a.b.values[g];
+    // log-prob of the stored action under N(mu, sigma), summed over the two dims (torch Normal.log_prob)
+    const float d0 = act.x - m0, d1 = act.y - m1, var0 = sg_0 * sg_0, var1 = sg_1 * sg_1;
+    const float lp = (-(d0 * d0) / (2.0f * var0) - logf(sg_0) - WL_PPO_LOG_SQRT_2PI)
+                   + (-(d1 * d1) / (2.0f * var1) - logf(sg_1) - WL_PPO_LOG_SQRT_2PI);
+    const float ratio = expf(lp - a.b.log_prob[g]);
+    const float lo = 1.0f - a.clip, hi = 1.0f + a.clip;
+    const float su1 = -A * ratio, su2 = -A * fminf(fmaxf(ratio, lo), hi);
+    const float w = ppo_max_share(su1, su2);
+    const float in_r = (ratio >= lo && ratio <= hi) ? 1.0f : 0.0f;      // clamp passes the gradient at its bounds
+    const float dratio = (w * a.inv_B) * -A + ((1.0f - w) * a.inv_B) * -A * in_r;
+    const float dlp = dratio * ratio;
+    d[0] = dlp * (d0 / var0);
+    d[1] = dlp * (d1 / var1);
+    d[3] = dlp * ((d0 * d0) * sg_0 / (var0 * var0) - 1.0f / sg_0);
+    d[4] = dlp * ((d1 * d1) * sg_1 / (var1 * var1) - 1.0f / sg_1);
+    float vl, dv;
+    if (a.clipped_value) {
+        const float dvo = vv - vo, vc = vo + fminf(fmaxf(dvo, -a.clip), a.clip);
+        const float l1 = (vv - R) * (vv - R), l2 = (vc - R) * (vc - R), wv = ppo_max_share(l1, l2);
+        const float in_v = (dvo >= -a.clip && dvo <= a.clip) ? 1.0f : 0.0f;
+        dv = (wv * a.inv_B) * (2.0f * (vv - R)) + ((1.0f - wv) * a.inv_B) * (2.0f * (vc - R)) * in_v;
+        vl = fmaxf(l1, l2);
+    } else {
+        dv = a.inv_B * (2.0f * (vv - R));
+        vl = (R - vv) * (R - vv);
+    }
+    d[2] = a.vcoef * dv;
+    d[5] = fmaxf(su1, su2);
+    d[6] = vl;
+    const float e0 = mo.x - m0, e1 = mo.y - m1;
+    d[7] = (logf(sg_0 / so0 + 1e-5f) + (so0 * so0 + e0 * e0) / (2.0f * var0) - 0.5f)
+         + (logf(sg_1 / so1 + 1e-5f) + (so1 * so1 + e1 * e1) / (2.0f * var1) - 0.5f);
+}
+
 __device__ __forceinline__ void ppo_store_elu(float* h0, const float acc[4][4]) {
 #pragma unroll
     for (int e = 0; e < 4; ++e)
@@ -137,44 +180,7 @@ wl_ppo_grad_kernel(const float* __restrict__ blob, int blob_floats, PolicyOffset
             if (p == 0) {
                 float* d = sd + s * WL_PPO_SD;
                 if (row < a.B) {
-                    const int64_t g = a.b.perm[a.row0 + row];
-                    m0 += b3a0; m1 += b3a1; vv += b3c;
-                    const float2 act = reinterpret_cast<const float2*>(a.b.actions)[g];
-                    const float2 mo = reinterpret_cast<const float2*>(a.b.mean)[g];
-                    const float A = (a.b.advantages[g] - adv_mean) / adv_den;
-                    const float R = a.b.returns[g], vo = a.b.values[g];
-                    // log-prob of the stored action under N(mu, sigma), summed over the two dims (torch Normal.log_prob)
-                    const float d0 = act.x - m0, d1 = act.y - m1, var0 = sg_0 * sg_0, var1 = sg_1 * sg_1;
-                    const float lp = (-(d0 * d0) / (2.0f * var0) - logf(sg_0) - WL_PPO_LOG_SQRT_2PI)
-                                   + (-(d1 * d1) / (2.0f * var1) - logf(sg_1) - WL_PPO_LOG_SQRT_2PI);
-                    const float ratio = expf(lp - a.b.log_prob[g]);
-                    const float lo = 1.0f - a.clip, hi = 1.0f + a.clip;
-                    const float su1 = -A * ratio, su2 = -A * fminf(fmaxf(ratio, lo), hi);
-                    const float w = ppo_max_share(su1, su2);
-                    const float in_r = (ratio >= lo && ratio <= hi) ? 1.0f : 0.0f;      // clamp passes the gradient at its bounds
-                    const float dratio = (w * a.inv_B) * -A + ((1.0f - w) * a.inv_B) * -A * in_r;
-                    const float dlp = dratio * ratio;
-                    d[0] = dlp * (d0 / var0);
-                    d[1] = dlp * (d1 / var1);
-                    d[3] = dlp * ((d0 * d0) * sg_0 / (var0 * var0) - 1.0f / sg_0);
-                    d[4] = dlp * ((d1 * d1) * sg_1 / (var1 * var1) - 1.0f / sg_1);
-                    float vl, dv;
-                    if (a.clipped_value) {
-                        const float dvo = vv - vo, vc = vo + fminf(fmaxf(dvo, -a.clip), a.clip);
-                        const float l1 = (vv - R) * (vv - R), l2 = (vc - R) * (vc - R), wv = ppo_max_share(l1, l2);
-                        const float in_v = (dvo >= -a.clip && dvo <= a.clip) ? 1.0f : 0.0f;
-                        dv = (wv * a.inv_B) * (2.0f * (vv - R)) + ((1.0f - wv) * a.inv_B) * (2.0f * (vc - R)) * in_v;
-                        vl = fmaxf(l1, l2);
-                    } else {
-                        dv = a.inv_B * (2.0f * (vv - R));
-                        vl = (R - vv) * (R - vv);
-                    }
-                    d[2] = a.vcoef * dv;
-                    d[5] = fmaxf(su1, su2);
-                    d[6] = vl;
-                    const float e0 = mo.x - m0, e1 = mo.y - m1;
-                    d[7] = (logf(sg_0 / so0 + 1e-5f) + (so0 * so0 + e0 * e0) / (2.0f * var0) - 0.5f)
-                         + (logf(sg_1 / so1 + 1e-5f) + (so1 * so1 + e1 * e1) / (2.0f * var1) - 0.5f);
+                    ppo_sample_derivs(a, row, m0 + b3a0, m1 + b3a1, vv + b3c, sg_0, sg_1, so0, so1, adv_mean, adv_den, d);
                 } else {
 #pragma unroll
                     for (int k = 0; k < WL_PPO_SD; ++k) d[k] = 0.0f;     // tail of a partial tile: no gradient

@@ -111,20 +111,37 @@ class PPOConfig:
         return cls(**{f.name: getattr(alg_cfg, f.name) for f in fields(cls) if hasattr(alg_cfg, f.name)})
 
 
+def activation_from_rsl_rl(policy_cfg) -> str:
+    """The hidden activation of an rsl_rl ``RslRlPpoActorCriticCfg``-like object (the reference's ``policy`` of an agent cfg:
+    "elu" for the Drift family, "relu" for Elevation and Visual), checked against the network the fused kernels run:
+    ``actor_hidden_dims == critic_hidden_dims == [64, 64]`` and ELU or ReLU."""
+    from .policy import check_activation
+    dims = [list(getattr(policy_cfg, k)) for k in ("actor_hidden_dims", "critic_hidden_dims")]
+    if dims != [[64, 64], [64, 64]]:
+        raise NotImplementedError(f"the fused actor-critic is [64, 64] for actor and critic, not {dims[0]} / {dims[1]}")
+    return check_activation(policy_cfg.activation)
+
+
 class FusedPPO:
     """rsl_rl ``PPO.update()`` (modified_rsl_rl_runner.py:118) [UPSTREAM-RECALL] on the device, training the blob that
     ``FusedPolicyRollout`` reads in place (``wl_ppo_update``: one gradient kernel + two finisher launches per mini-batch).
 
     Owns the Adam moments, the device state (learning rate, Adam step, statistics) and the workspace.  Nothing syncs the
     host, so with an explicit ``perm`` tensor refilled in place the update can be captured into the same CUDA graph as the
-    rollout.  Covers the Drift-family network only (obs_dim <= 16, [64, 64] ELU actor and critic, learned std)."""
+    rollout.  The network is [64, 64] actor and critic with a learned std: activation "elu" is the Drift family's
+    (obs_dim <= 16, ``wl_ppo_update``), "relu" the Elevation / Visual one (obs_dim <= 4096, ``wl_ppo_update_wide``)."""
 
-    def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None):
+    def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None, activation: str = "elu"):
+        from .policy import check_activation
         if cfg is None:
             cfg = PPOConfig()
         if cfg.schedule not in ("adaptive", "fixed"):
             raise ValueError(f"schedule must be 'adaptive' or 'fixed', not {cfg.schedule!r}")
         self.blob, self.obs_dim, self.cfg, self.device = blob, obs_dim, cfg, blob.device
+        self.activation = check_activation(activation)
+        wide = self.activation == "relu"
+        self._ws_query = lib.wl_ppo_wide_workspace_bytes if wide else lib.wl_ppo_workspace_bytes
+        self._update = lib.wl_ppo_update_wide if wide else lib.wl_ppo_update
         self.m = torch.zeros_like(blob)
         self.v = torch.zeros_like(blob)
         self.state = torch.zeros(lib.wl_ppo_state_floats(), dtype=torch.float32, device=blob.device)
@@ -134,9 +151,9 @@ class FusedPPO:
 
     def _workspace(self, batch: int) -> torch.Tensor:
         with torch.cuda.device(self.device):
-            need = lib.wl_ppo_workspace_bytes(self.obs_dim, batch, self.cfg.num_mini_batches)
+            need = self._ws_query(self.obs_dim, batch, self.cfg.num_mini_batches)
         if need == 0:
-            raise WlError(f"wl_ppo_workspace_bytes failed: {lib.wl_last_error().decode()}")
+            raise WlError(f"{self._ws_query.__name__} failed: {lib.wl_last_error().decode()}")
         if self.workspace.numel() < need:
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
         return self.workspace
@@ -162,9 +179,9 @@ class FusedPPO:
                         cfg.entropy_coef, cfg.max_grad_norm, cfg.desired_kl, int(cfg.schedule == "adaptive"),
                         int(cfg.use_clipped_value_loss), 0)
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        check(lib.wl_ppo_update(C.byref(p), C.byref(self._batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
-                                C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
-                                ws.numel(), stream), "wl_ppo_update")
+        check(self._update(C.byref(p), C.byref(self._batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
+                           C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
+                           ws.numel(), stream), self._update.__name__)
         k = cfg.num_learning_epochs * cfg.num_mini_batches
         return {"value_function": self.state[7] / k, "surrogate": self.state[6] / k, "entropy": self.state[8] / k,
                 "learning_rate": self.state[0], "kl": self.state[9]}
@@ -184,20 +201,20 @@ class PPOIteration:
     """One whole rsl_rl iteration on one GPU (modified_rsl_rl_runner.py:70-118): the fused rollout, the bootstrap value
     V(obs_T) from the blob, ``compute_returns`` (time_outs = truncated, as process_env_step), then ``FusedPPO.update``.
     ``capture=True`` records all of it as ONE CUDA graph; the mini-batch permutation is refilled in place before each
-    replay (``torch.randperm`` on the device unless the caller passes one)."""
+    replay (``torch.randperm`` on the device unless the caller passes one).  ``activation``: as ``FusedPPO``."""
 
-    def __init__(self, sim, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128):
+    def __init__(self, sim, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu"):
         from .policy import FusedPolicyRollout
         self.sim, self.blob, self.T = sim, blob, T
-        self.roll = FusedPolicyRollout(sim, blob, T)
-        self.ppo = FusedPPO(blob, sim.obs_dim, cfg)
+        self.roll = FusedPolicyRollout(sim, blob, T, activation=activation)
+        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation)
         self.perm = torch.empty(T * sim.num_envs, dtype=torch.int64, device=sim.device)
         self.graph = None
         self.stats = None
 
     def _bootstrap(self) -> torch.Tensor:
         from .policy import critic_value
-        return critic_value(self.blob, self.sim.obs_dim, self.roll.obs0)
+        return critic_value(self.blob, self.sim.obs_dim, self.roll.obs0, self.ppo.activation)
 
     def _learn(self):
         slab, cfg = self.roll.slab, self.ppo.cfg

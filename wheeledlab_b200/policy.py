@@ -95,15 +95,25 @@ def load_actor_critic_state_dict(sd: dict, obs_dim: int, out: torch.Tensor | Non
     return out
 
 
-def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor) -> torch.Tensor:
+ACTIVATIONS = {"elu": torch.nn.functional.elu, "relu": torch.nn.functional.relu}
+
+
+def check_activation(activation: str) -> str:
+    if activation not in ACTIVATIONS:
+        raise ValueError(f"activation must be 'elu' (the Drift family's network) or 'relu' (Elevation / Visual), not {activation!r}")
+    return activation
+
+
+def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu") -> torch.Tensor:
     """V(obs) [N] in torch from zero-copy views of the blob (the bootstrap value of compute_returns): a CUDA graph that
     captures it reads the weights the last update left in the blob."""
+    act = ACTIVATIONS[check_activation(activation)]
     _, critic, _ = _blob_layers(blob, obs_dim)
     x = obs
     for k, (w, b) in enumerate(critic):
         x = torch.addmm(b, x, w)
         if k < 2:
-            x = torch.nn.functional.elu(x)
+            x = act(x)
     return x.squeeze(-1)
 
 
@@ -127,13 +137,25 @@ def act_step(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions:
           "wl_act_step")
 
 
-class FusedPolicyRollout:
-    """T x wl_act_step captured as ONE CUDA graph: the reference's whole collection loop (modified_rsl_rl_runner.py:70-109)
-    with nothing but T kernel launches inside.  The blob is read at replay time, so refilling it in place
-    (pack_actor_critic(..., out=blob)) after each PPO update needs no re-capture."""
+def policy_act(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor, mean: torch.Tensor,
+               log_prob: torch.Tensor, value: torch.Tensor, step_counter: int):
+    """One launch (wl_policy_act): value / mean / sample / log-prob of `obs_in` [N, obs_dim] under the ReLU network in `blob`,
+    for any obs_dim up to 4096.  The env is not stepped: follow with sim.step(actions, step_counter)."""
+    po = WlPolicyOut(actions.data_ptr(), mean.data_ptr(), log_prob.data_ptr(), value.data_ptr())
+    check(lib.wl_policy_act(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(blob.data_ptr()), po, step_counter,
+                            _stream_ptr(sim.device)), "wl_policy_act")
 
-    def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None):
-        self.sim, self.blob, self.T = sim, blob, T
+
+class FusedPolicyRollout:
+    """T policy-and-step launches captured as ONE CUDA graph: the reference's whole collection loop
+    (modified_rsl_rl_runner.py:70-109).  activation "elu" (the Drift family): T x wl_act_step, the policy fused into the
+    step; "relu" (Elevation, Visual): T x (wl_policy_act, then wl_step).  The blob is read at replay time, so refilling it
+    in place (pack_actor_critic(..., out=blob)) after each PPO update needs no re-capture."""
+
+    def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu"):
+        self.sim, self.blob, self.T, self.activation = sim, blob, T, check_activation(activation)
+        if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
+            raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
         self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=True)
         # values / log-prob / mean go straight into the slab (= the all-gather send buffer) when it has those fields
         self.pol = (SimpleNamespace(values=self.slab.values, log_prob=self.slab.log_prob, mean=self.slab.mean)
@@ -149,8 +171,14 @@ class FusedPolicyRollout:
     def _body(self):
         self.slab.obs_in[0].copy_(self.obs0)
         for k in range(self.T):
-            act_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
-                     self.pol.values[k], self.slab.step_outputs(k), self.logs[k], WheeledSim.device_counter_plus(k))
+            t = WheeledSim.device_counter_plus(k)
+            if self.activation == "relu":
+                policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
+                           self.pol.values[k], t)
+                self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
+            else:
+                act_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
+                         self.pol.values[k], self.slab.step_outputs(k), self.logs[k], t)
         self.sim.advance_counter(self.T)
         self.obs0.copy_(self.slab.obs[self.T - 1])
 
