@@ -358,7 +358,8 @@ size_t wl_config_sizeof(void);
 int wl_set_step_counter(wl_sim* sim, int64_t value, void* stream);
 int wl_advance_counter(wl_sim* sim, int32_t K, void* stream);
 int wl_note_device_counter(wl_sim* sim, int64_t value);
-/* publish the extras["log"] row of the most recent step now (otherwise the next step's launch does it) */
+/* publish the extras["log"] row of the most recent step now (otherwise the next step's launch does it); once the flush
+ * has run on the stream, the library writes that step's log buffer no more, so it may be freed or reused */
 int wl_log_flush(wl_sim* sim, void* stream);
 /* live reward weights (what the next step will use): device pointer to WL_MAX_REW_TERMS floats inside the state buffer */
 float* wl_reward_weights(wl_sim* sim);

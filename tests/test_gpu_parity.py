@@ -314,7 +314,7 @@ def _elev_pair(n, seed=42):
 
 
 def test_scan_pipeline_walks_several_envs_per_cta():
-    """The pipelined ray-caster runs 888 persistent CTAs: with more envs than that every CTA re-uses its two stages
+    """The pipelined ray-caster runs min(N, 132 x 6 = 792) persistent CTAs on the H100: with more envs than that CTAs re-use their two stages
     (mbarrier phases flip), and the rows must still equal the oracle's and the plain-load kernel's bit for bit."""
     _need_gpu()
     n = 4000

@@ -1360,9 +1360,15 @@ __global__ void wl_curriculum_kernel(wl_globals* __restrict__ gl, CurrArgs a) {
     for (int t = 0; t < a.n; ++t)
         if ((a.fire_mask >> t) & 1u) gl->rew_weight[a.wslot][a.slots[t]] += a.inc[t];
 }
-// publish the log row of step t_next - 1 without stepping (idempotent; the next step's janitor would do the same)
+// publish the log row of step t_next - 1 without stepping, then drop its pointer: the caller may free or reuse the row's
+// buffer once this has run, so the next step's janitor must not write the row through it again (it still re-publishes
+// last_log, with the same values)
 __global__ void wl_flush_kernel(const __grid_constant__ wl_config c, wl_globals* __restrict__ gl, uint32_t t_next) {
-    if (t_next != 0u) publish_log_row(c, gl, (t_next + 2u) % 3u, threadIdx.x & 31);
+    if (t_next == 0u) return;
+    const uint32_t row = (t_next + 2u) % 3u;
+    publish_log_row(c, gl, row, threadIdx.x & 31);
+    __syncwarp();                                                      // every lane has read log_ptr[row]
+    if (threadIdx.x == 0) gl->log_ptr[row] = nullptr;
 }
 // counter jump: carry the weights over to the slot the next step reads, clear the accumulators and the pending log
 __global__ void wl_rearm_kernel(wl_globals* __restrict__ gl, uint32_t from_slot, uint32_t to_slot) {
@@ -1875,6 +1881,19 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
         if (cfg->hf_nx < 2 || cfg->hf_ny < 2 || cfg->hf_pitch < cfg->hf_nx || (cfg->hf_pitch & 3) || !(cfg->hf_cell > 0.0f))
             return fail(WL_EINVAL, "wl_create: bad height-field geometry (hf_pitch must be >= hf_nx and a multiple of 4)");
         if (((uintptr_t)d_heightfield & 15u) != 0) return fail(WL_EINVAL, "wl_create: height-field must be 16-byte aligned");
+        // The height scan reads every ray's 2x2 cell out of a WL_TILE_W x WL_TILE_H window staged in shared memory, and clamps
+        // the cell into the window, so a cell outside it is a wrong height, not a fault.  scan_pose starts the window
+        // reach = scan_half*sqrt2 + hf_cell below the base (rounded down to a sample; in x down again to a multiple of 4).  The
+        // 26 x 26 rays within +-scan_half span up to D = 2*scan_half*sqrt2 / hf_cell cells along an axis (yaw 45 deg), so they
+        // touch floor(D) + 2 cells: with the reach's cell and the +1 bilinear neighbour, floor(D) + 4 rows and floor(D) + 7
+        // columns.  The 1/64-cell margin absorbs the float32 rounding of the kernel's index arithmetic.  0.1 m at the
+        // task's 1.25 m half-width needs 39 of the 40 rows; the smallest cell accepted there is about 0.0956 m.
+        if ((WL_SCAN_SIDE - 1) * (double)cfg->scan_res > 2.0 * (double)cfg->scan_half * (1.0 + 1e-6))
+            return fail(WL_EINVAL, "wl_create: the height-scan grid must lie within +-scan_half (25 * scan_res <= 2 * scan_half)");
+        const int span = (int)floor(2.0 * (double)cfg->scan_half * 1.41421356237 / (double)cfg->hf_cell + 1.0 / 64.0);
+        if (span + 4 > WL_TILE_H || span + 7 > WL_TILE_W)
+            return fail(WL_EINVAL, "wl_create: hf_cell too small for scan_half: the height scan needs floor(2*scan_half*sqrt2/hf_cell) + 4 <= " +
+                                   std::to_string(WL_TILE_H) + " window rows (hf_cell > about scan_half / 13.08: 0.0956 m at scan_half 1.25 m)");
     }
     if (cfg->bounding != WL_BOUND_CLIP && cfg->bounding != WL_BOUND_NONE && cfg->bounding != WL_BOUND_TANH)
         return fail(WL_EUNSUPPORTED, "wl_create: unknown bounding strategy");

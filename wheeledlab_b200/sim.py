@@ -137,7 +137,8 @@ class WheeledSim:
         check(lib.wl_note_device_counter(self._h, value), "wl_note_device_counter")
 
     def flush_log(self):
-        """Publish the extras["log"] row of the most recent step now (otherwise the next step's launch does it)."""
+        """Publish the extras["log"] row of the most recent step now (otherwise the next step's launch does it).  Once this
+        has run on the stream, that step's `log` tensor is no longer written and may be freed."""
         check(lib.wl_log_flush(self._h, _stream_ptr(self.device)), "wl_log_flush")
 
     @property
