@@ -523,6 +523,32 @@ int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_va
            const uint8_t* d_time_outs, float gamma, float lam, float* d_returns, float* d_advantages, int32_t T,
            int32_t N, void* stream);
 
+/* ---- the runner's episode statistics over the [T, N] slab ------------------------------------------------------------
+ * rsl_rl's runner bookkeeping (modified_rsl_rl_runner.py:55-63, :99-109): per env, for t = 0..T-1,
+ *   cur_return += rewards[t] (fp32, in t order); cur_length += 1;
+ *   if terminated[t] | truncated[t]: append (cur_return, cur_length) to a deque(maxlen=100), envs in ascending id order
+ *   (the nonzero() order); then cur_return = cur_length = 0.
+ * d_cur_return / d_cur_length [N] f32 carry the running episodes between calls; *d_stats carries the deque (zero-fill it
+ * for an empty one) and receives the outputs.  The means are fp64 sums over the ring, oldest episode first, divided by
+ * `fill` (statistics.mean of the deque; 0 while it is empty).  Two launches, no float atomics, no host sync, graph-
+ * capturable; results are bit-identical run to run.  T in 1..4096. */
+#define WL_EPISODE_RING 100
+typedef struct wl_episode_stats_state {
+    float ring_return[WL_EPISODE_RING];  /* finished episodes: slot (head - fill + k) mod 100 holds the k-th oldest */
+    float ring_length[WL_EPISODE_RING];
+    int32_t fill;                        /* episodes in the ring (<= 100) */
+    int32_t head;                        /* slot the next finished episode goes to */
+    int32_t finished;                    /* output: episodes that finished during the last call */
+    int32_t _pad;
+    double mean_return;                  /* output: mean of ring_return over the ring (Train/mean_reward) */
+    double mean_length;                  /* output: mean of ring_length (Train/mean_episode_length) */
+} wl_episode_stats_state;
+/* workspace for wl_episode_stats (a (return, length) cell per (t, env) and a done word per (t, 32 envs)); 0 on bad T / N */
+size_t wl_episode_stats_workspace_bytes(int32_t T, int32_t N);
+int wl_episode_stats(const float* d_rewards, const uint8_t* d_terminated, const uint8_t* d_truncated, int32_t T, int32_t N,
+                     float* d_cur_return, float* d_cur_length, wl_episode_stats_state* d_stats, void* d_workspace,
+                     size_t workspace_bytes, void* stream);
+
 /* ---- the learner's data-parallel step for the small policy networks (SURVEY 8f-2) --------------------------------------
  * Gradient all-reduce fused with the Adam update, one kernel over peer memory: d_grads[r] = rank r's flat fp32 gradient
  * (this rank's own buffer and the P2P-mapped buffers of its peers, e.g. slices of one torch symmetric-memory allocation; the

@@ -128,6 +128,16 @@ lib.wl_camera.argtypes = [_vp, _vp, _i64, _vp, _vp]
 lib.wl_step_stage_a.argtypes = [_vp, _vp, _vp, _vp, _i64, _vp]
 lib.wl_step_stage_b.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]
 lib.wl_gae.argtypes = [_vp, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _vp, _vp, _i32, _i32, _vp]
+
+
+class WlEpisodeStatsState(C.Structure):
+    _fields_ = [("ring_return", C.c_float * 100), ("ring_length", C.c_float * 100), ("fill", _i32), ("head", _i32),
+                ("finished", _i32), ("_pad", _i32), ("mean_return", C.c_double), ("mean_length", C.c_double)]
+
+
+lib.wl_episode_stats_workspace_bytes.restype = _sz
+lib.wl_episode_stats_workspace_bytes.argtypes = [_i32, _i32]
+lib.wl_episode_stats.argtypes = [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]
 lib.wl_dp_adam_step.argtypes = [_vp, _vp, _vp, _i32, C.POINTER(_vp), C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _i32, _i32, _vp]
 
 
@@ -160,7 +170,7 @@ lib.wl_graph_upload.argtypes = [_vp, _vp]
 EXPORTED_SYMBOLS = [
     "wl_config_describe", "wl_config_sizeof", "wl_config_finalize", "wl_set_step_counter", "wl_advance_counter", "wl_note_device_counter", "wl_log_flush", "wl_reward_weights", "wl_set_seed", "wl_set_term_bits", "wl_set_peer_fanout", "wl_set_multicast_fanout", "wl_state_bytes", "wl_globals_offset", "wl_create", "wl_destroy",
     "wl_last_error", "wl_build_info", "wl_startup", "wl_reset", "wl_step", "wl_step_host", "wl_step_host_zero_copy", "wl_rollout", "wl_result_bytes", "wl_observe", "wl_curriculum",
-    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_policy_act", "wl_ppo_wide_workspace_bytes", "wl_ppo_update_wide", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_null", "wl_test_null_cfg",
+    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_policy_act", "wl_ppo_wide_workspace_bytes", "wl_ppo_update_wide", "wl_episode_stats_workspace_bytes", "wl_episode_stats", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_null", "wl_test_null_cfg",
 ]
 
 

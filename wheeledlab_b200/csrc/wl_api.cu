@@ -1530,6 +1530,7 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 
 #include "wl_ppo.cuh"
 #include "wl_wide.cuh"
+#include "wl_episode.cuh"
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2320,6 +2321,33 @@ int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_va
         wl_gae_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_rewards, d_values, d_last_values, d_dones, d_time_outs, gamma,
                                                                          lam, d_returns, d_advantages, T, N);
     return cuda_check(cudaGetLastError(), "wl_gae_kernel");
+}
+
+// workspace of wl_episode_stats: [(return, length) per (t, env)][done word per (t, 32 envs)], 256-byte aligned
+static size_t episode_words_off(int32_t T, int32_t N) { return align256(sizeof(float2) * (size_t)T * N); }
+size_t wl_episode_stats_workspace_bytes(int32_t T, int32_t N) {
+    if (T < 1 || T > WL_EP_MAX_T || N < 1) { fail(WL_EINVAL, "wl_episode_stats_workspace_bytes: T must be in 1..4096 and N >= 1"); return 0; }
+    return episode_words_off(T, N) + sizeof(uint32_t) * (size_t)T * ((N + 31) / 32);
+}
+
+int wl_episode_stats(const float* d_rewards, const uint8_t* d_terminated, const uint8_t* d_truncated, int32_t T, int32_t N,
+                     float* d_cur_return, float* d_cur_length, wl_episode_stats_state* d_stats, void* d_workspace,
+                     size_t workspace_bytes, void* stream) {
+    if (!d_rewards || !d_terminated || !d_truncated || !d_cur_return || !d_cur_length || !d_stats || !d_workspace)
+        return fail(WL_EINVAL, "wl_episode_stats: null argument");
+    const size_t need = wl_episode_stats_workspace_bytes(T, N);
+    if (need == 0) return fail(WL_EINVAL, "wl_episode_stats: T must be in 1..4096 and N >= 1");
+    if (workspace_bytes < need) return fail(WL_EINVAL, "wl_episode_stats: workspace smaller than wl_episode_stats_workspace_bytes(T, N)");
+    if (((uintptr_t)d_stats & 7u) != 0 || ((uintptr_t)d_workspace & 255u) != 0)
+        return fail(WL_EINVAL, "wl_episode_stats: d_stats must be 8-byte and d_workspace 256-byte aligned");
+    cudaStream_t cs = (cudaStream_t)stream;
+    float2* ep = reinterpret_cast<float2*>(d_workspace);
+    uint32_t* words = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(d_workspace) + episode_words_off(T, N));
+    wl_episode_walk_kernel<<<(N + WL_EP_WALK_THREADS - 1) / WL_EP_WALK_THREADS, WL_EP_WALK_THREADS, 0, cs>>>(
+        d_rewards, d_terminated, d_truncated, T, N, d_cur_return, d_cur_length, ep, words);
+    if (int rc = cuda_check(cudaGetLastError(), "wl_episode_walk_kernel")) return rc;
+    wl_episode_ring_kernel<<<1, WL_EP_RING_THREADS, 0, cs>>>(ep, words, T, N, d_stats);
+    return cuda_check(cudaGetLastError(), "wl_episode_ring_kernel");
 }
 
 int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, float beta1,
