@@ -512,6 +512,13 @@ typedef struct wl_policy_out {
 int32_t wl_policy_blob_floats(int32_t obs_dim, int32_t offsets[13]);
 int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, float* d_obs,
                 float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
+/* wl_act_step for playback (rsl_rl ActorCritic.act_inference, the runner's get_inference_policy()): the action is the
+ * actor mean -- no critic, no policy noise, no log-prob -- then the same env step, PDL trigger / wait, janitor and episode
+ * log as wl_act_step.  Writes d_actions [N,2] (8-byte aligned) and nothing else of a wl_policy_out; equals
+ * wl_actor_mean(d_obs_in, ..., WL_ACTIVATION_ELU) bit for bit, which equals the mean wl_act_step stores.  The tasks of
+ * wl_act_step only (obs_dim <= 16, not Elevation). */
+int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, float* d_actions, float* d_obs,
+                      float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
 
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out
@@ -617,6 +624,16 @@ int wl_ppo_update(const wl_ppo_params* params, const wl_ppo_batch* batch, float*
  * included), so a = mean + std * z matches it bit for bit for the same mean.  One launch; it does not step the env:
  * follow it with wl_step(out.actions, ..., the same step_counter). */
 int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter,
+                  void* stream);
+/* The actor mean alone, for any batch and without a sim handle: d_mean [n,2] (8-byte aligned) = actor(d_obs [n, obs_dim])
+ * under the network in d_policy_blob (16-byte aligned).  activation WL_ACTIVATION_ELU: wl_act_step's network, obs_dim
+ * 1..16, bit for bit the mean wl_act_step stores for the same rows; WL_ACTIVATION_RELU: obs_dim 1..4096, bit for bit the
+ * mean wl_policy_act stores.  One launch on the device that holds d_mean; it does not trigger dependents early, so a
+ * wl_step after it waits for every mean.  Bad arguments (n < 1, obs_dim out of range, ELU with obs_dim > 16, an unknown
+ * activation, a null or misaligned pointer) return WL_EINVAL / WL_EUNSUPPORTED before any device call. */
+#define WL_ACTIVATION_ELU 0
+#define WL_ACTIVATION_RELU 1
+int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d_policy_blob, int32_t activation, float* d_mean,
                   void* stream);
 /* rsl_rl PPO.update() on that network: the semantics, structs and d_state layout of wl_ppo_update (relu'(z) = (h > 0), 0
  * at z == 0 as torch's threshold_backward).  Per mini-batch: the gathered layer-1 forward, layers 2-3 and the loss with

@@ -4,7 +4,8 @@ Elevation and Visual, rsl_rl's PPO settings, save_interval 50).  One CUDA graph 
 
 Prints, per iteration, the reference runner's Train/mean_reward and Train/mean_episode_length (the last 100 finished
 episodes, once there is one), the episodes finished in the iteration, the learning rate, the losses and the iteration time.
-``--log-dir`` saves ``models/model_{it}.pt`` every ``--save-interval`` iterations; ``--resume PATH`` continues from one.
+``--log-dir`` saves ``models/model_{it}.pt`` every ``--save-interval`` iterations and the run's ``run.json`` (task, num_envs,
+seed, agent cfg; what ``tools/play_policy.py -p LOG_DIR`` reads); ``--resume PATH`` continues from one.
 
     python tools/ppo_train.py [--task elevation|visual] --envs 4096 --iters 50 [--log-dir DIR] [--resume DIR/models/model_25.pt] [--out log.txt]
 """
@@ -22,16 +23,6 @@ TASKS = {"drift": ("Isaac-MushrDriftRL-v0", "elu", "Drift"), "elevation": ("Isaa
          "visual": ("Isaac-MushrVisualRL-v0", "relu", "Visual (camera)")}
 
 
-def agent_cfg(activation: str, steps: int, save_interval: int) -> dict:
-    """The reference's agent cfg (``MushrPPORunnerCfg().to_dict()`` of the task's rsl_rl_ppo_cfg.py), the fields the runner reads."""
-    from dataclasses import asdict
-    from wheeledlab_b200.learner import PPOConfig
-    return {"num_steps_per_env": steps, "save_interval": save_interval, "empirical_normalization": False,
-            "policy": {"class_name": "ActorCritic", "init_noise_std": 1.0, "actor_hidden_dims": [64, 64],
-                       "critic_hidden_dims": [64, 64], "activation": activation},
-            "algorithm": {"class_name": "PPO", **asdict(PPOConfig())}}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--task", choices=sorted(TASKS), default="drift")
@@ -46,11 +37,15 @@ def main():
     a = ap.parse_args()
     import wheeledlab_b200 as wl
     from wheeledlab_b200.learner import FusedOnPolicyRunner
+    from wheeledlab_b200.runs import agent_cfg, save_run_config
     dev = "cuda:0"
     torch.manual_seed(a.seed)
     task_id, activation, name = TASKS[a.task]
     env = wl.make(task_id, device=dev, num_envs=a.envs, seed=a.seed)
-    runner = FusedOnPolicyRunner(env, agent_cfg(activation, a.steps, a.save_interval), log_dir=a.log_dir, device=dev)
+    agent = agent_cfg(activation, a.steps, a.save_interval)
+    runner = FusedOnPolicyRunner(env, agent, log_dir=a.log_dir, device=dev)
+    if a.log_dir:
+        save_run_config(a.log_dir, task_id, a.envs, a.seed, agent)
     head = (f"# {name} PPO (obs_dim {env.sim.obs_dim}, {activation}), {a.envs} envs x {a.steps} steps, rsl_rl agent cfg, seed {a.seed}, "
             f"one graph per iteration, {torch.cuda.get_device_name(0)}")
     if a.resume:

@@ -880,7 +880,10 @@ __device__ __forceinline__ void mlp_tile_store_elu(float* h0, int hstride, const
 #define WL_ACT_XS 20                             // padded observation row
 #define WL_ACT_HS (2 * WL_HID + 4)               // padded hidden row, [actor 64 | critic 64 | pad]
 
-template <int TASK>
+// INFER (wl_act_infer_step): the actor mean alone is the action -- no critic, no policy noise, no log-prob; only the actor
+// blocks of the blob are copied, and warps 0..3 run the actor with lanes 0-15 and 16-31 on different envs.  Each output
+// keeps its summation order, so the actions equal the mean the INFER = false instantiation stores, bit for bit.
+template <int TASK, bool INFER = false>
 __global__ void __launch_bounds__(WL_ACT_THREADS)
 wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl, Terrain T,
                         const float* __restrict__ obs_in, const float* __restrict__ blob, int blob_floats, PolicyOffsets po_off,
@@ -908,12 +911,19 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
         mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
         mbar_init_fence();
         const int a0 = po_off.o[0], a1 = po_off.o[2], c0 = po_off.o[6], c1 = po_off.o[8];
-        mbar_expect(&mbar[0], (uint32_t)((a1 - a0) + (c1 - c0)) * 4u);
-        bulk_g2s(sw + a0, blob + a0, (uint32_t)(a1 - a0) * 4u, &mbar[0]);
-        bulk_g2s(sw + c0, blob + c0, (uint32_t)(c1 - c0) * 4u, &mbar[0]);
-        mbar_expect(&mbar[1], (uint32_t)((c0 - a1) + (blob_floats - c1)) * 4u);
-        bulk_g2s(sw + a1, blob + a1, (uint32_t)(c0 - a1) * 4u, &mbar[1]);
-        bulk_g2s(sw + c1, blob + c1, (uint32_t)(blob_floats - c1) * 4u, &mbar[1]);
+        if constexpr (INFER) {                               // actor W1t | b1, then the rest of the actor
+            mbar_expect(&mbar[0], (uint32_t)(a1 - a0) * 4u);
+            bulk_g2s(sw + a0, blob + a0, (uint32_t)(a1 - a0) * 4u, &mbar[0]);
+            mbar_expect(&mbar[1], (uint32_t)(c0 - a1) * 4u);
+            bulk_g2s(sw + a1, blob + a1, (uint32_t)(c0 - a1) * 4u, &mbar[1]);
+        } else {
+            mbar_expect(&mbar[0], (uint32_t)((a1 - a0) + (c1 - c0)) * 4u);
+            bulk_g2s(sw + a0, blob + a0, (uint32_t)(a1 - a0) * 4u, &mbar[0]);
+            bulk_g2s(sw + c0, blob + c0, (uint32_t)(c1 - c0) * 4u, &mbar[0]);
+            mbar_expect(&mbar[1], (uint32_t)((c0 - a1) + (blob_floats - c1)) * 4u);
+            bulk_g2s(sw + a1, blob + a1, (uint32_t)(c0 - a1) * 4u, &mbar[1]);
+            bulk_g2s(sw + c1, blob + c1, (uint32_t)(blob_floats - c1) * 4u, &mbar[1]);
+        }
     }
     const uint32_t t = decode_step(gl, t_arg);
     const VisualMap vm = VIS ? visual_map(c, T.hf) : VisualMap{nullptr, nullptr};
@@ -934,7 +944,7 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     // the policy noise does not depend on the weights: draw it while the copies are in flight
     float z0 = 0.0f, z1 = 0.0f, zn[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     if (stepper) {
-        policy_noise(c.seed, L.gid, t, z0, z1);
+        if constexpr (!INFER) policy_noise(c.seed, L.gid, t, z0, z1);
         if (!ELEV && !VIS) quad_obs_noise(c, L.w, L.gid, t, RNG_OBS, 0u, zn);
     }
     __syncthreads();                                         // mbarrier init visible to every waiter; obs rows written
@@ -942,9 +952,9 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     // ---- MLPs: warp k takes envs 4k..4k+3 of the CTA; its 32 lanes tile the 128 (actor | critic) hidden columns 4 at a
     // time, so a lane holds 4 units x 4 envs in registers.  Layer exchanges stay warp-local (__syncwarp).  W1t has obs_dim
     // rows; rows obs_dim..nin1-1 read whatever follows in the blob and meet the zero padding of x.
-    {
-        const int lane = threadIdx.x & 31, net = lane >> 4, ucol = (lane & 15) * 4;
-        const int env0 = (threadIdx.x >> 5) * 4;
+    if (!INFER || stepper) {                                 // (INFER: warp k takes envs 8k..8k+7, half-warps 4 each)
+        const int lane = threadIdx.x & 31, net = INFER ? 0 : lane >> 4, ucol = (lane & 15) * 4;
+        const int env0 = INFER ? (threadIdx.x >> 5) * 8 + (lane >> 4) * 4 : (threadIdx.x >> 5) * 4;
         const int nin1 = (obs_dim + 3) & ~3;
         const int oW1 = net ? po_off.o[6] : po_off.o[0], oB1 = net ? po_off.o[7] : po_off.o[1];     // (no dynamic indexing of kernel params)
         const int oW2 = net ? po_off.o[8] : po_off.o[2], oB2 = net ? po_off.o[9] : po_off.o[3];
@@ -967,24 +977,35 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
 #pragma unroll
         for (int u = 0; u < 16; ++u) {
             const int j = 16 * L.w + u;
-            const float xa = hrow[j], xc = hrow[WL_HID + j];
-            m0 = fmaf(w3a[2 * j], xa, m0); m1 = fmaf(w3a[2 * j + 1], xa, m1);
-            vv = fmaf(w3c[j], xc, vv);
+            if constexpr (INFER) {
+                const float xa = hrow[j];
+                m0 = fmaf(w3a[2 * j], xa, m0); m1 = fmaf(w3a[2 * j + 1], xa, m1);
+            } else {
+                const float xa = hrow[j], xc = hrow[WL_HID + j];
+                m0 = fmaf(w3a[2 * j], xa, m0); m1 = fmaf(w3a[2 * j + 1], xa, m1);
+                vv = fmaf(w3c[j], xc, vv);
+            }
         }
         m0 += __shfl_xor_sync(0xffffffffu, m0, 1); m0 += __shfl_xor_sync(0xffffffffu, m0, 2);
         m1 += __shfl_xor_sync(0xffffffffu, m1, 1); m1 += __shfl_xor_sync(0xffffffffu, m1, 2);
-        vv += __shfl_xor_sync(0xffffffffu, vv, 1); vv += __shfl_xor_sync(0xffffffffu, vv, 2);
-        m0 += sw[po_off.o[5]]; m1 += sw[po_off.o[5] + 1]; vv += sw[po_off.o[11]];
         float2 a;
-        float lp;
-        gaussian_head(m0, m1, sw[po_off.o[12]], sw[po_off.o[12] + 1], z0, z1, a, lp);
-        if (L.live && L.w == 0) {
-            reinterpret_cast<float2*>(po.actions)[L.i] = a;
-            reinterpret_cast<float2*>(po.mean)[L.i] = make_float2(m0, m1);
-            po.log_prob[L.i] = lp;
-            po.value[L.i] = vv;
+        if constexpr (INFER) {
+            m0 += sw[po_off.o[5]]; m1 += sw[po_off.o[5] + 1];
+            a = make_float2(m0, m1);
+            if (L.live && L.w == 0) reinterpret_cast<float2*>(po.actions)[L.i] = a;
+        } else {
+            vv += __shfl_xor_sync(0xffffffffu, vv, 1); vv += __shfl_xor_sync(0xffffffffu, vv, 2);
+            m0 += sw[po_off.o[5]]; m1 += sw[po_off.o[5] + 1]; vv += sw[po_off.o[11]];
+            float lp;
+            gaussian_head(m0, m1, sw[po_off.o[12]], sw[po_off.o[12] + 1], z0, z1, a, lp);
+            if (L.live && L.w == 0) {
+                reinterpret_cast<float2*>(po.actions)[L.i] = a;
+                reinterpret_cast<float2*>(po.mean)[L.i] = make_float2(m0, m1);
+                po.log_prob[L.i] = lp;
+                po.value[L.i] = vv;
+            }
         }
-        // ---- the env step on the sampled action
+        // ---- the env step on the sampled action (INFER: on the mean)
         quad_env_step<TASK>(c, T, vm, gl->acc[t % 3u], wts, e, L, t, a, zn, obs + (size_t)obs_row_floats(c, TASK) * L.ii, rew, terminated_o, truncated_o);
         if (L.live) store_env_quad(st, n, L.i, L.w, e, ELEV);
     }
@@ -1530,6 +1551,7 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 
 #include "wl_ppo.cuh"
 #include "wl_wide.cuh"
+#include "wl_actor.cuh"
 #include "wl_episode.cuh"
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
@@ -2279,15 +2301,15 @@ int32_t wl_policy_blob_floats(int32_t obs_dim, int32_t offsets[13]) {
     return policy_offsets(obs_dim, offsets ? offsets : tmp);
 }
 
-int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, float* d_obs, float* d_rew,
-                uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
-    if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value || !d_obs || !d_rew ||
-        !d_terminated || !d_truncated)
-        return fail(WL_EINVAL, "wl_act_step: null argument");
-    if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_act_step: blind-observation tasks only (obs_dim <= 16)");
-    if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, "wl_act_step: obs_dim > 16");
+// wl_act_step and wl_act_infer_step: the same launch of wl_act_step_quad_kernel<task, infer> (arguments checked by the caller
+// for null)
+static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out,
+                           float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter,
+                           void* stream) {
+    if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, std::string(fn) + ": blind-observation tasks only (obs_dim <= 16)");
+    if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))
-        return fail(WL_EINVAL, "wl_act_step: policy blob must be 16-byte aligned, actions/mean 8-byte aligned");
+        return fail(WL_EINVAL, std::string(fn) + ": policy blob must be 16-byte aligned, actions/mean 8-byte aligned");
     PolicyOffsets po;
     const int blob_floats = policy_offsets(sim->obs_dim, po.o);
     const int n = sim->cfg.num_envs, grid = (n + WL_ACT_ENVS - 1) / WL_ACT_ENVS + 1;      // + the janitor CTA
@@ -2299,13 +2321,35 @@ int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, 
     if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
         cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_VISUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_VISUAL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_DRIFT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         attr_set[sim->device] = true;
     }
     with_task<WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
-        launch_k(wl_act_step_quad_kernel<task>, grid, WL_ACT_THREADS, smem, cs, g_pdl, sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated, d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
+        launch_k(infer ? wl_act_step_quad_kernel<task, true> : wl_act_step_quad_kernel<task, false>, grid, WL_ACT_THREADS, smem, cs, g_pdl,
+                 sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated,
+                 d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
     });
-    if (int rc = launched(sim, "wl_act_step_quad_kernel")) return rc;
+    if (int rc = launched(sim, infer ? "wl_act_step_quad_kernel<infer>" : "wl_act_step_quad_kernel")) return rc;
     return post_step(sim, step_counter, cs);
+}
+
+int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, float* d_obs, float* d_rew,
+                uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value || !d_obs || !d_rew ||
+        !d_terminated || !d_truncated)
+        return fail(WL_EINVAL, "wl_act_step: null argument");
+    return act_step_launch(false, "wl_act_step", sim, d_obs_in, d_policy_blob, out, d_obs, d_rew, d_terminated, d_truncated, d_log,
+                           step_counter, stream);
+}
+
+int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, float* d_actions, float* d_obs, float* d_rew,
+                      uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs_in || !d_policy_blob || !d_actions || !d_obs || !d_rew || !d_terminated || !d_truncated)
+        return fail(WL_EINVAL, "wl_act_infer_step: null argument");
+    const wl_policy_out out{d_actions, nullptr, nullptr, nullptr};
+    return act_step_launch(true, "wl_act_infer_step", sim, d_obs_in, d_policy_blob, out, d_obs, d_rew, d_terminated, d_truncated, d_log,
+                           step_counter, stream);
 }
 
 int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_values, const uint8_t* d_dones,
@@ -2499,6 +2543,40 @@ int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob
     wl_policy_act_kernel<<<(n + WL_WIDE_ROWS - 1) / WL_WIDE_ROWS, WL_WIDE_THREADS, policy_act_smem(), (cudaStream_t)stream>>>(
         d_obs_in, n, D, d_policy_blob, blob_floats, po, pc, out, sim->globals, sim->cfg.seed, sim->cfg.env_id_offset, (uint32_t)step_counter);
     return launched(sim, "wl_policy_act_kernel");
+}
+
+int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d_policy_blob, int32_t activation, float* d_mean,
+                  void* stream) {
+    if (!d_obs || !d_policy_blob || !d_mean) return fail(WL_EINVAL, "wl_actor_mean: null argument");
+    if (n < 1) return fail(WL_EINVAL, "wl_actor_mean: n must be >= 1");
+    if (activation != WL_ACTIVATION_ELU && activation != WL_ACTIVATION_RELU)
+        return fail(WL_EINVAL, "wl_actor_mean: activation must be WL_ACTIVATION_ELU or WL_ACTIVATION_RELU");
+    if (obs_dim < 1 || obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, "wl_actor_mean: obs_dim must be in 1..4096");
+    if (activation == WL_ACTIVATION_ELU && obs_dim > 16)
+        return fail(WL_EUNSUPPORTED, "wl_actor_mean: the ELU network (wl_act_step's) takes obs_dim <= 16");
+    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)d_mean & 7u) || ((uintptr_t)d_obs & 3u))
+        return fail(WL_EINVAL, "wl_actor_mean: policy blob must be 16-byte aligned, mean 8-byte aligned, obs 4-byte aligned");
+    // device guard: the launch goes to the device that holds the output
+    cudaPointerAttributes pa;
+    if (int rc = cuda_check(cudaPointerGetAttributes(&pa, d_mean), "wl_actor_mean")) return rc;
+    if (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) return fail(WL_EINVAL, "wl_actor_mean: d_mean is not device memory");
+    int cur = -1;
+    if (cudaGetDevice(&cur) == cudaSuccess && cur != pa.device) cudaSetDevice(pa.device);
+    const size_t smem = actor_mean_smem();
+    static bool attr_set[64] = {false};
+    if (pa.device >= 0 && pa.device < 64 && !attr_set[pa.device]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_actor_mean_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_actor_mean")) return rc;
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_actor_mean_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_actor_mean")) return rc;
+        attr_set[pa.device] = true;
+    }
+    PolicyOffsets po;
+    policy_offsets(obs_dim, po.o);
+    const int grid = (n + WL_AM_ROWS - 1) / WL_AM_ROWS;
+    if (activation == WL_ACTIVATION_RELU)
+        wl_actor_mean_kernel<true><<<grid, WL_AM_THREADS, smem, (cudaStream_t)stream>>>(d_obs, n, obs_dim, d_policy_blob, po, reinterpret_cast<float2*>(d_mean));
+    else
+        wl_actor_mean_kernel<false><<<grid, WL_AM_THREADS, smem, (cudaStream_t)stream>>>(d_obs, n, obs_dim, d_policy_blob, po, reinterpret_cast<float2*>(d_mean));
+    return cuda_check(cudaGetLastError(), "wl_actor_mean_kernel");
 }
 
 // workspace of wl_ppo_update_wide: wl_ppo_update's, then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)

@@ -486,6 +486,17 @@ class FusedOnPolicyRunner:
                 self.callback(k, log)
         return self.last_log
 
+    def get_inference_policy(self, device=None):
+        """rsl_rl's ``get_inference_policy``: ``policy(obs) -> actions``, the actor mean (``policy.InferencePolicy``) over the
+        runner's live blob with the runner's activation, so later ``learn`` / ``load`` calls are seen.  The policy runs on
+        the env's device: another `device` raises."""
+        from .policy import InferencePolicy
+        if device is not None:
+            norm = lambda x: (x.type, x.index if x.index is not None or x.type != "cuda" else torch.cuda.current_device())
+            if norm(torch.device(device)) != norm(torch.device(self.device)):
+                raise ValueError(f"device {device} is not the env's device {self.device}: the policy runs where the env's blob is")
+        return InferencePolicy(self.blob, self.env.sim.obs_dim, self.activation)
+
     def save(self, path: str, infos=None):
         """rsl_rl's checkpoint: {"model_state_dict", "optimizer_state_dict", "iter", "infos"}."""
         from .policy import actor_critic_state_dict

@@ -13,7 +13,7 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import WlPolicyOut, check, lib
+from ._lib import WL_ACTIVATION, WlPolicyOut, check, lib
 from .distributed import RolloutSlab
 from .sim import WheeledSim, _stream_ptr
 
@@ -117,6 +117,56 @@ def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation
     return x.squeeze(-1)
 
 
+def _device_tensor(name: str, t, device, shape=None, ndim=None) -> None:
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name} must be a torch.Tensor")
+    if t.device.type != "cuda" or (device is not None and t.device != device):
+        raise ValueError(f"{name} must be on {device or 'a CUDA device'}, not {t.device}")
+    if t.dtype != torch.float32:
+        raise ValueError(f"{name} must be float32, not {t.dtype}")
+    if ndim is not None and t.dim() != ndim:
+        raise ValueError(f"{name} must have {ndim} dimension(s), not shape {tuple(t.shape)}")
+    if shape is not None and tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name} must have shape {tuple(shape)}, not {tuple(t.shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+
+
+def actor_mean(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu", out: torch.Tensor | None = None) -> torch.Tensor:
+    """The actor mean [N, 2] of `obs` [N, obs_dim] under the network in `blob` -- rsl_rl ``ActorCritic.act_inference``, the
+    deterministic action a trained policy is played with.  One launch (wl_actor_mean) on the current stream of obs's
+    device; into `out` [N, 2] when given (capturable), else into a new tensor.  "elu": the Drift family's network
+    (obs_dim <= 16), bit for bit the mean wl_act_step stores; "relu": Elevation / Visual (obs_dim <= 4096), bit for bit
+    wl_policy_act's mean."""
+    check_activation(activation)
+    _device_tensor("obs", obs, None, ndim=2)
+    dev = obs.device
+    if obs.shape[1] != obs_dim:
+        raise ValueError(f"obs must have shape [N, {obs_dim}], not {tuple(obs.shape)}")
+    if obs.shape[0] < 1:
+        raise ValueError("obs must have at least one row")
+    _device_tensor("blob", blob, dev, shape=(blob_layout(obs_dim)[1],))
+    if out is None:
+        out = torch.empty((obs.shape[0], 2), dtype=torch.float32, device=dev)
+    else:
+        _device_tensor("out", out, dev, shape=(obs.shape[0], 2))
+    check(lib.wl_actor_mean(C.c_void_p(obs.data_ptr()), obs.shape[0], obs_dim, C.c_void_p(blob.data_ptr()), WL_ACTIVATION[activation],
+                            C.c_void_p(out.data_ptr()), _stream_ptr(dev)), "wl_actor_mean")
+    return out
+
+
+class InferencePolicy:
+    """rsl_rl's ``runner.get_inference_policy()``: ``policy(obs) -> actions [N, 2]``, the actor mean (actor_mean), a new
+    tensor per call (play_policy.py appends the actions without cloning) unless `out` is given.  The blob is read at call
+    time, so later updates and loads into it are seen.  Works under ``torch.inference_mode()``."""
+
+    def __init__(self, blob: torch.Tensor, obs_dim: int, activation: str = "elu"):
+        self.blob, self.obs_dim, self.activation = blob, obs_dim, check_activation(activation)
+
+    def __call__(self, obs: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+        return actor_mean(self.blob, self.obs_dim, obs, self.activation, out)
+
+
 class PolicyBuffers:
     """[T, N] storage of what alg.act() records per step (rsl_rl RolloutStorage fields)."""
 
@@ -137,6 +187,17 @@ def act_step(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions:
           "wl_act_step")
 
 
+def act_infer_step(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor, out, log: torch.Tensor | None,
+                   step_counter: int):
+    """One launch (wl_act_infer_step): the actor mean of `obs_in` under the ELU network in `blob` into `actions`, then
+    env.step(actions) into `out`."""
+    obs, rew, term, trunc = out
+    check(lib.wl_act_infer_step(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(blob.data_ptr()), C.c_void_p(actions.data_ptr()),
+                                C.c_void_p(obs.data_ptr()), C.c_void_p(rew.data_ptr()), C.c_void_p(term.data_ptr()),
+                                C.c_void_p(trunc.data_ptr()), C.c_void_p(log.data_ptr()) if log is not None else None, step_counter,
+                                _stream_ptr(sim.device)), "wl_act_infer_step")
+
+
 def policy_act(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor, mean: torch.Tensor,
                log_prob: torch.Tensor, value: torch.Tensor, step_counter: int):
     """One launch (wl_policy_act): value / mean / sample / log-prob of `obs_in` [N, obs_dim] under the ReLU network in `blob`,
@@ -150,16 +211,26 @@ class FusedPolicyRollout:
     """T policy-and-step launches captured as ONE CUDA graph: the reference's whole collection loop
     (modified_rsl_rl_runner.py:70-109).  activation "elu" (the Drift family): T x wl_act_step, the policy fused into the
     step; "relu" (Elevation, Visual): T x (wl_policy_act, then wl_step).  The blob is read at replay time, so refilling it
-    in place (pack_actor_critic(..., out=blob)) after each PPO update needs no re-capture."""
+    in place (pack_actor_critic(..., out=blob)) after each PPO update needs no re-capture.
 
-    def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu"):
+    ``deterministic=True`` plays the policy instead (play_policy.py's loop): the action is the actor mean, with no critic and
+    no noise -- T x wl_act_infer_step for "elu", T x (wl_actor_mean, then wl_step) for "relu" -- and the slab has no
+    policy fields.  ``slab.obs[k]`` / ``slab.actions[k]`` are what play_policy.py appends at step k, so
+    ``recording.save_slab(playback_dir, play_name, roll.slab)`` writes its rollouts file."""
+
+    def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu",
+                 deterministic: bool = False):
         self.sim, self.blob, self.T, self.activation = sim, blob, T, check_activation(activation)
+        self.deterministic = bool(deterministic)
         if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
             raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
-        self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=True)
+        self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=not self.deterministic)
         # values / log-prob / mean go straight into the slab (= the all-gather send buffer) when it has those fields
-        self.pol = (SimpleNamespace(values=self.slab.values, log_prob=self.slab.log_prob, mean=self.slab.mean)
-                    if hasattr(self.slab, "values") else PolicyBuffers(T, sim.num_envs, sim.device))
+        if self.deterministic:
+            self.pol = None
+        else:
+            self.pol = (SimpleNamespace(values=self.slab.values, log_prob=self.slab.log_prob, mean=self.slab.mean)
+                        if hasattr(self.slab, "values") else PolicyBuffers(T, sim.num_envs, sim.device))
         self.logs = torch.zeros((T, 16), dtype=torch.float32, device=sim.device)
         # slab.obs_in[k] = the observation actions[k] / log_prob[k] / values[k] / mean[k] were computed from (rsl_rl
         # RolloutStorage.observations[k]); slab.obs[k] = obs_in[k+1] = what step k returned
@@ -172,7 +243,14 @@ class FusedPolicyRollout:
         self.slab.obs_in[0].copy_(self.obs0)
         for k in range(self.T):
             t = WheeledSim.device_counter_plus(k)
-            if self.activation == "relu":
+            if self.deterministic:
+                if self.activation == "relu":
+                    actor_mean(self.blob, self.sim.obs_dim, self.slab.obs_in[k], "relu", out=self.slab.actions[k])
+                    self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
+                else:
+                    act_infer_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.slab.step_outputs(k),
+                                   self.logs[k], t)
+            elif self.activation == "relu":
                 policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
                            self.pol.values[k], t)
                 self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
