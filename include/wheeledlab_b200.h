@@ -369,13 +369,21 @@ int wl_set_term_bits(wl_sim* sim, uint8_t* d_term_bits);
 /* Fused rollout-slab fan-out (multi-GPU, SURVEY 8e): every output row wl_step writes (observation, reward, terminated,
  * truncated) is ALSO stored at `pointer + byte_deltas[k]` for k < n_peers -- byte_deltas[k] = base of peer k's symmetric
  * (P2P-mapped, NVLink) gathered buffer minus the base of the local one -- so the learner-facing concat of the rollout is
- * complete when the step kernels are: no separate collective.  n_peers = 0 switches it off.  Drift-family tasks. */
+ * complete when the step kernels are: no separate collective.  Drift-family tasks; at most WL_MAX_PEERS (8) deltas, each a
+ * multiple of 16 (WL_EINVAL otherwise: full rows leave as 16-byte stores).  n_peers = 0 switches it off, the multicast
+ * delta included.
+ * Only wl_step carries the fan-out, and only when it runs the 8-envs-per-CTA kernel (variant 8: Drift family, N <= 33 792,
+ * default or wl_set_kernel_variant 8).  While a peer or multicast delta is set, wl_step on any other variant and
+ * wl_rollout, wl_act_step, wl_act_infer_step, wl_step_stage_a / _b, wl_step_host and wl_step_host_zero_copy return
+ * WL_EUNSUPPORTED before any device work and leave the handle as it was.  wl_observe, wl_reset and wl_policy_act write no
+ * step rows and ignore it. */
 int wl_set_peer_fanout(wl_sim* sim, int32_t n_peers, const int64_t* byte_deltas);
 /* NVSwitch multicast form of the fan-out: `mc_byte_delta` = (multicast alias of the symmetric buffer) - (this rank's mapping of
- * it); the 8-envs-per-CTA step kernel (variant 8) then sends every full, aligned output row with ONE multimem.st that the
- * switch replicates into all ranks' buffers (NVLink egress 1x instead of (world-1)x); rows it cannot send that way (partial
- * CTA, unaligned pointers, other kernel variants) still go peer by peer through wl_set_peer_fanout's deltas, so set both.
- * 0 switches it off.  torch: _SymmetricMemory.multicast_ptr. */
+ * it); wl_step's variant-8 kernel then sends every full, aligned output row with ONE multimem.st that the switch replicates
+ * into all ranks' buffers (NVLink egress 1x instead of (world-1)x); the rows it cannot send that way (partial CTA, unaligned
+ * pointers) go peer by peer through wl_set_peer_fanout's deltas.  So the peer deltas must be set first: a nonzero delta on
+ * a handle without them, or one that is not a multiple of 16, is WL_EINVAL.  0 switches it off.  The calls that refuse the
+ * peer fan-out refuse this one too.  torch: _SymmetricMemory.multicast_ptr. */
 int wl_set_multicast_fanout(wl_sim* sim, int64_t mc_byte_delta);
 /* ManagerBasedEnv.seed(): re-key the counter-based generator for all later launches (startup draws are not repeated) */
 int wl_set_seed(wl_sim* sim, uint64_t seed);

@@ -1831,12 +1831,17 @@ int wl_set_term_bits(wl_sim* sim, uint8_t* d_term_bits) {
     sim->term_bits = d_term_bits;
     return WL_OK;
 }
+// The packed rows leave as 16-byte stores at pointer + delta, so every delta must keep that alignment.  The multicast delta
+// is only a shortcut for the rows that qualify: the others go peer by peer, so it needs the peer deltas set first, and
+// switching the peers off switches it off too.
 int wl_set_peer_fanout(wl_sim* sim, int32_t n_peers, const int64_t* byte_deltas) {
     if (!sim || n_peers < 0 || n_peers > WL_MAX_PEERS || (n_peers > 0 && !byte_deltas)) return fail(WL_EINVAL, "wl_set_peer_fanout: bad argument");
     if (n_peers > 0 && sim->cfg.task != WL_TASK_DRIFT) return fail(WL_EUNSUPPORTED, "wl_set_peer_fanout: Drift-family tasks only");
+    for (int k = 0; k < n_peers; ++k)
+        if (byte_deltas[k] % 16 != 0) return fail(WL_EINVAL, "wl_set_peer_fanout: every byte delta must be a multiple of 16");
     const int32_t mc = sim->fan.mc; const long long mcd = sim->fan.mc_delta;
     memset(&sim->fan, 0, sizeof sim->fan);
-    sim->fan.mc = mc; sim->fan.mc_delta = mcd;
+    if (n_peers > 0) { sim->fan.mc = mc; sim->fan.mc_delta = mcd; }
     sim->fan.n = n_peers;
     for (int k = 0; k < n_peers; ++k) sim->fan.delta[k] = (long long)byte_deltas[k];
     return WL_OK;
@@ -1844,6 +1849,8 @@ int wl_set_peer_fanout(wl_sim* sim, int32_t n_peers, const int64_t* byte_deltas)
 int wl_set_multicast_fanout(wl_sim* sim, int64_t mc_byte_delta) {
     if (!sim) return fail(WL_EINVAL, "wl_set_multicast_fanout: null handle");
     if (mc_byte_delta != 0 && sim->cfg.task != WL_TASK_DRIFT) return fail(WL_EUNSUPPORTED, "wl_set_multicast_fanout: Drift-family tasks only");
+    if (mc_byte_delta != 0 && sim->fan.n == 0) return fail(WL_EINVAL, "wl_set_multicast_fanout: set the peer deltas first (wl_set_peer_fanout)");
+    if (mc_byte_delta % 16 != 0) return fail(WL_EINVAL, "wl_set_multicast_fanout: the byte delta must be a multiple of 16");
     sim->fan.mc = mc_byte_delta != 0 ? 1 : 0;
     sim->fan.mc_delta = (long long)mc_byte_delta;
     return WL_OK;
@@ -2028,6 +2035,14 @@ static int prep_step(wl_sim* sim, int64_t step_counter, int32_t n_steps, cudaStr
     sim->last_t = t + n_steps - 1;
     return WL_OK;
 }
+// The peer / multicast fan-out is carried by wl_step's duo kernel only.  Every other call that writes the rows of a step
+// (rollout, act step, staged step, host-transport step) refuses while it is set, before any device work: run without it,
+// every peer would keep stale rows with no error.
+static bool fan_set(const wl_sim* sim) { return sim->fan.n > 0 || sim->fan.mc; }
+static int refuse_fan(const wl_sim* sim, const char* fn) {
+    if (!fan_set(sim)) return WL_OK;
+    return fail(WL_EUNSUPPORTED, std::string(fn) + ": the peer fan-out is set, and only wl_step carries it (wl_set_peer_fanout(0) first)");
+}
 // after the step kernel(s): a curriculum boundary reached with a host-supplied counter is applied in place right away
 static int post_step(wl_sim* sim, int64_t step_counter, cudaStream_t cs) {
     if (step_counter < 0 || sim->cfg.curr_n <= 0) return WL_OK;
@@ -2065,6 +2080,8 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     // 8 = quad + aux warp (Drift family, small N: shortest dependent chain), 4 = quad, 1 = thread per env
     int variant = sim->variant ? sim->variant : ((n <= WL_QUAD_MAX_ENVS) ? ((sim->cfg.task == WL_TASK_DRIFT) ? 8 : 4) : 1);
     if (variant == 8 && sim->cfg.task != WL_TASK_DRIFT) variant = 4;
+    if (variant != 8 && fan_set(sim))                         // before prep_step: a refused call leaves the handle as it was
+        return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
     const float2* act = reinterpret_cast<const float2*>(d_action);
     cudaStream_t cs = (cudaStream_t)stream;
     const uint32_t t = (uint32_t)step_counter;               // negative (device base + k) stays encoded: see decode_step
@@ -2078,7 +2095,7 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
                              (((uintptr_t)d_terminated | (uintptr_t)d_truncated) & 7u) == 0;
         if (sim->fan.mc && rows_ok)
             launch_k(wl_step_duo_kernel<2, 0u>, grid, duo_block(sim, wl_step_duo_kernel<2, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
-        else if (sim->fan.n > 0 || sim->fan.mc)
+        else if (fan_set(sim))
             launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
         else
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
@@ -2086,8 +2103,6 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
                 launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
             });
         cta_threads = sim->duo_threads;
-    } else if (sim->fan.n > 0) {
-        return fail(WL_EUNSUPPORTED, "wl_step: the peer fan-out is implemented by the Drift-family small-N kernel (variant 8) only");
     } else if (variant == 4) {
 #ifndef WL_QUAD_BS
 #define WL_QUAD_BS 32
@@ -2141,6 +2156,7 @@ int wl_step_stage_a(wl_sim* sim, const float* d_action, float* d_rew, uint8_t* d
     if (!sim || !d_action || !d_rew || !d_term_bits) return fail(WL_EINVAL, "wl_step_stage_a: null argument");
     if ((uintptr_t)d_action & 7u) return fail(WL_EINVAL, "wl_step_stage_a: action must be 8-byte aligned");
     if (step_counter < 0) return fail(WL_EINVAL, "wl_step_stage_a: the staged step takes the host's step counter");
+    if (int rc = refuse_fan(sim, "wl_step_stage_a")) return rc;
     {   // stage a reads W(t) like a full step: re-arm on a counter jump, but the step is only committed by stage b
         const int64_t keep = sim->last_t;
         if (int rc = prep_step(sim, step_counter, 1, (cudaStream_t)stream)) return rc;
@@ -2154,6 +2170,7 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
                     float* d_obs, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
     if (!sim || !d_term_bits || !d_obs || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_step_stage_b: null argument");
     if (step_counter < 0) return fail(WL_EINVAL, "wl_step_stage_b: the staged step takes the host's step counter");
+    if (int rc = refuse_fan(sim, "wl_step_stage_b")) return rc;
     if (int rc = prep_step(sim, step_counter, 1, (cudaStream_t)stream)) return rc;
     if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, (uint32_t)step_counter,
                                  StageIO{const_cast<uint8_t*>(d_term_bits), d_extra_terminated, d_extra_truncated}, (cudaStream_t)stream))
@@ -2168,6 +2185,7 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
                uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
     if (!sim || !d_obs || !d_rew || !d_terminated || !d_truncated || !d_log) return fail(WL_EINVAL, "wl_rollout: null argument");
     if (K < 1) return fail(WL_EINVAL, "wl_rollout: K must be >= 1");
+    if (int rc = refuse_fan(sim, "wl_rollout")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_rollout: the elevation step is two kernels (use wl_step)");
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam) return fail(WL_EUNSUPPORTED, "wl_rollout: the camera term is a second kernel (use wl_step)");
     if (sim->cfg.curr_n > 0) {
@@ -2198,6 +2216,7 @@ size_t wl_result_bytes(int32_t num_envs) { return (size_t)num_envs * 6u; }
 int wl_step_host(wl_sim* sim, const float* h_action, float* d_action, float* d_obs, void* d_result, float* d_log,
                  void* h_result, float* h_obs, int64_t step_counter, void* stream) {
     if (!sim || !h_action || !d_action || !d_obs || !d_result || !h_result) return fail(WL_EINVAL, "wl_step_host: null argument");
+    if (int rc = refuse_fan(sim, "wl_step_host")) return rc;     // (its rows are the caller's result block, not a slab's)
     const size_t n = (size_t)sim->cfg.num_envs;
     cudaStream_t cs = (cudaStream_t)stream;
     ensure_device(sim);
@@ -2226,6 +2245,7 @@ static void* host_alias(wl_sim* sim, const void* h) {
 int wl_step_host_zero_copy(wl_sim* sim, const float* h_action, float* d_obs, float* d_log, void* h_result,
                            int64_t step_counter, void* stream) {
     if (!sim || !h_action || !d_obs || !h_result) return fail(WL_EINVAL, "wl_step_host_zero_copy: null argument");
+    if (int rc = refuse_fan(sim, "wl_step_host_zero_copy")) return rc;
     const size_t n = (size_t)sim->cfg.num_envs;
     const float* da = reinterpret_cast<const float*>(host_alias(sim, h_action));
     void* dr = host_alias(sim, h_result);
@@ -2306,6 +2326,7 @@ int32_t wl_policy_blob_floats(int32_t obs_dim, int32_t offsets[13]) {
 static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out,
                            float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter,
                            void* stream) {
+    if (int rc = refuse_fan(sim, fn)) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, std::string(fn) + ": blind-observation tasks only (obs_dim <= 16)");
     if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))

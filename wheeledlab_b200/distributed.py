@@ -96,7 +96,10 @@ class SymmetricRolloutSlab:
     rank (torch.distributed._symmetric_memory).  Rank r's slab is slot r of its own buffer; the step kernel stores every
     output row there AND at the same offset of every peer's buffer (WheeledSim.set_peer_fanout), so after the last step of
     the rollout plus one barrier every rank holds the concatenated rollout -- no all-gather, no staging copy, the transfer
-    rides along with the steps.  ``slab`` is the local RolloutSlab, ``gathered()`` the [world, ...] views."""
+    rides along with the steps.  ``slab`` is the local RolloutSlab, ``gathered()`` the [world, ...] views.  Only
+    ``sim.step`` (Drift family, the 8-envs-per-CTA kernel) carries the fan-out, and only the obs, rewards, terminated and
+    truncated rows: while a slab is attached, the rollout, act-step, staged and host-transport steps raise WlError.  The
+    other fields (actions, policy fields) are the caller's to exchange."""
 
     def __init__(self, T: int, n_local: int, obs_dim: int, act_dim: int, device, group=None, policy_fields: bool = False):
         import torch.distributed._symmetric_memory as symm

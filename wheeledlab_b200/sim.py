@@ -115,14 +115,18 @@ class WheeledSim:
 
     def set_peer_fanout(self, byte_deltas):
         """Every output row of step() is also stored at pointer + delta for each delta (peer symmetric buffers, see
-        distributed.SymmetricRolloutSlab); [] switches the fan-out off."""
+        distributed.SymmetricRolloutSlab); [] switches the fan-out off, the multicast delta included.  At most 8 deltas,
+        each a multiple of 16.  Only step() on the 8-envs-per-CTA kernel (Drift family, N <= 33 792) carries it: while it
+        is set, rollout, act_step, the staged and host-transport steps and step() on another kernel variant raise WlError
+        and leave the handle unchanged."""
         n = len(byte_deltas)
         arr = (C.c_int64 * max(1, n))(*byte_deltas)
         check(lib.wl_set_peer_fanout(self._h, n, arr), "wl_set_peer_fanout")
 
     def set_multicast_fanout(self, mc_byte_delta: int):
         """NVSwitch multicast alias of the symmetric buffer (SymmetricRolloutSlab.mc_delta): full output rows leave with one
-        multimem.st replicated by the switch; 0 switches it off.  Keep set_peer_fanout's deltas set as well."""
+        multimem.st replicated by the switch; 0 switches it off.  The other rows go peer by peer, so set_peer_fanout's
+        deltas must be set first (WlError otherwise)."""
         check(lib.wl_set_multicast_fanout(self._h, int(mc_byte_delta)), "wl_set_multicast_fanout")
 
     def set_step_counter(self, value: int):
