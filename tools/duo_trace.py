@@ -7,7 +7,10 @@
 `run` steps M independent env sets round-robin inside one CUDA graph, as bench.py does, so that the working set is larger
 than L2 and every launch starts cold.  Every warp that owns envs stamps %globaltimer at its hand-offs and records %smid and
 %warpid (csrc/wl_api.cu, WL_DUO_TRACE).  Times are ns after the launch's first warp entry, median over launches of the
-per-launch median warp, except where a row says otherwise.  The traced build is a diagnostic build: its stamps and
+per-launch median warp, except where a row says otherwise.  "pass k cycles" rows are SM clock cycles (%clock) of the env
+warp's sub-step pass k (pass 0 from bar.sync 1), median over env warps, split by whether an aux warp on the same SM
+scheduler (%warpid % 4) was between its bar.arrive 1 and bar.arrive 3 (issuing the noise, push and reset draws) at any time
+during the pass.  The traced build is a diagnostic build: its stamps and
 records cost time of their own, so compare traces with traces, and bench.py figures with bench.py figures."""
 import argparse
 import json
@@ -20,7 +23,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 
-# DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64
+# DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64; ck[6] u32
 TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
      [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3"]
 
@@ -40,6 +43,34 @@ def build(out: Path, defines):
 def _median(xs):
     xs = sorted(xs)
     return xs[len(xs) // 2] if xs else None
+
+
+def pass_cycles(recs):
+    """per pass 0..3: env-warp cycles, all / while an aux warp on the same scheduler was drawing / while none was"""
+    import numpy as np
+    env, aux = recs[recs["role"] == 0], recs[recs["role"] == 1]
+    ek = env["smid"].astype(np.int64) * 4 + env["warpid"] % 4
+    ak = aux["smid"].astype(np.int64) * 4 + aux["warpid"] % 4
+    a0, a1 = aux["ts"][:, 4].astype(np.int64), aux["ts"][:, 15].astype(np.int64)     # aux bar.arrive 1 .. bar.arrive 3
+    order = np.argsort(ak, kind="stable")
+    ak, a0, a1 = ak[order], a0[order], a1[order]
+    out = {}
+    for p in range(4):
+        cyc = (env["ck"][:, p + 1].astype(np.int64) - env["ck"][:, p].astype(np.int64)) & 0xFFFFFFFF
+        t0 = env["ts"][:, 4 if p == 0 else 4 + p].astype(np.int64)
+        t1 = env["ts"][:, 5 + p].astype(np.int64)
+        ok = (env["ck"][:, p + 1] != 0) & (env["ck"][:, p] != 0) & (t0 > 0) & (t1 > 0)
+        busy = np.zeros(len(env), dtype=bool)
+        lo, hi = np.searchsorted(ak, ek, "left"), np.searchsorted(ak, ek, "right")
+        for i in np.nonzero(ok)[0]:
+            s0, s1 = a0[lo[i]:hi[i]], a1[lo[i]:hi[i]]
+            busy[i] = bool(np.any((s0 > 0) & (s0 < t1[i]) & (s1 > t0[i])))
+        m = lambda x: float(np.median(x)) if len(x) else None
+        out[f"pass {p} cycles"] = m(cyc[ok])
+        out[f"pass {p} cycles, aux warp drawing on the scheduler"] = m(cyc[ok & busy])
+        out[f"pass {p} cycles, no aux warp drawing on the scheduler"] = m(cyc[ok & ~busy])
+        out[f"pass {p}: fraction of env warps with an aux warp drawing on the scheduler"] = float(busy[ok].mean()) if ok.any() else None
+    return out
 
 
 def summarize(recs, tag, n_launch_expected):
@@ -104,6 +135,7 @@ def summarize(recs, tag, n_launch_expected):
         "env warps entering after the previous launch's last store (median)": _median(late_cta),
         "launches whose last env-warp store is from such a late warp": int(sum(last_is_late)),
     })
+    out.update(pass_cycles(recs))
     return out
 
 
@@ -142,8 +174,8 @@ def run(args):
     g.replay(); torch.cuda.synchronize()
     per_launch = 2 * ((E + 7) // 8)
     dtype = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
-                      ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR))])
-    assert dtype.itemsize == 168
+                      ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
+    assert dtype.itemsize == 192
     cap = per_launch * R
     buf = torch.zeros(cap * dtype.itemsize, dtype=torch.uint8, device=dev)
     lib.wl_duo_trace_arm.argtypes = [C.c_void_p, C.c_uint32]

@@ -223,6 +223,14 @@ __device__ __forceinline__ void dc_limits(const wl_config& c, float effort_limit
     hi = r_clamp(c.dc_saturation * (1.0f - ratio), 0.0f, effort_limit);
     lo = r_clamp(c.dc_saturation * (-1.0f - ratio), -effort_limit, 0.0f);
 }
+// the same limits as a select instead of an early return (no divergent region where it runs inside the sub-step loop)
+__device__ __forceinline__ void dc_limits_sel(const wl_config& c, float effort_limit, float omega, float& lo, float& hi) {
+    const bool on = effort_limit > 0.0f;
+    const float ratio = omega * c.d_inv_dc_vel_limit;
+    const float h = r_clamp(c.dc_saturation * (1.0f - ratio), 0.0f, effort_limit);
+    const float l = r_clamp(c.dc_saturation * (-1.0f - ratio), -effort_limit, 0.0f);
+    hi = on ? h : 0.0f; lo = on ? l : 0.0f;
+}
 
 // ---- terrain -----------------------------------------------------------------------
 struct Terrain { const float* __restrict__ hf; };
@@ -295,8 +303,9 @@ __device__ __forceinline__ void steer_step(const wl_config& c, float target, flo
 struct WheelOut { V3 F, Tq; float omega; };
 
 // one wheel: contact, Pacejka slip force with the implicit-stick cap, spin update.  `i` = wheel index
-// [bl, br, fl, fr]; (sn, cs) = sin/cos of its steer angle (front wheels only).
-template <int TASK>
+// [bl, br, fl, fr]; (sn, cs) = sin/cos of its steer angle (front wheels only).  SEL: the front / rear tyre direction is a
+// select between both forms, not a branch on i (for a warp whose lanes hold different wheels)
+template <int TASK, bool SEL = false>
 __device__ __forceinline__ WheelOut wheel_force(const wl_config& c, const Terrain& T, const StepConsts& k, const M3& R,
                                                 const Chassis& b, V3 vb, int i, float sn, float cs, float omega, float target,
                                                 float eff_lo, float eff_hi, float kd, float hI, float idk, float fxk, float Dmu, float Cmu) {
@@ -330,7 +339,13 @@ __device__ __forceinline__ WheelOut wheel_force(const wl_config& c, const Terrai
     if (ce > c.susp_travel) Fz = fm(c.bump_k, ce - c.susp_travel, Fz);
     Fz = (comp > 0.0f) ? r_max(Fz, 0.0f) : 0.0f;
     V3 ft;
-    if (i >= 2) { float d = fm(cs, nb.x, sn * nb.y); ft = V3{fm(-d, nb.x, cs), fm(-d, nb.y, sn), -(d * nb.z)}; }
+    if (SEL) {
+        const float df = fm(cs, nb.x, sn * nb.y), dr = nb.x;
+        const bool front = i >= 2;
+        ft.x = front ? fm(-df, nb.x, cs) : fm(-dr, nb.x, 1.0f);
+        ft.y = front ? fm(-df, nb.y, sn) : -(dr * nb.y);
+        ft.z = front ? -(df * nb.z) : -(dr * nb.z);
+    } else if (i >= 2) { float d = fm(cs, nb.x, sn * nb.y); ft = V3{fm(-d, nb.x, cs), fm(-d, nb.y, sn), -(d * nb.z)}; }
     else { float d = nb.x; ft = V3{fm(-d, nb.x, 1.0f), -(d * nb.y), -(d * nb.z)}; }
     // |ft|^2 = 1 - d^2: normalise with the binomial series of (1 - e)^(-1/2), e = 1 - |ft|^2 (no sqrt, no division)
     float en = 1.0f - dot(ft, ft);
@@ -384,8 +399,8 @@ __device__ __forceinline__ void chassis_integrate(const wl_config& c, const Step
 // LANES == 1: one thread owns the env and loops over the 4 wheels.
 // LANES == 4: four adjacent lanes own one env; lane (l & 3) owns wheel l & 3, the chassis is integrated
 //             redundantly (bit-identically) in all four, forces are summed with two butterfly shuffles.
-// Both sum as (F0 + F1) + (F2 + F3), the order the oracle uses.
-template <int TASK, int LANES>
+// Both sum as (F0 + F1) + (F2 + F3), the order the oracle uses.  SEL (LANES == 4): no divergent region in the pass.
+template <int TASK, int LANES, bool SEL = false>
 __device__ __forceinline__ void physics_substep(const wl_config& c, const Terrain& T, EnvState& e, Chassis& b,
                                                 const float wheel_target[4], const float eff_lo[4], const float eff_hi[4],
                                                 const float steer_target[2], const StepConsts& k) {
@@ -414,7 +429,7 @@ __device__ __forceinline__ void physics_substep(const wl_config& c, const Terrai
         // region inside the sub-step; rear wheels then take (sin, cos) = (0, 1)
         steer_step(c, steer_target[0], e.steer[0], e.steer_vel[0], sn, cs);
         sn = (i >= 2) ? sn : 0.0f; cs = (i >= 2) ? cs : 1.0f;
-        WheelOut w = wheel_force<TASK>(c, T, k, R, b, vb, i, sn, cs, e.omega[0], wheel_target[0], eff_lo[0], eff_hi[0], e.kd[0],
+        WheelOut w = wheel_force<TASK, SEL>(c, T, k, R, b, vb, i, sn, cs, e.omega[0], wheel_target[0], eff_lo[0], eff_hi[0], e.kd[0],
                                        k.hI[0], k.idk[0], k.fxk[0], e.D[0], e.C[0]);
         e.omega[0] = w.omega;
         float v6[6] = {w.F.x, w.F.y, w.F.z, w.Tq.x, w.Tq.y, w.Tq.z};
@@ -441,9 +456,10 @@ __device__ __forceinline__ Chassis chassis_from_env(const wl_config& c, const En
 // effort: the DC-motor effort limit per wheel (LANES == 4: slot 0 = this lane's wheel); the speed-dependent limits are
 // formed once per physics step.  With a fixed spec (K != 0) the trip counts are constants but the loops stay rolled: fully
 // unrolled, the 4 x 1 Drift sub-steps were no faster on H100 (DESIGN.md 6e) and cost ~900 more static instructions
-// `pass_done` is called after every sub-step (the duo kernel's phase trace, WL_DUO_TRACE; empty otherwise).
+// SEL: the pass has no divergent region (dc_limits_sel, physics_substep<..., SEL>).  `pass_done` is called after every
+// sub-step (the duo kernel's phase trace, WL_DUO_TRACE; empty otherwise).
 struct NoPassHook { __device__ __forceinline__ void operator()(const EnvState&) const {} };
-template <int TASK, int LANES, uint32_t K = 0, typename PassHook = NoPassHook>
+template <int TASK, int LANES, uint32_t K = 0, bool SEL = false, typename PassHook = NoPassHook>
 __device__ __forceinline__ void run_substeps(const wl_config& c, const Terrain& T, EnvState& e, Chassis& b, const float target[4],
                                              const float effort[4], const float steer_target[2], const StepConsts& kc,
                                              PassHook pass_done = {}) {
@@ -451,9 +467,12 @@ __device__ __forceinline__ void run_substeps(const wl_config& c, const Terrain& 
     for (int d = 0; d < S::decimation(c); ++d) {
         float lo[4], hi[4];
 #pragma unroll
-        for (int w = 0; w < 4 / LANES; ++w) dc_limits(c, effort[w], e.omega[w], lo[w], hi[w]);
+        for (int w = 0; w < 4 / LANES; ++w) {
+            if (SEL) dc_limits_sel(c, effort[w], e.omega[w], lo[w], hi[w]);
+            else dc_limits(c, effort[w], e.omega[w], lo[w], hi[w]);
+        }
         for (int j = 0; j < S::substeps(c); ++j) {
-            physics_substep<TASK, LANES>(c, T, e, b, target, lo, hi, steer_target, kc);
+            physics_substep<TASK, LANES, SEL>(c, T, e, b, target, lo, hi, steer_target, kc);
             pass_done(e);
         }
     }
