@@ -569,9 +569,11 @@ int wl_episode_stats(const float* d_rewards, const uint8_t* d_terminated, const 
  * (this rank's own buffer and the P2P-mapped buffers of its peers, e.g. slices of one torch symmetric-memory allocation; the
  * same rank order on every rank, so every replica forms the identical mean); d_param / d_m / d_v = this rank's flat
  * parameters and Adam moments, n floats each.  `step` = 1, 2, ... (bias correction).  The caller brackets the launch with
- * barriers (all gradients written before; none overwritten until every rank has read them).  n_ranks = 1 is plain Adam. */
-int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, float beta1,
-                    float beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream);
+ * barriers (all gradients written before; none overwritten until every rank has read them).  n_ranks = 1 is plain Adam.
+ * The betas are doubles so that 1 - beta^step and 1 - beta are formed from the caller's values as torch.optim.Adam forms
+ * them (an fp32 0.999 puts 1 - 0.999^step ~1.3e-5 off); they reach the update as fp32, as torch's kernels receive them. */
+int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, double beta1,
+                    double beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream);
 
 /* ---- the learner: rsl_rl PPO.update() for the Drift-family actor-critic, trained in the act-step blob in place -------
  * rsl_rl PPO.update() (modified_rsl_rl_runner.py:118; rsl-rl-lib >= 2.3.0) [UPSTREAM-RECALL] on the network wl_act_step

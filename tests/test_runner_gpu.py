@@ -87,7 +87,10 @@ def _slab(T, N, case, it, g):
 
 CASES = [(1, 1, "random"), (1, 33, "random"), (1, 4096, "random"), (128, 1, "random"), (128, 33, "random"), (128, 4096, "random"),
          (128, 33, "none"), (128, 4096, "exactly_100"), (128, 4096, "burst"), (1, 4096, "burst"), (128, 33, "sparse"),
-         (128, 4096, "sparse"), (128, 4096, "t0"), (128, 33, "both"), (128, 4096, "both"), (7, 1000, "random")]
+         (128, 4096, "sparse"), (128, 4096, "t0"), (128, 33, "both"), (128, 4096, "both"), (7, 1000, "random"),
+         # T > 1024 runs the ring kernel's 1024-step loop more than once (4096 = WL_EP_MAX_T); N = 1057 has 34 done words
+         # per row, neither a multiple of 32 nor one chunk
+         (17, 1057, "random"), (1025, 1057, "random"), (4096, 33, "random"), (4096, 1057, "both"), (128, 1057, "burst")]
 
 
 @pytest.mark.parametrize("T,N,case", CASES)

@@ -141,7 +141,7 @@ class WlEpisodeStatsState(C.Structure):
 lib.wl_episode_stats_workspace_bytes.restype = _sz
 lib.wl_episode_stats_workspace_bytes.argtypes = [_i32, _i32]
 lib.wl_episode_stats.argtypes = [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]
-lib.wl_dp_adam_step.argtypes = [_vp, _vp, _vp, _i32, C.POINTER(_vp), C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _i32, _i32, _vp]
+lib.wl_dp_adam_step.argtypes = [_vp, _vp, _vp, _i32, C.POINTER(_vp), C.c_float, C.c_double, C.c_double, C.c_float, C.c_float, _i32, _i32, _vp]
 
 
 class WlPpoParams(C.Structure):

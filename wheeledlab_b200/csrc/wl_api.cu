@@ -1554,14 +1554,15 @@ __device__ __forceinline__ void adam_update(float* param, float* m, float* v, in
     param[i] = p - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
 }
 __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__ m, float* __restrict__ v, const __grid_constant__ GradPeers gp,
-                                  float lr, float beta1, float beta2, float eps, float weight_decay, float bc1, float bc2, int n) {
+                                  float lr, float beta1, float cb1, float beta2, float cb2, float eps, float weight_decay, float bc1,
+                                  float bc2, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     float g = 0.0f;
     for (int r = 0; r < gp.n; ++r) g += __ldcg(gp.g[r] + i);           // (L2-coherent loads: peers have just written)
     g = g / (float)gp.n;
     if (weight_decay != 0.0f) g = fmaf(weight_decay, param[i], g);
-    adam_update(param, m, v, i, g, lr, beta1, 1.0f - beta1, beta2, 1.0f - beta2, eps, bc1, bc2);
+    adam_update(param, m, v, i, g, lr, beta1, cb1, beta2, cb2, eps, bc1, bc2);
 }
 
 #include "wl_ppo.cuh"
@@ -2430,15 +2431,18 @@ int wl_episode_stats(const float* d_rewards, const uint8_t* d_terminated, const 
     return cuda_check(cudaGetLastError(), "wl_episode_ring_kernel");
 }
 
-int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, float beta1,
-                    float beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream) {
+int wl_dp_adam_step(float* d_param, float* d_m, float* d_v, int32_t n_ranks, const float* const* d_grads, float lr, double beta1,
+                    double beta2, float eps, float weight_decay, int32_t step, int32_t n, void* stream) {
     if (!d_param || !d_m || !d_v || !d_grads || n_ranks < 1 || n_ranks > WL_MAX_PEERS || n < 1 || step < 1)
         return fail(WL_EINVAL, "wl_dp_adam_step: bad argument");
     GradPeers gp; memset(&gp, 0, sizeof gp);
     gp.n = n_ranks;
     for (int r = 0; r < n_ranks; ++r) { if (!d_grads[r]) return fail(WL_EINVAL, "wl_dp_adam_step: null gradient pointer"); gp.g[r] = d_grads[r]; }
-    const float bc1 = 1.0f - powf(beta1, (float)step), bc2 = 1.0f - powf(beta2, (float)step);
-    wl_dp_adam_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(d_param, d_m, d_v, gp, lr, beta1, beta2, eps, weight_decay, bc1, bc2, n);
+    // torch forms 1 - beta^t and 1 - beta from the Python (double) betas, as wl_ppo_step_kernel does; in fp32, 0.999f exceeds
+    // 0.999 by 1.3e-8 and 1 - 0.999f^t is ~1.3e-5 off for the first thousand steps
+    const float bc1 = (float)(1.0 - pow(beta1, (double)step)), bc2 = (float)(1.0 - pow(beta2, (double)step));
+    wl_dp_adam_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(d_param, d_m, d_v, gp, lr, (float)beta1, (float)(1.0 - beta1),
+                                                                         (float)beta2, (float)(1.0 - beta2), eps, weight_decay, bc1, bc2, n);
     return cuda_check(cudaGetLastError(), "wl_dp_adam_kernel");
 }
 

@@ -24,11 +24,30 @@ from ._lib import WlEpisodeStatsState, WlError, WlPpoBatch, WlPpoParams, check, 
 
 def compute_returns(rewards: torch.Tensor, values: torch.Tensor, last_values: torch.Tensor, dones: torch.Tensor,
                     gamma: float, lam: float, time_outs: torch.Tensor | None = None):
-    """rewards/values [T,N] f32, last_values [N] f32, dones/time_outs [T,N] u8|bool (CUDA, contiguous) -> (returns, advantages)."""
+    """rewards/values [T,N] f32, last_values [N] f32, dones/time_outs [T,N] u8|bool (CUDA, contiguous) -> (returns, advantages).
+    Every tensor is checked before the launch (the kernel reads raw pointers: a wrong dtype is misread, a short or host
+    tensor is read out of bounds); ``time_outs=None`` is the same as all-zero time-outs."""
+    if rewards.dim() != 2:
+        raise ValueError(f"compute_returns: rewards must be [T, N], not {tuple(rewards.shape)}")
     T, N = rewards.shape
-    for x in (rewards, values, last_values, dones):
+    named = [("rewards", rewards, (T, N)), ("values", values, (T, N)), ("last_values", last_values, (N,)), ("dones", dones, (T, N))]
+    if time_outs is not None:
+        named.append(("time_outs", time_outs, (T, N)))
+    for name, x, _ in named:
+        flag = name in ("dones", "time_outs")
+        if flag and x.dtype not in (torch.uint8, torch.bool):
+            raise ValueError(f"compute_returns: {name} must be uint8 or bool, not {x.dtype}")
+        if not flag and x.dtype != torch.float32:
+            raise ValueError(f"compute_returns: {name} must be float32, not {x.dtype}")
+    for name, x, shape in named:
+        if tuple(x.shape) != shape:
+            raise ValueError(f"compute_returns: {name} must have shape {list(shape)}, not {list(x.shape)}")
+    for name, x, _ in named:
+        if x.device != rewards.device:
+            raise ValueError(f"compute_returns: {name} is on {x.device}, rewards on {rewards.device}")
+    for name, x, _ in named:
         if not (x.is_cuda and x.is_contiguous()):
-            raise ValueError("compute_returns expects contiguous CUDA tensors")
+            raise ValueError(f"compute_returns: {name} must be a contiguous CUDA tensor")
     d8 = dones.view(torch.uint8) if dones.dtype == torch.bool else dones
     t8 = None if time_outs is None else (time_outs.view(torch.uint8) if time_outs.dtype == torch.bool else time_outs)
     ret, adv = torch.empty_like(rewards), torch.empty_like(rewards)
@@ -75,6 +94,11 @@ class EpisodeStatistics:
 
     def update(self, rewards: torch.Tensor, terminated: torch.Tensor, truncated: torch.Tensor):
         """rewards [T, N] f32, terminated / truncated [T, N] u8|bool (the rollout slab's fields)."""
+        if rewards.dtype != torch.float32:
+            raise ValueError(f"EpisodeStatistics.update: rewards must be float32, not {rewards.dtype}")
+        for x in (terminated, truncated):
+            if x.dtype not in (torch.uint8, torch.bool):
+                raise ValueError(f"EpisodeStatistics.update: terminated / truncated must be uint8 or bool, not {x.dtype}")
         for x in (rewards, terminated, truncated):
             if not (x.is_cuda and x.is_contiguous()) or tuple(x.shape) != (self.T, self.num_envs):
                 raise ValueError(f"EpisodeStatistics.update expects contiguous [{self.T}, {self.num_envs}] CUDA tensors")
@@ -97,7 +121,12 @@ class DataParallelAdam:
     fused into the update kernel (``wl_dp_adam_step``): parameters and gradients live in flat buffers (``p.data`` / ``p.grad``
     are views), the flat gradient sits in torch symmetric memory so every rank reads its peers' gradients over NVLink inside
     the update kernel -- one launch per optimiser step, no NCCL call.  world_size 1 (or no process group) is plain fused Adam.
-    Matches ``torch.optim.Adam`` (amsgrad off, decoupled weight decay off) on the rank-averaged gradient."""
+    Matches ``torch.optim.Adam`` (amsgrad off, decoupled weight decay off) on the rank-averaged gradient.
+
+    ``Module.zero_grad()`` (``set_to_none=True`` by default) drops the seated views, and the next backward writes a fresh
+    ``p.grad``.  ``step()`` notices a gradient that is no longer its view of the flat buffer (another storage or shape),
+    copies it into the flat buffer and seats the view again, so the update always uses the gradient ``p.grad`` holds; a
+    parameter whose ``p.grad`` is None is refused (``torch.optim.Adam`` would skip it, the fused update cannot)."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, group=None):
         import torch.distributed as dist
@@ -123,18 +152,32 @@ class DataParallelAdam:
         self.m = torch.zeros(n, dtype=torch.float32, device=dev)
         self.v = torch.zeros(n, dtype=torch.float32, device=dev)
         off = 0
+        self._grad_views = []
         with torch.no_grad():
             for p in self.params:                          # re-seat parameters and gradients as views of the flat buffers
                 k = p.numel()
                 self.flat_p[off:off + k].copy_(p.detach().reshape(-1))
                 p.data = self.flat_p[off:off + k].view_as(p)
                 p.grad = self.flat_g[off:off + k].view_as(p)
+                self._grad_views.append(p.grad)
                 off += k
 
     def zero_grad(self):
         self.flat_g.zero_()
 
+    def _gather_detached_grads(self):
+        """Copy every gradient that is not (any more) the seated view into the flat buffer and seat the view again."""
+        with torch.no_grad():
+            for i, (p, view) in enumerate(zip(self.params, self._grad_views)):
+                g = p.grad
+                if g is None:
+                    raise ValueError(f"DataParallelAdam.step: parameter {i} has no gradient (p.grad is None)")
+                if g.data_ptr() != view.data_ptr() or g.shape != view.shape:
+                    view.copy_(g)
+                    p.grad = view
+
     def step(self):
+        self._gather_detached_grads()
         self.t += 1
         stream = C.c_void_p(torch.cuda.current_stream(self.flat_p.device).cuda_stream)
         if self.handle is not None:
