@@ -654,6 +654,30 @@ size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_m
 int wl_ppo_update_wide(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
                        float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the data-parallel PPO update: rsl_rl's multi-GPU PPO.update() [UPSTREAM-RECALL] ------------------------------------
+ * n_ranks replicas of the update above (activation WL_ACTIVATION_ELU: wl_ppo_update's network; WL_ACTIVATION_RELU:
+ * wl_ppo_update_wide's), each on its own rows, with the gradient and the KL averaged across the ranks inside every
+ * mini-batch: each rank's reduced gradient (entropy term included) and kl_mean are summed in rank order 0..n_ranks-1 and
+ * divided by n_ranks, then the KL rule, clip_grad_norm_ and Adam run on the average, so every replica forms the same bits.
+ * Rank-local as in the single-rank update: advantage normalisation, the permutation, the loss statistics in d_state.
+ * d_exchange[r] (r < n_ranks, 256-byte aligned) = rank r's exchange buffer of wl_ppo_dp_exchange_bytes(obs_dim) bytes, the
+ * same rank order on every rank: this process's own buffers and the P2P-mapped buffers of its peers (e.g. one torch
+ * symmetric-memory allocation), zero-filled once before the first call and left to the calls afterwards.  The call runs
+ * n_local ranks, local_ranks[l] being the rank of the l-th entry of the per-rank arrays (batches, d_blob, d_adam_m,
+ * d_adam_v, d_state, d_workspace: wl_ppo_update's arguments, one per local rank; workspace_bytes as wl_ppo_workspace_bytes /
+ * wl_ppo_wide_workspace_bytes); their exchange buffers must be on one device.  One local rank per process is the
+ * multi-process form; all ranks local (one device, one stream) runs the whole exchange in one process.  Each mini-batch
+ * waits on the device for every peer's row (no host sync, graph-capturable: the round counter lives in the buffers); a
+ * wait that exceeds 60 s sets word 1 of the rank's own buffer (uint32, nonzero = failed), after which the call leaves
+ * blob, moments and d_state untouched.  n_ranks = 1 gives wl_ppo_update / wl_ppo_update_wide's results bit for bit.
+ * Bad arguments (n_ranks outside 1..WL_MAX_PEERS, a null or misaligned exchange buffer, a local rank index out of range or
+ * repeated, local buffers on different devices, and every argument error of the single-rank entries) return WL_EINVAL
+ * before any launch. */
+size_t wl_ppo_dp_exchange_bytes(int32_t obs_dim);
+int wl_ppo_update_dp(const wl_ppo_params* params, int32_t activation, int32_t n_ranks, void* const* d_exchange, int32_t n_local,
+                     const int32_t* local_ranks, const wl_ppo_batch* batches, float* const* d_blob, float* const* d_adam_m,
+                     float* const* d_adam_v, float* const* d_state, void* const* d_workspace, size_t workspace_bytes, void* stream);
+
 /* A caller that drives wl_step through a CUDA graph of K steps (how a rollout is meant to be issued: one launch per K steps)
  * pays the upload of the instantiated graph to the device on its FIRST launch; this moves that
  * upload to set-up time.  graph_exec = cudaGraphExec_t (torch: CUDAGraph.raw_cuda_graph_exec()). */

@@ -8,6 +8,9 @@ episodes, once there is one), the episodes finished in the iteration, the learni
 seed, agent cfg; what ``tools/play_policy.py -p LOG_DIR`` reads); ``--resume PATH`` continues from one.
 
     python tools/ppo_train.py [--task elevation|visual] --envs 4096 --iters 50 [--log-dir DIR] [--resume DIR/models/model_25.pt] [--out log.txt]
+
+Under ``torchrun --nproc-per-node=R`` it trains data-parallel (rsl_rl's multi-GPU PPO, DESIGN 6j): ``--envs`` per rank, rank r
+simulating envs r * envs .. (r + 1) * envs - 1 of one big run on cuda:LOCAL_RANK; only rank 0 prints and writes.
 """
 from __future__ import annotations
 
@@ -38,26 +41,29 @@ def main():
     import wheeledlab_b200 as wl
     from wheeledlab_b200.learner import FusedOnPolicyRunner
     from wheeledlab_b200.runs import agent_cfg, save_run_config
-    dev = "cuda:0"
+    import os
+    rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
+    dev = f"cuda:{int(os.environ.get('LOCAL_RANK', '0'))}"
     torch.manual_seed(a.seed)
     task_id, activation, name = TASKS[a.task]
-    env = wl.make(task_id, device=dev, num_envs=a.envs, seed=a.seed)
+    env = wl.make(task_id, device=dev, num_envs=a.envs, seed=a.seed, env_id_offset=rank * a.envs)
     agent = agent_cfg(activation, a.steps, a.save_interval)
     runner = FusedOnPolicyRunner(env, agent, log_dir=a.log_dir, device=dev)
-    if a.log_dir:
+    if a.log_dir and rank == 0:
         save_run_config(a.log_dir, task_id, a.envs, a.seed, agent)
-    head = (f"# {name} PPO (obs_dim {env.sim.obs_dim}, {activation}), {a.envs} envs x {a.steps} steps, rsl_rl agent cfg, seed {a.seed}, "
-            f"one graph per iteration, {torch.cuda.get_device_name(0)}")
+    head = (f"# {name} PPO (obs_dim {env.sim.obs_dim}, {activation}), {a.envs} envs x {a.steps} steps" + (f" x {world} ranks" if world > 1 else "")
+            + f", rsl_rl agent cfg, seed {a.seed}, one graph per iteration, {torch.cuda.get_device_name(dev)}")
     if a.resume:
         runner.load(a.resume)
         env.common_step_counter = runner.current_learning_iteration * a.steps     # continue the curriculum where it was
         head += f"; resumed from {Path(a.resume).name} at iteration {runner.current_learning_iteration}"
     lines = [head, "iter  Train/mean_reward  Train/mean_episode_length  finished  learning_rate  value_loss  surrogate  entropy  ms"]
-    print(lines[0]); print(lines[1])
+    if rank == 0:
+        print(lines[0]); print(lines[1])
 
     def log(it, s):
         mr, ml = s.get("Train/mean_reward", float("nan")), s.get("Train/mean_episode_length", float("nan"))
-        ms = a.steps * a.envs / s["Perf/total_fps"] * 1e3
+        ms = a.steps * a.envs * world / s["Perf/total_fps"] * 1e3
         line = (f"{it:4d}  {mr:17.4f}  {ml:25.2f}  {s['Episodes/finished']:8d}  {s['Loss/learning_rate']:13.3e}  "
                 f"{s['Loss/value_function']:10.4f}  {s['Loss/surrogate']:9.4f}  {s['Loss/entropy']:7.4f}  {ms:6.2f}")
         print(line, flush=True)
@@ -65,7 +71,7 @@ def main():
 
     runner.callback = log
     runner.learn(a.iters)
-    if a.out:
+    if a.out and rank == 0:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text("\n".join(lines) + "\n")
 

@@ -2455,6 +2455,8 @@ static size_t ppo_grad_smem(int obs_dim) {
 
 // workspace of wl_ppo_update: [reduced row][fp64 block sums of squares][one gradient row per CTA], each 256-byte aligned
 struct PpoWorkspace { int blob_floats, rowlen, ctas, norm_parts; size_t norm_off, rows_off, bytes; };
+// (wl_ppo_update_wide's: wl_ppo_update's, then H1 and dZ1 of a mini-batch)
+struct PpoWideWorkspace { PpoWorkspace w; size_t h1_off, dz_off, bytes; };
 static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_batches, int sms, PpoWorkspace& w) {
     int32_t off[13];
     w.blob_floats = policy_offsets(obs_dim, off);
@@ -2493,26 +2495,79 @@ size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_b
     return ppo_workspace("wl_ppo_workspace_bytes", obs_dim, batch, num_mini_batches, w) ? 0 : w.bytes;
 }
 
+// the host-side checks of one rank's arguments to a PPO update entry (fn names the entry in the message)
+static int ppo_check_args(const char* fn, const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_blob, const float* d_adam_m,
+                          const float* d_adam_v, const float* d_state, const void* d_workspace) {
+    if (!p || !b) return fail(WL_EINVAL, std::string(fn) + ": null params / batch");
+    if (!b->obs || !b->actions || !b->values || !b->log_prob || !b->mean || !b->returns || !b->advantages || !b->perm)
+        return fail(WL_EINVAL, std::string(fn) + ": null array in batch");
+    if (!d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
+        return fail(WL_EINVAL, std::string(fn) + ": null d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
+    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, std::string(fn) + ": num_learning_epochs must be >= 1");
+    return WL_OK;
+}
+
+static int ppo_wide_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWideWorkspace& x);
+
+// the workspace layout of the update (narrow: wl_ppo_update's, wide: wl_ppo_update_wide's) and the checks against it
+static int ppo_check_layout(const char* fn, bool wide, const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_blob,
+                            const float* d_adam_m, const float* d_adam_v, const void* d_workspace, size_t workspace_bytes,
+                            PpoWideWorkspace& x) {
+    if (wide) {
+        if (int rc = ppo_wide_workspace(fn, p->obs_dim, p->batch, p->num_mini_batches, x)) return rc;
+    } else {
+        if (int rc = ppo_workspace(fn, p->obs_dim, p->batch, p->num_mini_batches, x.w)) return rc;
+        x.bytes = x.w.bytes;
+    }
+    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
+    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
+    if (workspace_bytes < x.bytes)
+        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (" + (wide ? "wl_ppo_wide_workspace_bytes" : "wl_ppo_workspace_bytes") +
+                                   " gives " + std::to_string(x.bytes) + ")");
+    return WL_OK;
+}
+
+static size_t ppo_grad_smem(int obs_dim);
+static size_t ppo_wide_grad_smem();
+static size_t ppo_wide_dw1_smem();
+
+// The gradient phase of one mini-batch (a.row0): one gradient row per CTA in the workspace.  Narrow: wl_ppo_grad_kernel;
+// wide: the gathered layer-1 forward, the layers 2-3 gradient kernel and the split-K dW1.
+static void ppo_grad_phase(bool wide, const PpoWideWorkspace& x, const PolicyOffsets& po, const PolicyOffsets& pc, const PpoArgs& a,
+                           const float* d_blob, const float* d_state, char* ws, cudaStream_t cs) {
+    const PpoWorkspace& w = x.w;
+    float* rows = (float*)(ws + w.rows_off);
+    if (!wide) {
+        wl_ppo_grad_kernel<<<w.ctas, WL_PPO_THREADS, ppo_grad_smem(a.obs_dim), cs>>>(d_blob, w.blob_floats, po, a, d_state, rows, w.rowlen);
+        return;
+    }
+    float* H1 = (float*)(ws + x.h1_off);
+    float* dZ1 = (float*)(ws + x.dz_off);
+    const dim3 dw1_grid((unsigned)((a.obs_dim + WL_DW1_K - 1) / WL_DW1_K), (unsigned)w.ctas);
+    wl_ppo_wide_fwd_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE, cs>>>(d_blob, po, a, H1);
+    wl_ppo_wide_grad_kernel<<<w.ctas, WL_PPO_THREADS, ppo_wide_grad_smem(), cs>>>(d_blob, w.blob_floats, po, pc, a, d_state, H1, dZ1,
+                                                                                 rows, w.rowlen);
+    wl_ppo_wide_dw1_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
+}
+
+// the per-mini-batch arguments of every update entry
+static void ppo_launch_args(const wl_ppo_params* p, const wl_ppo_batch* b, PpoArgs& a, PpoStepArgs& sa) {
+    const int B = p->batch / p->num_mini_batches;
+    a.b = *b; a.obs_dim = p->obs_dim; a.B = B; a.tiles = (B + WL_PPO_TILE - 1) / WL_PPO_TILE;
+    a.clip = p->clip_param; a.vcoef = p->value_loss_coef; a.inv_B = 1.0f / (float)B; a.clipped_value = p->use_clipped_value_loss != 0;
+    sa = PpoStepArgs{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
+}
+
 int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
                   void* d_workspace, size_t workspace_bytes, void* stream) {
-    if (!p || !b) return fail(WL_EINVAL, "wl_ppo_update: null params / batch");
-    if (!b->obs || !b->actions || !b->values || !b->log_prob || !b->mean || !b->returns || !b->advantages || !b->perm)
-        return fail(WL_EINVAL, "wl_ppo_update: null array in batch");
-    if (!d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
-        return fail(WL_EINVAL, "wl_ppo_update: null d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
-    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, "wl_ppo_update: num_learning_epochs must be >= 1");
-    PpoWorkspace w;
-    if (int rc = ppo_workspace("wl_ppo_update", p->obs_dim, p->batch, p->num_mini_batches, w)) return rc;
-    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
-        return fail(WL_EINVAL, "wl_ppo_update: d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
-    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
-        return fail(WL_EINVAL, "wl_ppo_update: d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
-    if (workspace_bytes < w.bytes)
-        return fail(WL_EINVAL, "wl_ppo_update: workspace_bytes too small (wl_ppo_workspace_bytes gives " + std::to_string(w.bytes) + ")");
+    if (int rc = ppo_check_args("wl_ppo_update", p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
+    PpoWideWorkspace x;
+    if (int rc = ppo_check_layout("wl_ppo_update", false, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x)) return rc;
+    const PpoWorkspace& w = x.w;
     PolicyOffsets po;
     policy_offsets(p->obs_dim, po.o);
-    const int B = p->batch / p->num_mini_batches;
-    const size_t smem = ppo_grad_smem(p->obs_dim);
     cudaStream_t cs = (cudaStream_t)stream;
     char* ws = (char*)d_workspace;
     float* red = (float*)ws;
@@ -2521,18 +2576,17 @@ int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, 
     wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
     if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
     PpoArgs a;
-    a.b = *b; a.obs_dim = p->obs_dim; a.B = B; a.tiles = (B + WL_PPO_TILE - 1) / WL_PPO_TILE;
-    a.clip = p->clip_param; a.vcoef = p->value_loss_coef; a.inv_B = 1.0f / (float)B; a.clipped_value = p->use_clipped_value_loss != 0;
-    PpoStepArgs sa{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
+    PpoStepArgs sa;
+    ppo_launch_args(p, b, a, sa);
     for (int e = 0; e < p->num_learning_epochs; ++e) {
         for (int i = 0; i < p->num_mini_batches; ++i) {
-            a.row0 = (int64_t)i * B;
+            a.row0 = (int64_t)i * a.B;
             sa.update_index = e * p->num_mini_batches + i;
-            wl_ppo_grad_kernel<<<w.ctas, WL_PPO_THREADS, smem, cs>>>(d_blob, w.blob_floats, po, a, d_state, rows, w.rowlen);
+            ppo_grad_phase(false, x, po, po, a, d_blob, d_state, ws, cs);
             wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
                                                                p->entropy_coef, red, norm_part);
-            wl_ppo_step_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
-                                                                 w.blob_floats, po, p->obs_dim, sa);
+            wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                        w.blob_floats, po, p->obs_dim, sa, nullptr);
             if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel")) return rc;
         }
     }
@@ -2620,7 +2674,6 @@ int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d
 }
 
 // workspace of wl_ppo_update_wide: wl_ppo_update's, then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
-struct PpoWideWorkspace { PpoWorkspace w; size_t h1_off, dz_off, bytes; };
 static int ppo_wide_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWideWorkspace& x) {
     if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
     if (obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
@@ -2644,53 +2697,137 @@ size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_m
 
 int wl_ppo_update_wide(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
                        void* d_workspace, size_t workspace_bytes, void* stream) {
-    if (!p || !b) return fail(WL_EINVAL, "wl_ppo_update_wide: null params / batch");
-    if (!b->obs || !b->actions || !b->values || !b->log_prob || !b->mean || !b->returns || !b->advantages || !b->perm)
-        return fail(WL_EINVAL, "wl_ppo_update_wide: null array in batch");
-    if (!d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
-        return fail(WL_EINVAL, "wl_ppo_update_wide: null d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
-    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, "wl_ppo_update_wide: num_learning_epochs must be >= 1");
+    if (int rc = ppo_check_args("wl_ppo_update_wide", p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
     PpoWideWorkspace x;
-    if (int rc = ppo_wide_workspace("wl_ppo_update_wide", p->obs_dim, p->batch, p->num_mini_batches, x)) return rc;
+    if (int rc = ppo_check_layout("wl_ppo_update_wide", true, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x)) return rc;
     const PpoWorkspace& w = x.w;
-    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
-        return fail(WL_EINVAL, "wl_ppo_update_wide: d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
-    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
-        return fail(WL_EINVAL, "wl_ppo_update_wide: d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
-    if (workspace_bytes < x.bytes)
-        return fail(WL_EINVAL, "wl_ppo_update_wide: workspace_bytes too small (wl_ppo_wide_workspace_bytes gives " + std::to_string(x.bytes) + ")");
     PolicyOffsets po, pc;
     policy_offsets(p->obs_dim, po.o);
     wide_compact_offsets(po, w.blob_floats, pc);
-    const int B = p->batch / p->num_mini_batches;
     cudaStream_t cs = (cudaStream_t)stream;
     char* ws = (char*)d_workspace;
     float* red = (float*)ws;
     double* norm_part = (double*)(ws + w.norm_off);
     float* rows = (float*)(ws + w.rows_off);
-    float* H1 = (float*)(ws + x.h1_off);
-    float* dZ1 = (float*)(ws + x.dz_off);
     wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
     if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
     PpoArgs a;
-    a.b = *b; a.obs_dim = p->obs_dim; a.B = B; a.tiles = (B + WL_PPO_TILE - 1) / WL_PPO_TILE;
-    a.clip = p->clip_param; a.vcoef = p->value_loss_coef; a.inv_B = 1.0f / (float)B; a.clipped_value = p->use_clipped_value_loss != 0;
-    PpoStepArgs sa{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
-    const dim3 dw1_grid((unsigned)((p->obs_dim + WL_DW1_K - 1) / WL_DW1_K), (unsigned)w.ctas);
+    PpoStepArgs sa;
+    ppo_launch_args(p, b, a, sa);
     for (int e = 0; e < p->num_learning_epochs; ++e) {
         for (int i = 0; i < p->num_mini_batches; ++i) {
-            a.row0 = (int64_t)i * B;
+            a.row0 = (int64_t)i * a.B;
             sa.update_index = e * p->num_mini_batches + i;
-            wl_ppo_wide_fwd_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE, cs>>>(d_blob, po, a, H1);
-            wl_ppo_wide_grad_kernel<<<w.ctas, WL_PPO_THREADS, ppo_wide_grad_smem(), cs>>>(d_blob, w.blob_floats, po, pc, a, d_state, H1, dZ1,
-                                                                                         rows, w.rowlen);
-            wl_ppo_wide_dw1_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
+            ppo_grad_phase(true, x, po, pc, a, d_blob, d_state, ws, cs);
             wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
                                                                p->entropy_coef, red, norm_part);
-            wl_ppo_step_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
-                                                                 w.blob_floats, po, p->obs_dim, sa);
+            wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                        w.blob_floats, po, p->obs_dim, sa, nullptr);
             if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_update_wide kernels")) return rc;
         }
+    }
+    return WL_OK;
+}
+
+// ---- the data-parallel update (DESIGN 6j) ---------------------------------------------------------------------------
+static size_t ppo_dp_slot_bytes(int rowlen) { return align256(sizeof(float) * (size_t)rowlen); }
+
+size_t wl_ppo_dp_exchange_bytes(int32_t obs_dim) {
+    if (obs_dim < 1 || obs_dim > WL_WIDE_MAX_OBS) { fail(WL_EINVAL, "wl_ppo_dp_exchange_bytes: obs_dim must be in 1..4096"); return 0; }
+    int32_t off[13];
+    const int rowlen = (policy_offsets(obs_dim, off) + WL_PPO_STATS + 3) & ~3;
+    return WL_PPO_DP_HEADER + 2 * ppo_dp_slot_bytes(rowlen);
+}
+
+int wl_ppo_update_dp(const wl_ppo_params* p, int32_t activation, int32_t n_ranks, void* const* d_exchange, int32_t n_local,
+                     const int32_t* local_ranks, const wl_ppo_batch* batches, float* const* d_blob, float* const* d_adam_m,
+                     float* const* d_adam_v, float* const* d_state, void* const* d_workspace, size_t workspace_bytes, void* stream) {
+    static const char* fn = "wl_ppo_update_dp";
+    if (!p) return fail(WL_EINVAL, "wl_ppo_update_dp: null params");
+    if (activation != WL_ACTIVATION_ELU && activation != WL_ACTIVATION_RELU)
+        return fail(WL_EINVAL, "wl_ppo_update_dp: activation must be WL_ACTIVATION_ELU or WL_ACTIVATION_RELU");
+    if (n_ranks < 1 || n_ranks > WL_MAX_PEERS) return fail(WL_EINVAL, "wl_ppo_update_dp: n_ranks must be in 1..8 (WL_MAX_PEERS)");
+    if (!d_exchange) return fail(WL_EINVAL, "wl_ppo_update_dp: null d_exchange");
+    PpoExchange ex; memset(&ex, 0, sizeof ex);
+    ex.n = n_ranks;
+    for (int r = 0; r < n_ranks; ++r) {
+        if (!d_exchange[r] || ((uintptr_t)d_exchange[r] & 255u))
+            return fail(WL_EINVAL, "wl_ppo_update_dp: exchange buffer " + std::to_string(r) + " is null or not 256-byte aligned");
+        ex.buf[r] = (const char*)d_exchange[r];
+    }
+    if (n_local < 1 || n_local > n_ranks || !local_ranks) return fail(WL_EINVAL, "wl_ppo_update_dp: n_local must be in 1..n_ranks, local_ranks non-null");
+    bool seen[WL_MAX_PEERS] = {false};
+    for (int l = 0; l < n_local; ++l) {
+        const int r = local_ranks[l];
+        if (r < 0 || r >= n_ranks) return fail(WL_EINVAL, "wl_ppo_update_dp: local rank index " + std::to_string(r) + " out of 0..n_ranks-1");
+        if (seen[r]) return fail(WL_EINVAL, "wl_ppo_update_dp: local rank " + std::to_string(r) + " given twice");
+        seen[r] = true;
+    }
+    if (!batches || !d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
+        return fail(WL_EINVAL, "wl_ppo_update_dp: null per-rank array");
+    for (int l = 0; l < n_local; ++l)
+        if (int rc = ppo_check_args(fn, p, &batches[l], d_blob[l], d_adam_m[l], d_adam_v[l], d_state[l], d_workspace[l])) return rc;
+    if (activation == WL_ACTIVATION_ELU && p->obs_dim > 16)
+        return fail(WL_EUNSUPPORTED, "wl_ppo_update_dp: obs_dim > 16 (the network wl_act_step runs)");
+    // every local rank's exchange buffer on one device: the call runs them in one stream
+    int dev0 = -1;
+    for (int l = 0; l < n_local; ++l) {
+        cudaPointerAttributes pa;
+        if (cudaPointerGetAttributes(&pa, d_exchange[local_ranks[l]]) != cudaSuccess || pa.type != cudaMemoryTypeDevice) {
+            cudaGetLastError();
+            return fail(WL_EINVAL, "wl_ppo_update_dp: local exchange buffer " + std::to_string(local_ranks[l]) + " is not device memory");
+        }
+        if (l == 0) dev0 = pa.device;
+        else if (pa.device != dev0) return fail(WL_EINVAL, "wl_ppo_update_dp: local ranks' exchange buffers are on different devices");
+    }
+    const bool wide = activation == WL_ACTIVATION_RELU;
+    PpoWideWorkspace x;
+    for (int l = 0; l < n_local; ++l)
+        if (int rc = ppo_check_layout(fn, wide, p, &batches[l], d_blob[l], d_adam_m[l], d_adam_v[l], d_workspace[l], workspace_bytes, x)) return rc;
+    const PpoWorkspace& w = x.w;
+    PolicyOffsets po, pc;
+    policy_offsets(p->obs_dim, po.o);
+    if (wide) wide_compact_offsets(po, w.blob_floats, pc);
+    else pc = po;
+    cudaStream_t cs = (cudaStream_t)stream;
+    const size_t slot = ppo_dp_slot_bytes(w.rowlen);
+    for (int l = 0; l < n_local; ++l)
+        wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(batches[l].advantages, p->batch, d_blob[l], po.o[12], d_state[l]);
+    if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
+    PpoArgs a;
+    PpoStepArgs sa;
+    ppo_launch_args(p, &batches[0], a, sa);
+    const int K = p->num_learning_epochs * p->num_mini_batches;
+    for (int k = 0; k < K; ++k) {
+        const size_t slot_off = WL_PPO_DP_HEADER + (size_t)(k & 1) * slot;
+        a.row0 = (int64_t)(k % p->num_mini_batches) * a.B;
+        sa.update_index = k;
+        // every local rank publishes before any waits: in the one-process form the waits never spin
+        for (int l = 0; l < n_local; ++l) {
+            char* ws = (char*)d_workspace[l];
+            char* own = (char*)d_exchange[local_ranks[l]];
+            a.b = batches[l];
+            ppo_grad_phase(wide, x, po, pc, a, d_blob[l], d_state[l], ws, cs);
+            wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>((const float*)(ws + w.rows_off), w.ctas, w.rowlen, w.blob_floats, po,
+                                                               p->obs_dim, d_blob[l], p->entropy_coef, (float*)(own + slot_off),
+                                                               (double*)(ws + w.norm_off));
+            wl_ppo_dp_publish_kernel<<<1, 1, 0, cs>>>((uint32_t*)own);
+        }
+        for (int l = 0; l < n_local; ++l) {
+            char* ws = (char*)d_workspace[l];
+            uint32_t* own = (uint32_t*)d_exchange[local_ranks[l]];
+            wl_ppo_dp_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(ex, own, slot_off, w.rowlen, w.blob_floats, po, p->obs_dim, a.inv_B,
+                                                                  (float*)ws, (double*)(ws + w.norm_off));
+            wl_ppo_step_kernel<true><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob[l], d_adam_m[l], d_adam_v[l], d_state[l], (const float*)ws,
+                                                                       (const double*)(ws + w.norm_off), w.norm_parts, w.blob_floats, po,
+                                                                       p->obs_dim, sa, own + 1);
+        }
+        if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_update_dp kernels")) return rc;
+    }
+    if (K & 1) {       // the no-row round: the next call starts on slot 0 again (see wl_ppo.cuh)
+        for (int l = 0; l < n_local; ++l) wl_ppo_dp_publish_kernel<<<1, 1, 0, cs>>>((uint32_t*)d_exchange[local_ranks[l]]);
+        for (int l = 0; l < n_local; ++l) wl_ppo_dp_wait_kernel<<<1, 1, 0, cs>>>(ex, (uint32_t*)d_exchange[local_ranks[l]]);
+        if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_dp_wait_kernel")) return rc;
     }
     return WL_OK;
 }

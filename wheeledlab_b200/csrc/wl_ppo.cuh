@@ -283,18 +283,24 @@ struct PpoStepArgs {
 };
 
 // One CTA: global norm -> clip coefficient, KL -> learning rate (before this step, as rsl_rl), statistics, then Adam on every
-// parameter of the blob in place (padding entries are never touched).
+// parameter of the blob in place (padding entries are never touched).  DP: `red` is the row wl_ppo_dp_reduce_kernel wrote,
+// whose KL column already holds the mean over the ranks of each rank's kl_mean; a nonzero exchange error word (a peer wait
+// that timed out) leaves everything untouched.
+template <bool DP>
 __global__ void __launch_bounds__(WL_PPO_FIN_THREADS)
 wl_ppo_step_kernel(float* __restrict__ blob, float* __restrict__ m, float* __restrict__ v, float* __restrict__ state,
                    const float* __restrict__ red, const double* __restrict__ norm_part, int nparts, int blob_floats,
-                   PolicyOffsets po, int obs_dim, PpoStepArgs a) {
+                   PolicyOffsets po, int obs_dim, PpoStepArgs a, const uint32_t* __restrict__ dp_error) {
+    if constexpr (DP) {
+        if (*(const volatile uint32_t*)dp_error) return;
+    }
     __shared__ float s_coef, s_lr, s_bc1, s_bc2;
     if (threadIdx.x == 0) {
         double n2 = 0.0;
         for (int i = 0; i < nparts; ++i) n2 += norm_part[i];
         const float norm = (float)sqrt(n2);
         const float coef = fminf(a.max_grad_norm / (norm + 1e-6f), 1.0f);         // clip_grad_norm_: always applied
-        const float kl = red[blob_floats + 2] * a.inv_B;
+        const float kl = DP ? red[blob_floats + 2] : red[blob_floats + 2] * a.inv_B;
         float lr = state[0];
         if (a.adaptive) {
             if (kl > a.desired_kl * 2.0f) lr = fmaxf(1e-5f, lr / 1.5f);
@@ -349,4 +355,100 @@ wl_ppo_begin_kernel(const float* __restrict__ adv, int n, const float* __restric
         state[5] = (float)sqrt(n > 1 ? sh[0] / (n - 1) : 0.0);
         state[6] = 0.0f; state[7] = 0.0f; state[8] = 0.0f; state[9] = 0.0f;
     }
+}
+
+// ---- data-parallel update (DESIGN 6j): every rank's reduced row averaged across ranks inside each mini-batch ----------
+// Each rank owns an exchange buffer, symmetric across ranks (same layout, P2P-mapped or on one device): a 256-byte header
+// (word 0: the rank's epoch, the number of rows it has published; word 1: its error word) and two slots of one reduced row
+// each, mini-batch parity.  Per mini-batch: wl_ppo_reduce_kernel writes the rank's own reduced row into slot (k & 1) of its
+// buffer, wl_ppo_dp_publish_kernel bumps the epoch, wl_ppo_dp_reduce_kernel waits for every rank's epoch to reach its own
+// and averages the R slots into the rank's workspace row, and wl_ppo_step_kernel<true> steps on that average.
+//
+// Why two slots and one flag per mini-batch are enough: a rank overwrites its slot of mini-batch k + 2 (wl_ppo_reduce_kernel
+// of k + 2) only after its DP reduce of k + 1 has passed the wait, i.e. after every peer published k + 1.  A peer publishes
+// k + 1 after its reduce of k + 1, which its stream runs after its DP reduce of k -- its last read of anyone's slot of k.
+// So nobody still reads the slot being overwritten.  This needs the parity to alternate across calls as well: a call with
+// an odd number of mini-batches ends with one more publish / wait round that carries no row (wl_ppo_dp_wait_kernel).
+#define WL_PPO_DP_HEADER 256
+#define WL_PPO_DP_TIMEOUT_NS 60000000000ull       // 60 s: far beyond any rank skew of a healthy run (a checkpoint write included)
+
+struct PpoExchange { int32_t n; int32_t pad; const char* buf[WL_MAX_PEERS]; };
+
+__device__ __forceinline__ uint32_t ppo_ld_acquire_sys(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint64_t ppo_globaltimer() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// One thread: bump this rank's epoch, a release store at system scope.  The reduce kernel before it on the stream wrote the
+// slot; the fence makes those writes visible system-wide before the flag that a peer acquires over NVLink.
+__global__ void wl_ppo_dp_publish_kernel(uint32_t* __restrict__ own) {
+    const uint32_t e = *(volatile uint32_t*)own + 1u;
+    __threadfence_system();
+    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(own), "r"(e) : "memory");
+}
+
+// Wait until every rank's epoch has reached this rank's own (acquire loads at system scope), bounded by %globaltimer: on
+// timeout, or if an earlier wait timed out, the rank's error word is set and false returned (no trap: the step kernel then
+// skips, the host raises when it reads the error word back).
+__device__ bool ppo_dp_wait(const PpoExchange& ex, uint32_t* own) {
+    volatile uint32_t* err = own + 1;
+    if (*err) return false;
+    const uint32_t target = *(volatile uint32_t*)own;
+    const uint64_t t0 = ppo_globaltimer();
+    for (int r = 0; r < ex.n; ++r) {
+        const uint32_t* e = reinterpret_cast<const uint32_t*>(ex.buf[r]);
+        while ((int32_t)(ppo_ld_acquire_sys(e) - target) < 0) {
+            if (ppo_globaltimer() - t0 > WL_PPO_DP_TIMEOUT_NS) { *err = 1u; __threadfence_system(); return false; }
+            __nanosleep(256);
+        }
+    }
+    return true;
+}
+
+// The no-row round that keeps the slot parity alternating across calls with an odd number of mini-batches.
+__global__ void wl_ppo_dp_wait_kernel(const __grid_constant__ PpoExchange ex, uint32_t* __restrict__ own) { ppo_dp_wait(ex, own); }
+
+// One CTA per 256 columns, as wl_ppo_reduce_kernel: column c of `red` = (sum over ranks 0..R-1 of slot c) / R for the
+// parameters, in rank order on every rank (so every replica forms the same bits); the fp64 sum of squares of the averaged
+// parameter columns per block (tree in thread order); the KL column = (sum_r kl_mean_r) / R with kl_mean_r = slot_r[KL] *
+// inv_B; the surrogate / value-loss columns stay this rank's own (rsl_rl reduces neither).
+__global__ void __launch_bounds__(256)
+wl_ppo_dp_reduce_kernel(const __grid_constant__ PpoExchange ex, uint32_t* __restrict__ own, size_t slot_off, int rowlen,
+                        int blob_floats, PolicyOffsets po, int obs_dim, float inv_B, float* __restrict__ red,
+                        double* __restrict__ norm_part) {
+    __shared__ double sq[256];
+    __shared__ int s_ok;
+    if (threadIdx.x == 0) {
+        s_ok = ppo_dp_wait(ex, own);
+        __threadfence_system();
+    }
+    __syncthreads();
+    if (!s_ok) return;
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    const bool param = c < blob_floats && ppo_is_param(c, po, obs_dim);
+    const float rn = (float)ex.n;
+    float g = 0.0f;
+    if (param) {
+        for (int r = 0; r < ex.n; ++r) g += __ldcg(reinterpret_cast<const float*>(ex.buf[r] + slot_off) + c);
+        g = g / rn;
+    } else if (c == blob_floats + 2) {
+        for (int r = 0; r < ex.n; ++r) g += __ldcg(reinterpret_cast<const float*>(ex.buf[r] + slot_off) + c) * inv_B;
+        g = g / rn;
+    } else if (c >= blob_floats && c < blob_floats + WL_PPO_STATS) {
+        g = reinterpret_cast<const float*>(reinterpret_cast<const char*>(own) + slot_off)[c];
+    }
+    if (c < rowlen) red[c] = g;
+    sq[threadIdx.x] = param ? (double)g * (double)g : 0.0;
+    __syncthreads();
+    for (int s = 128; s > 0; s >>= 1) {
+        if (threadIdx.x < s) sq[threadIdx.x] += sq[threadIdx.x + s];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) norm_part[blockIdx.x] = sq[0];
 }

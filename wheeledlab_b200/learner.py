@@ -19,7 +19,7 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import WlEpisodeStatsState, WlError, WlPpoBatch, WlPpoParams, check, lib
+from ._lib import WL_ACTIVATION, WlEpisodeStatsState, WlError, WlPpoBatch, WlPpoParams, check, lib
 
 
 def compute_returns(rewards: torch.Tensor, values: torch.Tensor, last_values: torch.Tensor, dones: torch.Tensor,
@@ -231,15 +231,21 @@ class FusedPPO:
     Owns the Adam moments, the device state (learning rate, Adam step, statistics) and the workspace.  Nothing syncs the
     host, so with an explicit ``perm`` tensor refilled in place the update can be captured into the same CUDA graph as the
     rollout.  The network is [64, 64] actor and critic with a learned std: activation "elu" is the Drift family's
-    (obs_dim <= 16, ``wl_ppo_update``), "relu" the Elevation / Visual one (obs_dim <= 4096, ``wl_ppo_update_wide``)."""
+    (obs_dim <= 16, ``wl_ppo_update``), "relu" the Elevation / Visual one (obs_dim <= 4096, ``wl_ppo_update_wide``).
 
-    def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None, activation: str = "elu"):
+    With an ``exchange`` (``PPOExchange``) the update is rsl_rl's multi-GPU one (``wl_ppo_update_dp``, DESIGN 6j): this
+    replica is rank ``exchange.rank`` of ``exchange.n_ranks``, and the gradient and KL are averaged across the ranks inside
+    every mini-batch.  ``update_local_ranks`` runs several replicas of one process together."""
+
+    def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None, activation: str = "elu",
+                 exchange: "PPOExchange | None" = None):
         from .policy import check_activation
         if cfg is None:
             cfg = PPOConfig()
         if cfg.schedule not in ("adaptive", "fixed"):
             raise ValueError(f"schedule must be 'adaptive' or 'fixed', not {cfg.schedule!r}")
         self.blob, self.obs_dim, self.cfg, self.device = blob, obs_dim, cfg, blob.device
+        self.exchange = exchange
         self.activation = check_activation(activation)
         wide = self.activation == "relu"
         self._ws_query = lib.wl_ppo_wide_workspace_bytes if wide else lib.wl_ppo_workspace_bytes
@@ -260,11 +266,8 @@ class FusedPPO:
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
         return self.workspace
 
-    def update(self, slab, returns: torch.Tensor, advantages: torch.Tensor, perm: torch.Tensor | None = None) -> dict:
-        """One PPO update over the slab (obs_in / actions / values / log_prob / mean, [T, N, ...]) with returns and
-        advantages [T, N] from ``compute_returns``.  perm: int64 [T*N] permutation (default: ``torch.randperm`` on the
-        device, as rsl_rl).  Returns device tensors keyed like rsl_rl's loss dict (means over the epochs x mini-batches)
-        plus the learning rate and the last mini-batch's KL."""
+    def _prepare(self, slab, returns: torch.Tensor, advantages: torch.Tensor, perm: torch.Tensor | None):
+        """Check the update's tensors, size the workspace, keep the batch struct alive: (params, batch, workspace)."""
         cfg = self.cfg
         n = returns.numel()
         if perm is None:
@@ -280,13 +283,28 @@ class FusedPPO:
         p = WlPpoParams(self.obs_dim, n, cfg.num_learning_epochs, cfg.num_mini_batches, cfg.clip_param, cfg.value_loss_coef,
                         cfg.entropy_coef, cfg.max_grad_norm, cfg.desired_kl, int(cfg.schedule == "adaptive"),
                         int(cfg.use_clipped_value_loss), 0)
-        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        check(self._update(C.byref(p), C.byref(self._batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
-                           C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
-                           ws.numel(), stream), self._update.__name__)
-        k = cfg.num_learning_epochs * cfg.num_mini_batches
+        return p, self._batch, ws
+
+    def _stats(self) -> dict:
+        k = self.cfg.num_learning_epochs * self.cfg.num_mini_batches
         return {"value_function": self.state[7] / k, "surrogate": self.state[6] / k, "entropy": self.state[8] / k,
                 "learning_rate": self.state[0], "kl": self.state[9]}
+
+    def update(self, slab, returns: torch.Tensor, advantages: torch.Tensor, perm: torch.Tensor | None = None) -> dict:
+        """One PPO update over the slab (obs_in / actions / values / log_prob / mean, [T, N, ...]) with returns and
+        advantages [T, N] from ``compute_returns``.  perm: int64 [T*N] permutation (default: ``torch.randperm`` on the
+        device, as rsl_rl).  Returns device tensors keyed like rsl_rl's loss dict (means over the epochs x mini-batches)
+        plus the learning rate and the last mini-batch's KL (with an exchange: this rank's losses, the ranks' mean KL)."""
+        if self.exchange is not None:
+            if self.exchange.one_process and self.exchange.n_ranks > 1:
+                raise ValueError("FusedPPO.update: the ranks of a one-process exchange update together (update_local_ranks)")
+            return update_local_ranks([self], [(slab, returns, advantages, perm)])[0]
+        p, batch, ws = self._prepare(slab, returns, advantages, perm)
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        check(self._update(C.byref(p), C.byref(batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
+                           C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
+                           ws.numel(), stream), self._update.__name__)
+        return self._stats()
 
     @property
     def history(self) -> torch.Tensor:
@@ -295,7 +313,8 @@ class FusedPPO:
         return self.state[10:10 + 2 * k].view(k, 2)
 
     def last_gradient(self) -> torch.Tensor:
-        """The last mini-batch's reduced gradient (before clipping), blob layout (device view of the workspace)."""
+        """The last mini-batch's reduced gradient (before clipping; with an exchange, the ranks' average), blob layout
+        (device view of the workspace)."""
         return self.workspace[:4 * self.blob.numel()].view(torch.float32)
 
     def optimizer_state_dict(self) -> dict:
@@ -350,6 +369,86 @@ class FusedPPO:
         self.state[0] = self.cfg.learning_rate
 
 
+class PPOExchange:
+    """The exchange of a data-parallel PPO update (``wl_ppo_update_dp``, DESIGN 6j): ``n_ranks``, this replica's ``rank`` and
+    the ``n_ranks`` exchange buffers in rank order (``ptrs``; ``buffer`` is this rank's own, a uint8 device tensor of
+    ``wl_ppo_dp_exchange_bytes(obs_dim)`` bytes).  ``symmetric`` allocates it in torch symmetric memory for one rank per
+    process; ``local`` allocates the ranks of one process (one device), for the one-process form."""
+
+    def __init__(self, n_ranks: int, rank: int, ptrs, buffer: torch.Tensor, handle=None, one_process: bool = False):
+        if not 0 <= rank < n_ranks or len(ptrs) != n_ranks:
+            raise ValueError(f"rank {rank} of {n_ranks} with {len(ptrs)} buffers")
+        self.n_ranks, self.rank, self.buffer, self.handle = n_ranks, rank, buffer, handle
+        self.one_process = one_process
+        self.ptrs = (C.c_void_p * n_ranks)(*ptrs)
+
+    @staticmethod
+    def nbytes(obs_dim: int) -> int:
+        need = lib.wl_ppo_dp_exchange_bytes(obs_dim)
+        if need == 0:
+            raise WlError(f"wl_ppo_dp_exchange_bytes failed: {lib.wl_last_error().decode()}")
+        return need
+
+    @classmethod
+    def symmetric(cls, obs_dim: int, device, group=None) -> "PPOExchange":
+        """This rank's exchange over the ranks of `group` (default: the world), every buffer P2P-mapped to every rank."""
+        import torch.distributed as dist
+        import torch.distributed._symmetric_memory as symm
+        group = group if group is not None else dist.group.WORLD
+        buf = symm.empty(cls.nbytes(obs_dim), dtype=torch.uint8, device=device)
+        buf.zero_()
+        handle = symm.rendezvous(buf, group.group_name)
+        handle.barrier()                                   # every buffer is zero before any rank publishes into it
+        return cls(dist.get_world_size(group), dist.get_rank(group), [int(x) for x in handle.buffer_ptrs], buf, handle)
+
+    @classmethod
+    def local(cls, n_ranks: int, obs_dim: int, device) -> list:
+        """The exchanges of n_ranks ranks that all live in this process on one device (``update_local_ranks``)."""
+        bufs = [torch.zeros(cls.nbytes(obs_dim), dtype=torch.uint8, device=device) for _ in range(n_ranks)]
+        ptrs = [b.data_ptr() for b in bufs]
+        return [cls(n_ranks, r, ptrs, bufs[r], one_process=True) for r in range(n_ranks)]
+
+    def failed(self) -> bool:
+        """Whether a peer wait of this rank timed out (its error word; one sync).  The update then stops stepping."""
+        return bool(self.buffer[4:8].view(torch.int32).item())
+
+    def check(self):
+        if self.failed():
+            raise WlError(f"data-parallel PPO update: rank {self.rank} timed out waiting for its peers' gradients "
+                          f"(the parameters were left as they were)")
+
+
+def update_local_ranks(ppos: list, inputs: list) -> list:
+    """One data-parallel update of the replicas ``ppos`` (``FusedPPO`` with exchanges of the same ranks, each its own
+    rank) in one call: inputs[l] = (slab, returns, advantages, perm) of ppos[l], as ``FusedPPO.update``.  With every rank
+    of the exchange local (``PPOExchange.local``) this is the one-process form: the whole exchange on one device and
+    stream.  Returns each replica's statistics."""
+    if not ppos or len(ppos) != len(inputs):
+        raise ValueError("update_local_ranks: one (slab, returns, advantages, perm) per replica")
+    ex0 = ppos[0].exchange
+    for q in ppos:
+        if q.exchange is None or list(q.exchange.ptrs) != list(ex0.ptrs):
+            raise ValueError("update_local_ranks: every replica needs an exchange over the same rank buffers")
+        if q.activation != ppos[0].activation or q.cfg != ppos[0].cfg or q.obs_dim != ppos[0].obs_dim:
+            raise ValueError("update_local_ranks: the replicas must share the network, obs_dim and PPOConfig")
+    if len({q.exchange.rank for q in ppos}) != len(ppos):
+        raise ValueError("update_local_ranks: two replicas hold the same rank")
+    if ex0.one_process and len(ppos) != ex0.n_ranks:
+        raise ValueError(f"update_local_ranks: a one-process exchange updates all {ex0.n_ranks} ranks together, not {len(ppos)}")
+    prepared = [q._prepare(*x) for q, x in zip(ppos, inputs)]
+    nl = len(ppos)
+    vp = lambda xs: (C.c_void_p * nl)(*[x.data_ptr() for x in xs])
+    batches = (WlPpoBatch * nl)(*[b for _, b, _ in prepared])
+    ranks = (C.c_int32 * nl)(*[q.exchange.rank for q in ppos])
+    ws = [w for _, _, w in prepared]
+    q0 = ppos[0]
+    stream = C.c_void_p(torch.cuda.current_stream(q0.device).cuda_stream)
+    check(lib.wl_ppo_update_dp(C.byref(prepared[0][0]), WL_ACTIVATION[q0.activation], ex0.n_ranks, ex0.ptrs, nl, ranks, batches,
+                               vp([q.blob for q in ppos]), vp([q.m for q in ppos]), vp([q.v for q in ppos]),
+                               vp([q.state for q in ppos]), vp(ws), min(w.numel() for w in ws), stream), "wl_ppo_update_dp")
+    return [q._stats() for q in ppos]
+
+
 def _adam_param_group(lr: float) -> dict:
     """torch.optim.Adam's param group as this torch version writes it, for 13 parameters with rsl_rl's settings."""
     group = torch.optim.Adam([torch.zeros(1, requires_grad=True) for _ in range(13)], lr=lr).state_dict()["param_groups"][0]
@@ -371,11 +470,11 @@ class PPOIteration:
     SUMMARY = ("Loss/value_function", "Loss/surrogate", "Loss/entropy", "Loss/learning_rate", "Policy/mean_noise_std")
 
     def __init__(self, sim, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu",
-                 episode_stats: bool = False):
+                 episode_stats: bool = False, exchange: PPOExchange | None = None):
         from .policy import FusedPolicyRollout
         self.sim, self.blob, self.T = sim, blob, T
         self.roll = FusedPolicyRollout(sim, blob, T, activation=activation)
-        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation)
+        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation, exchange=exchange)
         self.perm = torch.empty(T * sim.num_envs, dtype=torch.int64, device=sim.device)
         self.graph = None
         self.stats = None
@@ -391,14 +490,19 @@ class PPOIteration:
         from .policy import critic_value
         return critic_value(self.blob, self.sim.obs_dim, self.roll.obs0, self.ppo.activation)
 
-    def _learn(self):
+    def _returns(self):
         slab, cfg = self.roll.slab, self.ppo.cfg
         if self.episodes is not None:
             self.episodes.update(slab.rewards, slab.terminated, slab.truncated)
         last_values = self._bootstrap()
-        ret, adv = compute_returns(slab.rewards, slab.values, last_values, slab.terminated | slab.truncated, cfg.gamma, cfg.lam,
-                                   time_outs=slab.truncated)
-        stats = self.ppo.update(slab, ret, adv, self.perm)
+        return compute_returns(slab.rewards, slab.values, last_values, slab.terminated | slab.truncated, cfg.gamma, cfg.lam,
+                               time_outs=slab.truncated)
+
+    def _learn(self):
+        ret, adv = self._returns()
+        return self._summarise(self.ppo.update(self.roll.slab, ret, adv, self.perm))
+
+    def _summarise(self, stats):
         if self.summary is not None:
             from .policy import blob_layout
             o_std = blob_layout(self.sim.obs_dim)[0][12]
@@ -439,6 +543,99 @@ class PPOIteration:
         return self.stats
 
 
+class LocalRanksIteration:
+    """The one-process form of a data-parallel iteration: R ``PPOIteration`` s of this process (each with its own sim, blob
+    and an exchange from ``PPOExchange.local``) run as one -- every rollout, then every bootstrap and GAE, then one
+    ``update_local_ranks`` -- and ``capture=True`` records all of it as ONE CUDA graph.  ``run(perms)`` takes one
+    permutation per rank (default: ``torch.randperm`` each)."""
+
+    def __init__(self, its: list):
+        if not its or any(it.ppo.exchange is None for it in its):
+            raise ValueError("LocalRanksIteration: every iteration needs an exchange")
+        self.its, self.graph, self.stats = its, None, None
+
+    def _learn(self):
+        inputs = [(it.roll.slab, *it._returns(), it.perm) for it in self.its]
+        stats = update_local_ranks([it.ppo for it in self.its], inputs)
+        return [it._summarise(st) for it, st in zip(self.its, stats)]
+
+    def _body(self):
+        for it in self.its:
+            it.roll._body()
+        return self._learn()
+
+    def start(self, step_counter: int = 0, capture: bool = True):
+        its = self.its
+        dev = its[0].sim.device
+        for it in its:
+            it.ppo._workspace(it.perm.numel())
+        if not capture:
+            for it in its:
+                it.roll.capture(step_counter)
+            return self
+        for it in its:
+            it.sim.observe(step_counter, 0, out=it.roll.obs0)
+            it.sim.set_step_counter(step_counter)
+        self.graph = torch.cuda.CUDAGraph()
+        s = its[0].roll._stream
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):
+            for it in its:
+                it._bootstrap()                            # warm-up: cuBLAS cannot create its handle under capture
+            with torch.cuda.graph(self.graph, stream=s):
+                self.stats = self._body()
+        torch.cuda.current_stream(dev).wait_stream(s)
+        for it in its:
+            it.sim.set_step_counter(step_counter)
+            it.roll._base = step_counter
+        return self
+
+    def run(self, perms=None) -> list:
+        for k, it in enumerate(self.its):
+            it.perm.copy_(perms[k] if perms is not None else torch.randperm(it.perm.numel(), device=it.perm.device))
+        if self.graph is None:
+            for it in self.its:
+                it.roll.run()
+            self.stats = self._learn()
+            return self.stats
+        self.graph.replay()
+        for it in self.its:
+            it.roll._base += it.T
+            it.sim.note_device_counter(it.roll._base)
+        return self.stats
+
+
+def _data_parallel_world(sim, device) -> tuple:
+    """(world size, rank) of the runner: (1, 0) without a process group or ``WORLD_SIZE`` > 1; otherwise the process group's
+    (initialised here with NCCL if ``WORLD_SIZE`` > 1 asks for one, as rsl_rl does [UPSTREAM-RECALL]) after the checks that
+    keep the ranks apart: this rank on ``cuda:LOCAL_RANK``, its env shard at ``env_id_offset = rank * num_envs`` (else the
+    ranks would simulate the same envs), no two ranks on one GPU (a peer wait could stall behind the other process)."""
+    import torch.distributed as dist
+    if dist.is_initialized():
+        world, rank = dist.get_world_size(), dist.get_rank()
+    else:
+        world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
+    if world <= 1:
+        return 1, 0
+    if world > 8:
+        raise NotImplementedError(f"the data-parallel update exchanges over at most 8 ranks (one node), not {world}")
+    local = int(os.environ.get("LOCAL_RANK", rank))
+    if torch.device(device) != torch.device(f"cuda:{local}"):
+        raise ValueError(f"rank {rank} runs on {device}, not cuda:{local} (LOCAL_RANK): one GPU per rank")
+    offset = int(sim.cfg.env_id_offset)
+    if offset != rank * sim.num_envs:
+        raise ValueError(f"rank {rank}'s env shard starts at env_id_offset {offset}, not rank * num_envs = {rank * sim.num_envs}: "
+                         "the ranks would simulate the same envs")
+    if not dist.is_initialized():
+        torch.cuda.set_device(torch.device(device))
+        dist.init_process_group(backend="nccl")
+    uuids = [None] * world
+    dist.all_gather_object(uuids, str(torch.cuda.get_device_properties(torch.device(device)).uuid))
+    if len(set(uuids)) != world:
+        raise ValueError(f"two ranks share a GPU (device UUIDs {uuids}): one GPU per rank")
+    return world, rank
+
+
 class FusedOnPolicyRunner:
     """rsl_rl's ``OnPolicyRunner`` as the reference drives it (``modified_rsl_rl_runner.py``, ``train_rl.py:95-116``), over
     ``PPOIteration``: ``FusedOnPolicyRunner(env, agent_cfg.to_dict(), log_dir, device)``, ``learn(n)``, ``save`` / ``load``
@@ -449,7 +646,14 @@ class FusedOnPolicyRunner:
     The agent cfg dict is read for ``num_steps_per_env``, ``save_interval``, ``policy`` (``activation_from_rsl_rl``,
     ``init_noise_std``) and ``algorithm`` (``PPOConfig.from_rsl_rl``).  The weights start as the reference's do: torch
     ``nn.Linear`` defaults from torch's global generator, std = ``init_noise_std``.  No writer: ``callback(it, scalars)``,
-    if set, receives each iteration's scalars (also kept in ``self.last_log``)."""
+    if set, receives each iteration's scalars (also kept in ``self.last_log``).
+
+    Data-parallel as rsl_rl [UPSTREAM-RECALL] when ``torch.distributed`` is initialised with a world larger than 1 (or, not
+    initialised, when ``WORLD_SIZE`` > 1: the runner then initialises NCCL itself), one process per GPU under ``torchrun``:
+    each rank rolls out its own env shard (``env_id_offset = rank * num_envs``), the PPO update averages gradient and KL
+    across the ranks inside every mini-batch (``FusedPPO`` with a ``PPOExchange`` in symmetric memory), ``learn`` first
+    broadcasts rank 0's weights, only rank 0 saves checkpoints and calls ``callback``, and ``Perf/total_fps`` counts the
+    env-steps of every rank.  Every rank loads the same checkpoint."""
 
     @staticmethod
     def settings(train_cfg) -> SimpleNamespace:
@@ -476,6 +680,7 @@ class FusedOnPolicyRunner:
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
+        self.world, self.rank = _data_parallel_world(sim, device)
         self.cfg, self.device, self.log_dir = s.cfg, sim.device, log_dir
         self.num_steps_per_env, self.save_interval, self.activation, self.alg_cfg = s.num_steps_per_env, s.save_interval, s.activation, s.alg_cfg
         D = sim.obs_dim
@@ -483,7 +688,9 @@ class FusedOnPolicyRunner:
         mk = lambda out: torch.nn.Sequential(torch.nn.Linear(D, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
         std = torch.full((2,), s.init_noise_std)
         self.blob = pack_actor_critic(mk(2), mk(1), std, D, sim.device)
-        self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True)
+        exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
+        self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True,
+                               exchange=exchange)
         self.alg = self.it.ppo
         self.current_learning_iteration = 0
         self.callback = None
@@ -500,6 +707,9 @@ class FusedOnPolicyRunner:
         if init_at_random_ep_len:
             env.episode_length_buf = torch.randint_like(env.episode_length_buf, high=int(env.max_episode_length))
         it.episodes.reset()
+        if self.world > 1:
+            import torch.distributed as dist
+            dist.broadcast(self.blob, src=0)          # every replica starts from rank 0's weights (rsl_rl's learn)
         it.start(env.common_step_counter, capture=True)
         names = sorted(env._log_index.items(), key=lambda kv: kv[1])
         ns = C.sizeof(WlEpisodeStatsState)
@@ -510,6 +720,8 @@ class FusedOnPolicyRunner:
             env.sim.flush_log()                       # publish the rollout's last episode-log row into the read-back block
             rb = it.readback.cpu()
             elapsed = time.perf_counter() - t0
+            if it.ppo.exchange is not None:
+                it.ppo.exchange.check()
             env.common_step_counter += T
             self.current_learning_iteration = k
             st = WlEpisodeStatsState.from_buffer_copy(bytes(rb[:ns].numpy()))
@@ -520,9 +732,11 @@ class FusedOnPolicyRunner:
                 log["Train/mean_reward"] = st.mean_return
                 log["Train/mean_episode_length"] = st.mean_length
             log.update({name: logs[col] for name, col in names})
-            log["Perf/total_fps"] = T * env.num_envs / elapsed
+            log["Perf/total_fps"] = T * env.num_envs * self.world / elapsed
             log["Episodes/finished"] = st.finished
             self.last_log = log
+            if self.rank != 0:
+                continue
             if self.log_dir is not None and k % self.save_interval == 0:
                 self.save(os.path.join(self.log_dir, "models", f"model_{k}.pt"))
             if self.callback is not None:
