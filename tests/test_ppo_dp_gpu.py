@@ -187,6 +187,9 @@ def test_emulated_ranks_follow_the_torch_restatement(R, D, activation, over):
     from wheeledlab_b200.policy import actor_critic_state_dict
     cfg = PPOConfig(num_learning_epochs=2, num_mini_batches=4, **over)
     blob, batches = _synthetic(D, activation, R, 8192, seed=7 * R + D)
+    if activation == "relu":      # every ReLU unit and loss branch of the first mini-batch clear of its edge on every rank
+        from test_ppo_wide_numerics_cpu import apply_margins
+        apply_margins(blob, D, batches, 0, 8192, cfg)
     ref32, tr32 = torch_dp_update(blob.clone(), D, cfg, activation, batches, torch.float32)
     ref64, tr64 = torch_dp_update(blob.clone(), D, cfg, activation, batches, torch.float64)
     ppos = _replicas(blob, D, cfg, activation, R)

@@ -1,7 +1,8 @@
 """wl_ppo_update_wide (FusedPPO(activation="relu")) against the torch restatement of rsl_rl PPO.update() with ReLU
 (tests/ppo_reference_relu.py over tests/ppo_reference.py) run in fp32 and fp64 on the same permutation.
 err(x) = ||x - x_fp64|| / ||x_fp64||; the fused update must stay within max(4 * err(torch fp32), 1e-6) of the fp64 run,
-each layer's weight and bias taken together."""
+each layer's weight and bias taken together.  One-mini-batch gradients are taken on margin batches, where no ReLU unit or
+loss branch lies within rounding of its edge; tests/test_ppo_wide_numerics_gpu.py checks each kernel per element."""
 import copy
 from types import SimpleNamespace
 
@@ -87,7 +88,13 @@ def _padding_mask(D):
 def _check_gradient(D, n, cfg, seed=0, branches=False, edit=None):
     from wheeledlab_b200.learner import FusedPPO
     from wheeledlab_b200.policy import actor_critic_state_dict
-    blob, slab, ret, adv, perm = _synthetic(D, n, seed, edit)
+    if edit is None and cfg.num_learning_epochs * cfg.num_mini_batches == 1:
+        # every ReLU pre-activation and loss branch clear of its edge by 4 rounding bounds (tests/test_ppo_wide_numerics_cpu.py):
+        # fused, torch fp32 and fp64 take the same masks whatever the seed and the SM count
+        from test_ppo_wide_numerics_cpu import margin_batch
+        blob, slab, ret, adv, perm = margin_batch(D, n, seed, DEV, cfg=cfg)
+    else:
+        blob, slab, ret, adv, perm = _synthetic(D, n, seed, edit)
     (r32, s32), (r64, s64) = _references(blob.clone(), D, slab, ret, adv, perm, cfg, keep_grads=True)
     ppo = FusedPPO(blob, D, cfg, activation="relu")
     out = ppo.update(slab, ret, adv, perm)
