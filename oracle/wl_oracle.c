@@ -1363,6 +1363,40 @@ int wlo_elev_terms(const wl_config* c_in, const float* root, const float* cmdb, 
     }
     return 0;
 }
+/* derived suspension joint state of every env (wl_derive_suspension): pos[n*4] = clamp(compression, +-susp_travel), vel[n*4] =
+ * compression rate (0 when comp <= 0), wheel order [bl, br, fl, fr].  The kernel's expression in the kernel's operation order:
+ * hub = pc + R rho, comp = (zt - hub_z) n_z + r, nb = R^T n, rc = rho - r nb, vc = vb + wb x rc, vel = -nb . vc */
+int wlo_derive_suspension(const wlo_sim* s, float* pos, float* vel) {
+    const wl_config* c = &s->cfg;
+    const real rw = (real)c->wheel_radius, tr = (real)c->susp_travel;
+    for (int li = 0; li < c->num_envs; ++li) {
+        const wlo_env* e = &s->env[li];
+        real R[9]; rotmat(e->q, R);
+        real cw[3], pc[3]; { real cc[3] = {(real)c->com[0], (real)c->com[1], (real)c->com[2]}; rot(R, cc, cw); }
+        for (int k = 0; k < 3; ++k) pc[k] = e->p[k] + cw[k];
+        real vb[3], wb[3]; rotT(R, e->v, vb); rotT(R, e->w, wb);
+        for (int i = 0; i < 4; ++i) {
+            real rho[3];
+            rho[0] = ((i >= 2) ? (real)c->hub_x_front : (real)c->hub_x_rear) - (real)c->com[0];
+            rho[1] = ((i & 1) ? -(real)c->hub_y : (real)c->hub_y) - (real)c->com[1];
+            rho[2] = (real)c->hub_z - (real)c->com[2];
+            real hubw[3]; rot(R, rho, hubw);
+            hubw[0] += pc[0]; hubw[1] += pc[1]; hubw[2] += pc[2];
+            real zt, nw[3]; terrain(s, hubw[0], hubw[1], &zt, nw);
+            real comp = fm(-(hubw[2] - zt), nw[2], rw);
+            real nb[3]; rotT(R, nw, nb);
+            real rc[3] = {fm(-rw, nb[0], rho[0]), fm(-rw, nb[1], rho[1]), fm(-rw, nb[2], rho[2])};
+            real vc[3]; cross(wb, rc, vc);
+            vc[0] += vb[0]; vc[1] += vb[1]; vc[2] += vb[2];
+            /* the dot product goes through memory so that its negation stays a sign flip: gcc folds -fma(a, b, c) into
+             * fnmsub = -(a b) - c, which gives +0 where the negated +0 is -0 (a resting wheel on a flat cell) */
+            volatile real d = vdot(nb, vc);
+            pos[4 * (size_t)li + i] = (float)r_clamp(comp, -tr, tr);
+            vel[4 * (size_t)li + i] = (float)((comp > K(0.0)) ? -d : K(0.0));
+        }
+    }
+    return 0;
+}
 int wlo_euler_xyz(const float* quat, float* out, int32_t n) {
     for (int i = 0; i < n; ++i) {
         real q[4] = {quat[4 * i], quat[4 * i + 1], quat[4 * i + 2], quat[4 * i + 3]}, e[3];

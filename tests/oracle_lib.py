@@ -57,6 +57,7 @@ def _load(path):
     lib.wlo_camera.argtypes = [vp, vp, i64, vp]
     lib.wlo_camera_post.argtypes = [vp, vp, vp, vp, i32]
     lib.wlo_camera_render.argtypes = [vp, i32, vp]
+    lib.wlo_derive_suspension.argtypes = [vp, vp, vp]
     lib.wlo_config_describe.restype = C.c_char_p
     return lib
 
@@ -202,6 +203,14 @@ class Oracle:
         out = np.zeros(npix, np.uint8)
         assert self.lib.wlo_camera_render(self._h, li, _p(out)) == 0
         return out
+
+    def suspension(self):
+        """Derived suspension joint state of the current state (wl_derive_suspension): (pos [n,4], vel [n,4]), wheel order
+        [bl, br, fl, fr]."""
+        pos = np.empty((self.n, 4), np.float32)
+        vel = np.empty((self.n, 4), np.float32)
+        assert self.lib.wlo_derive_suspension(self._h, _p(pos), _p(vel)) == 0
+        return pos, vel
 
     def any_reset(self) -> bool:
         """>= 1 env reset in the most recent step (the log row itself persists over steps without a reset)."""

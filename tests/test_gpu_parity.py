@@ -443,7 +443,8 @@ def test_visual_trajectory_bit_exact(variant):
 
 
 def test_articulation_views_and_suspension():
-    """env.scene["robot"].data.* (IsaacLab names): zero-copy root state, derived joint state incl. suspension."""
+    """env.scene["robot"].data.* (IsaacLab names): zero-copy root state, derived joint state incl. suspension.  A smoke check;
+    tests/test_articulation_cpu.py and tests/test_articulation_gpu.py are the tests of record for these views."""
     _need_gpu()
     import wheeledlab_b200 as wl
     env = wl.make("Isaac-MushrDriftRL-v0", num_envs=256, seed=1)
