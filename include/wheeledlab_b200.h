@@ -374,7 +374,7 @@ int wl_set_term_bits(wl_sim* sim, uint8_t* d_term_bits);
  * delta included.
  * Only wl_step carries the fan-out, and only when it runs the 8-envs-per-CTA kernel (variant 8: Drift family, N <= 33 792,
  * default or wl_set_kernel_variant 8).  While a peer or multicast delta is set, wl_step on any other variant and
- * wl_rollout, wl_act_step, wl_act_infer_step, wl_step_stage_a / _b, wl_step_host and wl_step_host_zero_copy return
+ * wl_rollout, wl_act_step, wl_act_infer_step, wl_policy_act_elu, wl_step_stage_a / _b, wl_step_host and wl_step_host_zero_copy return
  * WL_EUNSUPPORTED before any device work and leave the handle as it was.  wl_observe, wl_reset and wl_policy_act write no
  * step rows and ignore it. */
 int wl_set_peer_fanout(wl_sim* sim, int32_t n_peers, const int64_t* byte_deltas);
@@ -527,6 +527,16 @@ int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, 
  * wl_act_step only (obs_dim <= 16, not Elevation). */
 int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, float* d_actions, float* d_obs,
                       float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
+/* wl_act_step's policy without the env step, for a step launched separately (e.g. the staged step, whose Python terms run
+ * between wl_step_stage_a and wl_step_stage_b): for every env of `sim`, the actor mean, critic value, sampled action and
+ * log-prob of d_obs_in [N, obs_dim] under the ELU network in d_policy_blob into `out`.  For the same d_obs_in, blob, seed,
+ * env_id_offset and step_counter (a host counter or WL_DEVICE_COUNTER_PLUS(k)) all four outputs equal what wl_act_step
+ * stores, bit for bit.  One launch; no env state, janitor or episode log is touched, and it does not trigger dependents
+ * early, so a step launched after it with PDL waits for every action.  Returns before any launch: WL_EINVAL for a null
+ * or misaligned pointer (blob 16 bytes, actions / mean 8, obs_in / log_prob / value 4) or a counter out of range;
+ * WL_EUNSUPPORTED for obs_dim > 16 or while a peer / multicast fan-out is set (the step after it refuses it too). */
+int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter,
+                      void* stream);
 
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out

@@ -1026,6 +1026,87 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
     }
 }
 
+// wl_policy_act_elu: the policy of wl_act_step_quad_kernel<TASK, false> without the env step, for a step that is launched
+// separately (the staged step).  The same CTA of 32 envs x 8 lanes, the same blob copies on the two mbarriers, the same
+// mlp_tile_layer tiles, quad head butterfly and policy noise (global env id, decoded counter), so actions, mean, log-prob
+// and value equal what wl_act_step stores, bit for bit.  No janitor CTA, no env state, no episode log.  It does not trigger
+// dependents early: a step launched after it with PDL waits for every action.
+__global__ void __launch_bounds__(WL_ACT_THREADS)
+wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* __restrict__ gl, const float* __restrict__ obs_in,
+                         const float* __restrict__ blob, int blob_floats, PolicyOffsets po_off, wl_policy_out po, uint32_t t_arg,
+                         int obs_dim) {
+    extern __shared__ __align__(128) float smem[];
+    __shared__ __align__(8) uint64_t mbar[2];
+    float* sw = smem;                                        // the whole weight blob
+    float* sx = smem + blob_floats;                          // [32][WL_ACT_XS]
+    float* sh = sx + WL_ACT_ENVS * WL_ACT_XS;                // [32][WL_ACT_HS]
+    if (threadIdx.x == 0) {                                  // first-layer blocks on mbar[0], the rest on mbar[1]
+        mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
+        mbar_init_fence();
+        const int a0 = po_off.o[0], a1 = po_off.o[2], c0 = po_off.o[6], c1 = po_off.o[8];
+        mbar_expect(&mbar[0], (uint32_t)((a1 - a0) + (c1 - c0)) * 4u);
+        bulk_g2s(sw + a0, blob + a0, (uint32_t)(a1 - a0) * 4u, &mbar[0]);
+        bulk_g2s(sw + c0, blob + c0, (uint32_t)(c1 - c0) * 4u, &mbar[0]);
+        mbar_expect(&mbar[1], (uint32_t)((c0 - a1) + (blob_floats - c1)) * 4u);
+        bulk_g2s(sw + a1, blob + a1, (uint32_t)(c0 - a1) * 4u, &mbar[1]);
+        bulk_g2s(sw + c1, blob + c1, (uint32_t)(blob_floats - c1) * 4u, &mbar[1]);
+    }
+    const uint32_t t = decode_step(gl, t_arg);
+    const int n = c.num_envs;
+    const bool head = threadIdx.x < 4 * WL_ACT_ENVS;         // warps 0..3 own the env quads of the heads
+    const int q = (threadIdx.x >> 2) & (WL_ACT_ENVS - 1);
+    const QuadLane L = quad_lane(c, n, blockIdx.x * WL_ACT_ENVS + q, threadIdx.x & 3);
+    for (int k = threadIdx.x; k < WL_ACT_ENVS * 16; k += WL_ACT_THREADS) {
+        const int eq = k >> 4, j = k & 15, ei = min(blockIdx.x * WL_ACT_ENVS + eq, n - 1);
+        sx[eq * WL_ACT_XS + j] = j < obs_dim ? obs_in[(size_t)ei * obs_dim + j] : 0.0f;
+    }
+    float z0 = 0.0f, z1 = 0.0f;
+    if (head) policy_noise(c.seed, L.gid, t, z0, z1);
+    __syncthreads();                                         // mbarrier init visible to every waiter; obs rows written
+    mbar_wait_parity(&mbar[0], 0);
+    {                                                        // warp k: envs 4k..4k+3, lanes tile (actor | critic) 4 units each
+        const int lane = threadIdx.x & 31, net = lane >> 4, ucol = (lane & 15) * 4;
+        const int env0 = (threadIdx.x >> 5) * 4;
+        const int nin1 = (obs_dim + 3) & ~3;
+        const int oW1 = net ? po_off.o[6] : po_off.o[0], oB1 = net ? po_off.o[7] : po_off.o[1];
+        const int oW2 = net ? po_off.o[8] : po_off.o[2], oB2 = net ? po_off.o[9] : po_off.o[3];
+        float acc[4][4];
+        float* h0 = sh + env0 * WL_ACT_HS + net * WL_HID;
+        mlp_tile_layer(sw + oW1 + ucol, sw + oB1 + ucol, sx + env0 * WL_ACT_XS, WL_ACT_XS, nin1, acc);
+        mlp_tile_store_elu(h0 + ucol, WL_ACT_HS, acc);
+        __syncwarp();
+        mbar_wait_parity(&mbar[1], 0);
+        mlp_tile_layer(sw + oW2 + ucol, sw + oB2 + ucol, h0, WL_ACT_HS, WL_HID, acc);
+        __syncwarp();                                        // every lane has finished reading layer-1 activations
+        mlp_tile_store_elu(h0 + ucol, WL_ACT_HS, acc);
+    }
+    __syncthreads();                                         // layer-2 activations of all 32 envs are in shared memory
+    if (!head) return;
+    const float* hrow = sh + q * WL_ACT_HS;
+    const float* w3a = sw + po_off.o[4]; const float* w3c = sw + po_off.o[10];
+    float m0 = 0.0f, m1 = 0.0f, vv = 0.0f;
+#pragma unroll
+    for (int u = 0; u < 16; ++u) {
+        const int j = 16 * L.w + u;
+        const float xa = hrow[j], xc = hrow[WL_HID + j];
+        m0 = fmaf(w3a[2 * j], xa, m0); m1 = fmaf(w3a[2 * j + 1], xa, m1);
+        vv = fmaf(w3c[j], xc, vv);
+    }
+    m0 += __shfl_xor_sync(0xffffffffu, m0, 1); m0 += __shfl_xor_sync(0xffffffffu, m0, 2);
+    m1 += __shfl_xor_sync(0xffffffffu, m1, 1); m1 += __shfl_xor_sync(0xffffffffu, m1, 2);
+    vv += __shfl_xor_sync(0xffffffffu, vv, 1); vv += __shfl_xor_sync(0xffffffffu, vv, 2);
+    m0 += sw[po_off.o[5]]; m1 += sw[po_off.o[5] + 1]; vv += sw[po_off.o[11]];
+    float2 a;
+    float lp;
+    gaussian_head(m0, m1, sw[po_off.o[12]], sw[po_off.o[12] + 1], z0, z1, a, lp);
+    if (L.live && L.w == 0) {
+        reinterpret_cast<float2*>(po.actions)[L.i] = a;
+        reinterpret_cast<float2*>(po.mean)[L.i] = make_float2(m0, m1);
+        po.log_prob[L.i] = lp;
+        po.value[L.i] = vv;
+    }
+}
+
 // K consecutive env.step()s in ONE launch (synthetic / scripted-action rollouts, SURVEY 7.7): the state stays in registers
 // for the whole rollout, every step still writes its observation / reward / done rows ([K,N,...] slab) and its episode-log
 // row.  actions == nullptr => U[-1,1]^2 drawn in-kernel from the counter-based generator (and stored to act_out).
@@ -2387,6 +2468,34 @@ int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_
     const wl_policy_out out{d_actions, nullptr, nullptr, nullptr};
     return act_step_launch(true, "wl_act_infer_step", sim, d_obs_in, d_policy_blob, out, d_obs, d_rew, d_terminated, d_truncated, d_log,
                            step_counter, stream);
+}
+
+int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
+        return fail(WL_EINVAL, "wl_policy_act_elu: null argument");
+    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u) || ((uintptr_t)d_obs_in & 3u) ||
+        ((uintptr_t)out.log_prob & 3u) || ((uintptr_t)out.value & 3u))
+        return fail(WL_EINVAL, "wl_policy_act_elu: policy blob must be 16-byte aligned, actions/mean 8-byte aligned, obs_in/log_prob/value 4-byte aligned");
+    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
+        return fail(WL_EINVAL, "wl_policy_act_elu: step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+    // no step rows are written, but the step that consumes these actions refuses the fan-out: refuse it here already
+    if (int rc = refuse_fan(sim, "wl_policy_act_elu")) return rc;
+    if (sim->obs_dim < 1 || sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, "wl_policy_act_elu: obs_dim > 16 (the network wl_act_step runs)");
+    ensure_device(sim);
+    PolicyOffsets po;
+    const int blob_floats = policy_offsets(sim->obs_dim, po.o);
+    const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS));
+    static bool attr_set[64] = {false};                       // the attribute is per device
+    if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_elu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024),
+                                "wl_policy_act_elu"))
+            return rc;
+        attr_set[sim->device] = true;
+    }
+    const int n = sim->cfg.num_envs;
+    wl_policy_act_elu_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
+        sim->cfg, sim->globals, d_obs_in, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, sim->obs_dim);
+    return launched(sim, "wl_policy_act_elu_kernel");
 }
 
 int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_values, const uint8_t* d_dones,

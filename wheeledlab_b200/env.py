@@ -421,9 +421,24 @@ class ManagerBasedRLEnv:
 
     def _step_staged(self, action: torch.Tensor):
         """env.step with Python terms in the loop: stage a (A-E) -> terminations -> rewards -> stage b (F-I)."""
+        log = torch.empty(16, dtype=torch.float32, device=self.device) if self.log_episode_info else None
+        obs, rew, terminated, truncated, extra = self.staged_step(action, log=log)
+        if log is not None:
+            self.extras["log"] = _LazyLog(log, self._log_index, extra, env=self)
+        return {"policy": self._append_py_obs(obs)}, rew, terminated, truncated, self.extras
+
+    def staged_step(self, action: torch.Tensor, rew: torch.Tensor | None = None, term_bits: torch.Tensor | None = None, out=None,
+                    log: torch.Tensor | None = None):
+        """One staged step at ``common_step_counter`` -- stage a, the Python termination terms, then the Python reward terms
+        (func * weight * step_dt, weight 0 skipped, per-episode sums kept), stage b -- into the caller's buffers where given:
+        rew [N] f32, term_bits [N] u8, out = (obs [N, obs_dim] f32, terminated [N] u8, truncated [N] u8), log f32[16] (the
+        episode-log row, written by the next launch on the handle).  Advances ``common_step_counter`` by one and sets the
+        termination manager's masks.  Returns (obs, rew, terminated, truncated, extra): `extra` holds the Python terms'
+        ``Episode_Reward/<name>`` / ``Episode_Termination/<name>`` entries as 0-dim device tensors when `log` is given,
+        else None.  env.step and the runner's staged rollout both run their Python terms through this."""
         t = self.common_step_counter
         sim, tm = self.sim, self.termination_manager
-        rew, bits = sim.step_stage_a(action, t)
+        rew, bits = sim.step_stage_a(action, t, rew=rew, term_bits=term_bits)
         built_in_to = (bits & 1).bool()
         built_in_term = (bits & 0xFE).bool()
         self._term_bits_staged = bits            # per-term masks of the built-in terms (get_term)
@@ -446,11 +461,11 @@ class ManagerBasedRLEnv:
             val = term.func(self, **term.params).to(torch.float32) * (term.weight * self.step_dt)
             rew += val
             self._py_sums[term.name] += val
-        log = torch.empty(16, dtype=torch.float32, device=self.device) if self.log_episode_info else None
-        obs, term_u8, trunc_u8 = sim.step_stage_b(bits, t, extra_term, extra_to, log=log)
+        obs, term_u8, trunc_u8 = sim.step_stage_b(bits, t, extra_term, extra_to, out=out, log=log)
         self.common_step_counter = t + 1
         terminated, truncated = term_u8.view(torch.bool), trunc_u8.view(torch.bool)
         tm.terminated, tm.time_outs = terminated, truncated
+        extra = None
         if log is not None:
             done = terminated | truncated
             cnt = done.sum().clamp(min=1).to(torch.float32)
@@ -461,8 +476,12 @@ class ManagerBasedRLEnv:
                 sums.masked_fill_(done, 0.0)
             for term in self._py_terms:
                 extra["Episode_Termination/" + term.name] = (fired[term.name] & done).sum()
-            self.extras["log"] = _LazyLog(log, self._log_index, extra, env=self)
-        return {"policy": self._append_py_obs(obs)}, rew, terminated, truncated, self.extras
+        return obs, rew, terminated, truncated, extra
+
+    @property
+    def python_log_names(self) -> list:
+        """The extras["log"] keys of the Python reward and termination terms, in the order staged_step's `extra` has them."""
+        return ["Episode_Reward/" + t.name for t in self._py_rewards] + ["Episode_Termination/" + t.name for t in self._py_terms]
 
     def step(self, action: torch.Tensor):
         if self._needs_reset:

@@ -470,21 +470,26 @@ class PPOIteration:
     SUMMARY = ("Loss/value_function", "Loss/surrogate", "Loss/entropy", "Loss/learning_rate", "Policy/mean_noise_std")
 
     def __init__(self, sim, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu",
-                 episode_stats: bool = False, exchange: PPOExchange | None = None):
+                 episode_stats: bool = False, exchange: PPOExchange | None = None, rollout=None, extra_readback_bytes: int = 0):
         from .policy import FusedPolicyRollout
         self.sim, self.blob, self.T = sim, blob, T
-        self.roll = FusedPolicyRollout(sim, blob, T, activation=activation)
+        self.roll = rollout if rollout is not None else FusedPolicyRollout(sim, blob, T, activation=activation)
         self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation, exchange=exchange)
         self.perm = torch.empty(T * sim.num_envs, dtype=torch.int64, device=sim.device)
         self.graph = None
         self.stats = None
-        self.episodes = self.readback = self.summary = None
+        self.episodes = self.readback = self.summary = self.readback_extra = None
         if episode_stats:
             ns = C.sizeof(WlEpisodeStatsState)
-            self.readback = torch.zeros(ns + 4 * len(self.SUMMARY) + 4 * 16 * T, dtype=torch.uint8, device=sim.device)
+            end_logs = ns + 4 * len(self.SUMMARY) + 4 * 16 * T
+            extra_at = (end_logs + 7) & ~7
+            self.readback = torch.zeros(extra_at + extra_readback_bytes if extra_readback_bytes else end_logs, dtype=torch.uint8,
+                                        device=sim.device)
             self.episodes = EpisodeStatistics(sim.num_envs, T, sim.device, state=self.readback[:ns])
             self.summary = self.readback[ns:ns + 4 * len(self.SUMMARY)].view(torch.float32)
-            self.roll.logs = self.readback[ns + 4 * len(self.SUMMARY):].view(torch.float32).view(T, 16)
+            self.roll.logs = self.readback[ns + 4 * len(self.SUMMARY):end_logs].view(torch.float32).view(T, 16)
+            if extra_readback_bytes:
+                self.readback_extra = self.readback[extra_at:]          # (8-byte aligned)
 
     def _bootstrap(self) -> torch.Tensor:
         from .policy import critic_value
@@ -540,6 +545,47 @@ class PPOIteration:
         self.graph.replay()
         self.roll._base += self.T
         self.sim.note_device_counter(self.roll._base)
+        return self.stats
+
+
+class StagedPPOIteration(PPOIteration):
+    """``PPOIteration`` for an env with host-side Python reward / termination terms, on one GPU: the rollout is
+    ``policy.StagedPolicyRollout`` (T x (policy, ``env.staged_step``), eager: the terms are arbitrary torch code), and
+    everything after it -- ``wl_episode_stats``, bootstrap value, GAE, the update and the summary copy, the code
+    ``PPOIteration`` captures -- is ONE CUDA graph (``capture=True``).  The read-back block also carries the rollout's
+    ``py_logs`` (the Python terms' per-step log entries, f64 [T, len(py_names)]) after the episode-log rows.  The env's
+    ``common_step_counter`` advances by T during ``run``."""
+
+    def __init__(self, env, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu"):
+        from .policy import StagedPolicyRollout
+        roll = StagedPolicyRollout(env, blob, T, activation)
+        n_py = len(roll.py_names)
+        super().__init__(env.sim, blob, cfg, T, activation, episode_stats=True, rollout=roll, extra_readback_bytes=8 * T * n_py)
+        if n_py:
+            roll.py_logs = self.readback_extra.view(torch.float64).view(T, n_py)
+
+    def start(self, step_counter: int = 0, capture: bool = True):
+        roll, dev = self.roll, self.sim.device
+        self.ppo._workspace(self.perm.numel())                 # (allocated outside any capture)
+        roll.start(step_counter)
+        if capture:
+            self.graph = torch.cuda.CUDAGraph()
+            s = roll._stream
+            s.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(s):
+                self._bootstrap()                              # warm-up: cuBLAS cannot create its handle under capture
+                with torch.cuda.graph(self.graph, stream=s):
+                    self.stats = self._learn()
+            torch.cuda.current_stream(dev).wait_stream(s)
+        return self
+
+    def run(self, perm: torch.Tensor | None = None) -> dict:
+        self.perm.copy_(perm if perm is not None else torch.randperm(self.perm.numel(), device=self.perm.device))
+        self.roll.run()
+        if self.graph is None:
+            self.stats = self._learn()
+        else:
+            self.graph.replay()
         return self.stats
 
 
@@ -605,16 +651,20 @@ class LocalRanksIteration:
         return self.stats
 
 
+def _world_size() -> int:
+    """The runner's world size, without initialising anything: the process group's, else ``WORLD_SIZE`` (default 1)."""
+    import torch.distributed as dist
+    return dist.get_world_size() if dist.is_initialized() else int(os.environ.get("WORLD_SIZE", "1"))
+
+
 def _data_parallel_world(sim, device) -> tuple:
     """(world size, rank) of the runner: (1, 0) without a process group or ``WORLD_SIZE`` > 1; otherwise the process group's
     (initialised here with NCCL if ``WORLD_SIZE`` > 1 asks for one, as rsl_rl does [UPSTREAM-RECALL]) after the checks that
     keep the ranks apart: this rank on ``cuda:LOCAL_RANK``, its env shard at ``env_id_offset = rank * num_envs`` (else the
     ranks would simulate the same envs), no two ranks on one GPU (a peer wait could stall behind the other process)."""
     import torch.distributed as dist
-    if dist.is_initialized():
-        world, rank = dist.get_world_size(), dist.get_rank()
-    else:
-        world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
+    world = _world_size()
+    rank = dist.get_rank() if dist.is_initialized() else int(os.environ.get("RANK", "0"))
     if world <= 1:
         return 1, 0
     if world > 8:
@@ -640,8 +690,14 @@ class FusedOnPolicyRunner:
     """rsl_rl's ``OnPolicyRunner`` as the reference drives it (``modified_rsl_rl_runner.py``, ``train_rl.py:95-116``), over
     ``PPOIteration``: ``FusedOnPolicyRunner(env, agent_cfg.to_dict(), log_dir, device)``, ``learn(n)``, ``save`` / ``load``
     in rsl_rl's checkpoint format.  ``env`` is a ``wheeledlab_b200.env.ManagerBasedRLEnv`` (or a wrapper whose ``unwrapped``
-    is one) without host-side Python terms.  Each iteration is ONE CUDA graph -- rollout, ``wl_episode_stats``, bootstrap
-    value, GAE, PPO update -- plus the flush of the last episode-log row, and ONE read-back of what is logged.
+    is one).  Each iteration is ONE CUDA graph -- rollout, ``wl_episode_stats``, bootstrap value, GAE, PPO update -- plus
+    the flush of the last episode-log row, and ONE read-back of what is logged.
+
+    An env with host-side Python reward or termination terms (``add_reward_term`` / ``add_termination_term``) trains on one
+    GPU through ``StagedPPOIteration``: the rollout runs eagerly, T x (policy, staged step with the terms in between), and
+    the rest of the iteration is the same graph; the log gains ``Episode_Reward/<name>`` / ``Episode_Termination/<name>``
+    for each Python term, the T-step mean of what env.step's ``extras["log"]`` holds for it.  Python observation terms and
+    data-parallel runs with Python terms raise ``NotImplementedError``.
 
     The agent cfg dict is read for ``num_steps_per_env``, ``save_interval``, ``policy`` (``activation_from_rsl_rl``,
     ``init_noise_std``) and ``algorithm`` (``PPOConfig.from_rsl_rl``).  The weights start as the reference's do: torch
@@ -675,11 +731,16 @@ class FusedOnPolicyRunner:
         s = self.settings(train_cfg)
         self.env = getattr(env, "unwrapped", env)
         e = self.env
-        if getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None) or getattr(e, "_py_obs", None):
-            raise NotImplementedError("the fused rollout runs the kernels' MDP terms only: this env has host-side Python terms")
+        if getattr(e, "_py_obs", None):
+            raise NotImplementedError("Python observation terms (add_observation_term) widen the observation past the slab row the "
+                                      "staged step writes: an env with host-side Python terms trains with reward and termination terms only")
+        self.staged = bool(getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None))
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
+        if self.staged and _world_size() > 1:               # (before anything initialises NCCL)
+            raise NotImplementedError("data-parallel training of an env with host-side Python terms is not supported: the staged "
+                                      "rollout runs on one GPU")
         self.world, self.rank = _data_parallel_world(sim, device)
         self.cfg, self.device, self.log_dir = s.cfg, sim.device, log_dir
         self.num_steps_per_env, self.save_interval, self.activation, self.alg_cfg = s.num_steps_per_env, s.save_interval, s.activation, s.alg_cfg
@@ -688,9 +749,12 @@ class FusedOnPolicyRunner:
         mk = lambda out: torch.nn.Sequential(torch.nn.Linear(D, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
         std = torch.full((2,), s.init_noise_std)
         self.blob = pack_actor_critic(mk(2), mk(1), std, D, sim.device)
-        exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
-        self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True,
-                               exchange=exchange)
+        if self.staged:
+            self.it = StagedPPOIteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation)
+        else:
+            exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
+            self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True,
+                                   exchange=exchange)
         self.alg = self.it.ppo
         self.current_learning_iteration = 0
         self.callback = None
@@ -722,16 +786,21 @@ class FusedOnPolicyRunner:
             elapsed = time.perf_counter() - t0
             if it.ppo.exchange is not None:
                 it.ppo.exchange.check()
-            env.common_step_counter += T
+            if not self.staged:                       # (the staged step advances the env's counter itself, once per step)
+                env.common_step_counter += T
             self.current_learning_iteration = k
             st = WlEpisodeStatsState.from_buffer_copy(bytes(rb[:ns].numpy()))
             summary = rb[ns:ns + 4 * len(PPOIteration.SUMMARY)].view(torch.float32).tolist()
-            logs = rb[ns + 4 * len(PPOIteration.SUMMARY):].view(torch.float32).view(T, 16).double().mean(0).tolist()
+            o_logs = ns + 4 * len(PPOIteration.SUMMARY)
+            logs = rb[o_logs:o_logs + 4 * 16 * T].view(torch.float32).view(T, 16).double().mean(0).tolist()
             log = dict(zip(PPOIteration.SUMMARY, summary))
             if st.fill > 0:
                 log["Train/mean_reward"] = st.mean_return
                 log["Train/mean_episode_length"] = st.mean_length
             log.update({name: logs[col] for name, col in names})
+            if self.staged and it.roll.py_names:      # the Python terms' entries: T-step means of env.step's extras["log"]
+                py = rb[rb.numel() - 8 * T * len(it.roll.py_names):].view(torch.float64).view(T, -1).mean(0).tolist()
+                log.update(zip(it.roll.py_names, py))
             log["Perf/total_fps"] = T * env.num_envs * self.world / elapsed
             log["Episodes/finished"] = st.finished
             self.last_log = log

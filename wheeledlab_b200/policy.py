@@ -199,12 +199,15 @@ def act_infer_step(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, ac
 
 
 def policy_act(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor, mean: torch.Tensor,
-               log_prob: torch.Tensor, value: torch.Tensor, step_counter: int):
-    """One launch (wl_policy_act): value / mean / sample / log-prob of `obs_in` [N, obs_dim] under the ReLU network in `blob`,
-    for any obs_dim up to 4096.  The env is not stepped: follow with sim.step(actions, step_counter)."""
+               log_prob: torch.Tensor, value: torch.Tensor, step_counter: int, activation: str = "relu"):
+    """One launch: value / mean / sample / log-prob of `obs_in` [N, obs_dim] under the network in `blob`.  "relu"
+    (wl_policy_act): Elevation / Visual, any obs_dim up to 4096; "elu" (wl_policy_act_elu): the Drift family's network
+    (obs_dim <= 16), bit for bit what wl_act_step stores.  The env is not stepped: follow with a step on the same
+    step_counter (sim.step, or the staged step)."""
+    fn = lib.wl_policy_act if check_activation(activation) == "relu" else lib.wl_policy_act_elu
     po = WlPolicyOut(actions.data_ptr(), mean.data_ptr(), log_prob.data_ptr(), value.data_ptr())
-    check(lib.wl_policy_act(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(blob.data_ptr()), po, step_counter,
-                            _stream_ptr(sim.device)), "wl_policy_act")
+    check(fn(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(blob.data_ptr()), po, step_counter, _stream_ptr(sim.device)),
+          fn.__name__)
 
 
 class FusedPolicyRollout:
@@ -280,3 +283,46 @@ class FusedPolicyRollout:
         self._base += self.T
         self.sim.note_device_counter(self._base)
         return self.slab
+
+
+class StagedPolicyRollout:
+    """The collection loop of an env with host-side Python reward / termination terms: T x (policy, then the env's staged step
+    ``env.staged_step``: stage a -> Python terms -> stage b), issued eagerly because the terms are arbitrary torch code that
+    may sync the host.  The policy is ``policy_act`` (wl_policy_act_elu for "elu", wl_policy_act for "relu") on the host's
+    step counter, which the staged step advances by one per step.  The slab is filled as ``FusedPolicyRollout`` fills it
+    (``obs_in[k]`` -> actions / mean / log-prob / values [k]; rewards, ``obs[k] = obs_in[k+1]``, terminated, truncated [k];
+    ``logs[k]`` the episode-log row), and ``py_logs[k]`` [T, len(py_names)] f64 holds what env.step's ``extras["log"]`` has at
+    step k for each Python term's key (``py_names``)."""
+
+    def __init__(self, env, blob: torch.Tensor, T: int = 128, activation: str = "elu"):
+        sim = env.sim
+        if env._py_obs:
+            raise NotImplementedError("Python observation terms widen the observation past the slab row the staged step writes")
+        if (sim.num_envs * sim.obs_dim) % 2:
+            raise ValueError("the slab's observation rows are written pair-wise: num_envs * obs_dim must be even")
+        self.env, self.sim, self.blob, self.T, self.activation = env, sim, blob, T, check_activation(activation)
+        self.slab = RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=True)
+        self.logs = torch.zeros((T, 16), dtype=torch.float32, device=sim.device)
+        self.py_names = env.python_log_names
+        self.py_logs = torch.zeros((T, len(self.py_names)), dtype=torch.float64, device=sim.device)
+        self.obs0 = torch.empty((sim.num_envs, sim.obs_dim), dtype=torch.float32, device=sim.device)   # carried to the next run
+        self._bits = torch.empty(sim.num_envs, dtype=torch.uint8, device=sim.device)
+        self._stream = torch.cuda.Stream(device=sim.device)
+
+    def start(self, step_counter: int):
+        """Prime obs0 with the observation at `step_counter` (the env's ``common_step_counter``)."""
+        self.sim.observe(step_counter, 0, out=self.obs0)
+        return self
+
+    def run(self) -> RolloutSlab:
+        env, sim, slab = self.env, self.sim, self.slab
+        slab.obs_in[0].copy_(self.obs0)
+        for k in range(self.T):
+            policy_act(sim, slab.obs_in[k], self.blob, slab.actions[k], slab.mean[k], slab.log_prob[k], slab.values[k],
+                       env.common_step_counter, self.activation)
+            *_, extra = env.staged_step(slab.actions[k], rew=slab.rewards[k], term_bits=self._bits,
+                                        out=(slab.obs[k], slab.terminated[k], slab.truncated[k]), log=self.logs[k])
+            if self.py_names:
+                torch.stack([extra[name].to(torch.float64) for name in self.py_names], out=self.py_logs[k])
+        self.obs0.copy_(slab.obs[self.T - 1])
+        return slab
