@@ -501,6 +501,62 @@ int wl_step_stage_a(wl_sim* sim, const float* d_action, float* d_rew, uint8_t* d
 int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_extra_terminated, const uint8_t* d_extra_truncated,
                     float* d_obs, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
 
+/* ---- device terms: the reference's unregistered reward / termination functions, in CUDA (DESIGN.md 6l) -------------------
+ * A device term is one function of the library below, evaluated by a kernel between stage a and stage b with exactly the
+ * semantics of the same function registered as a Python term (terminations first, then rewards in registration order,
+ * fp32(f) * fp32(weight * step_dt), weight 0 skipped, per-episode sums).  E = elevation/mushr_elevation_env_cfg.py,
+ * V = visual/mushr_visual_env_cfg.py; params in the order listed.  Map terms (is_traversable*, vel_rew_trav,
+ * bool_is_not_traversable) need the Visual task. */
+#define WL_MAX_DEVICE_TERMS 8
+#define WL_TERM_E_FORWARD_VEL              1   /* clamp(v_b.x, max=1.2) */
+#define WL_TERM_E_FORWARD_WHEEL_SPIN       2   /* clamp(sum of the throttle joint velocities, max=200) */
+#define WL_TERM_E_CHANGE_IN_ELEVATION      3   /* v_w.z where > 0, else 0 */
+#define WL_TERM_E_ASCENDING                4   /* clamp(v_w.z, min=0) */
+#define WL_TERM_E_STEEP_PENALTY            5   /* (thresh_pitch) clamp(pitch - thresh, min=0), pitch wrapped to [0, 2 pi) */
+#define WL_TERM_E_ELEVATION_CONTINUITY     6   /* (threshold_elev) 50 |dz| on the ramp; keeps the previous z per env */
+#define WL_TERM_E_YAW_CHANGE_ON_ELEV       7   /* (threshold_yaw, threshold_z) */
+#define WL_TERM_E_UPRIGHT_PENALTY          8   /* (thresh_deg) */
+#define WL_TERM_E_ROLL_ON_ELEV             9   /* (z_start, roll_rate_thresh) */
+#define WL_TERM_E_LOW_VEL_PENALTY         10   /* (min_vel) */
+#define WL_TERM_V_IS_TRAVERSABLE          11   /* map */
+#define WL_TERM_V_IS_TRAVERSABLE_SPEED_SCALED 12   /* map */
+#define WL_TERM_V_VEL_REW_TRAV            13   /* map (speed_target_on_trav, speed_target_on_non_trav) */
+#define WL_TERM_V_LOW_SPEED_PENALTY       14   /* (low_speed_thresh) */
+#define WL_TERM_V_OFF_TRACK               15   /* (straight, corner_out_radius) */
+#define WL_TERM_V_BOOL_IS_NOT_TRAVERSABLE 16   /* map; 0 until common_step_counter // max_episode_length reaches 1000 */
+#define WL_TERM_V_ROLL_OVER               17   /* roll - pi in (-pi/2, pi/2), roll wrapped to [0, 2 pi) */
+#define WL_TERM_KINDS                     18
+#define WL_TERM_ROLE_REWARD      0
+#define WL_TERM_ROLE_TERMINATION 1   /* fires when the value is nonzero: terminated */
+#define WL_TERM_ROLE_TIME_OUT    2   /* fires when the value is nonzero: truncated */
+typedef struct wl_term_desc {
+    int32_t kind;        /* WL_TERM_* */
+    int32_t role;        /* WL_TERM_ROLE_* */
+    double weight;       /* reward weight (ignored for terminations); Python's weight * step_dt is formed in double */
+    double params[4];    /* the function's parameters as Python floats (unused ones 0) */
+} wl_term_desc;
+/* Store the handle's device terms (at most WL_MAX_DEVICE_TERMS, evaluated in this order) and allocate their per-env
+ * state: the reward terms' episode sums (zero) and elevation_continuity's previous elevation (unset: its first call sees
+ * no change).  The state survives env resets, as the reference's function attribute does; it is per handle.  n = 0 clears
+ * the table.  A set-up call: it allocates, clears the state and synchronises the device before it returns, and it is not
+ * capturable.  The old table's buffers are freed only after the new ones are ready (a failure leaves the handle as it
+ * was), so a graph captured with the old table must be captured again.  Refused before any device work: WL_EINVAL for a
+ * null handle, n outside 0..8, a null table with n > 0, an unknown kind or role, a non-finite weight or parameter;
+ * WL_EUNSUPPORTED for a map term on a task other than Visual. */
+int wl_set_device_terms(wl_sim* sim, const wl_term_desc* terms, int32_t n_terms);
+/* One env.step with the device terms: stage a, the term kernel, stage b (and the height scan / camera).  Same arguments
+ * as wl_step, plus d_term_log: NULL or float[WL_MAX_DEVICE_TERMS] on the device receiving, per term in table order,
+ * Episode_Reward/<name> (the mean episode sum over the envs done in this step / max_episode_length_s) or
+ * Episode_Termination/<name> (the number of done envs where it fired), then zeros; written by this call, fixed-order
+ * sums.  With no terms the call is wl_step itself and d_term_log is not written.
+ * step_counter is a host counter or WL_DEVICE_COUNTER_PLUS(k), so K calls and wl_advance_counter(K) form a replayable
+ * graph.  WL_EINVAL for a null argument or a misaligned action /
+ * obs, WL_EUNSUPPORTED while a peer / multicast fan-out is set, before any device work. */
+int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated,
+                  float* d_log, float* d_term_log, int64_t step_counter, void* stream);
+/* Device pointer to uint8[N]: bit k = device term k fired in the most recent wl_step_terms (NULL without terms). */
+uint8_t* wl_device_term_masks(const wl_sim* sim);
+
 /* ---- the step before env.step(): the policy (SURVEY 8f-1) ---------------------------------------------------------
  * alg.act(obs) of the rollout loop (modified_rsl_rl_runner.py:72; rsl_rl ActorCritic with the reference's sizes,
  * drifting/config/agents/mushr/rsl_rl_ppo_cfg.py:12-17: actor and critic 64x64 ELU MLPs, Gaussian head with a learned

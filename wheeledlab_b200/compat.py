@@ -131,12 +131,28 @@ def _lower_common(cfg, spec: T.TaskSpec):
     spec._curriculum_dirty = True
 
 
-def _lower_rewards(cfg, spec, table, handlers, allow_python_terms=False):
+def _device_term(spec, name, term, kind, device_terms) -> bool:
+    """With ``device_terms``, a term whose function is in the device-term library (by module AND name, before any
+    match by name against the built-in slots) joins ``spec.device_terms``; returns whether it did."""
+    from . import device_terms as dtm
+    if not device_terms or dtm.lookup(term.func) is None:
+        return False
+    if kind == "reward":
+        spec.device_terms.append((name, term.func, "reward", float(term.weight), dict(term.params or {})))
+    else:
+        spec.device_terms.append((name, term.func, "time_out" if getattr(term, "time_out", False) else "termination", 0.0,
+                                  dict(term.params or {})))
+    return True
+
+
+def _lower_rewards(cfg, spec, table, handlers, allow_python_terms=False, device_terms=False):
     c = spec.cfg
     names = [None] * len(table)
     for k in range(T_MAX := 8):
         c.rew_weight[k] = 0.0
     for name, term in _fields(getattr(cfg, "rewards", None)):
+        if _device_term(spec, name, term, "reward", device_terms):
+            continue
         fn = _ALIASES.get(_fname(term), _fname(term))
         if fn not in table:
             if allow_python_terms:      # the reference's own Python function, evaluated between the two halves of the staged step
@@ -186,16 +202,19 @@ def _lower_material_and_mass_events(events, c, seed):
         c.dr_wheel_mass[0], c.dr_wheel_mass[1] = wheel_mass
 
 
-def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: bool = False) -> T.TaskSpec:
+def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: bool = False, device_terms: bool = False) -> T.TaskSpec:
     """Build the TaskSpec for a reference env-cfg instance: the train cfgs of the four registered ids (Drift, F1Tenth drift,
     Elevation, Visual, incl. MushrVisualRLRandomEnvCfg) and their play cfgs (rewards / terminations / curriculum = None).
     With ``allow_python_terms`` reward / termination terms the kernels do not implement are kept as host-side terms that
-    call the cfg's own function (staged step, env.add_reward_term); otherwise they raise."""
+    call the cfg's own function (staged step, env.add_reward_term); otherwise they raise.  With ``device_terms`` such a
+    term whose function is in the device-term library (device_terms.REGISTRY) becomes a device term of the spec
+    (spec.device_terms, in cfg order, with the cfg's weight and params), matched by module and name before the
+    built-in terms are matched by name."""
     num_envs = int(cfg.scene.num_envs)
     seed = int(cfg.seed) if getattr(cfg, "seed", None) is not None else 42
     kind = _task_kind(cfg)
     if kind == "visual":
-        return _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms)
+        return _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device_terms)
     if kind == "drift":
         events = dict(_fields(cfg.events))
         randomize = "change_wheel_friction" in events
@@ -226,9 +245,11 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
             "side_slip": h_slip, "vel_dist": h_vel, "cross_track_dist": h_ctd,
             "turn_left_go_right": lambda p: setattr(c, "tlgr_ang_vel_thresh", p.get("ang_vel_thresh", math.pi / 4)),
             "energy_through_turn": lambda p: setattr(c, "energy_straight", p["straight"]),
-        }, allow_python_terms)
+        }, allow_python_terms, device_terms)
         for name, term in _fields(getattr(cfg, "terminations", None)):
             fn = _fname(term)
+            if _device_term(spec, name, term, "termination", device_terms):
+                continue
             if fn == "cart_off_track":
                 p = term.params
                 c.trk_straight, c.trk_corner_in, c.trk_corner_out = p["straight"], p["corner_in_radius"], p["corner_out_radius"]
@@ -268,12 +289,14 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     for _, t in _fields(cfg.observations.policy):
         if hasattr(t, "func") and _fname(t) == "world_height_map":
             c.scan_offset, c.scan_plane_init = float(t.params["offset"]), float(t.params["plane_init_value"])
-    _lower_rewards(cfg, spec, _ELEV_REWARDS, {}, allow_python_terms)
+    _lower_rewards(cfg, spec, _ELEV_REWARDS, {}, allow_python_terms, device_terms)
     term_bits = {"time_out": 0, "root_height_below_minimum": 1, "stuck": 2, "upright_bool": 3, "close_to_goal": 4}
     if getattr(cfg, "terminations", None) is not None:
         mask = 0
         for name, term in _fields(cfg.terminations):
             fn, p = _fname(term), (term.params or {})
+            if _device_term(spec, name, term, "termination", device_terms):
+                continue
             if fn not in term_bits:
                 if not allow_python_terms:
                     raise NotImplementedError(f"termination term {name} -> {fn} (pass allow_python_terms=True to run it host-side)")
@@ -310,7 +333,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     return spec
 
 
-def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms):
+def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device_terms=False):
     """MushrVisualRLEnvCfg / MushrVisualRLRandomEnvCfg / MushrVisualPlayEnvCfg (visual/mushr_visual_env_cfg.py:412-473)."""
     import numpy as np
     terrain = cfg.scene.terrain
@@ -345,11 +368,13 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms):
     off = cam.offset.pos
     c.vis_cam_pos[0], c.vis_cam_pos[1], c.vis_cam_pos[2] = 0.022995 + float(off[0]), 0.0175 + float(off[1]), 0.162178 + float(off[2])
     spec.obs_dim = 8 + c.vis_cam_w * (c.vis_cam_h - c.vis_cam_row0)
-    _lower_rewards(cfg, spec, _VIS_REWARDS, {}, allow_python_terms)
+    _lower_rewards(cfg, spec, _VIS_REWARDS, {}, allow_python_terms, device_terms)
     if getattr(cfg, "terminations", None) is not None:
         mask = 0
         for name, term in _fields(cfg.terminations):
             fn = _fname(term)
+            if _device_term(spec, name, term, "termination", device_terms):
+                continue
             if fn == "time_out":
                 mask |= 1
             elif fn == "out_of_map":
@@ -371,14 +396,14 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms):
     return spec
 
 
-def env_from_reference_cfg(cfg, render_mode=None, device=None, allow_python_terms: bool = False, **kwargs):
+def env_from_reference_cfg(cfg, render_mode=None, device=None, allow_python_terms: bool = False, device_terms: bool = False, **kwargs):
     """Entry point used by ``shims/isaaclab/envs:ManagerBasedRLEnv`` (gym kwargs: cfg=<env cfg>)."""
     from .env import ManagerBasedRLEnv
     kwargs.pop("env_cfg_entry_point", None); kwargs.pop("rsl_rl_cfg_entry_point", None); kwargs.pop("play_env_cfg_entry_point", None)
     if isinstance(cfg, (str, T.TaskSpec)):           # a gym id / an already lowered TaskSpec instead of a reference cfg object
         return ManagerBasedRLEnv(cfg, render_mode=render_mode, device=device or "cuda:0")
     dev = device or getattr(getattr(cfg, "sim", None), "device", None) or "cuda:0"
-    env = ManagerBasedRLEnv(spec_from_reference_cfg(cfg, allow_python_terms=allow_python_terms), render_mode=render_mode, device=dev)
+    env = ManagerBasedRLEnv(spec_from_reference_cfg(cfg, allow_python_terms=allow_python_terms, device_terms=device_terms), render_mode=render_mode, device=dev)
     env.cfg = cfg                                   # writer.log_config(self.env.cfg, ...) (modified_rsl_rl_runner.py:42-44)
     if not hasattr(cfg, "is_finite_horizon"):
         cfg.is_finite_horizon = False

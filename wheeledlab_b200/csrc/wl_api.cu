@@ -43,6 +43,7 @@ struct wl_sim {
     int step_variant;       // what the most recent wl_step launched (wl_step_launch_info): variant after the automatic choice
     int step_specialised;   // (the duo kernel ran a spec instantiation, not its generic body)
     int step_threads;       // (threads per CTA)
+    struct DevTerms* dterms;   // wl_set_device_terms: the term table and its per-env state (null: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1650,6 +1651,21 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 #include "wl_wide.cuh"
 #include "wl_actor.cuh"
 #include "wl_episode.cuh"
+#include "wl_terms.cuh"
+
+// the handle's device terms: the kernel's table and one device allocation holding the per-env state
+struct DevTerms {
+    TermTable tt;
+    TermBufs b;
+    uint8_t* tbits;     // [N] stage a's built-in termination bits when the handle records none (wl_set_term_bits)
+    void* block;
+};
+static void free_device_terms(wl_sim* sim) {
+    if (!sim->dterms) return;
+    cudaFree(sim->dterms->block);
+    delete sim->dterms;
+    sim->dterms = nullptr;
+}
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2092,7 +2108,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     return WL_OK;
 }
 
-int wl_destroy(wl_sim* sim) { delete sim; return WL_OK; }
+int wl_destroy(wl_sim* sim) { if (sim) free_device_terms(sim); delete sim; return WL_OK; }
 int32_t wl_obs_dim(const wl_sim* sim) { return sim ? sim->obs_dim : 0; }
 int wl_set_scan_tma(wl_sim* sim, int32_t use_tma) {
     if (!sim) return fail(WL_EINVAL, "wl_set_scan_tma: null handle");
@@ -2276,6 +2292,92 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
     return post_step(sim, step_counter, (cudaStream_t)stream);
+}
+
+int wl_set_device_terms(wl_sim* sim, const wl_term_desc* terms, int32_t n_terms) {
+    if (!sim) return fail(WL_EINVAL, "wl_set_device_terms: null handle");
+    if (n_terms < 0 || n_terms > WL_MAX_DEVICE_TERMS) return fail(WL_EINVAL, "wl_set_device_terms: at most 8 device terms");
+    if (n_terms > 0 && !terms) return fail(WL_EINVAL, "wl_set_device_terms: null term table");
+    TermTable tt;
+    memset(&tt, 0, sizeof tt);
+    tt.n = n_terms;
+    const double step_dt = (double)sim->cfg.sim_dt * (double)sim->cfg.decimation;      // TaskSpec.step_dt
+    for (int k = 0; k < n_terms; ++k) {
+        const wl_term_desc& d = terms[k];
+        if (d.kind < 1 || d.kind >= WL_TERM_KINDS) return fail(WL_EINVAL, "wl_set_device_terms: unknown term kind " + std::to_string(d.kind));
+        if (d.role < WL_TERM_ROLE_REWARD || d.role > WL_TERM_ROLE_TIME_OUT) return fail(WL_EINVAL, "wl_set_device_terms: unknown role");
+        if (!std::isfinite(d.weight)) return fail(WL_EINVAL, "wl_set_device_terms: non-finite weight");
+        for (int j = 0; j < 4; ++j)
+            if (!std::isfinite(d.params[j])) return fail(WL_EINVAL, "wl_set_device_terms: non-finite parameter");
+        const bool map = d.kind == WL_TERM_V_IS_TRAVERSABLE || d.kind == WL_TERM_V_IS_TRAVERSABLE_SPEED_SCALED ||
+                         d.kind == WL_TERM_V_VEL_REW_TRAV || d.kind == WL_TERM_V_BOOL_IS_NOT_TRAVERSABLE;
+        if (map && sim->cfg.task != WL_TASK_VISUAL)
+            return fail(WL_EUNSUPPORTED, "wl_set_device_terms: a traversability-map term needs the Visual task");
+        tt.kind[k] = d.kind;
+        tt.role[k] = d.role;
+        tt.scale[k] = d.role == WL_TERM_ROLE_REWARD ? (float)(d.weight * step_dt) : 0.0f;
+        tt.skip[k] = d.role == WL_TERM_ROLE_REWARD && d.weight == 0.0;
+        for (int j = 0; j < 4; ++j) tt.p[k][j] = (float)d.params[j];
+        if (d.kind == WL_TERM_V_OFF_TRACK) tt.p[k][2] = (float)(d.params[1] * d.params[1]);     // corner_out_radius**2 in double
+    }
+    ensure_device(sim);
+    if (n_terms == 0) { free_device_terms(sim); return WL_OK; }
+    const size_t n = (size_t)sim->cfg.num_envs, ctas = (n + WL_TERMS_BS - 1) / WL_TERMS_BS;
+    const size_t o_sums = 0, o_prev = align256(o_sums + WL_MAX_DEVICE_TERMS * n * 4), o_part = align256(o_prev + n * 4),
+                 o_bytes = align256(o_part + ctas * 16 * 4), bytes = o_bytes + 4 * align256(n);
+    // the new table and state are built completely before the old ones are dropped: a failure leaves the handle as it was
+    char* blk = nullptr;
+    if (int rc = cuda_check(cudaMalloc(&blk, bytes), "wl_set_device_terms: allocate")) return rc;
+    DevTerms* dt = new (std::nothrow) DevTerms();
+    if (!dt) { cudaFree(blk); return fail(WL_EINVAL, "wl_set_device_terms: out of host memory"); }
+    // cleared and finished before returning, so that a step on any stream afterwards sees the cleared state
+    int rc = cuda_check(cudaMemset(blk, 0, bytes), "wl_set_device_terms: clear");
+    if (!rc) rc = cuda_check(cudaMemset(blk + o_prev, 0xFF, n * 4), "wl_set_device_terms: clear");    // NaN: not called yet
+    if (!rc) rc = cuda_check(cudaDeviceSynchronize(), "wl_set_device_terms: synchronize");
+    if (rc) { cudaFree(blk); delete dt; return rc; }
+    dt->tt = tt;
+    dt->block = blk;
+    dt->b.sums = reinterpret_cast<float*>(blk + o_sums);
+    dt->b.prev = reinterpret_cast<float*>(blk + o_prev);
+    dt->b.part = reinterpret_cast<float*>(blk + o_part);
+    dt->b.extra_term = reinterpret_cast<uint8_t*>(blk + o_bytes);
+    dt->b.extra_to = dt->b.extra_term + align256(n);
+    dt->b.fired = dt->b.extra_to + align256(n);
+    dt->tbits = dt->b.fired + align256(n);
+    free_device_terms(sim);
+    sim->dterms = dt;
+    return WL_OK;
+}
+
+uint8_t* wl_device_term_masks(const wl_sim* sim) { return (sim && sim->dterms) ? sim->dterms->b.fired : nullptr; }
+
+int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated,
+                  float* d_log, float* d_term_log, int64_t step_counter, void* stream) {
+    if (!sim || !d_action || !d_obs || !d_rew || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_step_terms: null argument");
+    if (((uintptr_t)d_action & 7u) || ((uintptr_t)d_obs & 7u)) return fail(WL_EINVAL, "wl_step_terms: action/obs must be 8-byte aligned");
+    if (int rc = refuse_fan(sim, "wl_step_terms")) return rc;
+    cudaStream_t cs = (cudaStream_t)stream;
+    DevTerms* dt = sim->dterms;
+    if (!dt) return wl_step(sim, d_action, d_obs, d_rew, d_terminated, d_truncated, d_log, step_counter, stream);   // no terms: wl_step itself
+    if (int rc = prep_step(sim, step_counter, 1, cs)) return rc;
+    const uint32_t t = (uint32_t)step_counter;               // negative (device base + k) stays encoded: see decode_step
+    uint8_t* tbits = sim->term_bits ? sim->term_bits : dt->tbits;
+    if (int rc = launch_stage<1>(sim, reinterpret_cast<const float2*>(d_action), nullptr, d_rew, nullptr, nullptr, nullptr, t,
+                                 StageIO{tbits, nullptr, nullptr}, cs)) return rc;
+    const int n = sim->cfg.num_envs, ctas = (n + WL_TERMS_BS - 1) / WL_TERMS_BS;
+    wl_terms_kernel<<<ctas, WL_TERMS_BS, 0, cs>>>(dt->tt, sim->cfg, sim->state, sim->globals, sim->hf, t, d_rew, tbits, dt->b,
+                                                  d_term_log != nullptr);
+    if (int rc = launched(sim, "wl_terms_kernel")) return rc;
+    if (d_term_log) {
+        wl_terms_log_kernel<<<1, 9 * 32, 0, cs>>>(dt->tt, sim->cfg, dt->b.part, ctas, d_term_log);
+        if (int rc = launched(sim, "wl_terms_log_kernel")) return rc;
+    }
+    if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, t,
+                                 StageIO{tbits, dt->b.extra_term, dt->b.extra_to}, cs)) return rc;
+    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
+    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
+        if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc;   // t may be device-relative
+    return post_step(sim, step_counter, cs);
 }
 
 int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_out, float* d_obs, float* d_rew,

@@ -132,6 +132,9 @@ class TerminationManager:
         env = self._env
         if name in getattr(env, "_py_term_masks", {}):
             return env._py_term_masks[name]
+        for k, t in enumerate(getattr(env, "_dev_terms", ())):
+            if t.name == name and t.role != 0:
+                return ((env.sim.device_term_masks >> k) & 1).to(torch.bool)
         names = env.spec.termination_names
         for j, (n, is_to) in enumerate(names):
             if n == name:
@@ -304,6 +307,8 @@ class ManagerBasedRLEnv:
         # host-side (Python) MDP terms: evaluated between the two halves of the staged step (see add_reward_term)
         self._py_rewards, self._py_terms, self._py_obs = [], [], []
         self._py_sums = {}
+        self._dev_terms = []                     # device terms (add_device_reward_term): evaluated by wl_step_terms
+        self._term_log_ring = None
         for name, func, weight, params in self.spec.python_reward_terms:
             self.add_reward_term(name, func, weight, params)
         for name, func, time_out, params in self.spec.python_termination_terms:
@@ -315,6 +320,11 @@ class ManagerBasedRLEnv:
             from ._lib import check, lib
             self._term_bits = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
             check(lib.wl_set_term_bits(self.sim._h, C.c_void_p(self._term_bits.data_ptr())), "wl_set_term_bits")
+        for name, func, role, weight, params in self.spec.device_terms:
+            if role == "reward":
+                self.add_device_reward_term(name, func, weight, params)
+            else:
+                self.add_device_termination_term(name, func, role == "time_out", params)
         # event_manager.apply(mode="startup")
         self.sim.startup()
         self._needs_reset = True
@@ -394,6 +404,7 @@ class ManagerBasedRLEnv:
         func * weight * step_dt, accumulated per episode and logged as Episode_Reward/<name>).  It runs on the
         post-physics, PRE-reset state, exactly where ManagerBasedRLEnv.step calls the reward manager: the env switches
         to the staged step (wl_step_stage_a -> Python terms -> wl_step_stage_b)."""
+        self._refuse_mixing()
         self._py_rewards.append(SimpleNamespace(name=name, func=func, weight=float(weight), params=dict(params or {})))
         self._py_sums[name] = torch.zeros(self.num_envs, dtype=torch.float32, device=self.device)
         self.reward_manager.python_terms = [t.name for t in self._py_rewards]
@@ -401,8 +412,54 @@ class ManagerBasedRLEnv:
     def add_termination_term(self, name: str, func, time_out: bool = False, params: dict | None = None):
         """Register ``func(env, **params) -> [N] bool`` as a termination term (TerminationTermCfg semantics; evaluated
         before the rewards, OR-ed into terminated / time_outs, resets the env in the same step)."""
+        self._refuse_mixing()
         self._py_terms.append(SimpleNamespace(name=name, func=func, time_out=bool(time_out), params=dict(params or {})))
         self.termination_manager.python_terms = [t.name for t in self._py_terms]
+
+    # -- device terms: the reference's unregistered reward / termination functions, in CUDA (device_terms.py) ---------------
+    def _refuse_mixing(self, device: bool = False):
+        if (self._py_rewards or self._py_terms) if device else self._dev_terms:
+            raise NotImplementedError("an env runs either device terms or host-side Python reward / termination terms, not both")
+
+    def _add_device_term(self, name, func, role, weight, params):
+        from . import device_terms as dtm
+        self._refuse_mixing(device=True)
+        tk = dtm.lookup(func) if callable(func) else dtm.resolve(func)
+        if tk is None:
+            raise NotImplementedError(f"device term {name!r}: {getattr(func, '__module__', '?')}.{getattr(func, '__name__', func)} "
+                                      "is not in the device-term library (register it with add_reward_term as a Python term)")
+        if len(self._dev_terms) >= dtm.MAX_TERMS:
+            raise ValueError(f"at most {dtm.MAX_TERMS} device terms per env")
+        if any(t.name == name for t in self._dev_terms):
+            raise ValueError(f"device term {name!r} is already registered")
+        term = SimpleNamespace(name=name, kind=tk, role=role, weight=float(weight), params=dtm.param_values(tk, params))
+        table = [(t.kind.kind, t.role, t.weight, t.params) for t in self._dev_terms + [term]]
+        self.sim.set_device_terms(table)          # (refuses a map term off the Visual task; resets the terms' state)
+        self._dev_terms.append(term)
+        if self._term_bits is None:               # get_term of a built-in term: its own mask, not the union with the device terms
+            import ctypes as C
+            from ._lib import check, lib
+            self._term_bits = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
+            check(lib.wl_set_term_bits(self.sim._h, C.c_void_p(self._term_bits.data_ptr())), "wl_set_term_bits")
+
+    def add_device_reward_term(self, name: str, func, weight: float, params: dict | None = None):
+        """Register a library function (device_terms.REGISTRY: the reference function object, or a kind) as a reward
+        term evaluated on the device: the same value, weighting, episode sums and Episode_Reward/<name> entry as
+        add_reward_term would give it, inside env.step's launches (wl_step_terms) and capturable in a graph."""
+        from .device_terms import ROLE_REWARD
+        self._add_device_term(name, func, ROLE_REWARD, weight, params)
+
+    def add_device_termination_term(self, name: str, func, time_out: bool = False, params: dict | None = None):
+        """Register a library function as a termination term evaluated on the device (fires when its value is nonzero;
+        time_out=True truncates instead of terminating); get_term(name) and Episode_Termination/<name> cover it."""
+        from .device_terms import ROLE_TERMINATION, ROLE_TIME_OUT
+        self._add_device_term(name, func, ROLE_TIME_OUT if time_out else ROLE_TERMINATION, 0.0, params)
+
+    @property
+    def device_log_names(self) -> list:
+        """The extras["log"] keys of the device terms, in table order (the order of wl_step_terms' term_log)."""
+        from .device_terms import ROLE_REWARD
+        return [("Episode_Reward/" if t.role == ROLE_REWARD else "Episode_Termination/") + t.name for t in self._dev_terms]
 
     def add_observation_term(self, name: str, func, params: dict | None = None):
         """Register ``func(env, **params) -> [N, k]``; appended to the policy observation (after the built-in terms)."""
@@ -501,7 +558,13 @@ class ManagerBasedRLEnv:
         out, log = self._step_ring[t % self._ring_len]
         if not self.log_episode_info:
             log = None
-        obs, rew, term_u8, trunc_u8 = self.sim.step(action, t, out=out, log=log)
+        if self._dev_terms:
+            if self._term_log_ring is None:
+                self._term_log_ring = torch.zeros((self._ring_len, 8), dtype=torch.float32, device=self.device)
+            term_log = self._term_log_ring[t % self._ring_len] if log is not None else None
+            obs, rew, term_u8, trunc_u8 = self.sim.step_terms(action, t, out=out, log=log, term_log=term_log)
+        else:
+            obs, rew, term_u8, trunc_u8 = self.sim.step(action, t, out=out, log=log)
         self.common_step_counter = t + 1
         # curriculum: applied by the step kernel's last CTA (uses the incremented counter and fires only if >= 1 env
         # reset, like the reference's call from _reset_idx) -- no host logic, no sync
@@ -509,13 +572,15 @@ class ManagerBasedRLEnv:
         tm = self.termination_manager
         tm.terminated, tm.time_outs = terminated, truncated
         if log is not None:
-            self.extras["log"] = self._episode_log(log)
+            self.extras["log"] = self._episode_log(log, term_log if self._dev_terms else None)
         return {"policy": self._append_py_obs(obs)}, rew, terminated, truncated, self.extras
 
-    def _episode_log(self, log: torch.Tensor):
+    def _episode_log(self, log: torch.Tensor, term_log: torch.Tensor | None = None):
         """extras["log"] (RewardManager/TerminationManager.reset, SURVEY Appendix B): lazy views of the row the step
-        kernel's last CTA wrote -- device tensors, no extra launches, no host sync."""
-        return _LazyLog(log, self._log_index, env=self)
+        kernel's last CTA wrote -- device tensors, no extra launches, no host sync.  The device terms' entries are views
+        of the term_log row wl_step_terms wrote."""
+        extra = None if term_log is None else {k: term_log[j] for j, k in enumerate(self.device_log_names)}
+        return _LazyLog(log, self._log_index, extra, env=self)
 
     def step_host(self, action_host: torch.Tensor):
         """env.step() for a HOST-side caller: `action_host` is a CPU tensor [N,2] (pinned for best speed).  One C call
@@ -524,8 +589,8 @@ class ManagerBasedRLEnv:
         result views are overwritten by the next step_host call.  With ``env.host_obs = True`` the observations are returned in
         pinned HOST memory as well (a ring of _RING buffers): D2H copy after the step (transport "copy") or written by the
         kernel over PCIe (transport "zero_copy")."""
-        if self._py_rewards or self._py_terms:
-            raise NotImplementedError("step_host: host-side Python terms need the staged step (use env.step)")
+        if self._py_rewards or self._py_terms or self._dev_terms:
+            raise NotImplementedError("step_host: Python and device terms need the staged step (use env.step)")
         if self._needs_reset:
             self.reset()
         if self._host_io is None:
@@ -592,6 +657,11 @@ class ManagerBasedRLEnv:
         return self._host_io["h_action"]
 
 
-def make(task_id: str, cfg=None, render_mode=None, device="cuda:0", **kw) -> ManagerBasedRLEnv:
-    """gym.make(<id>, cfg=...) equivalent for the registered WheeledLab ids."""
+def make(task_id: str, cfg=None, render_mode=None, device="cuda:0", device_terms: bool = False, allow_python_terms: bool = False,
+         **kw) -> ManagerBasedRLEnv:
+    """gym.make(<id>, cfg=...) equivalent for the registered WheeledLab ids.  `cfg` may also be a reference env-cfg object,
+    lowered by compat.spec_from_reference_cfg with `device_terms` / `allow_python_terms`."""
+    if cfg is not None and not isinstance(cfg, (str, TaskSpec)):
+        from .compat import spec_from_reference_cfg
+        cfg = spec_from_reference_cfg(cfg, allow_python_terms=allow_python_terms, device_terms=device_terms)
     return ManagerBasedRLEnv(cfg if cfg is not None else task_id, render_mode=render_mode, device=device, **kw)

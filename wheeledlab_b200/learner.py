@@ -548,6 +548,20 @@ class PPOIteration:
         return self.stats
 
 
+def device_terms_iteration(env, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu",
+                           exchange: PPOExchange | None = None) -> PPOIteration:
+    """``PPOIteration`` (episode statistics on) for an env with device terms (``env.add_device_reward_term``): the rollout
+    is T x (``policy_act``, ``wl_step_terms``) on device counters, captured in the same graph as the episode statistics,
+    bootstrap, GAE and the update; ``exchange`` makes it one rank of a data-parallel run.  The read-back block carries the
+    rollout's ``term_logs`` [T, 8] f32 after the episode-log rows."""
+    from .policy import FusedPolicyRollout
+    sim = env.sim
+    roll = FusedPolicyRollout(sim, blob, T, activation=activation, device_terms=True)
+    it = PPOIteration(sim, blob, cfg, T, activation, episode_stats=True, exchange=exchange, rollout=roll, extra_readback_bytes=4 * 8 * T)
+    roll.term_logs = it.readback_extra.view(torch.float32).view(T, 8)
+    return it
+
+
 class StagedPPOIteration(PPOIteration):
     """``PPOIteration`` for an env with host-side Python reward / termination terms, on one GPU: the rollout is
     ``policy.StagedPolicyRollout`` (T x (policy, ``env.staged_step``), eager: the terms are arbitrary torch code), and
@@ -697,7 +711,9 @@ class FusedOnPolicyRunner:
     GPU through ``StagedPPOIteration``: the rollout runs eagerly, T x (policy, staged step with the terms in between), and
     the rest of the iteration is the same graph; the log gains ``Episode_Reward/<name>`` / ``Episode_Termination/<name>``
     for each Python term, the T-step mean of what env.step's ``extras["log"]`` holds for it.  Python observation terms and
-    data-parallel runs with Python terms raise ``NotImplementedError``.
+    data-parallel runs with Python terms raise ``NotImplementedError``.  An env with device terms (``add_device_reward_term``)
+    trains through ``device_terms_iteration``: its rollout (``policy_act`` then ``wl_step_terms``) is part of the one graph,
+    on one GPU or data-parallel, and the log gains each device term's ``Episode_*`` key as its T-step mean.
 
     The agent cfg dict is read for ``num_steps_per_env``, ``save_interval``, ``policy`` (``activation_from_rsl_rl``,
     ``init_noise_std``) and ``algorithm`` (``PPOConfig.from_rsl_rl``).  The weights start as the reference's do: torch
@@ -735,6 +751,7 @@ class FusedOnPolicyRunner:
             raise NotImplementedError("Python observation terms (add_observation_term) widen the observation past the slab row the "
                                       "staged step writes: an env with host-side Python terms trains with reward and termination terms only")
         self.staged = bool(getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None))
+        self.dev_names = e.device_log_names if getattr(e, "_dev_terms", None) else []
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
@@ -753,8 +770,9 @@ class FusedOnPolicyRunner:
             self.it = StagedPPOIteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation)
         else:
             exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
-            self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True,
-                                   exchange=exchange)
+            self.it = device_terms_iteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, exchange) \
+                if self.dev_names else PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation,
+                                                    episode_stats=True, exchange=exchange)
         self.alg = self.it.ppo
         self.current_learning_iteration = 0
         self.callback = None
@@ -798,6 +816,9 @@ class FusedOnPolicyRunner:
                 log["Train/mean_reward"] = st.mean_return
                 log["Train/mean_episode_length"] = st.mean_length
             log.update({name: logs[col] for name, col in names})
+            if self.dev_names:                        # the device terms' entries: T-step means of env.step's extras["log"]
+                dev = rb[rb.numel() - 4 * 8 * T:].view(torch.float32).view(T, 8)[:, :len(self.dev_names)].double().mean(0).tolist()
+                log.update(zip(self.dev_names, dev))
             if self.staged and it.roll.py_names:      # the Python terms' entries: T-step means of env.step's extras["log"]
                 py = rb[rb.numel() - 8 * T * len(it.roll.py_names):].view(torch.float64).view(T, -1).mean(0).tolist()
                 log.update(zip(it.roll.py_names, py))

@@ -219,12 +219,22 @@ class FusedPolicyRollout:
     ``deterministic=True`` plays the policy instead (play_policy.py's loop): the action is the actor mean, with no critic and
     no noise -- T x wl_act_infer_step for "elu", T x (wl_actor_mean, then wl_step) for "relu" -- and the slab has no
     policy fields.  ``slab.obs[k]`` / ``slab.actions[k]`` are what play_policy.py appends at step k, so
-    ``recording.save_slab(playback_dir, play_name, roll.slab)`` writes its rollouts file."""
+    ``recording.save_slab(playback_dir, play_name, roll.slab)`` writes its rollouts file.
+
+    ``device_terms=True`` rolls out an env whose handle has device terms (``wl_set_device_terms``): T x (``policy_act``,
+    then ``wl_step_terms``) on the same device counters, still one graph; ``term_logs[k]`` [T, 8] receives step k's
+    device-term ``Episode_*`` entries.  A graph must be captured after the handle's terms are set."""
 
     def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu",
-                 deterministic: bool = False):
+                 deterministic: bool = False, device_terms: bool = False):
         self.sim, self.blob, self.T, self.activation = sim, blob, T, check_activation(activation)
         self.deterministic = bool(deterministic)
+        self.device_terms = bool(device_terms)
+        if self.device_terms and self.deterministic:
+            raise ValueError("device_terms: the training rollout only")
+        if self.device_terms and (sim.num_envs * sim.obs_dim) % 2:
+            raise ValueError("the slab's observation rows are written pair-wise: num_envs * obs_dim must be even")
+        self.term_logs = torch.zeros((T, 8), dtype=torch.float32, device=sim.device) if self.device_terms else None
         if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
             raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
         self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=not self.deterministic)
@@ -253,6 +263,10 @@ class FusedPolicyRollout:
                 else:
                     act_infer_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.slab.step_outputs(k),
                                    self.logs[k], t)
+            elif self.device_terms:
+                policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
+                           self.pol.values[k], t, self.activation)
+                self.sim.step_terms(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k], term_log=self.term_logs[k])
             elif self.activation == "relu":
                 policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
                            self.pol.values[k], t)

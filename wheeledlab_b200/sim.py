@@ -36,6 +36,14 @@ def upload_graph(graph: "torch.cuda.CUDAGraph", stream=None):
     check(lib.wl_graph_upload(C.c_void_p(int(graph.raw_cuda_graph_exec())), C.c_void_p(st.cuda_stream)), "wl_graph_upload")
 
 
+def _device_u8_view(ptr: int, n: int, device) -> torch.Tensor:
+    """uint8 [n] tensor over device memory the library owns (through __cuda_array_interface__; torch does not own it)."""
+    class _Arr:
+        __cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (int(ptr), False), "version": 3}
+    with torch.cuda.device(device):
+        return torch.as_tensor(_Arr(), device=device)
+
+
 class WheeledSim:
     def __init__(self, spec: TaskSpec, device: str | torch.device = "cuda:0", heightfield: torch.Tensor | None = None):
         self.spec = spec
@@ -260,6 +268,41 @@ class WheeledSim:
                                   C.c_void_p(log.data_ptr()) if log is not None else None, step_counter, _stream_ptr(dev)),
               "wl_step_stage_b")
         return obs, term, trunc
+
+    def set_device_terms(self, terms):
+        """The handle's device terms (wl_set_device_terms): a list of (kind, role, weight, params[<= 4]) in evaluation
+        order; [] clears them.  Resets their per-env state (episode sums, elevation_continuity's previous elevation)."""
+        n = len(terms)
+        arr = (_lib.WlTermDesc * max(1, n))()
+        for k, (kind, role, weight, params) in enumerate(terms):
+            p = list(params) + [0.0] * (4 - len(params))
+            arr[k] = _lib.WlTermDesc(int(kind), int(role), float(weight), (C.c_double * 4)(*p))
+        with torch.cuda.device(self.device):
+            check(lib.wl_set_device_terms(self._h, arr, n), "wl_set_device_terms")
+
+    @property
+    def device_term_masks(self) -> torch.Tensor | None:
+        """uint8 [N] view: bit k = device term k fired in the most recent step_terms (None without device terms)."""
+        ptr = lib.wl_device_term_masks(self._h)
+        if not ptr:
+            return None
+        if getattr(self, "_dt_masks", None) is None or self._dt_masks.data_ptr() != ptr:
+            self._dt_masks = _device_u8_view(ptr, self.num_envs, self.device)
+        return self._dt_masks
+
+    def step_terms(self, action: torch.Tensor, step_counter: int = -1, out=None, log: torch.Tensor | None = None,
+                   term_log: torch.Tensor | None = None):
+        """step() with the device terms between stage a and stage b (wl_step_terms): same arguments and outputs, plus
+        `term_log` (float32[8] device tensor or None) receiving the device terms' Episode_* entries of this step."""
+        n = self.num_envs
+        if out is None:
+            out = (torch.empty((n, self.obs_dim), dtype=torch.float32, device=self.device), torch.empty(n, dtype=torch.float32, device=self.device),
+                   torch.empty(n, dtype=torch.uint8, device=self.device), torch.empty(n, dtype=torch.uint8, device=self.device))
+        obs, rew, term, trunc = out
+        ptr = lambda x: C.c_void_p(x.data_ptr()) if x is not None else None
+        check(lib.wl_step_terms(self._h, ptr(action), ptr(obs), ptr(rew), ptr(term), ptr(trunc), ptr(log), ptr(term_log),
+                                step_counter, _stream_ptr(self.device)), "wl_step_terms")
+        return obs, rew, term, trunc
 
     def observe(self, step_counter: int, call_idx: int = 0, out: torch.Tensor | None = None):
         obs = out if out is not None else torch.empty((self.num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
