@@ -594,6 +594,65 @@ int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_
 int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter,
                       void* stream);
 
+/* ---- the asymmetric actor-critic: a privileged critic observation group (DESIGN.md 6m) -----------------------------------
+ * rsl_rl's ActorCritic(num_actor_obs, num_critic_obs, ...) fed from extras["observations"]["critic"]
+ * (modified_rsl_rl_runner.py:51, :77-82): the actor reads the policy row, the critic a second row of its own width.
+ * Drift family only (policy obs_dim <= 16, ELU), critic width Dc <= WL_MAX_CRITIC_OBS.
+ *
+ * The critic row is the concatenation, in table order, of terms of this library; no noise is ever added:
+ *   kind                         width  content
+ *   WL_CRITIC_ROOT_POS_W           3    root position, world frame          } the BlindObsCfg terms, formed as the
+ *   WL_CRITIC_ROOT_EULER_XYZ       3    roll, pitch, yaw wrapped to [0, 2pi) } policy row forms them, without the
+ *   WL_CRITIC_BASE_LIN_VEL         3    linear velocity, body frame          } noise draw
+ *   WL_CRITIC_BASE_ANG_VEL         3    angular velocity, body frame         }
+ *   WL_CRITIC_LAST_ACTION          2    action_manager.action                }
+ *   WL_CRITIC_JOINT_VEL            4    throttle joint velocities [bl, br, fl, fr] (state group WL_G_WHEEL)
+ *   WL_CRITIC_JOINT_POS            2    steer joint positions L, R (WL_G_STEER)
+ *   WL_CRITIC_WHEEL_FRICTION       4    per-wheel peak friction coefficient of the env's DR bucket (WL_G_PMU_D)
+ *   WL_CRITIC_BASE_MASS            1    total mass (WL_G_PMASS)
+ *   WL_CRITIC_MOTOR_DAMPING        4    DC-motor damping per wheel (WL_G_PKD)
+ * clip > 0 clamps the term's floats to [-clip, clip] (ObservationTermCfg.clip, symmetric); 0 = no clip. */
+#define WL_MAX_CRITIC_OBS   32
+#define WL_MAX_CRITIC_TERMS 16
+#define WL_CRITIC_ROOT_POS_W      1
+#define WL_CRITIC_ROOT_EULER_XYZ  2
+#define WL_CRITIC_BASE_LIN_VEL    3
+#define WL_CRITIC_BASE_ANG_VEL    4
+#define WL_CRITIC_LAST_ACTION     5
+#define WL_CRITIC_JOINT_VEL       6
+#define WL_CRITIC_JOINT_POS       7
+#define WL_CRITIC_WHEEL_FRICTION  8
+#define WL_CRITIC_BASE_MASS       9
+#define WL_CRITIC_MOTOR_DAMPING  10
+#define WL_CRITIC_KINDS          11
+typedef struct wl_critic_term {
+    int32_t kind;        /* WL_CRITIC_* */
+    float clip;          /* symmetric clip bound, 0 = none */
+} wl_critic_term;
+/* Store the handle's critic table (a host-side set-up call: nothing is launched or allocated, and a failure leaves the
+ * handle as it was).  n_terms = 0 clears it.  WL_EINVAL: null handle, n_terms outside 0..WL_MAX_CRITIC_TERMS, a null table
+ * with n_terms > 0, an unknown kind, a negative or non-finite clip, a total width above WL_MAX_CRITIC_OBS;
+ * WL_EUNSUPPORTED: a task other than the Drift family.  A graph captured with the old table keeps the old table. */
+int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_terms);
+/* Dc: the width of the critic row (0 with no table) */
+int32_t wl_critic_obs_dim(const wl_sim* sim);
+/* d_critic_obs [N, Dc] (rows leave as 16-byte stores when it is 16-byte aligned) from the state the most recent step / reset left -- after wl_step, the
+ * post-reset state its observation row was formed from.  One launch, no generator and no counter; capturable.  For a handle
+ * whose noise_std are all 0 the five BlindObsCfg columns equal the policy row of wl_step (as fp32 values; a -0 that the
+ * policy row's "+ 0 * z" turned into +0 stays -0 here).  WL_EINVAL: a null pointer or one not 4-byte aligned, no table. */
+int wl_critic_observe(wl_sim* sim, float* d_critic_obs, void* stream);
+/* wl_policy_blob_floats with the critic's W1t block sized by critic_obs_dim: W1t[ceil4(critic_obs_dim)][64].  For
+ * critic_obs_dim == obs_dim the offsets and the total are wl_policy_blob_floats's. */
+int32_t wl_policy_blob_floats_asym(int32_t obs_dim, int32_t critic_obs_dim, int32_t offsets[13]);
+/* wl_policy_act_elu with the critic's first layer fed from d_critic_obs_in [N, critic_obs_dim] and a blob laid out by
+ * wl_policy_blob_floats_asym(obs_dim, critic_obs_dim).  The same CTA geometry, blob copies, layer tiles, head butterfly and
+ * policy noise: actions, mean and log-prob equal wl_policy_act_elu's for the same d_obs_in and actor blocks bit for bit,
+ * whatever the critic input is, and with critic_obs_dim == obs_dim and d_critic_obs_in == d_obs_in the value does too.
+ * Returns before any launch as wl_policy_act_elu does, plus WL_EINVAL for a null / misaligned d_critic_obs_in or
+ * critic_obs_dim outside 1..WL_MAX_CRITIC_OBS. */
+int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
+                       const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream);
+
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out
  * bootstrap of PPO.process_env_step (rewards += gamma * values * time_outs) folded in when d_time_outs != NULL:
@@ -690,6 +749,17 @@ size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_b
  * mini-batch's reduced gradient (before clipping) after the call. */
 int wl_ppo_update(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
                   float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* wl_ppo_update for the asymmetric network (rsl_rl PPO.update() with privileged observations): the critic's layer-1 forward
+ * and its dW1 are taken over d_critic_obs [batch, critic_obs_dim] (slab order, gathered through the same perm), the blob /
+ * moments are laid out by wl_policy_blob_floats_asym(params->obs_dim, critic_obs_dim).  The same three kernels per
+ * mini-batch, no float atomics, rows summed in CTA order; padding floats of the blob are never stepped.  With
+ * critic_obs_dim == obs_dim and d_critic_obs == batch->obs it leaves blob, moments and state equal to wl_ppo_update's, bit
+ * for bit.  critic_obs_dim in 1..WL_MAX_CRITIC_OBS; d_critic_obs 4-byte aligned; otherwise wl_ppo_update's checks. */
+size_t wl_ppo_asym_workspace_bytes(int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches);
+int wl_ppo_update_asym(const wl_ppo_params* params, const wl_ppo_batch* batch, const float* d_critic_obs, int32_t critic_obs_dim,
+                       float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes,
+                       void* stream);
 
 /* ---- the wide actor-critic: the Elevation / Visual policy and its PPO update -------------------------------------------
  * The same network and blob layout as above with ReLU instead of ELU between the layers (the reference's Elevation and

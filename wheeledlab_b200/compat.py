@@ -5,7 +5,8 @@
 ``shims/isaaclab``) to the entry point.  This module reads that object -- terms are recognised by the NAME of the
 function they reference, values are taken from the cfg (weights, params, dt, decimation, scales, noise, DR ranges) --
 and fills a ``TaskSpec``.  A term the kernels do not implement raises ``NotImplementedError`` (no silent fallback); the
-observation group is validated term by term (function, order, clip; BlindObs noise stds are read from the cfg).
+observation group is validated term by term (function, order, clip; BlindObs noise stds are read from the cfg).  A ``critic``
+group next to ``policy`` (Drift family) is lowered to the term table of the critic observation kernel (privileged.py).
 
 Reference files: wheeledlab_tasks/drifting/mushr_drift_env_cfg.py, f1tenth_drift_env_cfg.py,
 elevation/mushr_elevation_env_cfg.py, common/{actions,observations}.py.
@@ -89,6 +90,31 @@ def _validate_obs(cfg, expected, c, blind=False):
                     raise NotImplementedError(f"{name}: only zero-mean additive Gaussian noise is implemented")
                 std = float(n.std)
             c.noise_std[k] = std
+
+
+def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
+    """``cfg.observations.critic`` (an ObservationGroupCfg next to ``policy``) -> ``spec.critic_terms``, the term table of
+    ``wl_critic_observe``.  Anything the kernels do not do raises NotImplementedError naming the term; no group, no table."""
+    group = getattr(cfg.observations, "critic", None)
+    if group is None:
+        return
+    from . import privileged
+    if kind != "drift":
+        raise NotImplementedError(f"a critic observation group on the {kind.capitalize()} task is not implemented "
+                                  "(the asymmetric actor-critic covers the Drift family)")
+    if getattr(group, "concatenate_terms", True) is not True:
+        raise NotImplementedError("critic observation group: concatenate_terms=False is not implemented")
+    table = []
+    for name, t in _fields(group):
+        if not hasattr(t, "func"):
+            continue
+        noise = getattr(t, "noise", None) if getattr(group, "enable_corruption", False) or getattr(t, "noise", None) is not None else None
+        fn, clip = privileged.lower_term(name, t.func, getattr(t, "params", None), getattr(t, "clip", None), noise, getattr(t, "scale", None))
+        table.append((name, fn, clip))
+    if not table:
+        raise NotImplementedError("critic observation group: no terms")
+    privileged.check_width([(fn, c) for _, fn, c in table], "critic observation group " + ", ".join(n for n, _, _ in table))
+    spec.critic_terms = table
 
 
 def _lower_common(cfg, spec: T.TaskSpec):
@@ -213,6 +239,8 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     num_envs = int(cfg.scene.num_envs)
     seed = int(cfg.seed) if getattr(cfg, "seed", None) is not None else 42
     kind = _task_kind(cfg)
+    if getattr(cfg.observations, "critic", None) is not None and kind != "drift":
+        _lower_critic(cfg, None, kind)                      # (refused by name before anything is lowered)
     if kind == "visual":
         return _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device_terms)
     if kind == "drift":
@@ -225,6 +253,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
         c = spec.cfg
         _lower_common(cfg, spec)
         _validate_obs(cfg, _OBS_BLIND, c, blind=True)
+        _lower_critic(cfg, spec, kind)
 
         def h_slip(p):
             c.slip_min_thresh, c.slip_max_thresh = p["min_thresh"], p["max_thresh"]

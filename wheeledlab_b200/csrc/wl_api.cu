@@ -14,6 +14,8 @@
 
 using namespace wl;
 
+#include "wl_critic.cuh"
+
 // ---------------------------------------------------------------------------------------
 // handle
 // ---------------------------------------------------------------------------------------
@@ -44,6 +46,7 @@ struct wl_sim {
     int step_specialised;   // (the duo kernel ran a spec instantiation, not its generic body)
     int step_threads;       // (threads per CTA)
     struct DevTerms* dterms;   // wl_set_device_terms: the term table and its per-env state (null: none)
+    CriticTable critic;        // wl_set_critic_terms: the critic observation's columns (n_cols = 0: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -796,12 +799,13 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 struct PolicyOffsets { int32_t o[13]; };
 
-static int policy_offsets(int obs_dim, int32_t off[13]) {
+// critic_obs_dim: the width of the critic's input (the asymmetric network); 0 = obs_dim
+static int policy_offsets(int obs_dim, int32_t off[13], int critic_obs_dim = 0) {
     auto al = [](int x) { return (x + 3) & ~3; };
     int p = 0;
     for (int net = 0; net < 2; ++net) {
-        const int out = net == 0 ? 2 : 1;
-        off[net * 6 + 0] = p; p = al(p + al(obs_dim) * WL_HID);      // rows padded to a multiple of 4 (zeros)
+        const int out = net == 0 ? 2 : 1, in = (net == 1 && critic_obs_dim > 0) ? critic_obs_dim : obs_dim;
+        off[net * 6 + 0] = p; p = al(p + al(in) * WL_HID);           // rows padded to a multiple of 4 (zeros)
         off[net * 6 + 1] = p; p = al(p + WL_HID);
         off[net * 6 + 2] = p; p = al(p + WL_HID * WL_HID);
         off[net * 6 + 3] = p; p = al(p + WL_HID);
@@ -1032,15 +1036,21 @@ wl_act_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict_
 // mlp_tile_layer tiles, quad head butterfly and policy noise (global env id, decoded counter), so actions, mean, log-prob
 // and value equal what wl_act_step stores, bit for bit.  No janitor CTA, no env state, no episode log.  It does not trigger
 // dependents early: a step launched after it with PDL waits for every action.
-__global__ void __launch_bounds__(WL_ACT_THREADS)
-wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* __restrict__ gl, const float* __restrict__ obs_in,
-                         const float* __restrict__ blob, int blob_floats, PolicyOffsets po_off, wl_policy_out po, uint32_t t_arg,
-                         int obs_dim) {
+// ASYM (wl_policy_act_asym): the critic's first layer reads a second staged row, critic_in [N, critic_dim] padded to
+// WL_ACT_XC floats, and the blob's critic W1t block has ceil4(critic_dim) rows; everything else is the same code, so the
+// actor's outputs do not depend on the critic input and the critic's keep their summation order.
+#define WL_ACT_XC 36                             // padded critic observation row (critic_dim <= 32)
+template <bool ASYM>
+__device__ __forceinline__ void policy_act_elu_body(const wl_config& c, const wl_globals* __restrict__ gl, const float* __restrict__ obs_in,
+                                                    const float* __restrict__ critic_in, int critic_dim, const float* __restrict__ blob,
+                                                    int blob_floats, const PolicyOffsets& po_off, const wl_policy_out& po, uint32_t t_arg,
+                                                    int obs_dim) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar[2];
     float* sw = smem;                                        // the whole weight blob
     float* sx = smem + blob_floats;                          // [32][WL_ACT_XS]
     float* sh = sx + WL_ACT_ENVS * WL_ACT_XS;                // [32][WL_ACT_HS]
+    float* sxc = sh + WL_ACT_ENVS * WL_ACT_HS;               // ASYM: [32][WL_ACT_XC]
     if (threadIdx.x == 0) {                                  // first-layer blocks on mbar[0], the rest on mbar[1]
         mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
         mbar_init_fence();
@@ -1061,6 +1071,12 @@ wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* 
         const int eq = k >> 4, j = k & 15, ei = min(blockIdx.x * WL_ACT_ENVS + eq, n - 1);
         sx[eq * WL_ACT_XS + j] = j < obs_dim ? obs_in[(size_t)ei * obs_dim + j] : 0.0f;
     }
+    if constexpr (ASYM) {
+        for (int k = threadIdx.x; k < WL_ACT_ENVS * 32; k += WL_ACT_THREADS) {
+            const int eq = k >> 5, j = k & 31, ei = min(blockIdx.x * WL_ACT_ENVS + eq, n - 1);
+            sxc[eq * WL_ACT_XC + j] = j < critic_dim ? critic_in[(size_t)ei * critic_dim + j] : 0.0f;
+        }
+    }
     float z0 = 0.0f, z1 = 0.0f;
     if (head) policy_noise(c.seed, L.gid, t, z0, z1);
     __syncthreads();                                         // mbarrier init visible to every waiter; obs rows written
@@ -1073,7 +1089,8 @@ wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* 
         const int oW2 = net ? po_off.o[8] : po_off.o[2], oB2 = net ? po_off.o[9] : po_off.o[3];
         float acc[4][4];
         float* h0 = sh + env0 * WL_ACT_HS + net * WL_HID;
-        mlp_tile_layer(sw + oW1 + ucol, sw + oB1 + ucol, sx + env0 * WL_ACT_XS, WL_ACT_XS, nin1, acc);
+        if (ASYM && net) mlp_tile_layer(sw + oW1 + ucol, sw + oB1 + ucol, sxc + env0 * WL_ACT_XC, WL_ACT_XC, (critic_dim + 3) & ~3, acc);
+        else mlp_tile_layer(sw + oW1 + ucol, sw + oB1 + ucol, sx + env0 * WL_ACT_XS, WL_ACT_XS, nin1, acc);
         mlp_tile_store_elu(h0 + ucol, WL_ACT_HS, acc);
         __syncwarp();
         mbar_wait_parity(&mbar[1], 0);
@@ -1106,6 +1123,18 @@ wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* 
         po.log_prob[L.i] = lp;
         po.value[L.i] = vv;
     }
+}
+__global__ void __launch_bounds__(WL_ACT_THREADS)
+wl_policy_act_elu_kernel(const __grid_constant__ wl_config c, const wl_globals* __restrict__ gl, const float* __restrict__ obs_in,
+                         const float* __restrict__ blob, int blob_floats, PolicyOffsets po_off, wl_policy_out po, uint32_t t_arg,
+                         int obs_dim) {
+    policy_act_elu_body<false>(c, gl, obs_in, nullptr, 0, blob, blob_floats, po_off, po, t_arg, obs_dim);
+}
+__global__ void __launch_bounds__(WL_ACT_THREADS)
+wl_policy_act_asym_kernel(const __grid_constant__ wl_config c, const wl_globals* __restrict__ gl, const float* __restrict__ obs_in,
+                          const float* __restrict__ critic_in, int critic_dim, const float* __restrict__ blob, int blob_floats,
+                          PolicyOffsets po_off, wl_policy_out po, uint32_t t_arg, int obs_dim) {
+    policy_act_elu_body<true>(c, gl, obs_in, critic_in, critic_dim, blob, blob_floats, po_off, po, t_arg, obs_dim);
 }
 
 // K consecutive env.step()s in ONE launch (synthetic / scripted-action rollouts, SURVEY 7.7): the state stays in registers
@@ -2519,6 +2548,42 @@ int32_t wl_policy_blob_floats(int32_t obs_dim, int32_t offsets[13]) {
     int32_t tmp[13];
     return policy_offsets(obs_dim, offsets ? offsets : tmp);
 }
+int32_t wl_policy_blob_floats_asym(int32_t obs_dim, int32_t critic_obs_dim, int32_t offsets[13]) {
+    int32_t tmp[13];
+    return policy_offsets(obs_dim, offsets ? offsets : tmp, critic_obs_dim);
+}
+
+int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_terms) {
+    if (!sim) return fail(WL_EINVAL, "wl_set_critic_terms: null handle");
+    if (n_terms < 0 || n_terms > WL_MAX_CRITIC_TERMS) return fail(WL_EINVAL, "wl_set_critic_terms: at most 16 critic terms");
+    if (n_terms > 0 && !terms) return fail(WL_EINVAL, "wl_set_critic_terms: null term table");
+    if (sim->cfg.task != WL_TASK_DRIFT) return fail(WL_EUNSUPPORTED, "wl_set_critic_terms: the critic observation is implemented for the Drift family only");
+    CriticTable tb;
+    memset(&tb, 0, sizeof tb);
+    for (int k = 0; k < n_terms; ++k) {
+        const wl_critic_term& d = terms[k];
+        if (d.kind < 1 || d.kind >= WL_CRITIC_KINDS) return fail(WL_EINVAL, "wl_set_critic_terms: unknown term kind " + std::to_string(d.kind));
+        if (!std::isfinite(d.clip) || d.clip < 0.0f) return fail(WL_EINVAL, "wl_set_critic_terms: clip must be finite and >= 0");
+        if (tb.n_cols + critic_width(d.kind) > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, "wl_set_critic_terms: the critic row is wider than 32 floats");
+        for (int j = 0; j < critic_width(d.kind); ++j) {
+            tb.src[tb.n_cols] = (uint8_t)(critic_first(d.kind) + j);
+            tb.clip[tb.n_cols++] = d.clip;
+        }
+        tb.groups |= critic_groups(d.kind);
+    }
+    sim->critic = tb;
+    return WL_OK;
+}
+int32_t wl_critic_obs_dim(const wl_sim* sim) { return sim ? sim->critic.n_cols : 0; }
+int wl_critic_observe(wl_sim* sim, float* d_critic_obs, void* stream) {
+    if (!sim || !d_critic_obs) return fail(WL_EINVAL, "wl_critic_observe: null argument");
+    if ((uintptr_t)d_critic_obs & 3u) return fail(WL_EINVAL, "wl_critic_observe: d_critic_obs must be 4-byte aligned");
+    if (sim->critic.n_cols < 1) return fail(WL_EINVAL, "wl_critic_observe: no critic table (wl_set_critic_terms)");
+    ensure_device(sim);
+    const int n = sim->cfg.num_envs;
+    wl_critic_observe_kernel<<<(n + WL_CRITIC_BS - 1) / WL_CRITIC_BS, WL_CRITIC_BS, 0, (cudaStream_t)stream>>>(sim->critic, sim->state, n, d_critic_obs);
+    return launched(sim, "wl_critic_observe_kernel");
+}
 
 // wl_act_step and wl_act_infer_step: the same launch of wl_act_step_quad_kernel<task, infer> (arguments checked by the caller
 // for null)
@@ -2570,6 +2635,36 @@ int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_
     const wl_policy_out out{d_actions, nullptr, nullptr, nullptr};
     return act_step_launch(true, "wl_act_infer_step", sim, d_obs_in, d_policy_blob, out, d_obs, d_rew, d_terminated, d_truncated, d_log,
                            step_counter, stream);
+}
+
+int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
+                       const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
+    const char* fn = "wl_policy_act_asym";
+    if (!sim || !d_obs_in || !d_critic_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
+        return fail(WL_EINVAL, std::string(fn) + ": null argument");
+    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u) || ((uintptr_t)d_obs_in & 3u) ||
+        ((uintptr_t)d_critic_obs_in & 3u) || ((uintptr_t)out.log_prob & 3u) || ((uintptr_t)out.value & 3u))
+        return fail(WL_EINVAL, std::string(fn) + ": policy blob must be 16-byte aligned, actions/mean 8-byte aligned, obs_in/critic_obs_in/log_prob/value 4-byte aligned");
+    if (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
+    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
+        return fail(WL_EINVAL, std::string(fn) + ": step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+    if (int rc = refuse_fan(sim, fn)) return rc;
+    if (sim->obs_dim < 1 || sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    ensure_device(sim);
+    PolicyOffsets po;
+    const int blob_floats = policy_offsets(sim->obs_dim, po.o, critic_obs_dim);
+    const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS + WL_ACT_XC));
+    static bool attr_set[64] = {false};                       // the attribute is per device
+    if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_asym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024), fn))
+            return rc;
+        attr_set[sim->device] = true;
+    }
+    const int n = sim->cfg.num_envs;
+    wl_policy_act_asym_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
+        sim->cfg, sim->globals, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter,
+        sim->obs_dim);
+    return launched(sim, "wl_policy_act_asym_kernel");
 }
 
 int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
@@ -2668,9 +2763,9 @@ static size_t ppo_grad_smem(int obs_dim) {
 struct PpoWorkspace { int blob_floats, rowlen, ctas, norm_parts; size_t norm_off, rows_off, bytes; };
 // (wl_ppo_update_wide's: wl_ppo_update's, then H1 and dZ1 of a mini-batch)
 struct PpoWideWorkspace { PpoWorkspace w; size_t h1_off, dz_off, bytes; };
-static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_batches, int sms, PpoWorkspace& w) {
+static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_batches, int sms, PpoWorkspace& w, int32_t critic_obs_dim = 0) {
     int32_t off[13];
-    w.blob_floats = policy_offsets(obs_dim, off);
+    w.blob_floats = policy_offsets(obs_dim, off, critic_obs_dim);
     w.rowlen = (w.blob_floats + WL_PPO_STATS + 3) & ~3;
     const int tiles = (batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE;
     w.ctas = tiles < sms ? tiles : sms;
@@ -2799,6 +2894,78 @@ int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, 
             wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
                                                                         w.blob_floats, po, p->obs_dim, sa, nullptr);
             if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel")) return rc;
+        }
+    }
+    return WL_OK;
+}
+
+// ---- the asymmetric update (DESIGN 6m): wl_ppo_update's loop over wl_ppo_grad_asym_kernel and the asymmetric blob layout ----
+static size_t ppo_grad_asym_smem(int obs_dim, int critic_obs_dim) {
+    int32_t off[13];
+    return sizeof(float) * ((size_t)policy_offsets(obs_dim, off, critic_obs_dim) + 2 * WL_HID * WL_HID + WL_HID + 2 * WL_PPO_TILE * WL_PPO_XA +
+                            4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
+}
+static int ppo_asym_workspace(const char* fn, int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
+    if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
+    if (obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    if (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
+    if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
+    int dev = 0, sms = 0;
+    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
+    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
+    static bool attr_set[64] = {false};                       // per device, raised once to the widest network (see ppo_workspace)
+    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
+        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_asym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                     (int)ppo_grad_asym_smem(16, WL_MAX_CRITIC_OBS)), fn))
+            return rc;
+        attr_set[dev] = true;
+    }
+    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, w, critic_obs_dim);
+    return WL_OK;
+}
+
+size_t wl_ppo_asym_workspace_bytes(int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches) {
+    PpoWorkspace w;
+    return ppo_asym_workspace("wl_ppo_asym_workspace_bytes", obs_dim, critic_obs_dim, batch, num_mini_batches, w) ? 0 : w.bytes;
+}
+
+int wl_ppo_update_asym(const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_critic_obs, int32_t critic_obs_dim, float* d_blob,
+                       float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes, void* stream) {
+    const char* fn = "wl_ppo_update_asym";
+    if (int rc = ppo_check_args(fn, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
+    if (!d_critic_obs || ((uintptr_t)d_critic_obs & 3u)) return fail(WL_EINVAL, std::string(fn) + ": d_critic_obs is null or not 4-byte aligned");
+    PpoWorkspace w;
+    if (int rc = ppo_asym_workspace(fn, p->obs_dim, critic_obs_dim, p->batch, p->num_mini_batches, w)) return rc;
+    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
+    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
+    if (workspace_bytes < w.bytes)
+        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (wl_ppo_asym_workspace_bytes gives " + std::to_string(w.bytes) + ")");
+    PolicyOffsets po;
+    policy_offsets(p->obs_dim, po.o, critic_obs_dim);
+    cudaStream_t cs = (cudaStream_t)stream;
+    char* ws = (char*)d_workspace;
+    float* red = (float*)ws;
+    double* norm_part = (double*)(ws + w.norm_off);
+    float* rows = (float*)(ws + w.rows_off);
+    const size_t smem = ppo_grad_asym_smem(p->obs_dim, critic_obs_dim);
+    wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
+    if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
+    PpoArgs a;
+    PpoStepArgs sa;
+    ppo_launch_args(p, b, a, sa);
+    for (int e = 0; e < p->num_learning_epochs; ++e) {
+        for (int i = 0; i < p->num_mini_batches; ++i) {
+            a.row0 = (int64_t)i * a.B;
+            sa.update_index = e * p->num_mini_batches + i;
+            wl_ppo_grad_asym_kernel<<<w.ctas, WL_PPO_THREADS, smem, cs>>>(d_blob, w.blob_floats, po, a, d_critic_obs, critic_obs_dim, d_state,
+                                                                          rows, w.rowlen);
+            wl_ppo_reduce_asym_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, critic_obs_dim,
+                                                                    d_blob, p->entropy_coef, red, norm_part);
+            wl_ppo_step_asym_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                      w.blob_floats, po, p->obs_dim, critic_obs_dim, sa);
+            if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_asym_kernel / wl_ppo_reduce_asym_kernel / wl_ppo_step_asym_kernel")) return rc;
         }
     }
     return WL_OK;

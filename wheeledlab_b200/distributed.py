@@ -25,11 +25,18 @@ class RolloutSlab:
     Other fields: actions [T,N,A] f32,
     rewards [T,N] f32, terminated / truncated [T,N] u8 and -- with ``policy_fields`` -- what alg.act() records per step
     (rsl_rl RolloutStorage: values [T,N], actions_log_prob [T,N], action_mean [T,N,A]; written by wl_act_step).  Fields are
-    views of ONE flat byte buffer, so ONE all_gather_into_tensor moves the whole slab."""
+    views of ONE flat byte buffer, so ONE all_gather_into_tensor moves the whole slab.
 
-    def __init__(self, T: int, n_local: int, obs_dim: int, act_dim: int, device, policy_fields: bool = False, flat: torch.Tensor | None = None):
+    ``critic_obs_dim`` (the asymmetric actor-critic, one GPU) adds ``critic_obs_in`` [T+1, N, Dc], the critic rows: row k is
+    what ``values[k]`` was computed from, row T the bootstrap row.  It is a tensor of its own, NOT part of ``flat``: the
+    asymmetric network is refused in a data-parallel world, so no gather has to carry it; ``critic_obs_in`` is None otherwise."""
+
+    def __init__(self, T: int, n_local: int, obs_dim: int, act_dim: int, device, policy_fields: bool = False, flat: torch.Tensor | None = None,
+                 critic_obs_dim: int | None = None):
         self.T, self.n, self.obs_dim, self.act_dim = T, n_local, obs_dim, act_dim
         self.device = torch.device(device)
+        self.critic_obs_in = (torch.zeros((T + 1, n_local, critic_obs_dim), dtype=torch.float32, device=self.device)
+                              if critic_obs_dim else None)
         # name -> (dtype, trailing shape)
         self._fields = {"obs": (torch.float32, (obs_dim,)), "actions": (torch.float32, (act_dim,)), "rewards": (torch.float32, ()),
                         "terminated": (torch.uint8, ()), "truncated": (torch.uint8, ())}

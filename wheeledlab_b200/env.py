@@ -173,7 +173,7 @@ class ObservationManager:
         env = self._env
         obs = env.sim.observe(env.common_step_counter, self._calls)
         self._calls += 1
-        return {"policy": env._append_py_obs(obs)}
+        return env._obs_groups(obs)
 
 
 class _RobotData:
@@ -309,6 +309,7 @@ class ManagerBasedRLEnv:
         self._py_sums = {}
         self._dev_terms = []                     # device terms (add_device_reward_term): evaluated by wl_step_terms
         self._term_log_ring = None
+        self._critic_terms = []                  # the critic observation group (set_critic_observation)
         for name, func, weight, params in self.spec.python_reward_terms:
             self.add_reward_term(name, func, weight, params)
         for name, func, time_out, params in self.spec.python_termination_terms:
@@ -325,6 +326,8 @@ class ManagerBasedRLEnv:
                 self.add_device_reward_term(name, func, weight, params)
             else:
                 self.add_device_termination_term(name, func, role == "time_out", params)
+        if self.spec.critic_terms:
+            self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
         # event_manager.apply(mode="startup")
         self.sim.startup()
         self._needs_reset = True
@@ -382,6 +385,44 @@ class ManagerBasedRLEnv:
         obs = self.observation_manager.compute()
         return obs["policy"], {"observations": obs}
 
+    # -- the critic observation group (privileged.py, wl_critic_observe; DESIGN 6m) --------------------------------------------
+    def set_critic_observation(self, terms):
+        """Give the env a ``critic`` observation group next to ``policy``: `terms` is a list of (name, fn, params), `fn` a
+        function of the critic library (``privileged.wheel_friction`` / ``base_mass`` / ``motor_damping``, or IsaacLab's
+        ``root_pos_w``, ``root_euler_xyz``, ``base_lin_vel``, ``base_ang_vel``, ``last_action``, ``joint_vel``, ``joint_pos``
+        by name) or its name, `params` optionally holding ``clip=(-c, c)``.  The row is their concatenation, noise-free,
+        at most 32 floats, formed on the device.  From then on ``step`` / ``reset`` / ``get_observations`` put a fresh
+        ``[N, Dc]`` tensor at ``extras["observations"]["critic"]`` (and in the returned observation dict) and
+        ``observation_manager.group_obs_dim["critic"]`` is ``(Dc,)``; ``[]`` removes the group.  Drift family only, and not
+        together with host-side Python terms or device terms."""
+        from . import privileged
+        terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
+        if terms and (self._py_rewards or self._py_terms or self._py_obs):
+            raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
+        if terms and self._dev_terms:
+            raise NotImplementedError("a critic observation group together with device terms is not implemented")
+        table = []
+        for name, fn, params in terms:
+            p = dict(params or {})
+            table.append(privileged.lower_term(name, fn, p, clip=p.pop("clip", None)))
+        privileged.check_width(table)
+        dc = self.sim.set_critic_terms(table)     # (refuses a task outside the Drift family)
+        self._critic_terms = terms
+        if dc:
+            self.observation_manager.group_obs_dim["critic"] = (dc,)
+        else:
+            self.observation_manager.group_obs_dim.pop("critic", None)
+            self.extras.pop("observations", None)
+
+    def _obs_groups(self, obs: torch.Tensor) -> dict:
+        """The observation dict of the current state: ``policy`` and, with a critic group, a fresh ``critic`` row; the same
+        dict is what ``extras["observations"]`` holds then (RslRlVecEnvWrapper's convention, read by the reference's runner)."""
+        groups = {"policy": self._append_py_obs(obs)}
+        if self._critic_terms:
+            groups["critic"] = self.sim.critic_observe()
+            self.extras["observations"] = groups
+        return groups
+
     def _curriculum_fire_mask(self) -> int:
         """Counter conditions of increase_reward_weight_over_time (curriculums.py:23-35) -- the host-side restatement the
         golden-vector test checks; at run time the same conditions are evaluated on the device (log_finalize)."""
@@ -418,6 +459,9 @@ class ManagerBasedRLEnv:
 
     # -- device terms: the reference's unregistered reward / termination functions, in CUDA (device_terms.py) ---------------
     def _refuse_mixing(self, device: bool = False):
+        if getattr(self, "_critic_terms", None):
+            raise NotImplementedError("a critic observation group together with " + ("device terms" if device else "host-side Python terms")
+                                      + " is not implemented")
         if (self._py_rewards or self._py_terms) if device else self._dev_terms:
             raise NotImplementedError("an env runs either device terms or host-side Python reward / termination terms, not both")
 
@@ -573,7 +617,7 @@ class ManagerBasedRLEnv:
         tm.terminated, tm.time_outs = terminated, truncated
         if log is not None:
             self.extras["log"] = self._episode_log(log, term_log if self._dev_terms else None)
-        return {"policy": self._append_py_obs(obs)}, rew, terminated, truncated, self.extras
+        return self._obs_groups(obs), rew, terminated, truncated, self.extras
 
     def _episode_log(self, log: torch.Tensor, term_log: torch.Tensor | None = None):
         """extras["log"] (RewardManager/TerminationManager.reset, SURVEY Appendix B): lazy views of the row the step

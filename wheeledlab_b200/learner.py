@@ -235,11 +235,21 @@ class FusedPPO:
 
     With an ``exchange`` (``PPOExchange``) the update is rsl_rl's multi-GPU one (``wl_ppo_update_dp``, DESIGN 6j): this
     replica is rank ``exchange.rank`` of ``exchange.n_ranks``, and the gradient and KL are averaged across the ranks inside
-    every mini-batch.  ``update_local_ranks`` runs several replicas of one process together."""
+    every mini-batch.  ``update_local_ranks`` runs several replicas of one process together.
+
+    ``critic_obs_dim`` (None: the critic reads the policy row) trains the asymmetric network (``wl_ppo_update_asym``, DESIGN
+    6m): the blob is laid out by ``blob_layout(obs_dim, critic_obs_dim)`` and the slab carries ``critic_obs_in``
+    [T + 1, N, critic_obs_dim].  "elu" only, and not with an exchange (its buffers are sized by one obs_dim)."""
 
     def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None, activation: str = "elu",
-                 exchange: "PPOExchange | None" = None):
+                 exchange: "PPOExchange | None" = None, critic_obs_dim: int | None = None):
         from .policy import check_activation
+        if critic_obs_dim is not None and activation != "elu":
+            raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+        if critic_obs_dim is not None and exchange is not None:
+            raise NotImplementedError("a critic observation group in a data-parallel world is not implemented "
+                                      "(the exchange buffer is sized by one obs_dim)")
+        self.critic_obs_dim = critic_obs_dim
         if cfg is None:
             cfg = PPOConfig()
         if cfg.schedule not in ("adaptive", "fixed"):
@@ -259,9 +269,12 @@ class FusedPPO:
 
     def _workspace(self, batch: int) -> torch.Tensor:
         with torch.cuda.device(self.device):
-            need = self._ws_query(self.obs_dim, batch, self.cfg.num_mini_batches)
+            if self.critic_obs_dim is not None:
+                need = lib.wl_ppo_asym_workspace_bytes(self.obs_dim, self.critic_obs_dim, batch, self.cfg.num_mini_batches)
+            else:
+                need = self._ws_query(self.obs_dim, batch, self.cfg.num_mini_batches)
         if need == 0:
-            raise WlError(f"{self._ws_query.__name__} failed: {lib.wl_last_error().decode()}")
+            raise WlError(f"the PPO workspace query failed: {lib.wl_last_error().decode()}")
         if self.workspace.numel() < need:
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
         return self.workspace
@@ -273,7 +286,11 @@ class FusedPPO:
         if perm is None:
             perm = torch.randperm(n, device=self.device)
         arrays = (slab.obs_in, slab.actions, slab.values, slab.log_prob, slab.mean, returns, advantages, perm)
-        for x in arrays:
+        if self.critic_obs_dim is not None:
+            cobs = getattr(slab, "critic_obs_in", None)
+            if cobs is None or cobs.shape[-1] != self.critic_obs_dim or cobs.shape[0] * cobs.shape[1] < n:
+                raise ValueError(f"the slab must carry critic_obs_in [T + 1, N, {self.critic_obs_dim}]")
+        for x in arrays + ((slab.critic_obs_in,) if self.critic_obs_dim is not None else ()):
             if not (x.is_cuda and x.is_contiguous()):
                 raise ValueError("FusedPPO.update expects contiguous CUDA tensors")
         if perm.dtype != torch.int64 or perm.numel() != n:
@@ -301,6 +318,12 @@ class FusedPPO:
             return update_local_ranks([self], [(slab, returns, advantages, perm)])[0]
         p, batch, ws = self._prepare(slab, returns, advantages, perm)
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        if self.critic_obs_dim is not None:
+            check(lib.wl_ppo_update_asym(C.byref(p), C.byref(batch), C.c_void_p(slab.critic_obs_in.data_ptr()), self.critic_obs_dim,
+                                         C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()), C.c_void_p(self.v.data_ptr()),
+                                         C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), stream),
+                  "wl_ppo_update_asym")
+            return self._stats()
         check(self._update(C.byref(p), C.byref(batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
                            C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
                            ws.numel(), stream), self._update.__name__)
@@ -325,7 +348,7 @@ class FusedPPO:
         the current learning rate.  Reads the device state (one sync)."""
         from .policy import actor_critic_state_dict
         lr, step = (float(x) for x in self.state[:2].tolist())
-        m, v = actor_critic_state_dict(self.m, self.obs_dim), actor_critic_state_dict(self.v, self.obs_dim)
+        m, v = (actor_critic_state_dict(x, self.obs_dim, self.critic_obs_dim) for x in (self.m, self.v))
         state = {} if step == 0 else {i: {"step": torch.tensor(step), "exp_avg": m[k], "exp_avg_sq": v[k]} for i, k in enumerate(m)}
         return {"state": state, "param_groups": [_adam_param_group(lr)]}
 
@@ -346,7 +369,7 @@ class FusedPPO:
         g = groups[0]
         if tuple(g.get("betas", ())) != (0.9, 0.999) or g.get("eps") != 1e-8 or g.get("weight_decay", 0) != 0 or g.get("amsgrad", False):
             raise ValueError("the fused update runs Adam with betas (0.9, 0.999), eps 1e-8, no weight decay, no amsgrad (rsl_rl's)")
-        names = list(actor_critic_state_dict(self.m, self.obs_dim))
+        names = list(actor_critic_state_dict(self.m, self.obs_dim, self.critic_obs_dim))
         m = torch.zeros_like(self.m)
         v = torch.zeros_like(self.v)
         step = 0.0
@@ -357,7 +380,8 @@ class FusedPPO:
             try:
                 steps = {float(st[i]["step"]) for i in range(13)}
                 for out, key in ((m, "exp_avg"), (v, "exp_avg_sq")):
-                    load_actor_critic_state_dict({k: st[i][key] for i, k in enumerate(names)}, self.obs_dim, out=out)
+                    load_actor_critic_state_dict({k: st[i][key] for i, k in enumerate(names)}, self.obs_dim, out=out,
+                                                 critic_obs_dim=self.critic_obs_dim)
             except (KeyError, TypeError, RuntimeError) as e:
                 raise ValueError(f"malformed optimizer state: {e!r}") from None
             if len(steps) != 1:
@@ -465,16 +489,24 @@ class PPOIteration:
     ``episode_stats=True`` adds the runner's episode bookkeeping right after the rollout (``self.episodes``, an
     ``EpisodeStatistics``) and gathers everything the runner logs into one device block, ``self.readback``: the episode
     statistics' state, the update's statistics (``SUMMARY``) and the rollout's T episode-log rows (``roll.logs`` is a view of
-    it), so that one copy reads an iteration back."""
+    it), so that one copy reads an iteration back.
+
+    ``critic=True`` (a handle with a critic table, ``sim.set_critic_terms``) runs the asymmetric iteration, still one graph:
+    the rollout with ``critic=True``, the bootstrap value from the critic row ``critic_obs_in[T]``, and
+    ``wl_ppo_update_asym``; the blob is laid out by ``blob_layout(obs_dim, sim.critic_obs_dim)``."""
 
     SUMMARY = ("Loss/value_function", "Loss/surrogate", "Loss/entropy", "Loss/learning_rate", "Policy/mean_noise_std")
 
     def __init__(self, sim, blob: torch.Tensor, cfg: PPOConfig | None = None, T: int = 128, activation: str = "elu",
-                 episode_stats: bool = False, exchange: PPOExchange | None = None, rollout=None, extra_readback_bytes: int = 0):
+                 episode_stats: bool = False, exchange: PPOExchange | None = None, rollout=None, extra_readback_bytes: int = 0,
+                 critic: bool = False):
         from .policy import FusedPolicyRollout
         self.sim, self.blob, self.T = sim, blob, T
-        self.roll = rollout if rollout is not None else FusedPolicyRollout(sim, blob, T, activation=activation)
-        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation, exchange=exchange)
+        self.critic_obs_dim = sim.critic_obs_dim if critic else None
+        if critic and rollout is not None:
+            raise NotImplementedError("a critic observation group with a caller's rollout (device terms, Python terms) is not implemented")
+        self.roll = rollout if rollout is not None else FusedPolicyRollout(sim, blob, T, activation=activation, critic=critic)
+        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation, exchange=exchange, critic_obs_dim=self.critic_obs_dim)
         self.perm = torch.empty(T * sim.num_envs, dtype=torch.int64, device=sim.device)
         self.graph = None
         self.stats = None
@@ -493,6 +525,8 @@ class PPOIteration:
 
     def _bootstrap(self) -> torch.Tensor:
         from .policy import critic_value
+        if self.critic_obs_dim is not None:                    # cobs0 = critic_obs_in[T] once the rollout has run
+            return critic_value(self.blob, self.sim.obs_dim, self.roll.cobs0, "elu", self.critic_obs_dim)
         return critic_value(self.blob, self.sim.obs_dim, self.roll.obs0, self.ppo.activation)
 
     def _returns(self):
@@ -510,7 +544,7 @@ class PPOIteration:
     def _summarise(self, stats):
         if self.summary is not None:
             from .policy import blob_layout
-            o_std = blob_layout(self.sim.obs_dim)[0][12]
+            o_std = blob_layout(self.sim.obs_dim, self.critic_obs_dim)[0][12]
             self.summary.copy_(torch.stack([stats["value_function"], stats["surrogate"], stats["entropy"], stats["learning_rate"],
                                             self.blob[o_std:o_std + 2].mean()]))
         return stats
@@ -522,6 +556,8 @@ class PPOIteration:
             roll.capture(step_counter)
             return self
         sim.observe(step_counter, 0, out=roll.obs0)
+        if self.critic_obs_dim is not None:
+            sim.critic_observe(out=roll.cobs0)
         sim.set_step_counter(step_counter)
         self.graph = torch.cuda.CUDAGraph()
         s = roll._stream
@@ -725,7 +761,13 @@ class FusedOnPolicyRunner:
     each rank rolls out its own env shard (``env_id_offset = rank * num_envs``), the PPO update averages gradient and KL
     across the ranks inside every mini-batch (``FusedPPO`` with a ``PPOExchange`` in symmetric memory), ``learn`` first
     broadcasts rank 0's weights, only rank 0 saves checkpoints and calls ``callback``, and ``Perf/total_fps`` counts the
-    env-steps of every rank.  Every rank loads the same checkpoint."""
+    env-steps of every rank.  Every rank loads the same checkpoint.
+
+    An env with a ``critic`` observation group (``env.set_critic_observation``, or a reference cfg with
+    ``observations.critic``) trains the asymmetric network (DESIGN 6m): the critic is ``Linear(Dc, 64)``-first and reads the
+    critic row, the iteration is ``PPOIteration(critic=True)`` -- still one graph -- and checkpoints keep rsl_rl's keys with
+    ``critic.0.weight`` ``[64, Dc]``, as ``ActorCritic(num_actor_obs, num_critic_obs, ...)`` has it.  On one GPU with the ELU
+    network; with Python terms, device terms, ``activation="relu"`` or a data-parallel world it raises ``NotImplementedError``."""
 
     @staticmethod
     def settings(train_cfg) -> SimpleNamespace:
@@ -755,6 +797,17 @@ class FusedOnPolicyRunner:
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
+        self.critic_obs_dim = sim.critic_obs_dim if getattr(e, "_critic_terms", None) else None
+        if self.critic_obs_dim is not None:
+            if self.staged:
+                raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
+            if self.dev_names:
+                raise NotImplementedError("a critic observation group together with device terms is not implemented")
+            if s.activation != "elu":
+                raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+            if _world_size() > 1:                           # (before anything initialises NCCL)
+                raise NotImplementedError("a critic observation group in a data-parallel world (WORLD_SIZE > 1) is not implemented: "
+                                          "the exchange buffer is sized by one obs_dim")
         if self.staged and _world_size() > 1:               # (before anything initialises NCCL)
             raise NotImplementedError("data-parallel training of an env with host-side Python terms is not supported: the staged "
                                       "rollout runs on one GPU")
@@ -763,10 +816,12 @@ class FusedOnPolicyRunner:
         self.num_steps_per_env, self.save_interval, self.activation, self.alg_cfg = s.num_steps_per_env, s.save_interval, s.activation, s.alg_cfg
         D = sim.obs_dim
         act = torch.nn.ELU if self.activation == "elu" else torch.nn.ReLU
-        mk = lambda out: torch.nn.Sequential(torch.nn.Linear(D, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
+        mk = lambda out, nin=D: torch.nn.Sequential(torch.nn.Linear(nin, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
         std = torch.full((2,), s.init_noise_std)
-        self.blob = pack_actor_critic(mk(2), mk(1), std, D, sim.device)
-        if self.staged:
+        self.blob = pack_actor_critic(mk(2), mk(1, self.critic_obs_dim or D), std, D, sim.device, critic_obs_dim=self.critic_obs_dim)
+        if self.critic_obs_dim is not None:
+            self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, "elu", episode_stats=True, critic=True)
+        elif self.staged:
             self.it = StagedPPOIteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation)
         else:
             exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
@@ -842,26 +897,33 @@ class FusedOnPolicyRunner:
             norm = lambda x: (x.type, x.index if x.index is not None or x.type != "cuda" else torch.cuda.current_device())
             if norm(torch.device(device)) != norm(torch.device(self.device)):
                 raise ValueError(f"device {device} is not the env's device {self.device}: the policy runs where the env's blob is")
-        return InferencePolicy(self.blob, self.env.sim.obs_dim, self.activation)
+        return InferencePolicy(self.blob, self.env.sim.obs_dim, self.activation, self.critic_obs_dim)
 
     def save(self, path: str, infos=None):
         """rsl_rl's checkpoint: {"model_state_dict", "optimizer_state_dict", "iter", "infos"}."""
         from .policy import actor_critic_state_dict
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-        torch.save({"model_state_dict": actor_critic_state_dict(self.blob, self.env.sim.obs_dim),
+        torch.save({"model_state_dict": actor_critic_state_dict(self.blob, self.env.sim.obs_dim, self.critic_obs_dim),
                     "optimizer_state_dict": self.alg.optimizer_state_dict(),
                     "iter": self.current_learning_iteration, "infos": infos}, path)
 
     def load(self, path: str, load_optimizer: bool = True):
         """Load a checkpoint written by ``save`` or by rsl_rl into the blob (and the Adam state) in place; the next ``learn``
-        starts at its ``iter``.  Returns its ``infos``."""
+        starts at its ``iter``.  Returns its ``infos``.  A checkpoint whose actor or critic width is not the env's raises
+        ``ValueError`` before anything is written -- except with ``load_optimizer=False`` on an env without a critic group,
+        where a checkpoint of the asymmetric network loads its actor alone (what ``get_inference_policy`` and playback read)."""
         from .policy import load_actor_critic_state_dict
         d = torch.load(path, map_location=self.device)
         if not isinstance(d, dict) or not {"model_state_dict", "iter"} <= set(d) or (load_optimizer and "optimizer_state_dict" not in d):
             raise ValueError(f"{path}: not an rsl_rl checkpoint (model_state_dict, optimizer_state_dict, iter, infos)")
         D = self.env.sim.obs_dim
         try:
-            blob = load_actor_critic_state_dict(d["model_state_dict"], D, out=torch.zeros_like(self.blob))
+            w1 = d["model_state_dict"]["critic.0.weight"]
+            # playback of an asymmetric checkpoint on an env without the critic group (play_policy.py loads weights only):
+            # the actor is all that plays, so the critic of another width is left out instead of refused
+            actor_only = not load_optimizer and self.critic_obs_dim is None and w1.dim() == 2 and w1.shape[1] != D
+            blob = load_actor_critic_state_dict(d["model_state_dict"], D, out=self.blob.clone() if actor_only else torch.zeros_like(self.blob),
+                                                critic_obs_dim=self.critic_obs_dim, actor_only=actor_only)
         except (KeyError, TypeError, RuntimeError) as e:
             raise ValueError(f"{path}: malformed model_state_dict: {e!r}") from None
         if load_optimizer:

@@ -20,9 +20,14 @@ from .sim import WheeledSim, _stream_ptr
 HIDDEN = 64
 
 
-def blob_layout(obs_dim: int):
+def blob_layout(obs_dim: int, critic_obs_dim: int | None = None):
+    """Offsets and float count of the blob; ``critic_obs_dim`` (None: the critic reads the policy row) sizes the critic's
+    first layer for the asymmetric network (wl_policy_blob_floats_asym)."""
     off = (C.c_int32 * 13)()
-    total = lib.wl_policy_blob_floats(obs_dim, off)
+    if critic_obs_dim is None:
+        total = lib.wl_policy_blob_floats(obs_dim, off)
+    else:
+        total = lib.wl_policy_blob_floats_asym(obs_dim, critic_obs_dim, off)
     return list(off), total
 
 
@@ -33,15 +38,18 @@ def _linears(net):
     return ls
 
 
-def pack_actor_critic(actor, critic, std: torch.Tensor, obs_dim: int, device, out: torch.Tensor | None = None) -> torch.Tensor:
+def pack_actor_critic(actor, critic, std: torch.Tensor, obs_dim: int, device, out: torch.Tensor | None = None,
+                      critic_obs_dim: int | None = None) -> torch.Tensor:
     """actor / critic: torch modules holding three nn.Linear (obs->64->64->2 / ->1, ELU in between); std: [2].
-    Returns (or refills, when `out` is given -- e.g. after an optimiser step) the fp32 device blob wl_act_step reads."""
-    off, total = blob_layout(obs_dim)
+    Returns (or refills, when `out` is given -- e.g. after an optimiser step) the fp32 device blob wl_act_step reads.
+    ``critic_obs_dim``: the critic's input width when it reads a row of its own (wl_policy_act_asym's blob)."""
+    off, total = blob_layout(obs_dim, critic_obs_dim)
     blob = out if out is not None else torch.zeros(total, dtype=torch.float32, device=device)
     with torch.no_grad():
         for net_i, (net, nout) in enumerate(((actor, 2), (critic, 1))):
             ls = _linears(net)
-            if ls[0].in_features != obs_dim or ls[2].out_features != nout:
+            nin = obs_dim if net_i == 0 or critic_obs_dim is None else critic_obs_dim
+            if ls[0].in_features != nin or ls[2].out_features != nout:
                 raise ValueError("network shape does not match the task")
             for k, lin in enumerate(ls):
                 wt = lin.weight.detach().to(device=device, dtype=torch.float32).t().contiguous().reshape(-1)   # input-major
@@ -53,22 +61,24 @@ def pack_actor_critic(actor, critic, std: torch.Tensor, obs_dim: int, device, ou
     return blob
 
 
-def _blob_layers(blob: torch.Tensor, obs_dim: int):
+def _blob_layers(blob: torch.Tensor, obs_dim: int, critic_obs_dim: int | None = None):
     """Zero-copy views of the blob: per net, three (W [in, out] input-major, b [out]) pairs; plus std [2]."""
-    off, _ = blob_layout(obs_dim)
+    off, _ = blob_layout(obs_dim, critic_obs_dim)
     nets = []
     for net_i, nout in enumerate((2, 1)):
         o = off[net_i * 6:net_i * 6 + 6]
-        nets.append([(blob[o[0]:o[0] + obs_dim * HIDDEN].view(obs_dim, HIDDEN), blob[o[1]:o[1] + HIDDEN]),
+        nin = obs_dim if net_i == 0 or critic_obs_dim is None else critic_obs_dim
+        nets.append([(blob[o[0]:o[0] + nin * HIDDEN].view(nin, HIDDEN), blob[o[1]:o[1] + HIDDEN]),
                      (blob[o[2]:o[2] + HIDDEN * HIDDEN].view(HIDDEN, HIDDEN), blob[o[3]:o[3] + HIDDEN]),
                      (blob[o[4]:o[4] + HIDDEN * nout].view(HIDDEN, nout), blob[o[5]:o[5] + nout])])
     return nets[0], nets[1], blob[off[12]:off[12] + 2]
 
 
-def actor_critic_state_dict(blob: torch.Tensor, obs_dim: int) -> dict:
+def actor_critic_state_dict(blob: torch.Tensor, obs_dim: int, critic_obs_dim: int | None = None) -> dict:
     """The blob as an rsl_rl ActorCritic state dict (actor.0/2/4.weight|bias, critic.0/2/4.weight|bias, std) [UPSTREAM-RECALL]:
-    the ``model_state_dict`` of the checkpoints rsl_rl's runner saves and ``play_policy.py`` loads.  Tensors are copies."""
-    actor, critic, std = _blob_layers(blob, obs_dim)
+    the ``model_state_dict`` of the checkpoints rsl_rl's runner saves and ``play_policy.py`` loads.  Tensors are copies.
+    With ``critic_obs_dim`` ``critic.0.weight`` is [64, critic_obs_dim], as ActorCritic(num_actor_obs, num_critic_obs, ...) has it."""
+    actor, critic, std = _blob_layers(blob, obs_dim, critic_obs_dim)
     sd = {}
     for name, layers in (("actor", actor), ("critic", critic)):
         for k, (w, b) in enumerate(layers):
@@ -78,17 +88,26 @@ def actor_critic_state_dict(blob: torch.Tensor, obs_dim: int) -> dict:
     return sd
 
 
-def load_actor_critic_state_dict(sd: dict, obs_dim: int, out: torch.Tensor | None = None, device=None) -> torch.Tensor:
-    """Inverse of actor_critic_state_dict: fills `out` (or a new zeroed blob) from an rsl_rl ActorCritic state dict."""
+def load_actor_critic_state_dict(sd: dict, obs_dim: int, out: torch.Tensor | None = None, device=None,
+                                 critic_obs_dim: int | None = None, actor_only: bool = False) -> torch.Tensor:
+    """Inverse of actor_critic_state_dict: fills `out` (or a new zeroed blob) from an rsl_rl ActorCritic state dict.  Every
+    shape is checked before anything is written: a checkpoint whose actor or critic width does not match leaves `out` as it was.
+    ``actor_only``: the actor blocks and std alone, the critic's neither checked nor written -- what playback needs of a
+    checkpoint whose critic read a row of its own (the actor blocks sit at the same offsets in both layouts)."""
     if out is None:
-        out = torch.zeros(blob_layout(obs_dim)[1], dtype=torch.float32, device=device or sd["std"].device)
-    actor, critic, std = _blob_layers(out, obs_dim)
+        out = torch.zeros(blob_layout(obs_dim, critic_obs_dim)[1], dtype=torch.float32, device=device or sd["std"].device)
+    actor, critic, std = _blob_layers(out, obs_dim, critic_obs_dim)
+    nets = (("actor", actor),) if actor_only else (("actor", actor), ("critic", critic))
+    for name, layers in nets:
+        for k, (w, b) in enumerate(layers):
+            wt, bt = sd[f"{name}.{2 * k}.weight"], sd[f"{name}.{2 * k}.bias"]
+            if tuple(wt.shape) != (w.shape[1], w.shape[0]) or tuple(bt.shape) != tuple(b.shape):
+                width = f"obs_dim {obs_dim}" + ("" if critic_obs_dim is None else f" and critic width {critic_obs_dim}")
+                raise ValueError(f"{name}.{2 * k}: shape {tuple(wt.shape)} does not match the [64, 64] ELU network of {width}")
     with torch.no_grad():
-        for name, layers in (("actor", actor), ("critic", critic)):
+        for name, layers in nets:
             for k, (w, b) in enumerate(layers):
                 wt, bt = sd[f"{name}.{2 * k}.weight"], sd[f"{name}.{2 * k}.bias"]
-                if tuple(wt.shape) != (w.shape[1], w.shape[0]) or tuple(bt.shape) != tuple(b.shape):
-                    raise ValueError(f"{name}.{2 * k}: shape {tuple(wt.shape)} does not match the [64, 64] ELU network of obs_dim {obs_dim}")
                 w.copy_(wt.t())
                 b.copy_(bt)
         std.copy_(sd["std"])
@@ -104,11 +123,12 @@ def check_activation(activation: str) -> str:
     return activation
 
 
-def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu") -> torch.Tensor:
+def critic_value(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu",
+                 critic_obs_dim: int | None = None) -> torch.Tensor:
     """V(obs) [N] in torch from zero-copy views of the blob (the bootstrap value of compute_returns): a CUDA graph that
-    captures it reads the weights the last update left in the blob."""
+    captures it reads the weights the last update left in the blob.  With ``critic_obs_dim`` `obs` is the critic row."""
     act = ACTIVATIONS[check_activation(activation)]
-    _, critic, _ = _blob_layers(blob, obs_dim)
+    _, critic, _ = _blob_layers(blob, obs_dim, critic_obs_dim)
     x = obs
     for k, (w, b) in enumerate(critic):
         x = torch.addmm(b, x, w)
@@ -132,12 +152,14 @@ def _device_tensor(name: str, t, device, shape=None, ndim=None) -> None:
         raise ValueError(f"{name} must be contiguous")
 
 
-def actor_mean(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu", out: torch.Tensor | None = None) -> torch.Tensor:
+def actor_mean(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: str = "elu", out: torch.Tensor | None = None,
+               critic_obs_dim: int | None = None) -> torch.Tensor:
     """The actor mean [N, 2] of `obs` [N, obs_dim] under the network in `blob` -- rsl_rl ``ActorCritic.act_inference``, the
     deterministic action a trained policy is played with.  One launch (wl_actor_mean) on the current stream of obs's
     device; into `out` [N, 2] when given (capturable), else into a new tensor.  "elu": the Drift family's network
     (obs_dim <= 16), bit for bit the mean wl_act_step stores; "relu": Elevation / Visual (obs_dim <= 4096), bit for bit
-    wl_policy_act's mean."""
+    wl_policy_act's mean.  ``critic_obs_dim``: the blob is the asymmetric network's (blob_layout(obs_dim, critic_obs_dim));
+    the actor blocks sit at the same offsets, so it plays unchanged."""
     check_activation(activation)
     _device_tensor("obs", obs, None, ndim=2)
     dev = obs.device
@@ -145,7 +167,7 @@ def actor_mean(blob: torch.Tensor, obs_dim: int, obs: torch.Tensor, activation: 
         raise ValueError(f"obs must have shape [N, {obs_dim}], not {tuple(obs.shape)}")
     if obs.shape[0] < 1:
         raise ValueError("obs must have at least one row")
-    _device_tensor("blob", blob, dev, shape=(blob_layout(obs_dim)[1],))
+    _device_tensor("blob", blob, dev, shape=(blob_layout(obs_dim, critic_obs_dim)[1],))
     if out is None:
         out = torch.empty((obs.shape[0], 2), dtype=torch.float32, device=dev)
     else:
@@ -160,11 +182,11 @@ class InferencePolicy:
     tensor per call (play_policy.py appends the actions without cloning) unless `out` is given.  The blob is read at call
     time, so later updates and loads into it are seen.  Works under ``torch.inference_mode()``."""
 
-    def __init__(self, blob: torch.Tensor, obs_dim: int, activation: str = "elu"):
-        self.blob, self.obs_dim, self.activation = blob, obs_dim, check_activation(activation)
+    def __init__(self, blob: torch.Tensor, obs_dim: int, activation: str = "elu", critic_obs_dim: int | None = None):
+        self.blob, self.obs_dim, self.activation, self.critic_obs_dim = blob, obs_dim, check_activation(activation), critic_obs_dim
 
     def __call__(self, obs: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
-        return actor_mean(self.blob, self.obs_dim, obs, self.activation, out)
+        return actor_mean(self.blob, self.obs_dim, obs, self.activation, out, self.critic_obs_dim)
 
 
 class PolicyBuffers:
@@ -210,6 +232,23 @@ def policy_act(sim: WheeledSim, obs_in: torch.Tensor, blob: torch.Tensor, action
           fn.__name__)
 
 
+def policy_act_asym(sim: WheeledSim, obs_in: torch.Tensor, critic_obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor,
+                    mean: torch.Tensor, log_prob: torch.Tensor, value: torch.Tensor, step_counter: int):
+    """policy_act(..., "elu") for the asymmetric network (wl_policy_act_asym): the critic reads `critic_obs_in` [N, Dc] and the
+    blob is laid out by blob_layout(obs_dim, Dc); actions / mean / log-prob are wl_policy_act_elu's bit for bit."""
+    n = sim.num_envs
+    if critic_obs_in.dim() != 2 or not 1 <= critic_obs_in.shape[1] <= 32:
+        raise ValueError(f"critic_obs_in must have shape [N, Dc] with Dc in 1..32, not {tuple(critic_obs_in.shape)}")
+    _device_tensor("obs_in", obs_in, sim.device, shape=(n, sim.obs_dim))
+    _device_tensor("critic_obs_in", critic_obs_in, sim.device, shape=(n, critic_obs_in.shape[1]))
+    _device_tensor("blob", blob, sim.device, shape=(blob_layout(sim.obs_dim, critic_obs_in.shape[1])[1],))
+    for name, t, shape in (("actions", actions, (n, 2)), ("mean", mean, (n, 2)), ("log_prob", log_prob, (n,)), ("value", value, (n,))):
+        _device_tensor(name, t, sim.device, shape=shape)
+    po = WlPolicyOut(actions.data_ptr(), mean.data_ptr(), log_prob.data_ptr(), value.data_ptr())
+    check(lib.wl_policy_act_asym(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(critic_obs_in.data_ptr()), critic_obs_in.shape[-1],
+                                 C.c_void_p(blob.data_ptr()), po, step_counter, _stream_ptr(sim.device)), "wl_policy_act_asym")
+
+
 class FusedPolicyRollout:
     """T policy-and-step launches captured as ONE CUDA graph: the reference's whole collection loop
     (modified_rsl_rl_runner.py:70-109).  activation "elu" (the Drift family): T x wl_act_step, the policy fused into the
@@ -223,13 +262,30 @@ class FusedPolicyRollout:
 
     ``device_terms=True`` rolls out an env whose handle has device terms (``wl_set_device_terms``): T x (``policy_act``,
     then ``wl_step_terms``) on the same device counters, still one graph; ``term_logs[k]`` [T, 8] receives step k's
-    device-term ``Episode_*`` entries.  A graph must be captured after the handle's terms are set."""
+    device-term ``Episode_*`` entries.  A graph must be captured after the handle's terms are set.
+
+    ``critic=True`` rolls out the asymmetric network on a handle that has a critic table (``sim.set_critic_terms``): T x
+    (``policy_act_asym``, ``wl_step``, ``wl_critic_observe`` into row k + 1) on device counters, one graph.
+    ``slab.critic_obs_in`` [T + 1, N, Dc] holds the critic rows: row k is what ``values[k]`` was computed from, row T the
+    bootstrap row.  The blob is laid out by ``blob_layout(obs_dim, Dc)``.  "elu" only, and not with device terms."""
 
     def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu",
-                 deterministic: bool = False, device_terms: bool = False):
+                 deterministic: bool = False, device_terms: bool = False, critic: bool = False):
         self.sim, self.blob, self.T, self.activation = sim, blob, T, check_activation(activation)
         self.deterministic = bool(deterministic)
         self.device_terms = bool(device_terms)
+        self.critic = bool(critic)
+        if self.critic:
+            if self.deterministic:
+                raise ValueError("critic: the training rollout only (playback reads the actor alone)")
+            if self.device_terms:
+                raise NotImplementedError("a critic observation group together with device terms is not implemented")
+            if activation != "elu":
+                raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+            if sim.critic_obs_dim < 1:
+                raise ValueError("critic=True needs a critic table on the handle (sim.set_critic_terms)")
+            if (sim.num_envs * sim.obs_dim) % 2:
+                raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
         if self.device_terms and self.deterministic:
             raise ValueError("device_terms: the training rollout only")
         if self.device_terms and (sim.num_envs * sim.obs_dim) % 2:
@@ -237,7 +293,8 @@ class FusedPolicyRollout:
         self.term_logs = torch.zeros((T, 8), dtype=torch.float32, device=sim.device) if self.device_terms else None
         if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
             raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
-        self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=not self.deterministic)
+        self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=not self.deterministic,
+                                        critic_obs_dim=sim.critic_obs_dim if self.critic else None)
         # values / log-prob / mean go straight into the slab (= the all-gather send buffer) when it has those fields
         if self.deterministic:
             self.pol = None
@@ -248,15 +305,26 @@ class FusedPolicyRollout:
         # slab.obs_in[k] = the observation actions[k] / log_prob[k] / values[k] / mean[k] were computed from (rsl_rl
         # RolloutStorage.observations[k]); slab.obs[k] = obs_in[k+1] = what step k returned
         self.obs0 = torch.empty((sim.num_envs, sim.obs_dim), dtype=torch.float32, device=sim.device)    # carried to the next replay
+        if self.critic:
+            if self.slab.critic_obs_in is None or tuple(self.slab.critic_obs_in.shape) != (T + 1, sim.num_envs, sim.critic_obs_dim):
+                raise ValueError(f"critic=True needs a slab built with critic_obs_dim={sim.critic_obs_dim}")
+            self.cobs0 = torch.empty((sim.num_envs, sim.critic_obs_dim), dtype=torch.float32, device=sim.device)
         self.graph = None
         self._base = 0
         self._stream = torch.cuda.Stream(device=sim.device)
 
     def _body(self):
         self.slab.obs_in[0].copy_(self.obs0)
+        if self.critic:
+            self.slab.critic_obs_in[0].copy_(self.cobs0)
         for k in range(self.T):
             t = WheeledSim.device_counter_plus(k)
-            if self.deterministic:
+            if self.critic:
+                policy_act_asym(self.sim, self.slab.obs_in[k], self.slab.critic_obs_in[k], self.blob, self.slab.actions[k],
+                                self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t)
+                self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
+                self.sim.critic_observe(out=self.slab.critic_obs_in[k + 1])
+            elif self.deterministic:
                 if self.activation == "relu":
                     actor_mean(self.blob, self.sim.obs_dim, self.slab.obs_in[k], "relu", out=self.slab.actions[k])
                     self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
@@ -276,10 +344,14 @@ class FusedPolicyRollout:
                          self.pol.values[k], self.slab.step_outputs(k), self.logs[k], t)
         self.sim.advance_counter(self.T)
         self.obs0.copy_(self.slab.obs[self.T - 1])
+        if self.critic:
+            self.cobs0.copy_(self.slab.critic_obs_in[self.T])
 
     def capture(self, step_counter: int):
         sim = self.sim
         sim.observe(step_counter, 0, out=self.obs0)
+        if self.critic:
+            sim.critic_observe(out=self.cobs0)
         sim.set_step_counter(step_counter)
         self.graph = torch.cuda.CUDAGraph()
         s = self._stream

@@ -304,6 +304,36 @@ class WheeledSim:
                                 step_counter, _stream_ptr(self.device)), "wl_step_terms")
         return obs, rew, term, trunc
 
+    def set_critic_terms(self, terms):
+        """The handle's critic observation (wl_set_critic_terms): a list of term names of the library
+        (``_lib.WL_CRITIC_TERMS``) or (name, clip) pairs, concatenated in this order into the critic row; [] clears it.
+        Returns Dc, the row's width.  Nothing is launched; a graph captured earlier keeps the table it was captured with."""
+        pairs = [(t, 0.0) if isinstance(t, str) else (t[0], t[1] or 0.0) for t in terms]
+        for name, _ in pairs:
+            if name not in _lib.WL_CRITIC_TERMS:
+                raise ValueError(f"critic term {name!r} is not in the library {sorted(_lib.WL_CRITIC_TERMS)}")
+        arr = (_lib.WlCriticTerm * max(1, len(pairs)))()
+        for k, (name, clip) in enumerate(pairs):
+            arr[k] = _lib.WlCriticTerm(_lib.WL_CRITIC_TERMS[name][0], float(clip))
+        check(lib.wl_set_critic_terms(self._h, arr, len(pairs)), "wl_set_critic_terms")
+        return self.critic_obs_dim
+
+    @property
+    def critic_obs_dim(self) -> int:
+        return int(lib.wl_critic_obs_dim(self._h))
+
+    def critic_observe(self, out: torch.Tensor | None = None) -> torch.Tensor:
+        """The critic row [N, Dc] of the current state (wl_critic_observe): after step(), the post-reset state its
+        observation was formed from.  No noise, no counter; capturable."""
+        dc = self.critic_obs_dim
+        obs = out if out is not None else torch.empty((self.num_envs, dc), dtype=torch.float32, device=self.device)
+        if dc and (obs.dtype != torch.float32 or tuple(obs.shape) != (self.num_envs, dc) or not obs.is_contiguous()
+                   or not obs.is_cuda or obs.device.index != self.device.index):
+            raise ValueError(f"out must be a contiguous float32 [{self.num_envs}, {dc}] tensor on {self.device} (the table's row "
+                             f"is {dc} floats wide), not {obs.dtype} {tuple(obs.shape)} on {obs.device}")
+        check(lib.wl_critic_observe(self._h, C.c_void_p(obs.data_ptr()), _stream_ptr(self.device)), "wl_critic_observe")
+        return obs
+
     def observe(self, step_counter: int, call_idx: int = 0, out: torch.Tensor | None = None):
         obs = out if out is not None else torch.empty((self.num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
         check(lib.wl_observe(self._h, C.c_void_p(obs.data_ptr()), step_counter, call_idx, _stream_ptr(self.device)),

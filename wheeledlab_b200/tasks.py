@@ -66,6 +66,8 @@ class TaskSpec:
     python_termination_terms: list = field(default_factory=list)  # [(name, func, time_out, params)]
     # device terms (device_terms.py), evaluated by wl_step_terms: [(name, func, "reward" | "termination" | "time_out", weight, params)]
     device_terms: list = field(default_factory=list)
+    # the critic observation group (privileged.py, wl_critic_observe): [(name, library term, clip)] in row order; [] = none
+    critic_terms: list = field(default_factory=list)
 
     @property
     def step_dt(self) -> float:
