@@ -829,6 +829,14 @@ int wl_test_null_cfg(wl_sim* sim, int32_t grid, int32_t block, void* stream);   
 /* philox4x32-10: out[4*n] for counters (c0_base + i, c1, c2, c3), key from seed */
 int wl_test_philox(uint64_t seed, uint32_t c0_base, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t* d_out,
                    int32_t n, void* stream);
+/* the handle's device-term kernels (wl_terms_kernel, and wl_terms_log_kernel when d_term_log is not NULL) on a caller-given
+ * state: d_state in the handle's [group][N] float4 layout (the pre-reset state wl_step_stage_a leaves), d_done[N] the
+ * built-in termination bytes (nonzero: done), d_rew[N] in / out (the reward terms are added to it), d_term_log as in
+ * wl_step_terms.  It reads and updates the handle's term state (episode sums, previous elevations, the fired bits of
+ * wl_device_term_masks) exactly as wl_step_terms does; the handle's own state buffer is not touched.  WL_EINVAL for a null
+ * argument, a state that is not 16-byte aligned, a negative step counter or a handle without device terms. */
+int wl_test_device_terms(wl_sim* sim, const float* d_state, const uint8_t* d_done, float* d_rew, float* d_term_log,
+                         int64_t step_counter, void* stream);
 
 #ifdef __cplusplus
 }

@@ -244,6 +244,8 @@ typedef struct wlo_sim {
     float* hf;
     int32_t* vis_cells;       /* visual: spawn-candidate cell ids */
     uint8_t* vis_map;         /* visual: traversability map [rows, cols] */
+    struct wlo_dterms* dt;    /* wlo_set_device_terms: the term table and its per-env state (NULL: none) */
+    int32_t dt_run;           /* set by wlo_step_terms: env_step runs the device terms between E and F */
 } wlo_sim;
 
 static inline real dot3(real ax, real ay, real az, real bx, real by, real bz) { return fm(ax, bx, fm(ay, by, az * bz)); }
@@ -912,6 +914,219 @@ static void blind_obs(const wl_config* c, const wlo_env* e, uint32_t gid, uint32
 }
 
 /* ------------------------------------------------------------------------- */
+/* device terms: the twin of csrc/wl_terms.cuh (DESIGN.md 6l).  term_value has  */
+/* the kernel's expressions in its order; dterms_env is one thread of            */
+/* wl_terms_kernel; dterms_log is the 128-env tree per CTA, the lane-strided sum */
+/* over the CTAs and the butterfly of wl_terms_log_kernel.  Constants the torch  */
+/* expression takes as fp32 enter as fp32 in the fp64 build too (KF).            */
+/* ------------------------------------------------------------------------- */
+#define KF(x) ((real)(x##f))
+#define WLO_TERMS_BS 128
+typedef struct {
+    int32_t n;
+    int32_t kind[WL_MAX_DEVICE_TERMS], role[WL_MAX_DEVICE_TERMS], skip[WL_MAX_DEVICE_TERMS];
+    real scale[WL_MAX_DEVICE_TERMS];          /* reward: fp32(weight * step_dt) (fp64 build: the double product) */
+    real p[WL_MAX_DEVICE_TERMS][4];           /* the parameters as the fp32 constants torch compares with */
+} wlo_term_table;
+typedef struct wlo_dterms {
+    wlo_term_table tt;
+    real* sums;                               /* [WL_MAX_DEVICE_TERMS][N] */
+    real* prev;                               /* [N] elevation_continuity (NaN: not called yet) */
+    real* contrib;                            /* [N][9] the last step's per-env log contributions */
+    uint8_t* fired;                           /* [N] bit k: term k fired in the last step */
+    double log[WL_MAX_DEVICE_TERMS];          /* the last step's Episode_* entries */
+} wlo_dterms;
+
+/* wl_set_device_terms's host side: validation and the folding of weight and parameters */
+static int term_table(const wl_config* c, const wl_term_desc* d, int32_t n, wlo_term_table* tt) {
+    if (n < 0 || n > WL_MAX_DEVICE_TERMS || (n > 0 && !d)) return WL_EINVAL;
+    memset(tt, 0, sizeof *tt);
+    tt->n = n;
+    const double step_dt = (double)c->sim_dt * (double)c->decimation;
+    for (int k = 0; k < n; ++k) {
+        if (d[k].kind < 1 || d[k].kind >= WL_TERM_KINDS) return WL_EINVAL;
+        if (d[k].role < WL_TERM_ROLE_REWARD || d[k].role > WL_TERM_ROLE_TIME_OUT) return WL_EINVAL;
+        if (!isfinite(d[k].weight)) return WL_EINVAL;
+        for (int j = 0; j < 4; ++j) if (!isfinite(d[k].params[j])) return WL_EINVAL;
+        int map = d[k].kind == WL_TERM_V_IS_TRAVERSABLE || d[k].kind == WL_TERM_V_IS_TRAVERSABLE_SPEED_SCALED ||
+                  d[k].kind == WL_TERM_V_VEL_REW_TRAV || d[k].kind == WL_TERM_V_BOOL_IS_NOT_TRAVERSABLE;
+        if (map && c->task != WL_TASK_VISUAL) return WL_EUNSUPPORTED;
+        tt->kind[k] = d[k].kind;
+        tt->role[k] = d[k].role;
+#ifdef WLO_DOUBLE
+        tt->scale[k] = d[k].role == WL_TERM_ROLE_REWARD ? d[k].weight * step_dt : 0.0;
+#else
+        tt->scale[k] = d[k].role == WL_TERM_ROLE_REWARD ? (float)(d[k].weight * step_dt) : 0.0f;
+#endif
+        tt->skip[k] = d[k].role == WL_TERM_ROLE_REWARD && d[k].weight == 0.0;
+        for (int j = 0; j < 4; ++j) tt->p[k][j] = (real)(float)d[k].params[j];
+        if (d[k].kind == WL_TERM_V_OFF_TRACK) tt->p[k][2] = (real)(float)(d[k].params[1] * d[k].params[1]);
+    }
+    return 0;
+}
+
+/* the pre-reset quantities the terms read (TermIn) */
+typedef struct { real p[3], vw[3], vb[3], wb[3], q[4], spin; } wlo_term_in;
+static void term_in(const real p[3], const real q[4], const real v[3], const real w[3], const real omega[4], wlo_term_in* s) {
+    for (int k = 0; k < 3; ++k) { s->p[k] = p[k]; s->vw[k] = v[k]; }
+    for (int k = 0; k < 4; ++k) s->q[k] = q[k];
+    s->spin = (omega[0] + omega[1]) + (omega[2] + omega[3]);
+    real R[9]; rotmat(q, R);
+    rotT(R, v, s->vb); rotT(R, w, s->wb);
+}
+
+/* TraversabilityHashmapUtil.get_traversability at the root (the lookup of visual_terms) */
+static int term_traversable(const wl_config* c, const uint8_t* map, real x, real y) {
+    int xi = (int)((x + (real)c->vis_width / K(2.0) + (real)c->vis_row_spacing / K(2.0)) / (real)c->vis_row_spacing);
+    int yi = (int)((y + (real)c->vis_height / K(2.0) + (real)c->vis_col_spacing / K(2.0)) / (real)c->vis_col_spacing);
+    xi = xi < 0 ? 0 : (xi > c->vis_rows - 1 ? c->vis_rows - 1 : xi);
+    yi = yi < 0 ? 0 : (yi > c->vis_cols - 1 ? c->vis_cols - 1 : yi);
+    return map[(size_t)yi * c->vis_cols + xi] != 0;
+}
+
+static real term_value(const wl_config* c, const uint8_t* map, int kind, const real p[4], const wlo_term_in* s, uint32_t t,
+                       real* prev) {
+    switch (kind) {
+    case WL_TERM_E_FORWARD_VEL: return r_min(s->vb[0], KF(1.2));
+    case WL_TERM_E_FORWARD_WHEEL_SPIN: return r_min(s->spin, K(200.0));
+    case WL_TERM_E_CHANGE_IN_ELEVATION: return (s->vw[2] > K(0.0)) ? s->vw[2] : K(0.0);
+    case WL_TERM_E_ASCENDING: return r_max(s->vw[2], K(0.0));
+    case WL_TERM_E_STEEP_PENALTY: {
+        real e[3]; euler_xyz(s->q, e);
+        return r_max(e[1] - p[0], K(0.0));
+    }
+    case WL_TERM_E_ELEVATION_CONTINUITY: {
+        const real z = s->p[2] - KF(0.19);
+        const real d = z - ((*prev != *prev) ? z : *prev);
+        *prev = z;
+        return (z > p[0] && d != K(0.0)) ? r_fabs(K(50.0) * d) : K(0.0);
+    }
+    case WL_TERM_E_YAW_CHANGE_ON_ELEV: {
+        const real z = s->p[2] - KF(0.19), a = r_fabs(s->wb[2]);
+        return (z > p[1] && a > p[0]) ? K(2.0) * (a * a) : K(0.0);
+    }
+    case WL_TERM_E_UPRIGHT_PENALTY: {
+        const real w = s->q[0], x = s->q[1], y = s->q[2], z = s->q[3];
+        const real two_s = K(2.0) / (((w * w + x * x) + y * y) + z * z);
+        const real r22 = K(1.0) - two_s * (x * x + y * y);
+        if (!(r_fabs(r22) <= K(1.0))) return K(0.0);
+        const real deg = det_atan2(r_sqrt((K(1.0) - r22) * (K(1.0) + r22)), r22) * KF(57.29577951308232);
+        return (deg > p[0]) ? deg - p[0] : K(0.0);
+    }
+    case WL_TERM_E_ROLL_ON_ELEV: {
+        const real z = s->p[2] - KF(0.19), a = r_fabs(s->wb[0]);
+        return (z > p[0] && a > p[1]) ? a * K(2.0) : K(0.0);
+    }
+    case WL_TERM_E_LOW_VEL_PENALTY: return (s->vb[0] < p[0]) ? K(1.0) : K(0.0);
+    case WL_TERM_V_IS_TRAVERSABLE: return term_traversable(c, map, s->p[0], s->p[1]) ? K(1.0) : K(0.0);
+    case WL_TERM_V_IS_TRAVERSABLE_SPEED_SCALED: return (term_traversable(c, map, s->p[0], s->p[1]) ? K(1.0) : K(0.0)) * s->vb[0];
+    case WL_TERM_V_VEL_REW_TRAV: {
+        const real target = term_traversable(c, map, s->p[0], s->p[1]) ? p[0] : p[1];
+        const real sp = r_sqrt((s->vb[0] * s->vb[0] + s->vb[1] * s->vb[1]) + s->vb[2] * s->vb[2]);
+        const real d = sp - target;
+        const real sd = -(d * d) + target * target;
+        return (sd > K(0.0)) ? sd : K(0.0);
+    }
+    case WL_TERM_V_LOW_SPEED_PENALTY: {
+        const real sp = r_sqrt((s->vb[0] * s->vb[0] + s->vb[1] * s->vb[1]) + s->vb[2] * s->vb[2]);
+        return (sp < p[0]) ? K(1.0) : K(0.0);
+    }
+    case WL_TERM_V_OFF_TRACK: {
+        const real x = s->p[0], y = s->p[1];
+        int out;
+        if (r_fabs(y) < p[0]) out = r_fabs(x) > p[1];
+        else if (y > K(0.0)) { const real a = y - p[0]; out = a * a + x * x > p[2]; }
+        else { const real a = y + p[0]; out = a * a + x * x > p[2]; }
+        return out ? K(1.0) : K(0.0);
+    }
+    case WL_TERM_V_BOOL_IS_NOT_TRAVERSABLE:
+        if (t / (uint32_t)c->max_episode_length < 1000u) return K(0.0);
+        return term_traversable(c, map, s->p[0], s->p[1]) ? K(0.0) : K(1.0);
+    case WL_TERM_V_ROLL_OVER: {
+        real e[3]; euler_xyz(s->q, e);
+        const real roll = e[0] - KF(3.14159265358979323846);
+        return (roll < KF(1.57079632679489661923) && roll > -KF(1.57079632679489661923)) ? K(1.0) : K(0.0);
+    }
+    default: return K(0.0);
+    }
+}
+
+/* one env of wl_terms_kernel: terminations first, then the rewards added to *rew; the sums of env i (stride n) are kept or
+ * zeroed; contrib[9] = the log contributions ([k] done env's episode sum / fired flag, [8] done).  vals[k] (may be NULL):
+ * term k's value.  Returns the extra termination bits for the step's tmask (0x80 terminated, 1 time-out). */
+static uint32_t dterms_env(const wl_config* c, const uint8_t* map, const wlo_term_table* tt, const wlo_term_in* s, uint32_t t,
+                           real* prev, real* sums, size_t n, int builtin_done, real* rew, uint8_t* fired_o, real contrib[9],
+                           real* vals) {
+    uint32_t fired = 0u;
+    int x_term = 0, x_to = 0;
+    for (int k = 0; k < 9; ++k) contrib[k] = K(0.0);
+    for (int k = 0; k < tt->n; ++k) {
+        if (tt->role[k] == WL_TERM_ROLE_REWARD) continue;
+        const real v = term_value(c, map, tt->kind[k], tt->p[k], s, t, prev);
+        if (vals) vals[k] = v;
+        if (v != K(0.0)) {
+            fired |= 1u << k;
+            if (tt->role[k] == WL_TERM_ROLE_TIME_OUT) x_to = 1; else x_term = 1;
+        }
+    }
+    real r = *rew, ksum[WL_MAX_DEVICE_TERMS];
+    for (int k = 0; k < tt->n; ++k) {
+        ksum[k] = K(0.0);
+        if (tt->role[k] != WL_TERM_ROLE_REWARD || tt->skip[k]) continue;
+        const real f = term_value(c, map, tt->kind[k], tt->p[k], s, t, prev);
+        if (vals) vals[k] = f;
+        const real val = f * tt->scale[k];
+        r += val;
+        ksum[k] = sums[(size_t)k * n] + val;
+    }
+    *rew = r;
+    *fired_o = (uint8_t)fired;
+    const int done = builtin_done || x_term || x_to;
+    for (int k = 0; k < tt->n; ++k) {
+        if (tt->role[k] != WL_TERM_ROLE_REWARD) { contrib[k] = (done && ((fired >> k) & 1u)) ? K(1.0) : K(0.0); continue; }
+        if (tt->skip[k]) continue;
+        contrib[k] = done ? ksum[k] : K(0.0);
+        sums[(size_t)k * n] = done ? K(0.0) : ksum[k];
+    }
+    contrib[8] = done ? K(1.0) : K(0.0);
+    return (x_term ? 0x80u : 0u) | (x_to ? 1u : 0u);
+}
+
+/* the Episode_* entries from the per-env contributions [n][9], in the kernels' fixed order */
+static void dterms_log(const wl_config* c, const wlo_term_table* tt, const real* contrib, int n, double out[WL_MAX_DEVICE_TERMS]) {
+    const int ctas = (n + WLO_TERMS_BS - 1) / WLO_TERMS_BS;
+    real* part = (real*)calloc((size_t)ctas * 9, sizeof(real));
+    real red[WLO_TERMS_BS], col[9];
+    for (int g = 0; g < ctas; ++g)
+        for (int k = 0; k < 9; ++k) {
+            for (int j = 0; j < WLO_TERMS_BS; ++j) {
+                const int i = g * WLO_TERMS_BS + j;
+                red[j] = (i < n) ? contrib[(size_t)i * 9 + k] : K(0.0);
+            }
+            for (int h = WLO_TERMS_BS / 2; h > 0; h >>= 1)
+                for (int j = 0; j < h; ++j) red[j] += red[j + h];
+            part[(size_t)g * 9 + k] = red[0];
+        }
+    for (int k = 0; k < 9; ++k) {
+        real lane[32], nxt[32];
+        for (int l = 0; l < 32; ++l) {
+            real v = K(0.0);
+            for (int g = l; g < ctas; g += 32) v += part[(size_t)g * 9 + k];
+            lane[l] = v;
+        }
+        for (int o = 16; o > 0; o >>= 1) {
+            for (int l = 0; l < 32; ++l) nxt[l] = lane[l] + lane[l ^ o];
+            memcpy(lane, nxt, sizeof lane);
+        }
+        col[k] = lane[0];
+    }
+    free(part);
+    for (int j = 0; j < WL_MAX_DEVICE_TERMS; ++j)
+        out[j] = j >= tt->n ? 0.0
+               : (double)((tt->role[j] == WL_TERM_ROLE_REWARD) ? col[j] / r_max(col[8], K(1.0)) / (real)c->episode_length_s : col[j]);
+}
+
+/* ------------------------------------------------------------------------- */
 /* one env.step() for one env -- ordering per SURVEY 3.3 A..I                  */
 /* ------------------------------------------------------------------------- */
 typedef struct { double sum[WL_MAX_REW_TERMS]; double n_reset; double n_term[WL_MAX_TERM_TERMS]; int any; } step_log;
@@ -974,6 +1189,15 @@ static int env_step(wlo_sim* s, int li, const float* a_in, int64_t t, float* obs
         e->sums[k] += val;
     }
     *rew = (float)total;
+    if (s->dt_run) {      /* wl_step_terms: the device terms on the pre-reset state, between E and F */
+        wlo_dterms* dt = s->dt;
+        const size_t n = (size_t)c->num_envs;
+        wlo_term_in ti; term_in(e->p, e->q, e->v, e->w, e->omega, &ti);
+        real r = (real)*rew;
+        tmask |= dterms_env(c, s->vis_map, &dt->tt, &ti, (uint32_t)t, &dt->prev[li], dt->sums + li, n, tmask != 0u, &r,
+                            &dt->fired[li], dt->contrib + (size_t)li * 9, NULL);
+        *rew = (float)r;
+    }
     *term_o = (uint8_t)((tmask & ~1u) ? 1 : 0); *trunc_o = (uint8_t)(tmask & 1u);
     /* F. auto reset */
     if (tmask) {
@@ -1025,7 +1249,12 @@ wlo_sim* wlo_create(const wl_config* cfg, const float* heightfield) {
     for (int i = 0; i < cfg->num_envs; ++i) s->env[i].q[0] = K(1.0);
     return s;
 }
-void wlo_destroy(wlo_sim* s) { if (s) { free(s->env); free(s->hf); free(s->vis_cells); free(s->vis_map); free(s); } }
+static void free_dterms(wlo_sim* s) {
+    if (!s->dt) return;
+    free(s->dt->sums); free(s->dt->prev); free(s->dt->contrib); free(s->dt->fired); free(s->dt);
+    s->dt = NULL;
+}
+void wlo_destroy(wlo_sim* s) { if (s) { free_dterms(s); free(s->env); free(s->hf); free(s->vis_cells); free(s->vis_map); free(s); } }
 int wlo_is_double(void) {
 #ifdef WLO_DOUBLE
     return 1;
@@ -1134,6 +1363,81 @@ int wlo_step(wlo_sim* s, const float* action, float* obs, float* rew, uint8_t* t
         }
     }
     return err;
+}
+
+/* wl_set_device_terms: the table, zero episode sums, unset previous elevations; n = 0 clears it */
+int wlo_set_device_terms(wlo_sim* s, const wl_term_desc* terms, int32_t n_terms) {
+    wlo_term_table tt;
+    int rc = term_table(&s->cfg, terms, n_terms, &tt);
+    if (rc) return rc;
+    free_dterms(s);
+    if (n_terms == 0) return 0;
+    const size_t n = (size_t)s->cfg.num_envs;
+    wlo_dterms* dt = (wlo_dterms*)calloc(1, sizeof(wlo_dterms));
+    dt->tt = tt;
+    dt->sums = (real*)calloc(WL_MAX_DEVICE_TERMS * n, sizeof(real));
+    dt->prev = (real*)malloc(n * sizeof(real));
+    for (size_t i = 0; i < n; ++i) dt->prev[i] = (real)NAN;
+    dt->contrib = (real*)calloc(n * 9, sizeof(real));
+    dt->fired = (uint8_t*)calloc(n, 1);
+    s->dt = dt;
+    return 0;
+}
+/* wl_step_terms (with a term log): wlo_step with the device terms between E and F; no terms: wlo_step itself */
+int wlo_step_terms(wlo_sim* s, const float* action, float* obs, float* rew, uint8_t* terminated, uint8_t* truncated,
+                   int64_t step_counter, int nthreads) {
+    if (!s->dt) return wlo_step(s, action, obs, rew, terminated, truncated, step_counter, nthreads);
+    s->dt_run = 1;
+    int rc = wlo_step(s, action, obs, rew, terminated, truncated, step_counter, nthreads);
+    s->dt_run = 0;
+    dterms_log(&s->cfg, &s->dt->tt, s->dt->contrib, s->cfg.num_envs, s->dt->log);
+    return rc;
+}
+/* the last wlo_step_terms: fired bits [N] (wl_device_term_masks) and the Episode_* row [8]; per-env state: episode sums
+ * [8][N] and previous elevations [N] (either output may be NULL) */
+int wlo_get_device_terms(const wlo_sim* s, uint8_t* fired, double* term_log, double* sums, double* prev) {
+    if (!s->dt) return WL_EINVAL;
+    const size_t n = (size_t)s->cfg.num_envs;
+    if (fired) memcpy(fired, s->dt->fired, n);
+    if (term_log) memcpy(term_log, s->dt->log, sizeof s->dt->log);
+    if (sums) for (size_t k = 0; k < WL_MAX_DEVICE_TERMS * n; ++k) sums[k] = (double)s->dt->sums[k];
+    if (prev) for (size_t i = 0; i < n; ++i) prev[i] = (double)s->dt->prev[i];
+    return 0;
+}
+/* The term kernel on placed states: state in the product's [group][N] float4 layout (the pre-reset state stage a leaves),
+ * done[N] the built-in termination bytes, map the Visual traversability map [rows * cols] (NULL for other tasks), t the step
+ * counter.  In / out: prev[N], sums[8][N], rew[N] (the terms are added to it).  Out: fired[N], vals[N][8] (each term's
+ * value, 0 for a skipped reward term), term_log[8].  The arrays are double in both builds (fp32 values in the fp32 one). */
+int wlo_device_terms(const wl_config* c, const uint8_t* map, const wl_term_desc* terms, int32_t n_terms, const float* state,
+                     const uint8_t* done, int64_t t, double* prev, double* sums, double* rew, uint8_t* fired, double* vals,
+                     double* term_log) {
+    wlo_term_table tt;
+    int rc = term_table(c, terms, n_terms, &tt);
+    if (rc) return rc;
+    if (c->task == WL_TASK_VISUAL && !map) return WL_EINVAL;
+    const int n = c->num_envs;
+    real* contrib = (real*)calloc((size_t)n * 9, sizeof(real));
+    real* ksums = (real*)malloc((size_t)WL_MAX_DEVICE_TERMS * n * sizeof(real));
+    for (size_t k = 0; k < (size_t)WL_MAX_DEVICE_TERMS * n; ++k) ksums[k] = (real)sums[k];
+    for (int i = 0; i < n; ++i) {
+        const float* g;
+        real p[3], q[4], v[3], w[3], om[4];
+        g = state + ((size_t)WL_G_POS * n + i) * 4; for (int k = 0; k < 3; ++k) p[k] = g[k];
+        g = state + ((size_t)WL_G_QUAT * n + i) * 4; for (int k = 0; k < 4; ++k) q[k] = g[k];
+        g = state + ((size_t)WL_G_LINVEL * n + i) * 4; for (int k = 0; k < 3; ++k) v[k] = g[k];
+        g = state + ((size_t)WL_G_ANGVEL * n + i) * 4; for (int k = 0; k < 3; ++k) w[k] = g[k];
+        g = state + ((size_t)WL_G_WHEEL * n + i) * 4; for (int k = 0; k < 4; ++k) om[k] = g[k];
+        wlo_term_in ti; term_in(p, q, v, w, om, &ti);
+        real pv = (real)prev[i], r = (real)rew[i], vv[WL_MAX_DEVICE_TERMS] = {0};
+        dterms_env(c, map, &tt, &ti, (uint32_t)t, &pv, ksums + i, (size_t)n, done[i] != 0, &r, &fired[i],
+                   contrib + (size_t)i * 9, vv);
+        prev[i] = (double)pv; rew[i] = (double)r;
+        if (vals) for (int k = 0; k < WL_MAX_DEVICE_TERMS; ++k) vals[(size_t)i * WL_MAX_DEVICE_TERMS + k] = (double)vv[k];
+    }
+    for (size_t k = 0; k < (size_t)WL_MAX_DEVICE_TERMS * n; ++k) sums[k] = (double)ksums[k];
+    if (term_log) dterms_log(c, &tt, contrib, n, term_log);
+    free(contrib); free(ksums);
+    return 0;
 }
 
 int wlo_observe(wlo_sim* s, float* obs, int64_t step_counter, int32_t call_idx) {

@@ -351,7 +351,183 @@ def golden_camera():
                         aug=np.array(augs, dtype=np.float32), out=np.stack(outs).astype(np.float32))
 
 
+def _f32(x):
+    return float(np.float32(x))
+
+
+def _ulps(x):
+    """x as fp32 and its two fp32 neighbours."""
+    x = np.float32(x)
+    return [float(x), float(np.nextafter(x, np.float32(np.inf))), float(np.nextafter(x, np.float32(-np.inf)))]
+
+
+# the parameter sets of golden_device_terms: the ones the tests use plus every threshold a designed state sits on, exactly and
+# one fp32 ulp either side (the state's value is exact; the threshold moves)
+_Z29 = float(np.float32(np.float32(0.29) - np.float32(0.19)))          # pos.z = 0.29: z = pos.z - 0.19 in fp32
+_P_UP = float(np.float32(np.pi / 2))                                   # pitch of a |sin_pitch| >= 1 quaternion (nose up)
+_P_DN = float(np.float32(np.float32(-np.pi / 2) + np.float32(2 * np.pi)))   # nose down, wrapped
+DEVICE_TERM_PARAMS = {
+    "forward_vel": [()], "forward_wheel_spin": [()], "change_in_elevation": [()], "ascending": [()],
+    "steep_penalty": [(0.3,), (0.05,)] + [(v,) for x in (0.0, _P_UP, _P_DN) for v in _ulps(x)],
+    "yaw_change_onElev": [(0.5, 0.05)] + [(a, _Z29) for a in _ulps(0.5)] + [(0.25, z) for z in _ulps(_Z29)],
+    "upright_penalty": [(10.0,), (40.0,)],            # + the exact angles of the designed states, added below
+    "roll_on_elev": [(0.05, 0.3)] + [(_Z29, a) for a in _ulps(0.5)] + [(z, 0.25) for z in _ulps(_Z29)],
+    "low_vel_penalty": [(v,) for v in _ulps(0.1)],
+    "is_traversable": [()], "is_traversable_speed_scaled": [()],
+    "vel_rew_trav": [(1.0, 2.0), (1.5, 2.0), (2.0, 1.0)],
+    "low_speed_penalty": [(v,) for v in _ulps(0.3)] + [(v,) for v in _ulps(5.0)],
+    "off_track": [(2.0, 5.0), (5.0, 15.3), (20.0, 60.0), (2.0, 4.0)],
+    "roll_over": [()],
+}
+
+
+def golden_device_terms():
+    """The 17 functions of the device-term library (csrc/wl_terms.cuh), the reference's own code from
+    elevation/mushr_elevation_env_cfg.py and visual/mushr_visual_env_cfg.py, on random and designed states: every threshold
+    hit exactly and one fp32 ulp either side (identity or axis-aligned quaternions there, so that both rotations are exact),
+    pitch either side of 0 and |sin_pitch| >= 1, roll at pi and pi +- pi/2, r22 = +-1 with |q| != 1 and an r22 that rounds
+    below -1, every off_track boundary, positions on a traversability cell edge and one ulp either side, map cells beyond
+    every edge, the counter either side of bool_is_not_traversable's switch, and elevation_continuity over three-call
+    sequences (its function attribute cleared before each).  euler_xyz_from_quat and matrix_from_quat come from the
+    stand-in ([UPSTREAM-RECALL]); everything else is the reference's."""
+    from wheeledlab_tasks.elevation import mushr_elevation_env_cfg as E
+    from wheeledlab_tasks.visual import mushr_visual_env_cfg as V
+    f32 = np.float32
+    rng = np.random.default_rng(17)
+    rows = 24                                            # square, as the reference's 500 x 500 map (get_map_id clamps x to rows)
+    spacing, width = 0.5, rows * 0.5
+    trav_map = rng.random((rows, rows)) < 0.45
+    trav_map[0, 0], trav_map[0, 1], trav_map[-1, -1], trav_map[-1, -2] = True, False, True, False
+    max_len = 50                                         # the Visual task's max_episode_length (10 s / 0.2 s)
+
+    pos, quat, vel, ang, omega = [], [], [], [], []
+
+    def add(p=(0.0, 0.0, 0.29), q=(1.0, 0.0, 0.0, 0.0), v=(0.0, 0.0, 0.0), w=(0.0, 0.0, 0.0), om=(0.0, 0.0, 0.0, 0.0)):
+        pos.append(p); quat.append(q); vel.append(v); ang.append(w); omega.append(om)
+
+    # random states over the map and beyond it, some on the ramp (z - 0.19 above the thresholds), random unit quaternions
+    nr = 384
+    rq = rng.standard_normal((nr, 4)); rq /= np.linalg.norm(rq, axis=1, keepdims=True)
+    rq[: nr // 3, 1:3] *= 0.15; rq[: nr // 3] /= np.linalg.norm(rq[: nr // 3], axis=1, keepdims=True)   # mostly upright
+    for i in range(nr):
+        add(p=(rng.uniform(-8, 8), rng.uniform(-8, 8), rng.uniform(0.0, 0.6)), q=tuple(rq[i]), v=tuple(rng.normal(0, [1.5, 1.0, 0.5])),
+            w=tuple(rng.normal(0, [1.0, 1.0, 2.0])), om=tuple(rng.normal(40, 60, 4)))
+    # thresholds on identity quaternions (v_b = v_w, w_b = w_w exactly)
+    for vx in _ulps(1.2) + _ulps(0.1) + _ulps(0.3) + [2.0, 3.0, 4.0] + _ulps(2.0)[1:] + _ulps(4.0)[1:]:
+        add(v=(vx, 0.0, 0.0))
+    add(v=(3.0, 4.0, 0.0)); add(v=(0.0, 3.0, 4.0)); add(v=(-3.0, 0.0, -4.0))
+    for s in (_ulps(200.0)):
+        add(om=(s, 0.0, 0.0, 0.0))
+    add(om=(150.0, 25.0, 12.5, 12.5)); add(om=(-50.0, 250.0, 0.0, 0.0))
+    tiny = float(np.nextafter(f32(0), f32(1)))
+    for vz in (0.0, -0.0, tiny, -tiny, 1e-7, -1e-7, 0.5):
+        add(v=(0.2, 0.0, vz))
+    for a in _ulps(0.5) + [0.25]:
+        for z in (0.29, 0.19, 0.5):
+            add(p=(1.0, 1.0, z), w=(a, 0.0, a)); add(p=(1.0, 1.0, z), w=(-a, 0.0, -a))
+    # Euler-angle edges: |sin_pitch| >= 1 (non-unit quaternions), pitch just either side of 0, roll at pi and pi +- pi/2
+    for q in [(1.0, 0.0, 1.0, 0.0), (1.0, 0.0, -1.0, 0.0), (0.7071068, 0.0, 0.7071068, 0.0), (0.7071068, 0.0, -0.7071068, 0.0),
+              (1.0, 0.0, 1e-4, 0.0), (1.0, 0.0, -1e-4, 0.0), (1.0, 0.0, 1e-8, 0.0), (1.0, 0.0, -1e-8, 0.0),
+              (0.0, 1.0, 0.0, 0.0), (0.5, 0.5, 0.0, 0.0), (0.5, -0.5, 0.0, 0.0), (1.0, 1.0, 0.0, 0.0), (1.0, -1.0, 0.0, 0.0),
+              (0.0, 2.0, 0.0, 0.0), (2.0, 0.0, 0.0, 0.0), (0.0, 3.0, 0.0, 0.0), (0.0, 0.0, 2.0, 0.0), (0.0, 0.6, 0.8, 0.0),
+              (1e-3, 1.0, 0.0, 0.0), (1e-3, -1.0, 0.0, 0.0), (0.0, 1.0, 0.0, 1e-3), (0.0, 1.0, 0.0, -1e-3),
+              (1.0, 0.5, 0.5, 0.0), (1.0, -0.5, -0.5, 0.0)]:                 # roll = +-pi/2 exactly (cos_roll = 0)
+        add(q=q)              # at rest: with |q| != 1 the rotation matrix and quat_rotate_inverse scale v differently
+    # r22 that rounds below -1 (arccos is NaN there): w = z = 0, x^2 + y^2 in any summation order
+    found = 0
+    for _ in range(20000):
+        x, y = f32(rng.uniform(0.1, 3)), f32(rng.uniform(0.1, 3))
+        s = f32(x * x) + f32(y * y)
+        r22 = f32(1) - f32(f32(2) / s) * s
+        if r22 < -1:
+            add(q=(0.0, float(x), float(y), 0.0)); found += 1
+            if found == 6:
+                break
+    # off_track boundaries: |y| = straight, |x| = corner_out_radius, the circles (3-4-5 triangles), each +- one ulp
+    for (st, r) in ((2.0, 5.0), (2.0, 4.0)):
+        pts = [(r, 0.0), (-r, 0.0), (r, st), (r, -st), (0.0, st), (0.0, -st), (0.0, st + r), (0.0, -st - r)]
+        if r == 5.0:
+            pts += [(3.0, st + 4.0), (-3.0, st + 4.0), (3.0, -st - 4.0), (4.0, st + 3.0), (-4.0, -st - 3.0)]
+        for x, y in pts:
+            for xx in _ulps(x):
+                for yy in _ulps(y):
+                    add(p=(xx, yy, 0.1))
+    # |y| = straight with |x| = fp32(corner_out_radius): the straight test and the circle (r^2 rounded from double) disagree
+    for x, y in ((15.3, 0.0), (-15.3, 4.9), (15.3, 5.0), (-15.3, -5.0), (0.0, 20.3), (60.0, 0.0), (0.0, -80.0), (59.9, 19.9)):
+        for xx in _ulps(x):
+            add(p=(xx, y, 0.1))
+    # traversability: every cell edge (an integer quotient) and one ulp either side, along both axes; beyond every edge
+    for k in range(-1, rows + 2):
+        e = float(f32(k * spacing - width / 2 - spacing / 2))
+        for ee in _ulps(e):
+            add(p=(ee, 0.3, 0.1), v=(0.8, 0.0, 0.0)); add(p=(0.3, ee, 0.1), v=(0.8, 0.0, 0.0))
+    for x, y in ((-100.0, 0.0), (100.0, 0.0), (0.0, -100.0), (0.0, 100.0), (-100.0, -100.0), (100.0, 100.0), (-100.0, 100.0), (100.0, -100.0)):
+        add(p=(x, y, 0.1), v=(1.0, 0.0, 0.0))
+    n = len(pos)
+    P = torch.tensor(pos, dtype=torch.float32); Q = torch.tensor(quat, dtype=torch.float32)
+    VW = torch.tensor(vel, dtype=torch.float32); WW = torch.tensor(ang, dtype=torch.float32)
+    OM = torch.tensor(omega, dtype=torch.float32)
+
+    env = FakeEnv(n)
+    env.max_episode_length = max_len
+    env.scene["terrain"] = types.SimpleNamespace()
+    d = env.scene["robot"].data
+    d.root_pos_w, d.root_quat_w, d.root_lin_vel_w, d.root_ang_vel_w = P, Q, VW, WW
+    d.root_lin_vel_b = math_utils.quat_rotate_inverse(Q, VW)
+    d.root_ang_vel_b = math_utils.quat_rotate_inverse(Q, WW)
+    d.joint_vel = torch.zeros(n, 12); d.joint_vel[:, 0:4] = OM
+    V.TraversabilityHashmapUtil().set_traversability_hashmap(trav_map.tolist(), (rows, rows), (spacing, spacing))
+
+    params = dict(DEVICE_TERM_PARAMS)
+    deg = torch.rad2deg(torch.arccos(torch.tensor([1.0, 0.0, -1.0])))          # the exact angles of the designed states
+    params["upright_penalty"] = params["upright_penalty"] + [(v,) for x in deg.tolist() for v in _ulps(x)]
+    names = {"forward_vel": E.forward_vel, "forward_wheel_spin": E.forward_wheel_spin, "change_in_elevation": E.change_in_elevation,
+             "ascending": E.ascending, "steep_penalty": E.steep_penalty, "yaw_change_onElev": E.yaw_change_onElev,
+             "upright_penalty": E.upright_penalty, "roll_on_elev": E.roll_on_elev, "low_vel_penalty": E.low_vel_penalty,
+             "is_traversable": V.is_traversable, "is_traversable_speed_scaled": V.is_traversable_speed_scaled,
+             "vel_rew_trav": V.vel_rew_trav, "low_speed_penalty": V.low_speed_penalty, "off_track": V.off_track,
+             "roll_over": V.roll_over}
+    out = {"pos": P.numpy(), "quat": Q.numpy(), "vel_w": VW.numpy(), "ang_w": WW.numpy(), "omega": OM.numpy(),
+           "vel_b": d.root_lin_vel_b.numpy(), "ang_b": d.root_ang_vel_b.numpy(), "map": trav_map.astype(np.uint8),
+           "spacing": np.float64(spacing), "max_episode_length": np.int64(max_len), "n_random": np.int64(nr)}
+    for name, fn in names.items():
+        sig = [k for k in __import__("inspect").signature(fn).parameters if k not in ("env", "asset_cfg")]
+        vals = []
+        for ps in params[name]:
+            vals.append(fn(env, **dict(zip(sig, ps))).to(torch.float32).numpy())
+        out["p_" + name] = np.array(params[name], dtype=np.float64).reshape(len(params[name]), -1)
+        out["f_" + name] = np.stack(vals)
+    # bool_is_not_traversable: common_step_counter either side of 1000 episodes
+    ctrs = [1000 * max_len - 1, 1000 * max_len, 1000 * max_len + max_len - 1, 999 * max_len]
+    vals = []
+    for c in ctrs:
+        env.common_step_counter = c
+        vals.append(V.bool_is_not_traversable(env).to(torch.float32).numpy())
+    out["t_bool_is_not_traversable"] = np.array(ctrs, np.int64)
+    out["f_bool_is_not_traversable"] = np.stack(vals)
+    # elevation_continuity: three calls per sequence on the same envs, the attribute cleared before each sequence
+    zs = np.array([[0.29, 0.29, 0.29, 0.30, 0.50, 0.29, 0.10, 0.30, 0.29],
+                   [0.29, 0.35, 0.25, 0.29, 0.40, 0.30, 0.50, 0.30, 0.29],
+                   [0.29, 0.40, 0.20, 0.29, 0.30, 0.29, 0.05, 0.31, 0.30]], np.float32)
+    thr = _ulps(_Z29) + [0.05, -1.0]
+    ce = FakeEnv(zs.shape[1])
+    cd = ce.scene["robot"].data
+    seq = []
+    for tz in thr:
+        if hasattr(E.elevation_continuity, "prev_elevation"):
+            del E.elevation_continuity.prev_elevation
+        calls = []
+        for k in range(zs.shape[0]):
+            cd.root_pos_w = torch.zeros(zs.shape[1], 3); cd.root_pos_w[:, 2] = torch.from_numpy(zs[k])
+            calls.append(E.elevation_continuity(ce, threshold_elev=tz).to(torch.float32).numpy())
+        seq.append(np.stack(calls))
+    del E.elevation_continuity.prev_elevation
+    out["cont_z"], out["p_elevation_continuity"], out["f_elevation_continuity"] = zs, np.array(thr, np.float64)[:, None], np.stack(seq)
+    np.savez_compressed(HERE / "device_terms.npz", **out)
+
+
 if __name__ == "__main__":
+    golden_device_terms()
     golden_camera()
     golden_visual()
     golden_elevation()

@@ -58,6 +58,10 @@ def _load(path):
     lib.wlo_camera_post.argtypes = [vp, vp, vp, vp, i32]
     lib.wlo_camera_render.argtypes = [vp, i32, vp]
     lib.wlo_derive_suspension.argtypes = [vp, vp, vp]
+    lib.wlo_set_device_terms.argtypes = [vp, vp, i32]
+    lib.wlo_step_terms.argtypes = [vp, vp, vp, vp, vp, vp, i64, i32]
+    lib.wlo_get_device_terms.argtypes = [vp, vp, vp, vp, vp]
+    lib.wlo_device_terms.argtypes = [vp, vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp]
     lib.wlo_config_describe.restype = C.c_char_p
     return lib
 
@@ -112,6 +116,42 @@ def cfg_from_blob(path, **overrides):
     return cfg
 
 
+class TermDesc(C.Structure):
+    """wl_term_desc"""
+    _fields_ = [("kind", C.c_int32), ("role", C.c_int32), ("weight", C.c_double), ("params", C.c_double * 4)]
+
+
+MAX_DEVICE_TERMS = 8
+
+
+def term_table(terms):
+    """A wl_term_desc array from (kind, role, weight, params[<= 4]) rows."""
+    arr = (TermDesc * max(1, len(terms)))()
+    for k, (kind, role, weight, params) in enumerate(terms):
+        p = list(params) + [0.0] * (4 - len(params))
+        arr[k] = TermDesc(int(kind), int(role), float(weight), (C.c_double * 4)(*p))
+    return arr
+
+
+def device_terms(cfg, terms, state, done, t, vis_map=None, prev=None, sums=None, rew=None, kind="f32"):
+    """wlo_device_terms: the term kernel on placed states (state [16, N, 4] float32, done [N]).  Returns a dict of rew [N],
+    fired [N], vals [N, 8], term_log [8], prev [N] and sums [8, N] (float64; fp32 values in the fp32 build)."""
+    n = int(cfg.num_envs)
+    st = np.ascontiguousarray(state, np.float32)
+    assert st.shape == (NUM_GROUPS, n, 4)
+    dn = np.ascontiguousarray(done, np.uint8)
+    out = {"prev": np.full(n, np.nan) if prev is None else np.array(prev, np.float64),
+           "sums": np.zeros((MAX_DEVICE_TERMS, n)) if sums is None else np.array(sums, np.float64),
+           "rew": np.zeros(n) if rew is None else np.array(rew, np.float64),
+           "fired": np.zeros(n, np.uint8), "vals": np.zeros((n, MAX_DEVICE_TERMS)), "term_log": np.zeros(MAX_DEVICE_TERMS)}
+    m = None if vis_map is None else np.ascontiguousarray(vis_map, np.uint8)
+    tt = term_table(terms)
+    rc = get_lib(kind).wlo_device_terms(C.byref(cfg), _p(m), tt, len(terms), _p(st), _p(dn), int(t), _p(out["prev"]),
+                                        _p(out["sums"]), _p(out["rew"]), _p(out["fired"]), _p(out["vals"]), _p(out["term_log"]))
+    assert rc == 0, rc
+    return out
+
+
 class Oracle:
     """One oracle instance; mirrors the wl_* calls with host (numpy) buffers."""
 
@@ -157,6 +197,24 @@ class Oracle:
         rc = self.lib.wlo_step(self._h, _p(a), _p(obs), _p(rew), _p(term), _p(trunc), step_counter, self.threads)
         assert rc == 0, rc
         return obs, rew, term, trunc
+
+    def set_device_terms(self, terms):
+        """wl_set_device_terms: (kind, role, weight, params) rows; [] clears them."""
+        assert self.lib.wlo_set_device_terms(self._h, term_table(terms), len(terms)) == 0
+
+    def step_terms(self, action, step_counter):
+        """wl_step_terms: step() with the device terms; returns (obs, rew, term, trunc, fired [N], term_log [8])."""
+        a = np.ascontiguousarray(action, dtype=np.float32)
+        obs = np.empty((self.n, self.obs_dim), np.float32)
+        rew = np.empty(self.n, np.float32)
+        term = np.empty(self.n, np.uint8)
+        trunc = np.empty(self.n, np.uint8)
+        rc = self.lib.wlo_step_terms(self._h, _p(a), _p(obs), _p(rew), _p(term), _p(trunc), step_counter, self.threads)
+        assert rc == 0, rc
+        fired = np.empty(self.n, np.uint8)
+        tl = np.empty(MAX_DEVICE_TERMS, np.float64)
+        assert self.lib.wlo_get_device_terms(self._h, _p(fired), _p(tl), None, None) == 0
+        return obs, rew, term, trunc, fired, tl
 
     def observe(self, step_counter, call_idx=0):
         obs = np.empty((self.n, self.obs_dim), np.float32)

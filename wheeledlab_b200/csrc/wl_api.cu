@@ -3234,5 +3234,24 @@ int wl_test_philox(uint64_t seed, uint32_t c0_base, uint32_t c1, uint32_t c2, ui
     wl_philox_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(seed, c0_base, c1, c2, c3, reinterpret_cast<uint4*>(d_out), n);
     return cuda_check(cudaGetLastError(), "wl_philox_kernel");
 }
+int wl_test_device_terms(wl_sim* sim, const float* d_state, const uint8_t* d_done, float* d_rew, float* d_term_log,
+                         int64_t step_counter, void* stream) {
+    if (!sim || !d_state || !d_done || !d_rew) return fail(WL_EINVAL, "wl_test_device_terms: null argument");
+    if ((uintptr_t)d_state & 15u) return fail(WL_EINVAL, "wl_test_device_terms: state must be 16-byte aligned");
+    if (step_counter < 0) return fail(WL_EINVAL, "wl_test_device_terms: takes a host step counter");
+    DevTerms* dt = sim->dterms;
+    if (!dt) return fail(WL_EINVAL, "wl_test_device_terms: the handle has no device terms");
+    ensure_device(sim);
+    cudaStream_t cs = (cudaStream_t)stream;
+    const int n = sim->cfg.num_envs, ctas = (n + WL_TERMS_BS - 1) / WL_TERMS_BS;
+    wl_terms_kernel<<<ctas, WL_TERMS_BS, 0, cs>>>(dt->tt, sim->cfg, reinterpret_cast<const float4*>(d_state), sim->globals, sim->hf,
+                                                  (uint32_t)step_counter, d_rew, d_done, dt->b, d_term_log != nullptr);
+    if (int rc = launched(sim, "wl_terms_kernel")) return rc;
+    if (d_term_log) {
+        wl_terms_log_kernel<<<1, 9 * 32, 0, cs>>>(dt->tt, sim->cfg, dt->b.part, ctas, d_term_log);
+        if (int rc = launched(sim, "wl_terms_log_kernel")) return rc;
+    }
+    return WL_OK;
+}
 
 }  // extern "C"
