@@ -636,6 +636,30 @@ typedef struct wl_critic_term {
 int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_terms);
 /* Dc: the width of the critic row (0 with no table) */
 int32_t wl_critic_obs_dim(const wl_sim* sim);
+
+/* ---- reset-mode domain randomisation (IsaacLab EventTermCfg mode="reset", DESIGN.md 6n) --------------------------------
+ * The start-up events of wl_startup draw each env's parameters once.  A bit set here redraws that event's parameters for
+ * every env a call resets: the envs a step auto-reset (wl_step, wl_step_host, wl_step_host_zero_copy, wl_act_step,
+ * wl_act_infer_step, wl_step_stage_b, wl_step_terms) and the env_ids of wl_reset (all envs when NULL).  The draw is
+ * wl_startup's with the key (seed, env_id_offset + i, t, stream 12, k) instead of (.., 0, stream 6, k), t being the step
+ * counter of the call that reset the env (decoded from the device counter for WL_DEVICE_COUNTER_PLUS), k = 0 buckets,
+ * 1 gains, 2 base mass, 3 wheel masses.  The total mass is formed as wl_startup forms it, from the nominal mass: a
+ * component whose bit is clear is recomputed from its start-up key, so it keeps its start-up value bit for bit.
+ *   WL_RESET_EV_MATERIAL        randomize_rigid_body_material: WL_G_PMU_D, WL_G_PMU_C  (needs dr_enable)
+ *   WL_RESET_EV_ACTUATOR_GAINS  randomize_actuator_gains: WL_G_PKD                   (needs dr_enable, dr_kd_mask != 0)
+ *   WL_RESET_EV_BASE_MASS       randomize_rigid_body_mass on the base: WL_G_PMASS     (needs dr_enable)
+ *   WL_RESET_EV_WHEEL_MASS      randomize_rigid_body_mass on the wheels: WL_G_PMASS, WL_G_PIW (needs dr_wheel_mass_enable)
+ * A host-side set-up call kept per handle: nothing is launched.  With mask 0 (the default) no call launches anything new.
+ * With a non-zero mask every call listed above launches one more kernel on its stream after its own work, and wl_rollout
+ * returns WL_EUNSUPPORTED.  WL_EINVAL, leaving the handle as it was: a null handle, an unknown bit, a bit whose event the
+ * config does not have.  A graph captured with the old mask keeps the old mask. */
+#define WL_RESET_EV_MATERIAL       1u
+#define WL_RESET_EV_ACTUATOR_GAINS 2u
+#define WL_RESET_EV_BASE_MASS      4u
+#define WL_RESET_EV_WHEEL_MASS     8u
+int wl_set_reset_events(wl_sim* sim, uint32_t mask);
+/* the handle's mask (0 for a null handle) */
+uint32_t wl_reset_events(const wl_sim* sim);
 /* d_critic_obs [N, Dc] (rows leave as 16-byte stores when it is 16-byte aligned) from the state the most recent step / reset left -- after wl_step, the
  * post-reset state its observation row was formed from.  One launch, no generator and no counter; capturable.  For a handle
  * whose noise_std are all 0 the five BlindObsCfg columns equal the policy row of wl_step (as fp32 values; a -0 that the

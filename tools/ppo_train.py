@@ -37,6 +37,8 @@ def main():
     ap.add_argument("--log-dir", default=None, help="checkpoints go to LOG_DIR/models/model_{it}.pt")
     ap.add_argument("--resume", default=None, help="checkpoint to continue from (its iteration, weights and Adam state)")
     ap.add_argument("--out", default=None, help="also write the log here")
+    ap.add_argument("--reset-events", default="", help="DR events redrawn at every reset (mode='reset'), comma-separated: "
+                                                        "material, actuator_gains, base_mass, wheel_mass")
     a = ap.parse_args()
     import wheeledlab_b200 as wl
     from wheeledlab_b200.learner import FusedOnPolicyRunner
@@ -47,12 +49,16 @@ def main():
     torch.manual_seed(a.seed)
     task_id, activation, name = TASKS[a.task]
     env = wl.make(task_id, device=dev, num_envs=a.envs, seed=a.seed, env_id_offset=rank * a.envs)
+    events = [e for e in a.reset_events.split(",") if e]
+    if events:
+        env.sim.set_reset_events(**{e: True for e in events})
     agent = agent_cfg(activation, a.steps, a.save_interval)
     runner = FusedOnPolicyRunner(env, agent, log_dir=a.log_dir, device=dev)
     if a.log_dir and rank == 0:
         save_run_config(a.log_dir, task_id, a.envs, a.seed, agent)
     head = (f"# {name} PPO (obs_dim {env.sim.obs_dim}, {activation}), {a.envs} envs x {a.steps} steps" + (f" x {world} ranks" if world > 1 else "")
-            + f", rsl_rl agent cfg, seed {a.seed}, one graph per iteration, {torch.cuda.get_device_name(dev)}")
+            + f", rsl_rl agent cfg, seed {a.seed}" + (f", reset-mode DR: {', '.join(events)}" if events else "")
+            + f", one graph per iteration, {torch.cuda.get_device_name(dev)}")
     if a.resume:
         runner.load(a.resume)
         env.common_step_counter = runner.current_learning_iteration * a.steps     # continue the curriculum where it was

@@ -30,6 +30,7 @@ _OBS_ELEV = ["goal_relative_xyz", "root_euler_xyz", "base_lin_vel", "base_ang_ve
 _OBS_VIS_TAIL = ["base_lin_vel", "base_ang_vel", "last_action"]
 _CAMERA_FUNCS = {"camera_data_rgb_flattened_aug": "aug", "camera_data_rgb_flattened": "raw"}
 _BOUND = {None: T.BOUND_NONE, "clip": T.BOUND_CLIP, "tanh": T.BOUND_TANH}
+_RESET_EVENTS = ("material", "actuator_gains", "base_mass", "wheel_mass")     # the WL_RESET_EV_* bits, in bit order
 
 
 def _fields(obj):
@@ -200,11 +201,31 @@ def _lower_rewards(cfg, spec, table, handlers, allow_python_terms=False, device_
     T.set_curriculum(c, names, spec.curriculum)     # reward slots are known now
 
 
-def _lower_material_and_mass_events(events, c, seed):
-    """Startup DR events shared by the tasks (randomize_rigid_body_material / _mass, randomize_actuator_gains)."""
+def _event_mode(name, term) -> bool:
+    """Whether a DR event term is in IsaacLab's reset mode (True) or start-up mode (False); anything else is refused by name."""
+    mode = getattr(term, "mode", "startup")
+    if mode not in ("startup", "reset"):
+        raise NotImplementedError(f"event term {name}: mode {mode!r} (the DR events are implemented in 'startup' and 'reset' mode)")
+    if int(getattr(term, "min_step_count_between_reset", 0) or 0) != 0:
+        raise NotImplementedError(f"event term {name}: min_step_count_between_reset "
+                                  f"{term.min_step_count_between_reset} (only the default 0 is implemented)")
+    return mode == "reset"
+
+
+def _lower_material_and_mass_events(events, spec, seed):
+    """DR events shared by the tasks (randomize_rigid_body_material / _mass, randomize_actuator_gains): their ranges into the
+    config; those in mode="reset" into ``spec.reset_events`` (redrawn at every reset, wl_set_reset_events)."""
+    c = spec.cfg
     wheel_mass = None
+    reset = []
     for name, term in events.items():
         fn, p = _fname(term), (term.params or {})
+        if fn not in ("randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
+            continue
+        if _event_mode(name, term):
+            bodies = getattr(p.get("asset_cfg"), "body_names", None)
+            reset.append({"randomize_rigid_body_material": "material", "randomize_actuator_gains": "actuator_gains"}.get(
+                fn, "wheel_mass" if bodies is not None and "wheel" in str(bodies) else "base_mass"))
         if fn == "randomize_rigid_body_material":
             c.dr_num_buckets = int(p["num_buckets"])
             D, Cs = T.material_buckets(c.dr_num_buckets, p["static_friction_range"], p["dynamic_friction_range"],
@@ -226,6 +247,7 @@ def _lower_material_and_mass_events(events, c, seed):
     c.dr_wheel_mass_enable = 1 if wheel_mass is not None else 0
     if wheel_mass is not None:
         c.dr_wheel_mass[0], c.dr_wheel_mass[1] = wheel_mass
+    spec.reset_events = [e for e in _RESET_EVENTS if e in reset]
 
 
 def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: bool = False, device_terms: bool = False) -> T.TaskSpec:
@@ -308,7 +330,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
                 pass                                            # no-op without omni.isaac.sensor (quirk Q15)
             else:
                 raise NotImplementedError(f"event term {name} -> {fn}")
-        _lower_material_and_mass_events(events, c, seed)
+        _lower_material_and_mass_events(events, spec, seed)
         return spec
     # elevation (elevation/mushr_elevation_env_cfg.py)
     spec = T.elevation_task(num_envs=num_envs, seed=seed, env_id_offset=env_id_offset)
@@ -350,7 +372,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
                 c.elev_reset_vel[0], c.elev_reset_vel[1] = vr["x"]
         elif fn not in ("randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
             raise NotImplementedError(f"event term {name} -> {fn}")
-    _lower_material_and_mass_events(events, c, seed)
+    _lower_material_and_mass_events(events, spec, seed)
     cmds = dict(_fields(getattr(cfg, "commands", None)))
     for name, term in cmds.items():
         rng = getattr(term, "ranges", None)
@@ -418,7 +440,7 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device
         if fn not in ("reset_root_state", "randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
             raise NotImplementedError(f"event term {name} -> {fn}")
     if randomize:
-        _lower_material_and_mass_events(events, c, seed)
+        _lower_material_and_mass_events(events, spec, seed)
     else:                                                      # material table follows the (possibly overridden) ground friction
         D, Cs = T.material_buckets(1, (1.0, 1.0), (1.0, 1.0), True, c.ground_mu_s, c.ground_mu_d, seed)
         c.dr_bucket_D[0], c.dr_bucket_C[0] = D[0], Cs[0]

@@ -47,6 +47,7 @@ struct wl_sim {
     int step_threads;       // (threads per CTA)
     struct DevTerms* dterms;   // wl_set_device_terms: the term table and its per-env state (null: none)
     CriticTable critic;        // wl_set_critic_terms: the critic observation's columns (n_cols = 0: none)
+    uint32_t reset_ev;         // wl_set_reset_events: WL_RESET_EV_* bits of the events redrawn at every reset (0: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1375,6 +1376,9 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
     }
 }
 
+// (wl_reset_dr.cuh restates the DR draw below for its own kernel: this kernel is left as it is, machine code included)
+#include "wl_reset_dr.cuh"
+
 __global__ void wl_startup_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st) {
     const int n = c.num_envs;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2106,6 +2110,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     s->duo_kernel = nullptr;
     s->duo_threads = 64;
     s->step_variant = s->step_specialised = s->step_threads = 0;
+    s->reset_ev = 0;
     if (cfg->task == WL_TASK_ELEVATION) {
         typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -2193,6 +2198,14 @@ static int post_step(wl_sim* sim, int64_t step_counter, cudaStream_t cs) {
     wl_boundary_kernel<<<1, 32, 0, cs>>>(sim->cfg, sim->globals, (uint32_t)t_next);
     return launched(sim, "wl_boundary_kernel");
 }
+// after a call that reset envs: the reset-mode DR events of the handle (DESIGN 6n).  after_step: the envs the step just
+// reset, found by the kernel (n_ids = num_envs, ids = null); otherwise wl_reset's ids.  Mask 0: nothing is launched.
+static int reset_dr(wl_sim* sim, const int64_t* ids, int n_ids, int64_t step_counter, bool after_step, cudaStream_t cs) {
+    if (!sim->reset_ev) return WL_OK;
+    wl_reset_dr_kernel<<<(n_ids + WL_RESET_DR_BS - 1) / WL_RESET_DR_BS, WL_RESET_DR_BS, 0, cs>>>(
+        sim->cfg, sim->state, sim->globals, ids, n_ids, (uint32_t)step_counter, after_step, sim->reset_ev);
+    return launched(sim, "wl_reset_dr_kernel");
+}
 extern "C" {
 
 int wl_startup(wl_sim* sim, void* stream) {
@@ -2210,7 +2223,8 @@ int wl_reset(wl_sim* sim, const int64_t* d_env_ids, int32_t n_ids, int64_t step_
     if (n <= 0) return WL_OK;
     const int bs = 128;
     wl_reset_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, sim->hf, d_env_ids, n, (uint32_t)step_counter);
-    return launched(sim, "wl_reset_kernel");
+    if (int rc = launched(sim, "wl_reset_kernel")) return rc;
+    return reset_dr(sim, d_env_ids, n, step_counter, false, (cudaStream_t)stream);
 }
 
 int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated,
@@ -2265,6 +2279,7 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     if (int rc = launched(sim, "wl_step_kernel")) return rc;
     if (elev) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
     if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
+    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
     return post_step(sim, step_counter, cs);
 }
 
@@ -2320,6 +2335,7 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
     if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (cudaStream_t)stream)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
+    if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
     return post_step(sim, step_counter, (cudaStream_t)stream);
 }
 
@@ -2406,6 +2422,7 @@ int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew
     if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc;   // t may be device-relative
+    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
     return post_step(sim, step_counter, cs);
 }
 
@@ -2416,6 +2433,7 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
     if (int rc = refuse_fan(sim, "wl_rollout")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_rollout: the elevation step is two kernels (use wl_step)");
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam) return fail(WL_EUNSUPPORTED, "wl_rollout: the camera term is a second kernel (use wl_step)");
+    if (sim->reset_ev) return fail(WL_EUNSUPPORTED, "wl_rollout: the reset-mode DR events are a second kernel after each step (use wl_step)");
     if (sim->cfg.curr_n > 0) {
         if (step_counter < 0) return fail(WL_EINVAL, "wl_rollout: with curriculum terms the host must pass the step counter");
         const int64_t L = sim->cfg.max_episode_length;
@@ -2575,6 +2593,21 @@ int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_term
     return WL_OK;
 }
 int32_t wl_critic_obs_dim(const wl_sim* sim) { return sim ? sim->critic.n_cols : 0; }
+
+int wl_set_reset_events(wl_sim* sim, uint32_t mask) {
+    if (!sim) return fail(WL_EINVAL, "wl_set_reset_events: null handle");
+    const uint32_t all = WL_RESET_EV_MATERIAL | WL_RESET_EV_ACTUATOR_GAINS | WL_RESET_EV_BASE_MASS | WL_RESET_EV_WHEEL_MASS;
+    if (mask & ~all) return fail(WL_EINVAL, "wl_set_reset_events: unknown bit(s) " + std::to_string(mask & ~all));
+    const wl_config& c = sim->cfg;
+    if (mask && !c.dr_enable) return fail(WL_EINVAL, "wl_set_reset_events: the config has no DR events (dr_enable = 0)");
+    if ((mask & WL_RESET_EV_ACTUATOR_GAINS) && c.dr_kd_mask == 0)
+        return fail(WL_EINVAL, "wl_set_reset_events: the config has no randomize_actuator_gains event (dr_kd_mask = 0)");
+    if ((mask & WL_RESET_EV_WHEEL_MASS) && !c.dr_wheel_mass_enable)
+        return fail(WL_EINVAL, "wl_set_reset_events: the config has no wheel-mass event (dr_wheel_mass_enable = 0)");
+    sim->reset_ev = mask;
+    return WL_OK;
+}
+uint32_t wl_reset_events(const wl_sim* sim) { return sim ? sim->reset_ev : 0u; }
 int wl_critic_observe(wl_sim* sim, float* d_critic_obs, void* stream) {
     if (!sim || !d_critic_obs) return fail(WL_EINVAL, "wl_critic_observe: null argument");
     if ((uintptr_t)d_critic_obs & 3u) return fail(WL_EINVAL, "wl_critic_observe: d_critic_obs must be 4-byte aligned");
@@ -2616,6 +2649,7 @@ static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float*
                  d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
     });
     if (int rc = launched(sim, infer ? "wl_act_step_quad_kernel<infer>" : "wl_act_step_quad_kernel")) return rc;
+    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
     return post_step(sim, step_counter, cs);
 }
 

@@ -326,6 +326,8 @@ class ManagerBasedRLEnv:
                 self.add_device_reward_term(name, func, weight, params)
             else:
                 self.add_device_termination_term(name, func, role == "time_out", params)
+        if self.spec.reset_events:
+            self.sim.set_reset_events(**{name: True for name in self.spec.reset_events})
         if self.spec.critic_terms:
             self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
         # event_manager.apply(mode="startup")

@@ -318,6 +318,22 @@ class WheeledSim:
         check(lib.wl_set_critic_terms(self._h, arr, len(pairs)), "wl_set_critic_terms")
         return self.critic_obs_dim
 
+    def set_reset_events(self, material: bool = False, actuator_gains: bool = False, base_mass: bool = False,
+                         wheel_mass: bool = False) -> int:
+        """IsaacLab's mode="reset" for the start-up DR events (wl_set_reset_events): each event switched on here is drawn
+        again, on the device, for every env a step auto-resets or reset() resets; the others keep their start-up values.  All
+        False restores start-up DR.  Raises WlError, leaving the handle as it was, for an event the config does not have.
+        Nothing is launched; a graph captured earlier keeps the events it was captured with.  Returns the mask."""
+        on = {"material": material, "actuator_gains": actuator_gains, "base_mass": base_mass, "wheel_mass": wheel_mass}
+        mask = sum(bit for name, bit in _lib.WL_RESET_EVENTS.items() if on[name])
+        check(lib.wl_set_reset_events(self._h, mask), "wl_set_reset_events")
+        return mask
+
+    @property
+    def reset_events(self) -> int:
+        """The handle's WL_RESET_EV_* mask (0: every DR event in start-up mode)."""
+        return int(lib.wl_reset_events(self._h))
+
     @property
     def critic_obs_dim(self) -> int:
         return int(lib.wl_critic_obs_dim(self._h))

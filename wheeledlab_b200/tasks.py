@@ -68,6 +68,8 @@ class TaskSpec:
     device_terms: list = field(default_factory=list)
     # the critic observation group (privileged.py, wl_critic_observe): [(name, library term, clip)] in row order; [] = none
     critic_terms: list = field(default_factory=list)
+    # DR events in IsaacLab's mode="reset" (wl_set_reset_events): names of _lib.WL_RESET_EVENTS; [] = start-up DR only
+    reset_events: list = field(default_factory=list)
 
     @property
     def step_dt(self) -> float:
