@@ -501,6 +501,33 @@ int wl_step_stage_a(wl_sim* sim, const float* d_action, float* d_rew, uint8_t* d
 int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_extra_terminated, const uint8_t* d_extra_truncated,
                     float* d_obs, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
 
+/* ---- stage b cut once more, for HOST-SIDE (Python) event terms (IsaacLab EventTermCfg, DESIGN.md 6o) ----------------------
+ * ManagerBasedRLEnv.step runs the reset events inside _reset_idx, then the interval events, then the observation manager.
+ * Stage b1 = sections F and H of wl_step_stage_b with its arguments and checks (episode log, curriculum, auto-reset, the
+ * built-in interval pushes; the janitor, the reset-mode DR kernel and the curriculum boundary): writes d_terminated /
+ * d_truncated and leaves the post-reset, post-push state in the state buffer.  The caller may now write the state (root
+ * pose and velocity, episode_length_buf, ...).  Stage b2 = sections G and I (the Elevation command, the observation and its
+ * noise, the height scan / the Visual camera) formed from the state buffer as it is then, at the counter b1 was given
+ * (WL_EINVAL otherwise).  wl_step_stage_b1 + wl_step_stage_b2 with nothing written between them == wl_step_stage_b, bit for
+ * bit. */
+int wl_step_stage_b1(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_extra_terminated, const uint8_t* d_extra_truncated,
+                     uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream);
+int wl_step_stage_b2(wl_sim* sim, float* d_obs, int64_t step_counter, void* stream);
+/* Interval timers of up to WL_MAX_EVENT_TERMS host-side interval event terms (EventManager, is_global_time=False).
+ * wl_set_event_timers stores the terms' interval_range_s (lo_hi[2k], lo_hi[2k+1]), allocates time_left [n_terms][N] and
+ * draws it: time_left = u * (hi - lo) + lo, u = U[0,1) of the key (seed, env_id_offset + i, 0, stream 14, k).  A set-up call:
+ * it synchronises the device before it returns and is not capturable.  n_terms = 0 frees the table.  WL_EINVAL, leaving
+ * the handle as it was: a null handle, n_terms outside 0..8, a null table with n_terms > 0, a bound that is not finite,
+ * lo < 0 or lo > hi, a peer / multicast fan-out set.
+ * wl_event_timers, once per staged step between b1 and b2, per term k and env i with u_x, u_y from the key
+ * (seed, env_id_offset + i, step_counter, stream 13, k): time_left = u_x * (hi - lo) + lo where d_done[i] != 0 (the envs b1
+ * reset: d_terminated | d_truncated); then time_left -= step_dt; d_fired[k * N + i] = time_left < 1e-6, and where it fired
+ * time_left = u_y * (hi - lo) + lo.  One launch on `stream`.  WL_EINVAL before any launch: a null argument, a counter
+ * outside 0..2^31-1, no table, a fan-out set. */
+#define WL_MAX_EVENT_TERMS 8
+int wl_set_event_timers(wl_sim* sim, int32_t n_terms, const float* lo_hi);
+int wl_event_timers(wl_sim* sim, const uint8_t* d_done, uint8_t* d_fired, int64_t step_counter, void* stream);
+
 /* ---- device terms: the reference's unregistered reward / termination functions, in CUDA (DESIGN.md 6l) -------------------
  * A device term is one function of the library below, evaluated by a kernel between stage a and stage b with exactly the
  * semantics of the same function registered as a Python term (terminations first, then rewards in registration order,

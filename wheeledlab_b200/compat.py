@@ -212,6 +212,40 @@ def _event_mode(name, term) -> bool:
     return mode == "reset"
 
 
+EVENT_MODES = ("startup", "reset", "interval")
+MAX_INTERVAL_EVENTS = 8             # WL_MAX_EVENT_TERMS: the interval timers of one handle
+
+
+def check_event_term(name, mode, interval_range_s=None, is_global_time=False, min_step_count_between_reset=0):
+    """The refusals of a host-side (Python) event term, by name (env.add_event_term and the lowering of a cfg's event term)."""
+    if mode not in EVENT_MODES:
+        raise NotImplementedError(f"event term {name}: mode {mode!r} (Python event terms run in 'startup', 'reset' and 'interval' mode)")
+    if is_global_time:
+        raise NotImplementedError(f"event term {name}: is_global_time=True (the interval timers are per env and restart at reset)")
+    if int(min_step_count_between_reset or 0) != 0:
+        raise NotImplementedError(f"event term {name}: min_step_count_between_reset {min_step_count_between_reset} "
+                                  "(only the default 0 is implemented)")
+    if mode == "interval":
+        if interval_range_s is None:
+            raise ValueError(f"event term {name}: an interval event needs interval_range_s")
+        lo, hi = (float(v) for v in interval_range_s)
+        if not (math.isfinite(lo) and math.isfinite(hi) and 0.0 <= lo <= hi):
+            raise ValueError(f"event term {name}: interval_range_s {tuple(interval_range_s)} must be finite with 0 <= lo <= hi")
+
+
+def _python_event(spec, name, term, fn, allow_python_terms):
+    """An event term whose function the kernels do not lower: a host-side event term of the spec (spec.python_event_terms,
+    in cfg order) with ``allow_python_terms``, else refused by name."""
+    if not allow_python_terms:
+        raise NotImplementedError(f"event term {name} -> {fn}")
+    mode = getattr(term, "mode", "startup")
+    rng = getattr(term, "interval_range_s", None)
+    check_event_term(name, mode, rng, bool(getattr(term, "is_global_time", False)), getattr(term, "min_step_count_between_reset", 0))
+    if mode == "interval" and sum(1 for e in spec.python_event_terms if e[2] == "interval") >= MAX_INTERVAL_EVENTS:
+        raise NotImplementedError(f"event term {name}: more than {MAX_INTERVAL_EVENTS} Python interval event terms")
+    spec.python_event_terms.append((name, term.func, mode, dict(term.params or {}), tuple(float(v) for v in rng) if mode == "interval" else None))
+
+
 def _lower_material_and_mass_events(events, spec, seed):
     """DR events shared by the tasks (randomize_rigid_body_material / _mass, randomize_actuator_gains): their ranges into the
     config; those in mode="reset" into ``spec.reset_events`` (redrawn at every reset, wl_set_reset_events)."""
@@ -257,7 +291,9 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     call the cfg's own function (staged step, env.add_reward_term); otherwise they raise.  With ``device_terms`` such a
     term whose function is in the device-term library (device_terms.REGISTRY) becomes a device term of the spec
     (spec.device_terms, in cfg order, with the cfg's weight and params), matched by module and name before the
-    built-in terms are matched by name."""
+    built-in terms are matched by name.  With ``allow_python_terms`` an event term whose function the kernels do not lower
+    becomes a host-side event term (spec.python_event_terms, registered by the env with add_event_term) in startup, reset or
+    interval mode; the built-in event functions keep their own refusals."""
     num_envs = int(cfg.scene.num_envs)
     seed = int(cfg.seed) if getattr(cfg, "seed", None) is not None else 42
     kind = _task_kind(cfg)
@@ -329,7 +365,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
             elif fn == "disable_all_lidars":
                 pass                                            # no-op without omni.isaac.sensor (quirk Q15)
             else:
-                raise NotImplementedError(f"event term {name} -> {fn}")
+                _python_event(spec, name, term, fn, allow_python_terms)
         _lower_material_and_mass_events(events, spec, seed)
         return spec
     # elevation (elevation/mushr_elevation_env_cfg.py)
@@ -371,7 +407,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
             if "x" in vr:
                 c.elev_reset_vel[0], c.elev_reset_vel[1] = vr["x"]
         elif fn not in ("randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
-            raise NotImplementedError(f"event term {name} -> {fn}")
+            _python_event(spec, name, term, fn, allow_python_terms)
     _lower_material_and_mass_events(events, spec, seed)
     cmds = dict(_fields(getattr(cfg, "commands", None)))
     for name, term in cmds.items():
@@ -438,7 +474,7 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device
     for name, term in events.items():
         fn = _fname(term)
         if fn not in ("reset_root_state", "randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
-            raise NotImplementedError(f"event term {name} -> {fn}")
+            _python_event(spec, name, term, fn, allow_python_terms)
     if randomize:
         _lower_material_and_mass_events(events, spec, seed)
     else:                                                      # material table follows the (possibly overridden) ground friction

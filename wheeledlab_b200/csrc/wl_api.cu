@@ -15,6 +15,7 @@
 using namespace wl;
 
 #include "wl_critic.cuh"
+#include "wl_events.cuh"
 
 // ---------------------------------------------------------------------------------------
 // handle
@@ -48,6 +49,7 @@ struct wl_sim {
     struct DevTerms* dterms;   // wl_set_device_terms: the term table and its per-env state (null: none)
     CriticTable critic;        // wl_set_critic_terms: the critic observation's columns (n_cols = 0: none)
     uint32_t reset_ev;         // wl_set_reset_events: WL_RESET_EV_* bits of the events redrawn at every reset (0: none)
+    EventTable events;         // wl_set_event_timers: the interval terms' ranges and per-env timers (n = 0: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -198,6 +200,9 @@ __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool con
 // STAGE 0: the whole env.step.  STAGE 1 / 2: the same code cut after section E (wl_step_stage_a / wl_step_stage_b), so that
 // host-side (Python) reward and termination terms can run between "rewards" and "reset" exactly where the reference's
 // managers would call them; the state round-trips through HBM losslessly, so 1 + 2 == 0 bit for bit.
+// STAGE 3 / 4: stage 2 cut once more, after the interval pushes (wl_step_stage_b1: F, H) and before the commands and the
+// observation (wl_step_stage_b2: G, I), so that host-side event terms run in between (DESIGN 6o).  Stage 4 reads nothing
+// but the state buffer: whatever the host wrote there in between is what its command and observation are formed from.
 struct StageIO { uint8_t* tmask; const uint8_t* extra_terminated; const uint8_t* extra_truncated; };
 template <int TASK, int STAGE = 0>
 __global__ void __launch_bounds__(128, WL_STEP_MIN_BLOCKS)
@@ -216,9 +221,11 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
     uint32_t tmask = 0u;
     EnvState e;
     float wts[WL_MAX_REW_TERMS];            // W(t): issued with the state loads so the latency hides behind the integrator
-    load_weights(c, gl, t, wts);
-    if (STAGE != 1 && janitor_cta(c, gl, t, d_log, wts)) return;
-    if (STAGE == 2) {
+    if (STAGE != 4) load_weights(c, gl, t, wts);
+    if (STAGE != 1 && STAGE != 4 && janitor_cta(c, gl, t, d_log, wts)) return;
+    if (STAGE == 4) {
+        if (i < n) load_env(st, n, i, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
+    } else if (STAGE == 2 || STAGE == 3) {
         if (i < n) {
             load_env(st, n, i, e, ELEV, c.dr_wheel_mass_enable != 0, c.d_inv_Iw);
             tmask = sio.tmask[i];
@@ -271,10 +278,15 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
     }
     if (STAGE == 1) return;
     // F. auto-reset + per-step episode log (warp-shuffle reduction over the finished envs)
-    log_accumulate(gl->acc[t % 3u], done, tmask, e.sums);
+    if (STAGE != 4) log_accumulate(gl->acc[t % 3u], done, tmask, e.sums);
     if (i < n) {
         const uint32_t gid = (uint32_t)(c.env_id_offset + i);
         if (done) reset_env(c, TASK, vm, e, gid, t);
+        if (STAGE == 3) {                    // cut: H, then the post-reset, post-push state back to HBM for stage 4
+            if (!VIS && !ELEV) interval_pushes(c, e, gid, t, c.d_step_dt);
+            store_env(st, n, i, e, ELEV);
+            return;
+        }
         // G. commands   H. interval events (post-reset state)   I. observations
         if (VIS) {
             float o[8]; visual_proprio(c, e, o);
@@ -288,10 +300,10 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
 #pragma unroll
             for (int k = 0; k < 13; ++k) row[k] = o[k];
         } else {
-            interval_pushes(c, e, gid, t, c.d_step_dt);
+            if (STAGE != 4) interval_pushes(c, e, gid, t, c.d_step_dt);
             blind_obs(c, e, gid, t, RNG_OBS, 0u, obs + (size_t)WL_OBS_DIM_BLIND * i);
         }
-        store_env(st, n, i, e, ELEV);
+        if (STAGE != 4 || ELEV) store_env(st, n, i, e, ELEV);     // (stage 4 changes the command groups only)
     }
 }
 
@@ -1693,6 +1705,10 @@ struct DevTerms {
     uint8_t* tbits;     // [N] stage a's built-in termination bits when the handle records none (wl_set_term_bits)
     void* block;
 };
+static void free_event_timers(wl_sim* sim) {
+    if (sim->events.time_left) cudaFree(sim->events.time_left);
+    sim->events = EventTable{};
+}
 static void free_device_terms(wl_sim* sim) {
     if (!sim->dterms) return;
     cudaFree(sim->dterms->block);
@@ -2142,7 +2158,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     return WL_OK;
 }
 
-int wl_destroy(wl_sim* sim) { if (sim) free_device_terms(sim); delete sim; return WL_OK; }
+int wl_destroy(wl_sim* sim) { if (sim) { free_device_terms(sim); free_event_timers(sim); } delete sim; return WL_OK; }
 int32_t wl_obs_dim(const wl_sim* sim) { return sim ? sim->obs_dim : 0; }
 int wl_set_scan_tma(wl_sim* sim, int32_t use_tma) {
     if (!sim) return fail(WL_EINVAL, "wl_set_scan_tma: null handle");
@@ -2300,12 +2316,15 @@ int wl_duo_trace_arm(void* buf, uint32_t cap) {
 template <int STAGE>
 static int launch_stage(wl_sim* sim, const float2* act, float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated,
                         float* d_log, uint32_t t, StageIO sio, cudaStream_t cs) {
-    const int n = sim->cfg.num_envs, bs = pick_block(n), grid = (n + bs - 1) / bs + (STAGE == 2 ? 1 : 0);   // stage b: + the janitor CTA
+    const bool jan = STAGE == 2 || STAGE == 3;                                // stage b / b1: + the janitor CTA
+    const int n = sim->cfg.num_envs, bs = pick_block(n), grid = (n + bs - 1) / bs + (jan ? 1 : 0);
     Terrain T{sim->hf};
     with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
         wl_step_kernel<task, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
     });
-    return launched(sim, STAGE == 1 ? "wl_step_kernel<stage a>" : "wl_step_kernel<stage b>");
+    static const char* const names[] = {"wl_step_kernel", "wl_step_kernel<stage a>", "wl_step_kernel<stage b>", "wl_step_kernel<stage b1>",
+                                        "wl_step_kernel<stage b2>"};
+    return launched(sim, names[STAGE]);
 }
 extern "C" {
 
@@ -2337,6 +2356,73 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
         if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
     if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
     return post_step(sim, step_counter, (cudaStream_t)stream);
+}
+
+int wl_step_stage_b1(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_extra_terminated, const uint8_t* d_extra_truncated,
+                     uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter, void* stream) {
+    if (!sim || !d_term_bits || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_step_stage_b1: null argument");
+    if (step_counter < 0) return fail(WL_EINVAL, "wl_step_stage_b1: the staged step takes the host's step counter");
+    if (int rc = refuse_fan(sim, "wl_step_stage_b1")) return rc;
+    if (int rc = prep_step(sim, step_counter, 1, (cudaStream_t)stream)) return rc;
+    if (int rc = launch_stage<3>(sim, nullptr, nullptr, nullptr, d_terminated, d_truncated, d_log, (uint32_t)step_counter,
+                                 StageIO{const_cast<uint8_t*>(d_term_bits), d_extra_terminated, d_extra_truncated}, (cudaStream_t)stream))
+        return rc;
+    if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
+    return post_step(sim, step_counter, (cudaStream_t)stream);
+}
+
+int wl_step_stage_b2(wl_sim* sim, float* d_obs, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs) return fail(WL_EINVAL, "wl_step_stage_b2: null argument");
+    if (step_counter < 0 || step_counter != sim->last_t)
+        return fail(WL_EINVAL, "wl_step_stage_b2: step_counter must be that of the wl_step_stage_b1 before it");
+    if (int rc = refuse_fan(sim, "wl_step_stage_b2")) return rc;
+    ensure_device(sim);
+    if (int rc = launch_stage<4>(sim, nullptr, d_obs, nullptr, nullptr, nullptr, nullptr, (uint32_t)step_counter,
+                                 StageIO{nullptr, nullptr, nullptr}, (cudaStream_t)stream))
+        return rc;
+    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (cudaStream_t)stream)) return rc; }
+    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
+        if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
+    return WL_OK;
+}
+
+int wl_set_event_timers(wl_sim* sim, int32_t n_terms, const float* lo_hi) {
+    if (!sim) return fail(WL_EINVAL, "wl_set_event_timers: null handle");
+    if (n_terms < 0 || n_terms > WL_MAX_EVENT_TERMS) return fail(WL_EINVAL, "wl_set_event_timers: n_terms must be 0..8");
+    if (n_terms > 0 && !lo_hi) return fail(WL_EINVAL, "wl_set_event_timers: null range table");
+    if (fan_set(sim)) return fail(WL_EINVAL, "wl_set_event_timers: the peer fan-out is set, and event timers run with the staged step only");
+    EventTable et{};
+    et.n = n_terms;
+    for (int k = 0; k < n_terms; ++k) {
+        const float lo = lo_hi[2 * k], hi = lo_hi[2 * k + 1];
+        if (!std::isfinite(lo) || !std::isfinite(hi) || lo < 0.0f || lo > hi)
+            return fail(WL_EINVAL, "wl_set_event_timers: term " + std::to_string(k) + ": the range must be finite with 0 <= lo <= hi");
+        et.lo[k] = lo; et.hi[k] = hi;
+    }
+    ensure_device(sim);
+    if (n_terms == 0) { free_event_timers(sim); return WL_OK; }
+    const int n = sim->cfg.num_envs;
+    if (int rc = cuda_check(cudaMalloc(&et.time_left, sizeof(float) * (size_t)n_terms * n), "wl_set_event_timers: allocate")) return rc;
+    // drawn and finished before returning, so that a step on any stream afterwards sees the timers
+    wl_event_timers_init_kernel<<<(n + WL_EVENT_BS - 1) / WL_EVENT_BS, WL_EVENT_BS>>>(sim->cfg, et);
+    int rc = launched(sim, "wl_event_timers_init_kernel");
+    if (!rc) rc = cuda_check(cudaDeviceSynchronize(), "wl_set_event_timers: draw");
+    if (rc) { cudaFree(et.time_left); return rc; }
+    free_event_timers(sim);
+    sim->events = et;
+    return WL_OK;
+}
+
+int wl_event_timers(wl_sim* sim, const uint8_t* d_done, uint8_t* d_fired, int64_t step_counter, void* stream) {
+    if (!sim || !d_done || !d_fired) return fail(WL_EINVAL, "wl_event_timers: null argument");
+    if (step_counter < 0 || step_counter >= ((int64_t)1 << 31)) return fail(WL_EINVAL, "wl_event_timers: step_counter out of range (0 <= t < 2^31)");
+    if (sim->events.n < 1) return fail(WL_EINVAL, "wl_event_timers: no event timers (wl_set_event_timers)");
+    if (fan_set(sim)) return fail(WL_EINVAL, "wl_event_timers: the peer fan-out is set, and event timers run with the staged step only");
+    ensure_device(sim);
+    const int n = sim->cfg.num_envs;
+    wl_event_timers_kernel<<<(n + WL_EVENT_BS - 1) / WL_EVENT_BS, WL_EVENT_BS, 0, (cudaStream_t)stream>>>(sim->cfg, sim->events, d_done, d_fired,
+                                                                                                          (uint32_t)step_counter);
+    return launched(sim, "wl_event_timers_kernel");
 }
 
 int wl_set_device_terms(wl_sim* sim, const wl_term_desc* terms, int32_t n_terms) {

@@ -138,7 +138,7 @@ class TerminationManager:
         names = env.spec.termination_names
         for j, (n, is_to) in enumerate(names):
             if n == name:
-                bits = getattr(env, "_term_bits_staged", None) if (env._py_rewards or env._py_terms) else getattr(env, "_term_bits", None)
+                bits = getattr(env, "_term_bits_staged", None) if env._staged else getattr(env, "_term_bits", None)
                 if bits is not None:
                     return ((bits >> j) & 1).to(torch.bool)
                 others = [m for m, to in names if to == is_to]
@@ -306,6 +306,8 @@ class ManagerBasedRLEnv:
         self._host_obs_ring = None
         # host-side (Python) MDP terms: evaluated between the two halves of the staged step (see add_reward_term)
         self._py_rewards, self._py_terms, self._py_obs = [], [], []
+        self._py_events = []                     # host-side event terms (add_event_term): run between stage b1 and stage b2
+        self._event_fired = None                 # [interval terms, N] u8: wl_event_timers' fired bytes
         self._py_sums = {}
         self._dev_terms = []                     # device terms (add_device_reward_term): evaluated by wl_step_terms
         self._term_log_ring = None
@@ -333,6 +335,8 @@ class ManagerBasedRLEnv:
         # event_manager.apply(mode="startup")
         self.sim.startup()
         self._needs_reset = True
+        for name, func, mode, params, interval_range_s in self.spec.python_event_terms:
+            self.add_event_term(name, func, mode, params, interval_range_s)
 
     # -- gym surface ---------------------------------------------------------------------------
     @property
@@ -376,9 +380,12 @@ class ManagerBasedRLEnv:
         """No viewport: the reference renders through Omniverse RTX (video recording only, train_rl.py --video); returns None."""
         return None
 
-    def reset(self, seed=None, options=None):
-        self.sim.reset(None, self.common_step_counter)
-        self._needs_reset = False
+    def reset(self, seed=None, options=None, env_ids=None):
+        """Reset every env (or those of `env_ids`: _reset_idx), then run the reset-mode event terms on them, then observe."""
+        self.sim.reset(env_ids, self.common_step_counter)
+        if env_ids is None:
+            self._needs_reset = False
+        self._reset_events(None if env_ids is None else torch.as_tensor(env_ids, device=self.device).to(torch.int64).reshape(-1))
         obs = self.observation_manager.compute()
         return obs, self.extras
 
@@ -399,7 +406,7 @@ class ManagerBasedRLEnv:
         together with host-side Python terms or device terms."""
         from . import privileged
         terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
-        if terms and (self._py_rewards or self._py_terms or self._py_obs):
+        if terms and (self._py_rewards or self._py_terms or self._py_obs or self._py_events):
             raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
         if terms and self._dev_terms:
             raise NotImplementedError("a critic observation group together with device terms is not implemented")
@@ -459,12 +466,51 @@ class ManagerBasedRLEnv:
         self._py_terms.append(SimpleNamespace(name=name, func=func, time_out=bool(time_out), params=dict(params or {})))
         self.termination_manager.python_terms = [t.name for t in self._py_terms]
 
+    def add_event_term(self, name: str, func, mode: str, params: dict | None = None, interval_range_s=None, is_global_time: bool = False,
+                       min_step_count_between_reset: int = 0):
+        """Register ``func(env, env_ids, **params)`` as an event term (IsaacLab EventTermCfg semantics, DESIGN 6o).
+        ``"startup"``: called once, now (the env has started up), with env_ids None.  ``"reset"``: called with the sorted
+        int64 device tensor of the envs a step auto-reset, when there are any, after the built-in reset events and before the
+        observation; also from ``reset(env_ids)``.  ``"interval"``: per env, a timer drawn from ``interval_range_s`` = (lo, hi)
+        counts down by step_dt; the function is called with the envs whose timer ran out (timers restart at reset), after the
+        built-in pushes, in registration order.  Events write the state through ``scene["robot"].write_root_pose_to_sim`` /
+        ``write_root_velocity_to_sim``, the ``data`` views and ``episode_length_buf``.  The env then steps through the staged
+        step (stage a, b1, events, b2).  Refused by name: "prestartup" and other modes, is_global_time=True,
+        min_step_count_between_reset != 0, more than 8 interval terms."""
+        from .compat import MAX_INTERVAL_EVENTS, check_event_term
+        check_event_term(name, mode, interval_range_s, is_global_time, min_step_count_between_reset)
+        self._refuse_mixing()
+        intervals = [t for t in self._py_events if t.mode == "interval"]
+        if mode == "interval" and len(intervals) >= MAX_INTERVAL_EVENTS:
+            raise NotImplementedError(f"event term {name}: more than {MAX_INTERVAL_EVENTS} Python interval event terms")
+        term = SimpleNamespace(name=name, func=func, mode=mode, params=dict(params or {}),
+                               interval_range_s=None if mode != "interval" else tuple(float(v) for v in interval_range_s))
+        if mode == "startup":
+            func(self, None, **term.params)
+        elif mode == "interval":
+            self.sim.set_event_timers([t.interval_range_s for t in intervals + [term]])
+            self._event_fired = torch.zeros((len(intervals) + 1, self.num_envs), dtype=torch.uint8, device=self.device)
+        self._py_events.append(term)
+
+    def _reset_events(self, env_ids: torch.Tensor | None):
+        """The reset-mode event terms on `env_ids` (None: every env), in registration order."""
+        terms = [t for t in self._py_events if t.mode == "reset"]
+        if terms and env_ids is None:
+            env_ids = torch.arange(self.num_envs, dtype=torch.int64, device=self.device)
+        for term in terms:
+            term.func(self, env_ids, **term.params)
+
+    @property
+    def _staged(self) -> bool:
+        """Whether env.step runs the staged step: host-side reward, termination or event terms."""
+        return bool(self._py_rewards or self._py_terms or self._py_events)
+
     # -- device terms: the reference's unregistered reward / termination functions, in CUDA (device_terms.py) ---------------
     def _refuse_mixing(self, device: bool = False):
         if getattr(self, "_critic_terms", None):
             raise NotImplementedError("a critic observation group together with " + ("device terms" if device else "host-side Python terms")
                                       + " is not implemented")
-        if (self._py_rewards or self._py_terms) if device else self._dev_terms:
+        if (self._py_rewards or self._py_terms or getattr(self, "_py_events", None)) if device else self._dev_terms:
             raise NotImplementedError("an env runs either device terms or host-side Python reward / termination terms, not both")
 
     def _add_device_term(self, name, func, role, weight, params):
@@ -533,7 +579,8 @@ class ManagerBasedRLEnv:
     def staged_step(self, action: torch.Tensor, rew: torch.Tensor | None = None, term_bits: torch.Tensor | None = None, out=None,
                     log: torch.Tensor | None = None):
         """One staged step at ``common_step_counter`` -- stage a, the Python termination terms, then the Python reward terms
-        (func * weight * step_dt, weight 0 skipped, per-episode sums kept), stage b -- into the caller's buffers where given:
+        (func * weight * step_dt, weight 0 skipped, per-episode sums kept), stage b (with event terms: stage b1, the reset
+        events, the interval timers and events, stage b2) -- into the caller's buffers where given:
         rew [N] f32, term_bits [N] u8, out = (obs [N, obs_dim] f32, terminated [N] u8, truncated [N] u8), log f32[16] (the
         episode-log row, written by the next launch on the handle).  Advances ``common_step_counter`` by one and sets the
         termination manager's masks.  Returns (obs, rew, terminated, truncated, extra): `extra` holds the Python terms'
@@ -564,7 +611,10 @@ class ManagerBasedRLEnv:
             val = term.func(self, **term.params).to(torch.float32) * (term.weight * self.step_dt)
             rew += val
             self._py_sums[term.name] += val
-        obs, term_u8, trunc_u8 = sim.step_stage_b(bits, t, extra_term, extra_to, out=out, log=log)
+        if self._py_events:
+            obs, term_u8, trunc_u8 = self._events_stage_b(bits, t, extra_term, extra_to, out, log)
+        else:
+            obs, term_u8, trunc_u8 = sim.step_stage_b(bits, t, extra_term, extra_to, out=out, log=log)
         self.common_step_counter = t + 1
         terminated, truncated = term_u8.view(torch.bool), trunc_u8.view(torch.bool)
         tm.terminated, tm.time_outs = terminated, truncated
@@ -581,6 +631,26 @@ class ManagerBasedRLEnv:
                 extra["Episode_Termination/" + term.name] = (fired[term.name] & done).sum()
         return obs, rew, terminated, truncated, extra
 
+    def _events_stage_b(self, bits, t, extra_term, extra_to, out, log):
+        """Stage b with the event terms: b1 (log, auto-reset, built-in pushes), the reset events on the envs it reset, the
+        interval timers and the interval events on the envs each one fired for, then b2 (commands, observation)."""
+        sim, tm = self.sim, self.termination_manager
+        obs_out, b1_out = (None, None) if out is None else (out[0], out[1:])
+        term_u8, trunc_u8 = sim.step_stage_b1(bits, t, extra_term, extra_to, out=b1_out, log=log)
+        tm.terminated, tm.time_outs = term_u8.view(torch.bool), trunc_u8.view(torch.bool)
+        done = term_u8 | trunc_u8
+        if any(e.mode == "reset" for e in self._py_events):
+            ids = done.nonzero().squeeze(1)
+            if ids.numel():
+                self._reset_events(ids)
+        if self._event_fired is not None:
+            fired = sim.event_timers(done, t, self._event_fired)
+            for k, term in enumerate(e for e in self._py_events if e.mode == "interval"):
+                ids = fired[k].nonzero().squeeze(1)
+                if ids.numel():
+                    term.func(self, ids, **term.params)
+        return sim.step_stage_b2(t, out=obs_out), term_u8, trunc_u8
+
     @property
     def python_log_names(self) -> list:
         """The extras["log"] keys of the Python reward and termination terms, in the order staged_step's `extra` has them."""
@@ -591,7 +661,7 @@ class ManagerBasedRLEnv:
             self.reset()
         if action.dtype != torch.float32 or not action.is_contiguous() or str(action.device) != self.device:
             action = action.to(self.device, torch.float32).contiguous()
-        if self._py_rewards or self._py_terms:
+        if self._staged:
             return self._step_staged(action)
         t = self.common_step_counter
         # outputs live in a ring of preallocated buffers (no allocator call per step; a returned tensor stays valid for
@@ -635,7 +705,7 @@ class ManagerBasedRLEnv:
         result views are overwritten by the next step_host call.  With ``env.host_obs = True`` the observations are returned in
         pinned HOST memory as well (a ring of _RING buffers): D2H copy after the step (transport "copy") or written by the
         kernel over PCIe (transport "zero_copy")."""
-        if self._py_rewards or self._py_terms or self._dev_terms:
+        if self._py_rewards or self._py_terms or getattr(self, "_py_events", None) or self._dev_terms:
             raise NotImplementedError("step_host: Python and device terms need the staged step (use env.step)")
         if self._needs_reset:
             self.reset()

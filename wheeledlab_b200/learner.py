@@ -743,8 +743,8 @@ class FusedOnPolicyRunner:
     is one).  Each iteration is ONE CUDA graph -- rollout, ``wl_episode_stats``, bootstrap value, GAE, PPO update -- plus
     the flush of the last episode-log row, and ONE read-back of what is logged.
 
-    An env with host-side Python reward or termination terms (``add_reward_term`` / ``add_termination_term``) trains on one
-    GPU through ``StagedPPOIteration``: the rollout runs eagerly, T x (policy, staged step with the terms in between), and
+    An env with host-side Python reward, termination or event terms (``add_reward_term`` / ``add_termination_term`` /
+    ``add_event_term``) trains on one GPU through ``StagedPPOIteration``: the rollout runs eagerly, T x (policy, staged step with the terms in between), and
     the rest of the iteration is the same graph; the log gains ``Episode_Reward/<name>`` / ``Episode_Termination/<name>``
     for each Python term, the T-step mean of what env.step's ``extras["log"]`` holds for it.  Python observation terms and
     data-parallel runs with Python terms raise ``NotImplementedError``.  An env with device terms (``add_device_reward_term``)
@@ -792,7 +792,7 @@ class FusedOnPolicyRunner:
         if getattr(e, "_py_obs", None):
             raise NotImplementedError("Python observation terms (add_observation_term) widen the observation past the slab row the "
                                       "staged step writes: an env with host-side Python terms trains with reward and termination terms only")
-        self.staged = bool(getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None))
+        self.staged = bool(getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None) or getattr(e, "_py_events", None))
         self.dev_names = e.device_log_names if getattr(e, "_dev_terms", None) else []
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):

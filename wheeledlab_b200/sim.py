@@ -269,6 +269,45 @@ class WheeledSim:
               "wl_step_stage_b")
         return obs, term, trunc
 
+    def step_stage_b1(self, term_bits: torch.Tensor, step_counter: int, extra_terminated: torch.Tensor | None = None,
+                      extra_truncated: torch.Tensor | None = None, out=None, log: torch.Tensor | None = None):
+        """Sections F and H (wl_step_stage_b1): episode log, auto-reset of done envs (built-in bits | extras), the built-in
+        interval pushes; the post-reset state is left in the buffer for host-side event terms.  Returns (terminated u8,
+        truncated u8)."""
+        n, dev = self.num_envs, self.device
+        if out is None:
+            out = (torch.empty(n, dtype=torch.uint8, device=dev), torch.empty(n, dtype=torch.uint8, device=dev))
+        term, trunc = out
+        u8 = lambda x: None if x is None else C.c_void_p((x.view(torch.uint8) if x.dtype == torch.bool else x).data_ptr())
+        check(lib.wl_step_stage_b1(self._h, C.c_void_p(term_bits.data_ptr()), u8(extra_terminated), u8(extra_truncated),
+                                   C.c_void_p(term.data_ptr()), C.c_void_p(trunc.data_ptr()),
+                                   C.c_void_p(log.data_ptr()) if log is not None else None, step_counter, _stream_ptr(dev)),
+              "wl_step_stage_b1")
+        return term, trunc
+
+    def step_stage_b2(self, step_counter: int, out: torch.Tensor | None = None) -> torch.Tensor:
+        """Sections G and I (wl_step_stage_b2): commands and the observation of the state as it is now, at the counter the
+        preceding step_stage_b1 was given."""
+        obs = out if out is not None else torch.empty((self.num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
+        check(lib.wl_step_stage_b2(self._h, C.c_void_p(obs.data_ptr()), step_counter, _stream_ptr(self.device)), "wl_step_stage_b2")
+        return obs
+
+    def set_event_timers(self, ranges):
+        """The interval timers of host-side interval event terms (wl_set_event_timers): a list of (lo, hi) interval_range_s,
+        at most 8; each env's timers are drawn now.  [] frees them."""
+        n = len(ranges)
+        arr = (C.c_float * max(2, 2 * n))(*[float(v) for r in ranges for v in r])
+        with torch.cuda.device(self.device):
+            check(lib.wl_set_event_timers(self._h, n, arr), "wl_set_event_timers")
+
+    def event_timers(self, done: torch.Tensor, step_counter: int, fired: torch.Tensor) -> torch.Tensor:
+        """One step of the interval timers (wl_event_timers): redraw where `done` [N] (u8 / bool), count down, fire.
+        Writes fired [n_terms, N] u8 (1: the term fires for the env in this step) and returns it."""
+        d = done.view(torch.uint8) if done.dtype == torch.bool else done
+        check(lib.wl_event_timers(self._h, C.c_void_p(d.data_ptr()), C.c_void_p(fired.data_ptr()), step_counter,
+                                  _stream_ptr(self.device)), "wl_event_timers")
+        return fired
+
     def set_device_terms(self, terms):
         """The handle's device terms (wl_set_device_terms): a list of (kind, role, weight, params[<= 4]) in evaluation
         order; [] clears them.  Resets their per-env state (episode sums, elevation_continuity's previous elevation)."""

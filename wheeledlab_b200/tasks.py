@@ -64,6 +64,7 @@ class TaskSpec:
     # host-side (Python) MDP terms evaluated between the two halves of the staged step (env.add_*_term):
     python_reward_terms: list = field(default_factory=list)     # [(name, func, weight, params)]
     python_termination_terms: list = field(default_factory=list)  # [(name, func, time_out, params)]
+    python_event_terms: list = field(default_factory=list)      # [(name, func, mode, params, interval_range_s or None)]
     # device terms (device_terms.py), evaluated by wl_step_terms: [(name, func, "reward" | "termination" | "time_out", weight, params)]
     device_terms: list = field(default_factory=list)
     # the critic observation group (privileged.py, wl_critic_observe): [(name, library term, clip)] in row order; [] = none
