@@ -575,7 +575,8 @@ int wl_set_device_terms(wl_sim* sim, const wl_term_desc* terms, int32_t n_terms)
  * as wl_step, plus d_term_log: NULL or float[WL_MAX_DEVICE_TERMS] on the device receiving, per term in table order,
  * Episode_Reward/<name> (the mean episode sum over the envs done in this step / max_episode_length_s) or
  * Episode_Termination/<name> (the number of done envs where it fired), then zeros; written by this call, fixed-order
- * sums.  With no terms the call is wl_step itself and d_term_log is not written.
+ * sums.  With device event terms (wl_set_device_events) stage b runs cut: stage b1, the reset-mode DR kernel, the device
+ * events, stage b2.  With neither terms nor events the call is wl_step itself and d_term_log is not written.
  * step_counter is a host counter or WL_DEVICE_COUNTER_PLUS(k), so K calls and wl_advance_counter(K) form a replayable
  * graph.  WL_EINVAL for a null argument or a misaligned action /
  * obs, WL_EUNSUPPORTED while a peer / multicast fan-out is set, before any device work. */
@@ -583,6 +584,36 @@ int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew
                   float* d_log, float* d_term_log, int64_t step_counter, void* stream);
 /* Device pointer to uint8[N]: bit k = device term k fired in the most recent wl_step_terms (NULL without terms). */
 uint8_t* wl_device_term_masks(const wl_sim* sim);
+
+/* ---- device event terms: IsaacLab's push_by_setting_velocity in CUDA (DESIGN.md 6p) --------------------------------------
+ * Per term k, for the envs it fires for, each world-frame root velocity component c (0..5: x, y, z, roll, pitch, yaw) gains
+ * u * (hi_c - lo_c) + lo_c (fp32, no fma), u = U[0,1) of the key (seed, env_id_offset + i, step, stream 15, k) for c = 0..3
+ * (.x .. .w) and (seed, env_id_offset + i, step, stream 15, 8 + k) for c = 4, 5 (.x, .y); terms apply in table order.  A
+ * reset-mode term fires for the envs the step reset (terminated | truncated); an interval-mode term for the envs whose
+ * timer ran out, the timer of wl_event_timers (redraw at reset, count down by step_dt, fire below 1e-6, redraw) on a slot
+ * of its own: the j-th interval term of the table uses timer index j in the keys of streams 13 and 14.  Every task
+ * integrates all six components (chassis_integrate: 3-D velocity and body rates on the plane and on the height-field), so
+ * no component needs a zero range. */
+#define WL_MAX_DEVICE_EVENTS 8
+#define WL_EVENT_MODE_RESET    1
+#define WL_EVENT_MODE_INTERVAL 2
+typedef struct wl_device_event_desc {
+    int32_t mode;                 /* WL_EVENT_MODE_* */
+    float interval_range_s[2];    /* (lo, hi) of an interval term: finite, 0 <= lo <= hi; ignored in reset mode */
+    float velocity_range[6][2];   /* (lo, hi) per component x, y, z, roll, pitch, yaw: finite, lo <= hi */
+} wl_device_event_desc;
+/* Store the handle's device event terms and draw the interval terms' timers (key (seed, env_id_offset + i, 0, stream 14,
+ * j)).  n = 0 clears the table.  A set-up call: it allocates, draws and synchronises the device before it returns, and it
+ * is not capturable; a failure leaves the handle as it was.  Refused before any device work: WL_EINVAL for a null handle,
+ * n outside 0..8, a null table with n > 0, an unknown mode, a bound that is not finite, lo > hi, a negative interval bound,
+ * a peer / multicast fan-out set.  With a table, wl_step_terms applies the terms each step (stage a, the device terms,
+ * stage b1, the reset-mode DR kernel, wl_device_events, stage b2), and wl_step, wl_act_step, wl_act_infer_step, wl_rollout
+ * and the staged step refuse the handle (WL_EUNSUPPORTED): they would step it without the events. */
+int wl_set_device_events(wl_sim* sim, const wl_device_event_desc* table, int32_t n_terms);
+/* The device event terms of one step on the handle's state, after stage b1 wrote d_terminated / d_truncated: one launch
+ * on `stream`, capturable.  step_counter: the counter b1 was given (host value 0..2^31-1 or WL_DEVICE_COUNTER_PLUS(k)).
+ * WL_EINVAL before any launch: a null argument, a counter out of range, no table, a fan-out set. */
+int wl_device_events(wl_sim* sim, const uint8_t* d_terminated, const uint8_t* d_truncated, int64_t step_counter, void* stream);
 
 /* ---- the step before env.step(): the policy (SURVEY 8f-1) ---------------------------------------------------------
  * alg.act(obs) of the rollout loop (modified_rsl_rl_runner.py:72; rsl_rl ActorCritic with the reference's sizes,

@@ -246,6 +246,24 @@ def _python_event(spec, name, term, fn, allow_python_terms):
     spec.python_event_terms.append((name, term.func, mode, dict(term.params or {}), tuple(float(v) for v in rng) if mode == "interval" else None))
 
 
+def _device_event(spec, name, term, device_terms) -> bool:
+    """With ``device_terms``, an event term whose function is in the device event library (device_events.REGISTRY) becomes
+    a device event term of the spec (spec.device_events, in cfg order), after check_event_term's refusals and the
+    library's own; returns whether it did."""
+    from . import device_events as dev
+    if not device_terms or dev.lookup(term.func) is None:
+        return False
+    mode = getattr(term, "mode", "startup")
+    rng = getattr(term, "interval_range_s", None)
+    check_event_term(name, mode, rng, bool(getattr(term, "is_global_time", False)), getattr(term, "min_step_count_between_reset", 0))
+    dev.check_mode(name, mode)
+    if len(spec.device_events) >= dev.MAX_TERMS:
+        raise NotImplementedError(f"event term {name}: more than {dev.MAX_TERMS} device event terms")
+    dev.velocity_ranges(name, term.params)
+    spec.device_events.append((name, term.func, mode, dict(term.params or {}), tuple(float(v) for v in rng) if mode == "interval" else None))
+    return True
+
+
 def _lower_material_and_mass_events(events, spec, seed):
     """DR events shared by the tasks (randomize_rigid_body_material / _mass, randomize_actuator_gains): their ranges into the
     config; those in mode="reset" into ``spec.reset_events`` (redrawn at every reset, wl_set_reset_events)."""
@@ -293,7 +311,9 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     (spec.device_terms, in cfg order, with the cfg's weight and params), matched by module and name before the
     built-in terms are matched by name.  With ``allow_python_terms`` an event term whose function the kernels do not lower
     becomes a host-side event term (spec.python_event_terms, registered by the env with add_event_term) in startup, reset or
-    interval mode; the built-in event functions keep their own refusals."""
+    interval mode; the built-in event functions keep their own refusals.  With ``device_terms`` an Elevation or Visual event
+    term whose function is in the device event library (IsaacLab's push_by_setting_velocity) becomes a device event term
+    (spec.device_events, applied by wl_step_terms); the Drift family keeps lowering it onto its two built-in push slots."""
     num_envs = int(cfg.scene.num_envs)
     seed = int(cfg.seed) if getattr(cfg, "seed", None) is not None else 42
     kind = _task_kind(cfg)
@@ -406,7 +426,8 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
             c.elev_reset_yaw = float(pr["yaw"][1])
             if "x" in vr:
                 c.elev_reset_vel[0], c.elev_reset_vel[1] = vr["x"]
-        elif fn not in ("randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
+        elif fn not in ("randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass") and \
+                not _device_event(spec, name, term, device_terms):
             _python_event(spec, name, term, fn, allow_python_terms)
     _lower_material_and_mass_events(events, spec, seed)
     cmds = dict(_fields(getattr(cfg, "commands", None)))
@@ -473,7 +494,8 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device
         c.term_enable = mask
     for name, term in events.items():
         fn = _fname(term)
-        if fn not in ("reset_root_state", "randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass"):
+        if fn not in ("reset_root_state", "randomize_rigid_body_material", "randomize_actuator_gains", "randomize_rigid_body_mass") and \
+                not _device_event(spec, name, term, device_terms):
             _python_event(spec, name, term, fn, allow_python_terms)
     if randomize:
         _lower_material_and_mass_events(events, spec, seed)

@@ -50,6 +50,7 @@ struct wl_sim {
     CriticTable critic;        // wl_set_critic_terms: the critic observation's columns (n_cols = 0: none)
     uint32_t reset_ev;         // wl_set_reset_events: WL_RESET_EV_* bits of the events redrawn at every reset (0: none)
     EventTable events;         // wl_set_event_timers: the interval terms' ranges and per-env timers (n = 0: none)
+    struct DevEvents* devents; // wl_set_device_events: the device event terms and their timers (null: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1697,6 +1698,7 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 #include "wl_actor.cuh"
 #include "wl_episode.cuh"
 #include "wl_terms.cuh"
+#include "wl_dev_events.cuh"
 
 // the handle's device terms: the kernel's table and one device allocation holding the per-env state
 struct DevTerms {
@@ -1714,6 +1716,23 @@ static void free_device_terms(wl_sim* sim) {
     cudaFree(sim->dterms->block);
     delete sim->dterms;
     sim->dterms = nullptr;
+}
+// the handle's device event terms: the kernel's table (its timers point into `block`) and stage a's term bits
+struct DevEvents {
+    DevEventTable et;
+    uint8_t* tbits;     // [N] stage a's built-in termination bits when the handle records none (wl_set_term_bits)
+    void* block;
+};
+static void free_device_events(wl_sim* sim) {
+    if (!sim->devents) return;
+    cudaFree(sim->devents->block);
+    delete sim->devents;
+    sim->devents = nullptr;
+}
+// a call that steps the handle without its device event terms refuses it, before any device work
+static int refuse_devents(const wl_sim* sim, const char* fn) {
+    if (!sim->devents) return WL_OK;
+    return fail(WL_EUNSUPPORTED, std::string(fn) + ": the handle has device event terms, which wl_step_terms applies (wl_set_device_events(0) first)");
 }
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
@@ -2158,7 +2177,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     return WL_OK;
 }
 
-int wl_destroy(wl_sim* sim) { if (sim) { free_device_terms(sim); free_event_timers(sim); } delete sim; return WL_OK; }
+int wl_destroy(wl_sim* sim) { if (sim) { free_device_terms(sim); free_event_timers(sim); free_device_events(sim); } delete sim; return WL_OK; }
 int32_t wl_obs_dim(const wl_sim* sim) { return sim ? sim->obs_dim : 0; }
 int wl_set_scan_tma(wl_sim* sim, int32_t use_tma) {
     if (!sim) return fail(WL_EINVAL, "wl_set_scan_tma: null handle");
@@ -2247,6 +2266,7 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
             float* d_log, int64_t step_counter, void* stream) {
     if (!sim || !d_action || !d_obs || !d_rew || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_step: null argument");
     if (((uintptr_t)d_action & 7u) || ((uintptr_t)d_obs & 7u)) return fail(WL_EINVAL, "wl_step: action/obs must be 8-byte aligned");
+    if (int rc = refuse_devents(sim, "wl_step")) return rc;
     const int n = sim->cfg.num_envs;
     Terrain T{sim->hf};
     // 8 = quad + aux warp (Drift family, small N: shortest dependent chain), 4 = quad, 1 = thread per env
@@ -2333,6 +2353,7 @@ int wl_step_stage_a(wl_sim* sim, const float* d_action, float* d_rew, uint8_t* d
     if ((uintptr_t)d_action & 7u) return fail(WL_EINVAL, "wl_step_stage_a: action must be 8-byte aligned");
     if (step_counter < 0) return fail(WL_EINVAL, "wl_step_stage_a: the staged step takes the host's step counter");
     if (int rc = refuse_fan(sim, "wl_step_stage_a")) return rc;
+    if (int rc = refuse_devents(sim, "wl_step_stage_a")) return rc;
     {   // stage a reads W(t) like a full step: re-arm on a counter jump, but the step is only committed by stage b
         const int64_t keep = sim->last_t;
         if (int rc = prep_step(sim, step_counter, 1, (cudaStream_t)stream)) return rc;
@@ -2425,6 +2446,76 @@ int wl_event_timers(wl_sim* sim, const uint8_t* d_done, uint8_t* d_fired, int64_
     return launched(sim, "wl_event_timers_kernel");
 }
 
+}   // extern "C"
+static int launch_device_events(wl_sim* sim, const uint8_t* d_terminated, const uint8_t* d_truncated, uint32_t t, cudaStream_t cs) {
+    const int n = sim->cfg.num_envs;
+    wl_device_events_kernel<<<(n + WL_DEVICE_EVENTS_BS - 1) / WL_DEVICE_EVENTS_BS, WL_DEVICE_EVENTS_BS, 0, cs>>>(
+        sim->cfg, sim->devents->et, sim->state, sim->globals, d_terminated, d_truncated, t);
+    return launched(sim, "wl_device_events_kernel");
+}
+extern "C" {
+
+int wl_set_device_events(wl_sim* sim, const wl_device_event_desc* table, int32_t n_terms) {
+    if (!sim) return fail(WL_EINVAL, "wl_set_device_events: null handle");
+    if (n_terms < 0 || n_terms > WL_MAX_DEVICE_EVENTS) return fail(WL_EINVAL, "wl_set_device_events: n_terms must be 0..8");
+    if (n_terms > 0 && !table) return fail(WL_EINVAL, "wl_set_device_events: null term table");
+    if (fan_set(sim)) return fail(WL_EINVAL, "wl_set_device_events: the peer fan-out is set, and device events run with wl_step_terms only");
+    DevEventTable et{};
+    et.n = n_terms;
+    for (int k = 0; k < n_terms; ++k) {
+        const wl_device_event_desc& d = table[k];
+        const std::string term = "wl_set_device_events: term " + std::to_string(k);
+        if (d.mode != WL_EVENT_MODE_RESET && d.mode != WL_EVENT_MODE_INTERVAL) return fail(WL_EINVAL, term + ": unknown mode");
+        for (int j = 0; j < 6; ++j) {
+            const float lo = d.velocity_range[j][0], hi = d.velocity_range[j][1];
+            if (!std::isfinite(lo) || !std::isfinite(hi) || lo > hi)
+                return fail(WL_EINVAL, term + ": velocity range " + std::to_string(j) + " must be finite with lo <= hi");
+            et.lo[k][j] = lo; et.hi[k][j] = hi;
+        }
+        et.slot[k] = -1;
+        if (d.mode == WL_EVENT_MODE_INTERVAL) {
+            const float lo = d.interval_range_s[0], hi = d.interval_range_s[1];
+            if (!std::isfinite(lo) || !std::isfinite(hi) || lo < 0.0f || lo > hi)
+                return fail(WL_EINVAL, term + ": interval_range_s must be finite with 0 <= lo <= hi");
+            et.slot[k] = et.timers.n;
+            et.timers.lo[et.timers.n] = lo; et.timers.hi[et.timers.n] = hi;
+            ++et.timers.n;
+        }
+    }
+    ensure_device(sim);
+    if (n_terms == 0) { free_device_events(sim); return WL_OK; }
+    const size_t n = (size_t)sim->cfg.num_envs, o_bits = align256((size_t)et.timers.n * n * 4), bytes = o_bits + align256(n);
+    char* blk = nullptr;
+    if (int rc = cuda_check(cudaMalloc(&blk, bytes), "wl_set_device_events: allocate")) return rc;
+    DevEvents* de = new (std::nothrow) DevEvents();
+    if (!de) { cudaFree(blk); return fail(WL_EINVAL, "wl_set_device_events: out of host memory"); }
+    et.timers.time_left = et.timers.n ? reinterpret_cast<float*>(blk) : nullptr;
+    int rc = cuda_check(cudaMemset(blk + o_bits, 0, n), "wl_set_device_events: clear");
+    if (!rc && et.timers.n) {       // the interval timers, drawn as wl_set_event_timers draws them
+        wl_event_timers_init_kernel<<<(unsigned)((n + WL_EVENT_BS - 1) / WL_EVENT_BS), WL_EVENT_BS>>>(sim->cfg, et.timers);
+        rc = launched(sim, "wl_event_timers_init_kernel");
+    }
+    // finished before returning, so that a step on any stream afterwards sees the timers
+    if (!rc) rc = cuda_check(cudaDeviceSynchronize(), "wl_set_device_events: draw");
+    if (rc) { cudaFree(blk); delete de; return rc; }
+    de->et = et;
+    de->tbits = reinterpret_cast<uint8_t*>(blk + o_bits);
+    de->block = blk;
+    free_device_events(sim);
+    sim->devents = de;
+    return WL_OK;
+}
+
+int wl_device_events(wl_sim* sim, const uint8_t* d_terminated, const uint8_t* d_truncated, int64_t step_counter, void* stream) {
+    if (!sim || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_device_events: null argument");
+    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
+        return fail(WL_EINVAL, "wl_device_events: step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+    if (!sim->devents) return fail(WL_EINVAL, "wl_device_events: no device event terms (wl_set_device_events)");
+    if (fan_set(sim)) return fail(WL_EINVAL, "wl_device_events: the peer fan-out is set, and device events run with wl_step_terms only");
+    ensure_device(sim);
+    return launch_device_events(sim, d_terminated, d_truncated, (uint32_t)step_counter, (cudaStream_t)stream);
+}
+
 int wl_set_device_terms(wl_sim* sim, const wl_term_desc* terms, int32_t n_terms) {
     if (!sim) return fail(WL_EINVAL, "wl_set_device_terms: null handle");
     if (n_terms < 0 || n_terms > WL_MAX_DEVICE_TERMS) return fail(WL_EINVAL, "wl_set_device_terms: at most 8 device terms");
@@ -2489,26 +2580,36 @@ int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew
     if (int rc = refuse_fan(sim, "wl_step_terms")) return rc;
     cudaStream_t cs = (cudaStream_t)stream;
     DevTerms* dt = sim->dterms;
-    if (!dt) return wl_step(sim, d_action, d_obs, d_rew, d_terminated, d_truncated, d_log, step_counter, stream);   // no terms: wl_step itself
+    DevEvents* de = sim->devents;
+    if (!dt && !de) return wl_step(sim, d_action, d_obs, d_rew, d_terminated, d_truncated, d_log, step_counter, stream);   // wl_step itself
     if (int rc = prep_step(sim, step_counter, 1, cs)) return rc;
     const uint32_t t = (uint32_t)step_counter;               // negative (device base + k) stays encoded: see decode_step
-    uint8_t* tbits = sim->term_bits ? sim->term_bits : dt->tbits;
+    uint8_t* tbits = sim->term_bits ? sim->term_bits : dt ? dt->tbits : de->tbits;
     if (int rc = launch_stage<1>(sim, reinterpret_cast<const float2*>(d_action), nullptr, d_rew, nullptr, nullptr, nullptr, t,
                                  StageIO{tbits, nullptr, nullptr}, cs)) return rc;
     const int n = sim->cfg.num_envs, ctas = (n + WL_TERMS_BS - 1) / WL_TERMS_BS;
-    wl_terms_kernel<<<ctas, WL_TERMS_BS, 0, cs>>>(dt->tt, sim->cfg, sim->state, sim->globals, sim->hf, t, d_rew, tbits, dt->b,
-                                                  d_term_log != nullptr);
-    if (int rc = launched(sim, "wl_terms_kernel")) return rc;
-    if (d_term_log) {
-        wl_terms_log_kernel<<<1, 9 * 32, 0, cs>>>(dt->tt, sim->cfg, dt->b.part, ctas, d_term_log);
-        if (int rc = launched(sim, "wl_terms_log_kernel")) return rc;
+    if (dt) {
+        wl_terms_kernel<<<ctas, WL_TERMS_BS, 0, cs>>>(dt->tt, sim->cfg, sim->state, sim->globals, sim->hf, t, d_rew, tbits, dt->b,
+                                                      d_term_log != nullptr);
+        if (int rc = launched(sim, "wl_terms_kernel")) return rc;
+        if (d_term_log) {
+            wl_terms_log_kernel<<<1, 9 * 32, 0, cs>>>(dt->tt, sim->cfg, dt->b.part, ctas, d_term_log);
+            if (int rc = launched(sim, "wl_terms_log_kernel")) return rc;
+        }
     }
-    if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, t,
-                                 StageIO{tbits, dt->b.extra_term, dt->b.extra_to}, cs)) return rc;
+    const StageIO sio{tbits, dt ? dt->b.extra_term : nullptr, dt ? dt->b.extra_to : nullptr};
+    if (de) {   // stage b cut after the reset and the built-in pushes: the reset-mode DR, then the device events, then b2
+        if (int rc = launch_stage<3>(sim, nullptr, nullptr, nullptr, d_terminated, d_truncated, d_log, t, sio, cs)) return rc;
+        if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
+        if (int rc = launch_device_events(sim, d_terminated, d_truncated, t, cs)) return rc;
+        if (int rc = launch_stage<4>(sim, nullptr, d_obs, nullptr, nullptr, nullptr, nullptr, t, StageIO{nullptr, nullptr, nullptr}, cs)) return rc;
+    } else if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, t, sio, cs)) {
+        return rc;
+    }
     if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc;   // t may be device-relative
-    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
+    if (!de) { if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc; }
     return post_step(sim, step_counter, cs);
 }
 
@@ -2517,6 +2618,7 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
     if (!sim || !d_obs || !d_rew || !d_terminated || !d_truncated || !d_log) return fail(WL_EINVAL, "wl_rollout: null argument");
     if (K < 1) return fail(WL_EINVAL, "wl_rollout: K must be >= 1");
     if (int rc = refuse_fan(sim, "wl_rollout")) return rc;
+    if (int rc = refuse_devents(sim, "wl_rollout")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_rollout: the elevation step is two kernels (use wl_step)");
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam) return fail(WL_EUNSUPPORTED, "wl_rollout: the camera term is a second kernel (use wl_step)");
     if (sim->reset_ev) return fail(WL_EUNSUPPORTED, "wl_rollout: the reset-mode DR events are a second kernel after each step (use wl_step)");
@@ -2710,6 +2812,7 @@ static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float*
                            float* d_obs, float* d_rew, uint8_t* d_terminated, uint8_t* d_truncated, float* d_log, int64_t step_counter,
                            void* stream) {
     if (int rc = refuse_fan(sim, fn)) return rc;
+    if (int rc = refuse_devents(sim, fn)) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, std::string(fn) + ": blind-observation tasks only (obs_dim <= 16)");
     if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))

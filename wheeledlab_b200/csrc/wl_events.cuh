@@ -23,6 +23,18 @@ struct EventTable {
 // torch.rand's U[0, 1) (24 bits) scaled to [lo, hi) as the event manager scales it
 __device__ __forceinline__ float event_interval(uint32_t x, float lo, float hi) { return __fadd_rn(__fmul_rn(u01(x), __fsub_rn(hi, lo)), lo); }
 
+// one step of timer k at o = k * num_envs + i with the draws r: redraw a reset env (.x), count down, fire below 1e-6 and
+// redraw a fired one (.y); returns whether it fired (also the device event terms' timers, wl_dev_events.cuh)
+__device__ __forceinline__ bool event_timer_step(const EventTable& et, int k, size_t o, uint4 r, bool reset, float dt) {
+    float tl = et.time_left[o];
+    if (reset) tl = event_interval(r.x, et.lo[k], et.hi[k]);
+    tl = __fsub_rn(tl, dt);
+    const bool f = tl < 1.0e-6f;
+    if (f) tl = event_interval(r.y, et.lo[k], et.hi[k]);
+    et.time_left[o] = tl;
+    return f;
+}
+
 // the construction draw: key (seed, global env id, 0, RNG_EVENT_INIT, k)
 __global__ void __launch_bounds__(WL_EVENT_BS)
 wl_event_timers_init_kernel(const __grid_constant__ wl_config c, const __grid_constant__ EventTable et) {
@@ -46,13 +58,6 @@ wl_event_timers_kernel(const __grid_constant__ wl_config c, const __grid_constan
     const float dt = c.d_step_dt;
     for (int k = 0; k < et.n; ++k) {
         const size_t o = (size_t)k * n + i;
-        const uint4 r = philox4x32(c.seed, gid, t, RNG_EVENT, (uint32_t)k);
-        float tl = et.time_left[o];
-        if (reset) tl = event_interval(r.x, et.lo[k], et.hi[k]);
-        tl = __fsub_rn(tl, dt);
-        const bool f = tl < 1.0e-6f;
-        if (f) tl = event_interval(r.y, et.lo[k], et.hi[k]);
-        et.time_left[o] = tl;
-        fired[o] = f ? 1 : 0;
+        fired[o] = event_timer_step(et, k, o, philox4x32(c.seed, gid, t, RNG_EVENT, (uint32_t)k), reset, dt) ? 1 : 0;
     }
 }

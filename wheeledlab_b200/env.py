@@ -310,6 +310,7 @@ class ManagerBasedRLEnv:
         self._event_fired = None                 # [interval terms, N] u8: wl_event_timers' fired bytes
         self._py_sums = {}
         self._dev_terms = []                     # device terms (add_device_reward_term): evaluated by wl_step_terms
+        self._dev_events = []                    # device event terms (add_device_event_term): applied by wl_step_terms
         self._term_log_ring = None
         self._critic_terms = []                  # the critic observation group (set_critic_observation)
         for name, func, weight, params in self.spec.python_reward_terms:
@@ -328,6 +329,8 @@ class ManagerBasedRLEnv:
                 self.add_device_reward_term(name, func, weight, params)
             else:
                 self.add_device_termination_term(name, func, role == "time_out", params)
+        for name, func, mode, params, interval_range_s in self.spec.device_events:
+            self.add_device_event_term(name, func, mode, interval_range_s, params)
         if self.spec.reset_events:
             self.sim.set_reset_events(**{name: True for name in self.spec.reset_events})
         if self.spec.critic_terms:
@@ -408,7 +411,7 @@ class ManagerBasedRLEnv:
         terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
         if terms and (self._py_rewards or self._py_terms or self._py_obs or self._py_events):
             raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
-        if terms and self._dev_terms:
+        if terms and (self._dev_terms or self._dev_events):
             raise NotImplementedError("a critic observation group together with device terms is not implemented")
         table = []
         for name, fn, params in terms:
@@ -510,7 +513,8 @@ class ManagerBasedRLEnv:
         if getattr(self, "_critic_terms", None):
             raise NotImplementedError("a critic observation group together with " + ("device terms" if device else "host-side Python terms")
                                       + " is not implemented")
-        if (self._py_rewards or self._py_terms or getattr(self, "_py_events", None)) if device else self._dev_terms:
+        if (self._py_rewards or self._py_terms or getattr(self, "_py_events", None)) if device else \
+                (self._dev_terms or getattr(self, "_dev_events", None)):
             raise NotImplementedError("an env runs either device terms or host-side Python reward / termination terms, not both")
 
     def _add_device_term(self, name, func, role, weight, params):
@@ -546,6 +550,31 @@ class ManagerBasedRLEnv:
         time_out=True truncates instead of terminating); get_term(name) and Episode_Termination/<name> cover it."""
         from .device_terms import ROLE_TERMINATION, ROLE_TIME_OUT
         self._add_device_term(name, func, ROLE_TIME_OUT if time_out else ROLE_TERMINATION, 0.0, params)
+
+    def add_device_event_term(self, name: str, func, mode: str, interval_range_s=None, params: dict | None = None):
+        """Register an event function of the device event library (device_events.REGISTRY: IsaacLab's
+        ``push_by_setting_velocity``) as an event term applied on the device, inside env.step's launches (wl_step_terms) and
+        capturable in a graph (DESIGN 6p).  ``"reset"``: applied to the envs the step reset, after the reset and the
+        built-in pushes.  ``"interval"``: per env, a timer drawn from ``interval_range_s`` = (lo, hi) counts down by
+        step_dt, and the term applies where it ran out (timers restart at reset).  Terms apply in registration order, before
+        the step's command and observation.  ``env.reset()`` does not apply them.  Refused by name: what add_event_term
+        refuses, startup mode, a function the library does not have, a ninth term, host-side Python terms on the env."""
+        from . import device_events as dev
+        from .compat import check_event_term
+        check_event_term(name, mode, interval_range_s)
+        dev.check_mode(name, mode)
+        if dev.lookup(func) is None:
+            raise NotImplementedError(f"event term {name}: {getattr(func, '__module__', '?')}.{getattr(func, '__name__', func)} "
+                                      "is not in the device event library (register it with add_event_term as a Python event term)")
+        self._refuse_mixing(device=True)
+        if len(self._dev_events) >= dev.MAX_TERMS:
+            raise NotImplementedError(f"event term {name}: more than {dev.MAX_TERMS} device event terms")
+        if any(t.name == name for t in self._dev_events):
+            raise ValueError(f"device event term {name!r} is already registered")
+        term = SimpleNamespace(name=name, func=func, mode=mode, ranges=dev.velocity_ranges(name, params),
+                               interval_range_s=None if mode != "interval" else tuple(float(v) for v in interval_range_s))
+        self.sim.set_device_events([(t.mode, t.interval_range_s, t.ranges) for t in self._dev_events + [term]])
+        self._dev_events.append(term)
 
     @property
     def device_log_names(self) -> list:
@@ -674,7 +703,7 @@ class ManagerBasedRLEnv:
         out, log = self._step_ring[t % self._ring_len]
         if not self.log_episode_info:
             log = None
-        if self._dev_terms:
+        if self._dev_terms or self._dev_events:
             if self._term_log_ring is None:
                 self._term_log_ring = torch.zeros((self._ring_len, 8), dtype=torch.float32, device=self.device)
             term_log = self._term_log_ring[t % self._ring_len] if log is not None else None
@@ -705,7 +734,7 @@ class ManagerBasedRLEnv:
         result views are overwritten by the next step_host call.  With ``env.host_obs = True`` the observations are returned in
         pinned HOST memory as well (a ring of _RING buffers): D2H copy after the step (transport "copy") or written by the
         kernel over PCIe (transport "zero_copy")."""
-        if self._py_rewards or self._py_terms or getattr(self, "_py_events", None) or self._dev_terms:
+        if self._py_rewards or self._py_terms or getattr(self, "_py_events", None) or self._dev_terms or getattr(self, "_dev_events", None):
             raise NotImplementedError("step_host: Python and device terms need the staged step (use env.step)")
         if self._needs_reset:
             self.reset()

@@ -749,7 +749,8 @@ class FusedOnPolicyRunner:
     for each Python term, the T-step mean of what env.step's ``extras["log"]`` holds for it.  Python observation terms and
     data-parallel runs with Python terms raise ``NotImplementedError``.  An env with device terms (``add_device_reward_term``)
     trains through ``device_terms_iteration``: its rollout (``policy_act`` then ``wl_step_terms``) is part of the one graph,
-    on one GPU or data-parallel, and the log gains each device term's ``Episode_*`` key as its T-step mean.
+    on one GPU or data-parallel, and the log gains each device term's ``Episode_*`` key as its T-step mean.  An env with
+    device event terms (``add_device_event_term``) trains the same way; they add no log keys.
 
     The agent cfg dict is read for ``num_steps_per_env``, ``save_interval``, ``policy`` (``activation_from_rsl_rl``,
     ``init_noise_std``) and ``algorithm`` (``PPOConfig.from_rsl_rl``).  The weights start as the reference's do: torch
@@ -794,6 +795,7 @@ class FusedOnPolicyRunner:
                                       "staged step writes: an env with host-side Python terms trains with reward and termination terms only")
         self.staged = bool(getattr(e, "_py_rewards", None) or getattr(e, "_py_terms", None) or getattr(e, "_py_events", None))
         self.dev_names = e.device_log_names if getattr(e, "_dev_terms", None) else []
+        dev_step = bool(self.dev_names or getattr(e, "_dev_events", None))     # the rollout steps through wl_step_terms
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
@@ -801,7 +803,7 @@ class FusedOnPolicyRunner:
         if self.critic_obs_dim is not None:
             if self.staged:
                 raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
-            if self.dev_names:
+            if dev_step:
                 raise NotImplementedError("a critic observation group together with device terms is not implemented")
             if s.activation != "elu":
                 raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
@@ -826,7 +828,7 @@ class FusedOnPolicyRunner:
         else:
             exchange = PPOExchange.symmetric(D, sim.device) if self.world > 1 else None
             self.it = device_terms_iteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, exchange) \
-                if self.dev_names else PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation,
+                if dev_step else PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation,
                                                     episode_stats=True, exchange=exchange)
         self.alg = self.it.ppo
         self.current_learning_iteration = 0

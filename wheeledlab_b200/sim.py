@@ -343,6 +343,26 @@ class WheeledSim:
                                 step_counter, _stream_ptr(self.device)), "wl_step_terms")
         return obs, rew, term, trunc
 
+    def set_device_events(self, terms):
+        """The handle's device event terms (wl_set_device_events): a list of (mode, interval_range_s or None, velocity
+        ranges [6] of (lo, hi) in x, y, z, roll, pitch, yaw order), applied in this order; the interval terms' timers are
+        drawn now.  [] clears them.  From then on only step_terms steps the handle."""
+        n = len(terms)
+        arr = (_lib.WlDeviceEventDesc * max(1, n))()
+        for k, (mode, interval_range_s, ranges) in enumerate(terms):
+            d = arr[k]
+            d.mode = _lib.WL_EVENT_MODE[mode]
+            d.interval_range_s[0], d.interval_range_s[1] = interval_range_s if interval_range_s is not None else (0.0, 0.0)
+            for j, (lo, hi) in enumerate(ranges):
+                d.velocity_range[j][0], d.velocity_range[j][1] = float(lo), float(hi)
+        with torch.cuda.device(self.device):
+            check(lib.wl_set_device_events(self._h, arr, n), "wl_set_device_events")
+
+    def device_events(self, terminated: torch.Tensor, truncated: torch.Tensor, step_counter: int):
+        """The device event terms of one step on the state (wl_device_events), with the done bytes stage b1 wrote."""
+        u8 = lambda x: C.c_void_p((x.view(torch.uint8) if x.dtype == torch.bool else x).data_ptr())
+        check(lib.wl_device_events(self._h, u8(terminated), u8(truncated), step_counter, _stream_ptr(self.device)), "wl_device_events")
+
     def set_critic_terms(self, terms):
         """The handle's critic observation (wl_set_critic_terms): a list of term names of the library
         (``_lib.WL_CRITIC_TERMS``) or (name, clip) pairs, concatenated in this order into the critic row; [] clears it.

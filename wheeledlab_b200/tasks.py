@@ -67,6 +67,8 @@ class TaskSpec:
     python_event_terms: list = field(default_factory=list)      # [(name, func, mode, params, interval_range_s or None)]
     # device terms (device_terms.py), evaluated by wl_step_terms: [(name, func, "reward" | "termination" | "time_out", weight, params)]
     device_terms: list = field(default_factory=list)
+    # device event terms (device_events.py), applied by wl_step_terms: [(name, func, mode, params, interval_range_s or None)]
+    device_events: list = field(default_factory=list)
     # the critic observation group (privileged.py, wl_critic_observe): [(name, library term, clip)] in row order; [] = none
     critic_terms: list = field(default_factory=list)
     # DR events in IsaacLab's mode="reset" (wl_set_reset_events): names of _lib.WL_RESET_EVENTS; [] = start-up DR only
