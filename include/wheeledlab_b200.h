@@ -735,6 +735,58 @@ int32_t wl_policy_blob_floats_asym(int32_t obs_dim, int32_t critic_obs_dim, int3
 int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
                        const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream);
 
+/* ---- a modified policy observation group for the Drift family (DESIGN.md 6q) ----------------------------------------------
+ * IsaacLab's ObservationManager.compute for the "policy" group of a cfg whose terms differ from BlindObsCfg's: the row is
+ * the concatenation, in table order, of terms of the critic library (WL_CRITIC_*, with the widths listed there) and
+ *   WL_POLICY_PROJECTED_GRAVITY    3    the gravity direction (0, 0, -1) in the body frame (projected_gravity_b)
+ * Per term, in this order: the value; additive noise, only when the config's enable_corruption is set -- Gaussian
+ * (x + mean) + std * z, or uniform (x + u * (n_max - n_min)) + n_min, u in [0, 1); the clip [lo, hi] (r_clamp); the scale
+ * (x * s), one value or one per float.  Each step is one fp32 operation, no fma.  Parameters are the cfg's Python floats;
+ * each is rounded to fp32 as torch rounds a scalar operand, n_max - n_min is formed in double first, as Python forms it.
+ * Noise keys of column j (0-based in the row), env global id g, step counter t:
+ *   Gaussian, j < 12:  Philox (seed, g, t, 0, j / 4) after a step and (seed, g, t, 7, 3 call_idx + j / 4) for an observe
+ *                      call: the built-in row's own keys, so BlindObsCfg's five terms through a table are the built-in row;
+ *                      lanes (x, y) -> Box-Muller -> columns 4b, 4b + 1, lanes (z, w) -> 4b + 2, 4b + 3
+ *   otherwise:         Philox (seed, g, t, 16, 16 (call_idx + 1) + 8 u + j / 4), u = 1 for uniform noise, call_idx = -1
+ *                      after a step; word j % 4 (U[0,1) from its top 24 bits) or its Box-Muller lane as above
+ * so no two columns, steps or call indices share a key. */
+#define WL_MAX_POLICY_OBS   32
+#define WL_MAX_POLICY_TERMS 16
+#define WL_POLICY_PROJECTED_GRAVITY 11
+#define WL_POLICY_OBS_KINDS 12
+#define WL_NOISE_NONE     0
+#define WL_NOISE_GAUSSIAN 1   /* noise_params = (mean, std) */
+#define WL_NOISE_UNIFORM  2   /* noise_params = (n_min, n_max) */
+#define WL_POLICY_OBS_AFTER_STEP (-1)   /* wl_policy_observe's call_idx for the row of the step just taken */
+typedef struct wl_policy_term {
+    int32_t kind;             /* WL_CRITIC_* or WL_POLICY_PROJECTED_GRAVITY */
+    int32_t noise;            /* WL_NOISE_* */
+    double noise_params[2];
+    int32_t clip;             /* 1: clamp to [clip_range[0], clip_range[1]] */
+    int32_t n_scale;          /* 0: no scale; 1: scale[0] for every float; the term's width: scale[k] for float k */
+    double clip_range[2];
+    double scale[4];
+} wl_policy_term;
+/* Store the handle's policy table (a host-side set-up call: nothing is launched or allocated; every term is checked before
+ * the table is replaced, so a failure leaves the handle as it was).  n_terms = 0 clears it.  WL_EINVAL: a null handle,
+ * n_terms outside 0..WL_MAX_POLICY_TERMS, a null table with n_terms > 0, an unknown kind or noise model, n_scale not 0, 1 or
+ * the width, a parameter that is not finite, a total width above WL_MAX_POLICY_OBS; WL_EUNSUPPORTED: a task other than the
+ * Drift family, a peer / multicast fan-out set.  With a table, wl_act_step, wl_act_infer_step and wl_rollout return
+ * WL_EUNSUPPORTED (they hand their next call the built-in row); wl_step, wl_step_terms and wl_observe still write the
+ * built-in row.  wl_policy_act_elu, wl_policy_act and wl_policy_act_asym read rows of width Dp (and a blob laid out for
+ * Dp) from then on: the policy is trained and played on the table's row.  A graph captured with the old table keeps the old
+ * table. */
+int wl_set_policy_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms);
+/* Dp: the width of the policy row (0 with no table) */
+int32_t wl_policy_obs_dim(const wl_sim* sim);
+/* d_out [N, Dp] (16-byte stores when it is 16-byte aligned) from the state the most recent step / reset left -- after a
+ * step, the post-reset state of the envs it reset.  call_idx = WL_POLICY_OBS_AFTER_STEP: the row of the step taken at
+ * step_counter; call_idx >= 0: the row of wl_observe(step_counter, call_idx).  step_counter: a host value 0..2^31-1 or
+ * WL_DEVICE_COUNTER_PLUS(k).  One launch, capturable.  Before any launch: WL_EINVAL for a null pointer or one not 4-byte
+ * aligned, no table, a counter out of range, call_idx outside -1..2^27-1; WL_EUNSUPPORTED while a peer / multicast
+ * fan-out is set (only the built-in row carries it). */
+int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float* d_out, void* stream);
+
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out
  * bootstrap of PPO.process_env_step (rewards += gamma * values * time_outs) folded in when d_time_outs != NULL:

@@ -39,6 +39,10 @@ def base_ang_vel(env, asset_cfg: SceneEntityCfg = _ROBOT):
     return env.scene[asset_cfg.name].data.root_ang_vel_b
 
 
+def projected_gravity(env, asset_cfg: SceneEntityCfg = _ROBOT):
+    return env.scene[asset_cfg.name].data.projected_gravity_b
+
+
 def base_pos_z(env, asset_cfg: SceneEntityCfg = _ROBOT):
     return env.scene[asset_cfg.name].data.root_pos_w[:, 2].unsqueeze(-1)
 

@@ -9,7 +9,9 @@ policy: the action is the actor mean (rsl_rl's ``get_inference_policy``), T x ``
 ELU network, T x (``wl_actor_mean`` -> ``wl_step``) for the ReLU network of Elevation and Visual.  The task, num_envs, seed
 and agent cfg come from the run's ``run.json`` (``tools/ppo_train.py --log-dir``); without one, ``--task`` is needed and
 the activation follows the task.  ``-sd`` saves ``{'observations', 'actions'}`` as ``<playback-dir>/<play-name>-rollouts.pt``,
-the reference's file.  Prints the mean return and length of the episodes that finished during the playback.
+the reference's file.  Prints the mean return and length of the episodes that finished during the playback.  A run trained on
+a policy observation table (``policy_terms`` in ``run.json``, DESIGN 6q) plays on an env with the same table, through
+``wl_actor_mean`` on the table's row.
 """
 from __future__ import annotations
 
@@ -61,7 +63,8 @@ def resolve(args) -> dict:
     agent = run_cfg["agent_cfg"] if run_cfg is not None else agent_cfg(task_activation(task))
     num_envs = args.num_envs if args.num_envs is not None else (run_cfg or {}).get("num_envs")
     seed = args.seed if args.seed is not None else (run_cfg or {}).get("seed")
-    return {"task": task, "policy_path": policy_path, "playback_dir": playback_dir, "agent_cfg": agent, "num_envs": num_envs, "seed": seed}
+    return {"task": task, "policy_path": policy_path, "playback_dir": playback_dir, "agent_cfg": agent, "num_envs": num_envs, "seed": seed,
+            "policy_terms": (run_cfg or {}).get("policy_terms")}
 
 
 def play(r: dict, steps: int, device: str = "cuda:0"):
@@ -72,6 +75,9 @@ def play(r: dict, steps: int, device: str = "cuda:0"):
     from wheeledlab_b200.policy import FusedPolicyRollout
     kw = {k: r[k] for k in ("num_envs", "seed") if r[k] is not None}
     env = wl.make(r["task"], device=device, **kw)
+    if r.get("policy_terms"):
+        env.set_policy_observation([(name, fn, {"noise": tuple(nz) if nz else None, "clip": cl, "scale": sc})
+                                    for name, fn, nz, cl, sc in r["policy_terms"]])
     runner = FusedOnPolicyRunner(env, r["agent_cfg"], device=device)
     runner.load(r["policy_path"], load_optimizer=False)
     env.reset()

@@ -58,16 +58,21 @@ def _task_kind(cfg) -> str:
         return "visual"
     if "root_pos_w" in funcs:
         return "drift"
+    from ._lib import WL_POLICY_TERMS
+    if any(f in WL_POLICY_TERMS for f in funcs):           # a modified Drift group (lowered with device_terms only)
+        return "drift"
     raise NotImplementedError(f"observation group {funcs} is not one the fused step implements")
 
 
-def _validate_obs(cfg, expected, c, blind=False):
+def _validate_obs(cfg, expected, c, blind=False, task=None):
     """The observation group must be exactly what the kernel assembles: same term functions in the same order; noise stds
     (BlindObs) and clips are read from the cfg."""
     terms = [(k, t) for k, t in _fields(cfg.observations.policy) if hasattr(t, "func")]
     funcs = [_fname(t) for _, t in terms]
     if funcs != expected:
-        raise NotImplementedError(f"observation terms {funcs} differ from the kernel's {expected} (order matters)")
+        raise NotImplementedError(f"observation terms {funcs} differ from the kernel's {expected} (order matters)"
+                                  + (f"; a modified {task} policy group is not implemented (the policy observation table covers "
+                                     "the Drift family)" if task else ""))
     if getattr(cfg.observations.policy, "concatenate_terms", True) is not True:
         raise NotImplementedError("observation group must concatenate its terms")
     for k, (name, t) in enumerate(terms):
@@ -116,6 +121,38 @@ def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
         raise NotImplementedError("critic observation group: no terms")
     privileged.check_width([(fn, c) for _, fn, c in table], "critic observation group " + ", ".join(n for n, _, _ in table))
     spec.critic_terms = table
+
+
+def _lower_policy(cfg, spec: T.TaskSpec, c, device_terms: bool):
+    """``cfg.observations.policy`` of the Drift family: BlindObsCfg's group is validated onto the built-in row as before;
+    with ``device_terms`` any other group is lowered to ``spec.policy_terms``, the term table of ``wl_policy_observe``
+    (policy_obs.py), refusing by term name what the kernel does not do.  Without the flag a modified group raises."""
+    saved = (list(c.noise_std), c.obs_clip)
+    try:
+        _validate_obs(cfg, _OBS_BLIND, c, blind=True)
+        return
+    except NotImplementedError:
+        if not device_terms:
+            raise
+    c.noise_std[:], c.obs_clip = saved                      # the built-in row keeps the task's defaults
+    from . import policy_obs
+    group = cfg.observations.policy
+    if getattr(group, "concatenate_terms", True) is not True:
+        raise NotImplementedError("policy observation group: concatenate_terms=False is not implemented")
+    if getattr(group, "history_length", None):
+        raise NotImplementedError("policy observation group: history_length is not implemented")
+    table = []
+    for name, t in _fields(group):
+        if not hasattr(t, "func"):
+            continue
+        if getattr(t, "history_length", 0):
+            raise NotImplementedError(f"policy term {name}: history_length is not implemented")
+        table.append((name,) + policy_obs.lower_term(name, t.func, getattr(t, "params", None), getattr(t, "noise", None),
+                                                     getattr(t, "clip", None), getattr(t, "scale", None), getattr(t, "modifiers", None)))
+    if not table:
+        raise NotImplementedError("policy observation group: no terms")
+    policy_obs.check_width([t[1:] for t in table], "policy observation group " + ", ".join(t[0] for t in table))
+    spec.policy_terms = table
 
 
 def _lower_common(cfg, spec: T.TaskSpec):
@@ -330,7 +367,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
                             vehicle="f1tenth" if "f1tenth" in usd else "mushr")
         c = spec.cfg
         _lower_common(cfg, spec)
-        _validate_obs(cfg, _OBS_BLIND, c, blind=True)
+        _lower_policy(cfg, spec, c, device_terms)
         _lower_critic(cfg, spec, kind)
 
         def h_slip(p):
@@ -392,7 +429,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     spec = T.elevation_task(num_envs=num_envs, seed=seed, env_id_offset=env_id_offset)
     c = spec.cfg
     _lower_common(cfg, spec)
-    _validate_obs(cfg, _OBS_ELEV, c)
+    _validate_obs(cfg, _OBS_ELEV, c, task="Elevation")
     for _, t in _fields(cfg.observations.policy):
         if hasattr(t, "func") and _fname(t) == "world_height_map":
             c.scan_offset, c.scan_plane_init = float(t.params["offset"]), float(t.params["plane_init_value"])
@@ -453,7 +490,7 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device
     spec = T.visual_task(num_envs=num_envs, seed=seed, env_id_offset=env_id_offset, traversability=trav, camera=cam_mode, randomize=randomize)
     c = spec.cfg
     _lower_common(cfg, spec)
-    _validate_obs(cfg, [funcs[0]] + _OBS_VIS_TAIL, c)
+    _validate_obs(cfg, [funcs[0]] + _OBS_VIS_TAIL, c, task="Visual")
     # map geometry (VisualTerrainImporterCfg :63-124) and ground material (:126-135)
     c.vis_row_spacing, c.vis_col_spacing = float(terrain.row_spacing), float(terrain.col_spacing)
     c.vis_width, c.vis_height = float(terrain.width), float(terrain.height)

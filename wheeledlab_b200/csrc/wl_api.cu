@@ -15,6 +15,7 @@
 using namespace wl;
 
 #include "wl_critic.cuh"
+#include "wl_policy_obs.cuh"
 #include "wl_events.cuh"
 
 // ---------------------------------------------------------------------------------------
@@ -51,6 +52,7 @@ struct wl_sim {
     uint32_t reset_ev;         // wl_set_reset_events: WL_RESET_EV_* bits of the events redrawn at every reset (0: none)
     EventTable events;         // wl_set_event_timers: the interval terms' ranges and per-env timers (n = 0: none)
     struct DevEvents* devents; // wl_set_device_events: the device event terms and their timers (null: none)
+    PolicyObsTable pobs;       // wl_set_policy_terms: the policy observation's columns (n_cols = 0: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1734,6 +1736,14 @@ static int refuse_devents(const wl_sim* sim, const char* fn) {
     if (!sim->devents) return WL_OK;
     return fail(WL_EUNSUPPORTED, std::string(fn) + ": the handle has device event terms, which wl_step_terms applies (wl_set_device_events(0) first)");
 }
+// a call that hands its next call the built-in policy row refuses a handle with a policy table, before any device work
+static int refuse_pobs(const wl_sim* sim, const char* fn) {
+    if (sim->pobs.n_cols == 0) return WL_OK;
+    return fail(WL_EUNSUPPORTED, std::string(fn) + ": the handle has a policy observation table, whose row wl_policy_observe forms "
+                                 "(wl_set_policy_terms(0) first)");
+}
+// the width of the row the policy kernels read: the policy table's when the handle has one, else the built-in row's
+static int policy_in_dim(const wl_sim* sim) { return sim->pobs.n_cols ? sim->pobs.n_cols : sim->obs_dim; }
 
 __global__ void wl_detmath_kernel(int op, const float* __restrict__ in, const float* __restrict__ in2, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2619,6 +2629,7 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
     if (K < 1) return fail(WL_EINVAL, "wl_rollout: K must be >= 1");
     if (int rc = refuse_fan(sim, "wl_rollout")) return rc;
     if (int rc = refuse_devents(sim, "wl_rollout")) return rc;
+    if (int rc = refuse_pobs(sim, "wl_rollout")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_rollout: the elevation step is two kernels (use wl_step)");
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam) return fail(WL_EUNSUPPORTED, "wl_rollout: the camera term is a second kernel (use wl_step)");
     if (sim->reset_ev) return fail(WL_EUNSUPPORTED, "wl_rollout: the reset-mode DR events are a second kernel after each step (use wl_step)");
@@ -2782,6 +2793,61 @@ int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_term
 }
 int32_t wl_critic_obs_dim(const wl_sim* sim) { return sim ? sim->critic.n_cols : 0; }
 
+int wl_set_policy_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) {
+    const std::string fn = "wl_set_policy_terms: ";
+    if (!sim) return fail(WL_EINVAL, fn + "null handle");
+    if (n_terms < 0 || n_terms > WL_MAX_POLICY_TERMS) return fail(WL_EINVAL, fn + "at most 16 policy terms");
+    if (n_terms > 0 && !terms) return fail(WL_EINVAL, fn + "null term table");
+    if (sim->cfg.task != WL_TASK_DRIFT) return fail(WL_EUNSUPPORTED, fn + "a policy observation table is implemented for the Drift family only");
+    if (fan_set(sim)) return fail(WL_EUNSUPPORTED, fn + "the peer fan-out is set, and only the built-in row carries it");
+    PolicyObsTable tb;
+    memset(&tb, 0, sizeof tb);
+    for (int k = 0; k < n_terms; ++k) {
+        const wl_policy_term& d = terms[k];
+        const std::string at = fn + "term " + std::to_string(k) + ": ";
+        if (d.kind < 1 || d.kind >= WL_POLICY_OBS_KINDS) return fail(WL_EINVAL, at + "unknown term kind " + std::to_string(d.kind));
+        if (d.noise < WL_NOISE_NONE || d.noise > WL_NOISE_UNIFORM) return fail(WL_EINVAL, at + "unknown noise model " + std::to_string(d.noise));
+        const int w = policy_obs_width(d.kind);
+        if (d.n_scale != 0 && d.n_scale != 1 && d.n_scale != w) return fail(WL_EINVAL, at + "n_scale must be 0, 1 or the term's width");
+        bool finite = std::isfinite(d.noise_params[0]) && std::isfinite(d.noise_params[1]) && std::isfinite(d.clip_range[0]) &&
+                      std::isfinite(d.clip_range[1]);
+        for (int s = 0; s < 4; ++s) finite = finite && std::isfinite(d.scale[s]);
+        if (!finite) return fail(WL_EINVAL, at + "a noise, clip or scale parameter is not finite");
+        if (tb.n_cols + w > WL_MAX_POLICY_OBS) return fail(WL_EINVAL, fn + "the policy row is wider than 32 floats");
+        for (int j = 0; j < w; ++j, ++tb.n_cols) {
+            const int c = tb.n_cols;
+            tb.src[c] = (uint8_t)(policy_obs_first(d.kind) + j);
+            tb.noise[c] = (uint8_t)d.noise;
+            tb.na[c] = (float)d.noise_params[0];
+            tb.nb[c] = d.noise == WL_NOISE_UNIFORM ? (float)(d.noise_params[1] - d.noise_params[0]) : (float)d.noise_params[1];
+            tb.flags[c] = (uint8_t)((d.clip ? WL_POBS_CLIP : 0u) | (d.n_scale ? WL_POBS_SCALE : 0u));
+            tb.lo[c] = (float)d.clip_range[0];
+            tb.hi[c] = (float)d.clip_range[1];
+            tb.scale[c] = d.n_scale ? (float)d.scale[d.n_scale == 1 ? 0 : j] : 1.0f;
+        }
+        tb.groups |= policy_obs_groups(d.kind);
+    }
+    sim->pobs = tb;
+    return WL_OK;
+}
+int32_t wl_policy_obs_dim(const wl_sim* sim) { return sim ? sim->pobs.n_cols : 0; }
+int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float* d_out, void* stream) {
+    const std::string fn = "wl_policy_observe: ";
+    if (!sim || !d_out) return fail(WL_EINVAL, fn + "null argument");
+    if ((uintptr_t)d_out & 3u) return fail(WL_EINVAL, fn + "d_out must be 4-byte aligned");
+    if (sim->pobs.n_cols < 1) return fail(WL_EINVAL, fn + "no policy table (wl_set_policy_terms)");
+    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
+        return fail(WL_EINVAL, fn + "step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+    if (call_idx < WL_POLICY_OBS_AFTER_STEP || call_idx >= (1 << 27)) return fail(WL_EINVAL, fn + "call_idx must be in -1..2^27-1");
+    if (fan_set(sim)) return fail(WL_EUNSUPPORTED, fn + "the peer fan-out is set, and only the built-in row carries it");
+    ensure_device(sim);
+    const int n = sim->cfg.num_envs;
+    wl_policy_observe_kernel<<<(n + WL_POBS_ENVS - 1) / WL_POBS_ENVS, WL_POBS_THREADS, 0, (cudaStream_t)stream>>>(
+        sim->pobs, sim->state, sim->globals, n, sim->cfg.seed, sim->cfg.env_id_offset, sim->cfg.enable_corruption, (uint32_t)step_counter,
+        call_idx, d_out);
+    return launched(sim, "wl_policy_observe_kernel");
+}
+
 int wl_set_reset_events(wl_sim* sim, uint32_t mask) {
     if (!sim) return fail(WL_EINVAL, "wl_set_reset_events: null handle");
     const uint32_t all = WL_RESET_EV_MATERIAL | WL_RESET_EV_ACTUATOR_GAINS | WL_RESET_EV_BASE_MASS | WL_RESET_EV_WHEEL_MASS;
@@ -2813,6 +2879,7 @@ static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float*
                            void* stream) {
     if (int rc = refuse_fan(sim, fn)) return rc;
     if (int rc = refuse_devents(sim, fn)) return rc;
+    if (int rc = refuse_pobs(sim, fn)) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, std::string(fn) + ": blind-observation tasks only (obs_dim <= 16)");
     if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))
@@ -2872,10 +2939,11 @@ int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic
     if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
         return fail(WL_EINVAL, std::string(fn) + ": step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
     if (int rc = refuse_fan(sim, fn)) return rc;
-    if (sim->obs_dim < 1 || sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    const int D = policy_in_dim(sim);
+    if (D < 1 || D > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
     ensure_device(sim);
     PolicyOffsets po;
-    const int blob_floats = policy_offsets(sim->obs_dim, po.o, critic_obs_dim);
+    const int blob_floats = policy_offsets(D, po.o, critic_obs_dim);
     const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS + WL_ACT_XC));
     static bool attr_set[64] = {false};                       // the attribute is per device
     if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
@@ -2885,8 +2953,7 @@ int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic
     }
     const int n = sim->cfg.num_envs;
     wl_policy_act_asym_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
-        sim->cfg, sim->globals, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter,
-        sim->obs_dim);
+        sim->cfg, sim->globals, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
     return launched(sim, "wl_policy_act_asym_kernel");
 }
 
@@ -2900,10 +2967,11 @@ int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_
         return fail(WL_EINVAL, "wl_policy_act_elu: step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
     // no step rows are written, but the step that consumes these actions refuses the fan-out: refuse it here already
     if (int rc = refuse_fan(sim, "wl_policy_act_elu")) return rc;
-    if (sim->obs_dim < 1 || sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, "wl_policy_act_elu: obs_dim > 16 (the network wl_act_step runs)");
+    const int D = policy_in_dim(sim);
+    if (D < 1 || D > 16) return fail(WL_EUNSUPPORTED, "wl_policy_act_elu: obs_dim > 16 (the network wl_act_step runs)");
     ensure_device(sim);
     PolicyOffsets po;
-    const int blob_floats = policy_offsets(sim->obs_dim, po.o);
+    const int blob_floats = policy_offsets(D, po.o);
     const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS));
     static bool attr_set[64] = {false};                       // the attribute is per device
     if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
@@ -2914,7 +2982,7 @@ int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_
     }
     const int n = sim->cfg.num_envs;
     wl_policy_act_elu_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
-        sim->cfg, sim->globals, d_obs_in, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, sim->obs_dim);
+        sim->cfg, sim->globals, d_obs_in, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
     return launched(sim, "wl_policy_act_elu_kernel");
 }
 
@@ -3226,7 +3294,7 @@ static int wide_attributes(int dev, const char* fn) {
 int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
     if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
         return fail(WL_EINVAL, "wl_policy_act: null argument");
-    const int D = sim->obs_dim, n = sim->cfg.num_envs;
+    const int D = policy_in_dim(sim), n = sim->cfg.num_envs;
     if (D < 1 || D > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, "wl_policy_act: obs_dim must be in 1..4096");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))
         return fail(WL_EINVAL, "wl_policy_act: policy blob must be 16-byte aligned, actions/mean 8-byte aligned");

@@ -171,7 +171,10 @@ class ObservationManager:
     def compute(self):
         """Re-samples the observation noise, like the reference (SURVEY 3.4)."""
         env = self._env
-        obs = env.sim.observe(env.common_step_counter, self._calls)
+        if env._policy_terms:                    # (the table's row only: the built-in row would be thrown away)
+            obs = env.sim.policy_observe(env.common_step_counter, self._calls)
+        else:
+            obs = env.sim.observe(env.common_step_counter, self._calls)
         self._calls += 1
         return env._obs_groups(obs)
 
@@ -313,6 +316,8 @@ class ManagerBasedRLEnv:
         self._dev_events = []                    # device event terms (add_device_event_term): applied by wl_step_terms
         self._term_log_ring = None
         self._critic_terms = []                  # the critic observation group (set_critic_observation)
+        self._policy_terms = []                  # a modified policy observation group (set_policy_observation)
+        self._policy_ring = None
         for name, func, weight, params in self.spec.python_reward_terms:
             self.add_reward_term(name, func, weight, params)
         for name, func, time_out, params in self.spec.python_termination_terms:
@@ -335,6 +340,8 @@ class ManagerBasedRLEnv:
             self.sim.set_reset_events(**{name: True for name in self.spec.reset_events})
         if self.spec.critic_terms:
             self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
+        if self.spec.policy_terms:
+            self.set_policy_observation([(name, fn, {"noise": nz, "clip": cl, "scale": sc}) for name, fn, nz, cl, sc in self.spec.policy_terms])
         # event_manager.apply(mode="startup")
         self.sim.startup()
         self._needs_reset = True
@@ -426,6 +433,35 @@ class ManagerBasedRLEnv:
             self.observation_manager.group_obs_dim.pop("critic", None)
             self.extras.pop("observations", None)
 
+    # -- a modified policy observation group (policy_obs.py, wl_policy_observe; DESIGN 6q) ------------------------------------
+    def set_policy_observation(self, terms):
+        """Replace the built-in ``policy`` row by the concatenation of `terms`, a list of (name, fn, params): `fn` a function
+        of the policy library (IsaacLab's ``root_pos_w``, ``root_euler_xyz``, ``base_lin_vel``, ``base_ang_vel``,
+        ``last_action``, ``joint_vel``, ``joint_pos``, ``projected_gravity`` by name, or ``privileged.wheel_friction`` /
+        ``base_mass`` / ``motor_damping``) or its name; `params` may hold ``noise`` (an ``AdditiveGaussianNoiseCfg`` /
+        ``AdditiveUniformNoiseCfg`` or ``("gaussian", mean, std)`` / ``("uniform", n_min, n_max)``, drawn when the config's
+        enable_corruption is set), ``clip=(lo, hi)`` and ``scale`` (a number or one per float), applied in that order after
+        the value, as IsaacLab's ObservationManager does; anything else in `params` goes to the function.  At most 32 floats,
+        formed on the device.  From then on ``step`` / ``reset`` / ``get_observations`` return that row as ``"policy"`` and
+        ``observation_manager.group_obs_dim["policy"]`` is ``(Dp,)``; ``[]`` restores the built-in row.  Drift family only;
+        it combines with device terms, device events and a critic group, not with host-side Python terms."""
+        from . import policy_obs
+        terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
+        if terms and (self._py_rewards or self._py_terms or self._py_obs or self._py_events):
+            raise NotImplementedError("a policy observation table together with host-side Python terms is not implemented")
+        table = []
+        for name, fn, params in terms:
+            p = dict(params or {})
+            table.append(policy_obs.lower_term(name, fn, p, p.pop("noise", None), p.pop("clip", None), p.pop("scale", None)))
+        policy_obs.check_width(table)
+        dp = self.sim.set_policy_terms(table)    # (refuses a task outside the Drift family)
+        self._policy_terms = terms
+        self._policy_ring = None
+        d = dp or self.spec.obs_dim
+        self.observation_manager.group_obs_dim["policy"] = (d,)
+        self.single_observation_space = {"policy": _Box(-math.inf, math.inf, (d,))}
+        self.observation_space = {"policy": _Box(-math.inf, math.inf, (self.num_envs, d))}
+
     def _obs_groups(self, obs: torch.Tensor) -> dict:
         """The observation dict of the current state: ``policy`` and, with a critic group, a fresh ``critic`` row; the same
         dict is what ``extras["observations"]`` holds then (RslRlVecEnvWrapper's convention, read by the reference's runner)."""
@@ -510,6 +546,8 @@ class ManagerBasedRLEnv:
 
     # -- device terms: the reference's unregistered reward / termination functions, in CUDA (device_terms.py) ---------------
     def _refuse_mixing(self, device: bool = False):
+        if getattr(self, "_policy_terms", None) and not device:
+            raise NotImplementedError("a policy observation table together with host-side Python terms is not implemented")
         if getattr(self, "_critic_terms", None):
             raise NotImplementedError("a critic observation group together with " + ("device terms" if device else "host-side Python terms")
                                       + " is not implemented")
@@ -584,6 +622,8 @@ class ManagerBasedRLEnv:
 
     def add_observation_term(self, name: str, func, params: dict | None = None):
         """Register ``func(env, **params) -> [N, k]``; appended to the policy observation (after the built-in terms)."""
+        if self._policy_terms:
+            raise NotImplementedError("a policy observation table together with host-side Python observation terms is not implemented")
         term = SimpleNamespace(name=name, func=func, params=dict(params or {}))
         k = int(func(self, **term.params).reshape(self.num_envs, -1).shape[1])
         self._py_obs.append(term)
@@ -710,6 +750,11 @@ class ManagerBasedRLEnv:
             obs, rew, term_u8, trunc_u8 = self.sim.step_terms(action, t, out=out, log=log, term_log=term_log)
         else:
             obs, rew, term_u8, trunc_u8 = self.sim.step(action, t, out=out, log=log)
+        if self._policy_terms:                   # the built-in row above is scratch; the table's row is the observation
+            if self._policy_ring is None:
+                self._policy_ring = torch.empty((self._ring_len, self.num_envs, self.sim.policy_obs_dim), dtype=torch.float32,
+                                                device=self.device)
+            obs = self.sim.policy_observe(t, out=self._policy_ring[t % self._ring_len])
         self.common_step_counter = t + 1
         # curriculum: applied by the step kernel's last CTA (uses the incremented counter and fires only if >= 1 env
         # reset, like the reference's call from _reset_idx) -- no host logic, no sync
@@ -736,6 +781,8 @@ class ManagerBasedRLEnv:
         kernel over PCIe (transport "zero_copy")."""
         if self._py_rewards or self._py_terms or getattr(self, "_py_events", None) or self._dev_terms or getattr(self, "_dev_events", None):
             raise NotImplementedError("step_host: Python and device terms need the staged step (use env.step)")
+        if self._policy_terms:
+            raise NotImplementedError("step_host: a policy observation table's row is formed by a second kernel (use env.step)")
         if self._needs_reset:
             self.reset()
         if self._host_io is None:

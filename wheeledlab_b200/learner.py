@@ -506,7 +506,7 @@ class PPOIteration:
         if critic and rollout is not None:
             raise NotImplementedError("a critic observation group with a caller's rollout (device terms, Python terms) is not implemented")
         self.roll = rollout if rollout is not None else FusedPolicyRollout(sim, blob, T, activation=activation, critic=critic)
-        self.ppo = FusedPPO(blob, sim.obs_dim, cfg, activation, exchange=exchange, critic_obs_dim=self.critic_obs_dim)
+        self.ppo = FusedPPO(blob, sim.policy_width, cfg, activation, exchange=exchange, critic_obs_dim=self.critic_obs_dim)
         self.perm = torch.empty(T * sim.num_envs, dtype=torch.int64, device=sim.device)
         self.graph = None
         self.stats = None
@@ -526,8 +526,8 @@ class PPOIteration:
     def _bootstrap(self) -> torch.Tensor:
         from .policy import critic_value
         if self.critic_obs_dim is not None:                    # cobs0 = critic_obs_in[T] once the rollout has run
-            return critic_value(self.blob, self.sim.obs_dim, self.roll.cobs0, "elu", self.critic_obs_dim)
-        return critic_value(self.blob, self.sim.obs_dim, self.roll.obs0, self.ppo.activation)
+            return critic_value(self.blob, self.sim.policy_width, self.roll.cobs0, "elu", self.critic_obs_dim)
+        return critic_value(self.blob, self.sim.policy_width, self.roll.obs0, self.ppo.activation)
 
     def _returns(self):
         slab, cfg = self.roll.slab, self.ppo.cfg
@@ -544,7 +544,7 @@ class PPOIteration:
     def _summarise(self, stats):
         if self.summary is not None:
             from .policy import blob_layout
-            o_std = blob_layout(self.sim.obs_dim, self.critic_obs_dim)[0][12]
+            o_std = blob_layout(self.sim.policy_width, self.critic_obs_dim)[0][12]
             self.summary.copy_(torch.stack([stats["value_function"], stats["surrogate"], stats["entropy"], stats["learning_rate"],
                                             self.blob[o_std:o_std + 2].mean()]))
         return stats
@@ -555,9 +555,7 @@ class PPOIteration:
         if not capture:
             roll.capture(step_counter)
             return self
-        sim.observe(step_counter, 0, out=roll.obs0)
-        if self.critic_obs_dim is not None:
-            sim.critic_observe(out=roll.cobs0)
+        roll.observe0(step_counter)
         sim.set_step_counter(step_counter)
         self.graph = torch.cuda.CUDAGraph()
         s = roll._stream
@@ -670,7 +668,7 @@ class LocalRanksIteration:
                 it.roll.capture(step_counter)
             return self
         for it in its:
-            it.sim.observe(step_counter, 0, out=it.roll.obs0)
+            it.roll.observe0(step_counter)
             it.sim.set_step_counter(step_counter)
         self.graph = torch.cuda.CUDAGraph()
         s = its[0].roll._stream
@@ -768,7 +766,13 @@ class FusedOnPolicyRunner:
     ``observations.critic``) trains the asymmetric network (DESIGN 6m): the critic is ``Linear(Dc, 64)``-first and reads the
     critic row, the iteration is ``PPOIteration(critic=True)`` -- still one graph -- and checkpoints keep rsl_rl's keys with
     ``critic.0.weight`` ``[64, Dc]``, as ``ActorCritic(num_actor_obs, num_critic_obs, ...)`` has it.  On one GPU with the ELU
-    network; with Python terms, device terms, ``activation="relu"`` or a data-parallel world it raises ``NotImplementedError``."""
+    network; with Python terms, device terms, ``activation="relu"`` or a data-parallel world it raises ``NotImplementedError``.
+
+    An env with a policy observation table (``env.set_policy_observation``, or a reference cfg whose ``observations.policy``
+    was lowered with ``device_terms=True``; DESIGN 6q) trains its policy on the table's row: the actor (and, without a critic
+    group, the critic) is ``Linear(Dp, 64)``-first, the rollout runs the policy kernel on the slab row, the step, then
+    ``wl_policy_observe`` into the next slab row, one graph, with device terms, a critic group or data-parallel, and
+    checkpoints keep rsl_rl's keys with ``actor.0.weight`` ``[64, Dp]``."""
 
     @staticmethod
     def settings(train_cfg) -> SimpleNamespace:
@@ -816,7 +820,10 @@ class FusedOnPolicyRunner:
         self.world, self.rank = _data_parallel_world(sim, device)
         self.cfg, self.device, self.log_dir = s.cfg, sim.device, log_dir
         self.num_steps_per_env, self.save_interval, self.activation, self.alg_cfg = s.num_steps_per_env, s.save_interval, s.activation, s.alg_cfg
-        D = sim.obs_dim
+        D = sim.policy_width                          # (the policy table's width, DESIGN 6q, else the built-in row's)
+        if self.activation == "elu" and D > 16:
+            raise NotImplementedError(f"the ELU network takes a policy row of at most 16 floats, not {D} (the policy table's width; "
+                                      'activation="relu" takes up to 32)')
         act = torch.nn.ELU if self.activation == "elu" else torch.nn.ReLU
         mk = lambda out, nin=D: torch.nn.Sequential(torch.nn.Linear(nin, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
         std = torch.full((2,), s.init_noise_std)
@@ -899,13 +906,13 @@ class FusedOnPolicyRunner:
             norm = lambda x: (x.type, x.index if x.index is not None or x.type != "cuda" else torch.cuda.current_device())
             if norm(torch.device(device)) != norm(torch.device(self.device)):
                 raise ValueError(f"device {device} is not the env's device {self.device}: the policy runs where the env's blob is")
-        return InferencePolicy(self.blob, self.env.sim.obs_dim, self.activation, self.critic_obs_dim)
+        return InferencePolicy(self.blob, self.env.sim.policy_width, self.activation, self.critic_obs_dim)
 
     def save(self, path: str, infos=None):
         """rsl_rl's checkpoint: {"model_state_dict", "optimizer_state_dict", "iter", "infos"}."""
         from .policy import actor_critic_state_dict
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-        torch.save({"model_state_dict": actor_critic_state_dict(self.blob, self.env.sim.obs_dim, self.critic_obs_dim),
+        torch.save({"model_state_dict": actor_critic_state_dict(self.blob, self.env.sim.policy_width, self.critic_obs_dim),
                     "optimizer_state_dict": self.alg.optimizer_state_dict(),
                     "iter": self.current_learning_iteration, "infos": infos}, path)
 
@@ -918,7 +925,7 @@ class FusedOnPolicyRunner:
         d = torch.load(path, map_location=self.device)
         if not isinstance(d, dict) or not {"model_state_dict", "iter"} <= set(d) or (load_optimizer and "optimizer_state_dict" not in d):
             raise ValueError(f"{path}: not an rsl_rl checkpoint (model_state_dict, optimizer_state_dict, iter, infos)")
-        D = self.env.sim.obs_dim
+        D = self.env.sim.policy_width
         try:
             w1 = d["model_state_dict"]["critic.0.weight"]
             # playback of an asymmetric checkpoint on an env without the critic group (play_policy.py loads weights only):

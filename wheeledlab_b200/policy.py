@@ -239,9 +239,9 @@ def policy_act_asym(sim: WheeledSim, obs_in: torch.Tensor, critic_obs_in: torch.
     n = sim.num_envs
     if critic_obs_in.dim() != 2 or not 1 <= critic_obs_in.shape[1] <= 32:
         raise ValueError(f"critic_obs_in must have shape [N, Dc] with Dc in 1..32, not {tuple(critic_obs_in.shape)}")
-    _device_tensor("obs_in", obs_in, sim.device, shape=(n, sim.obs_dim))
+    _device_tensor("obs_in", obs_in, sim.device, shape=(n, sim.policy_width))
     _device_tensor("critic_obs_in", critic_obs_in, sim.device, shape=(n, critic_obs_in.shape[1]))
-    _device_tensor("blob", blob, sim.device, shape=(blob_layout(sim.obs_dim, critic_obs_in.shape[1])[1],))
+    _device_tensor("blob", blob, sim.device, shape=(blob_layout(sim.policy_width, critic_obs_in.shape[1])[1],))
     for name, t, shape in (("actions", actions, (n, 2)), ("mean", mean, (n, 2)), ("log_prob", log_prob, (n,)), ("value", value, (n,))):
         _device_tensor(name, t, sim.device, shape=shape)
     po = WlPolicyOut(actions.data_ptr(), mean.data_ptr(), log_prob.data_ptr(), value.data_ptr())
@@ -267,7 +267,13 @@ class FusedPolicyRollout:
     ``critic=True`` rolls out the asymmetric network on a handle that has a critic table (``sim.set_critic_terms``): T x
     (``policy_act_asym``, ``wl_step``, ``wl_critic_observe`` into row k + 1) on device counters, one graph.
     ``slab.critic_obs_in`` [T + 1, N, Dc] holds the critic rows: row k is what ``values[k]`` was computed from, row T the
-    bootstrap row.  The blob is laid out by ``blob_layout(obs_dim, Dc)``.  "elu" only, and not with device terms."""
+    bootstrap row.  The blob is laid out by ``blob_layout(obs_dim, Dc)``.  "elu" only, and not with device terms.
+
+    On a handle with a policy observation table (``sim.set_policy_terms``, DESIGN 6q) every step is the policy kernel of the
+    network on ``slab.obs_in[k]`` (``wl_policy_act_elu`` / ``wl_policy_act`` / ``wl_policy_act_asym``, or ``wl_actor_mean``
+    when deterministic), the step writing its built-in row to a scratch buffer, then ``wl_policy_observe`` into
+    ``slab.obs[k]`` = ``obs_in[k + 1]`` (and ``wl_critic_observe`` with a critic), still one graph; the slab and the blob
+    are sized by the table's width."""
 
     def __init__(self, sim: WheeledSim, blob: torch.Tensor, T: int = 128, slab: RolloutSlab | None = None, activation: str = "elu",
                  deterministic: bool = False, device_terms: bool = False, critic: bool = False):
@@ -293,8 +299,12 @@ class FusedPolicyRollout:
         self.term_logs = torch.zeros((T, 8), dtype=torch.float32, device=sim.device) if self.device_terms else None
         if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
             raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
-        self.slab = slab or RolloutSlab(T, sim.num_envs, sim.obs_dim, 2, sim.device, policy_fields=not self.deterministic,
+        self.table = sim.policy_obs_dim > 0
+        D = sim.policy_width
+        self.slab = slab or RolloutSlab(T, sim.num_envs, D, 2, sim.device, policy_fields=not self.deterministic,
                                         critic_obs_dim=sim.critic_obs_dim if self.critic else None)
+        # with a table the step's built-in row is scratch: the policy reads wl_policy_observe's row
+        self._scratch = torch.empty((sim.num_envs, sim.obs_dim), dtype=torch.float32, device=sim.device) if self.table else None
         # values / log-prob / mean go straight into the slab (= the all-gather send buffer) when it has those fields
         if self.deterministic:
             self.pol = None
@@ -304,7 +314,7 @@ class FusedPolicyRollout:
         self.logs = torch.zeros((T, 16), dtype=torch.float32, device=sim.device)
         # slab.obs_in[k] = the observation actions[k] / log_prob[k] / values[k] / mean[k] were computed from (rsl_rl
         # RolloutStorage.observations[k]); slab.obs[k] = obs_in[k+1] = what step k returned
-        self.obs0 = torch.empty((sim.num_envs, sim.obs_dim), dtype=torch.float32, device=sim.device)    # carried to the next replay
+        self.obs0 = torch.empty((sim.num_envs, D), dtype=torch.float32, device=sim.device)    # carried to the next replay
         if self.critic:
             if self.slab.critic_obs_in is None or tuple(self.slab.critic_obs_in.shape) != (T + 1, sim.num_envs, sim.critic_obs_dim):
                 raise ValueError(f"critic=True needs a slab built with critic_obs_dim={sim.critic_obs_dim}")
@@ -313,13 +323,46 @@ class FusedPolicyRollout:
         self._base = 0
         self._stream = torch.cuda.Stream(device=sim.device)
 
+    def _step_outputs(self, k: int):
+        """What the step writes at k: the slab's row k, or with a table the scratch row (the table's row follows it)."""
+        if not self.table:
+            return self.slab.step_outputs(k)
+        return (self._scratch,) + self.slab.step_outputs(k)[1:]
+
+    def _table_step(self, k: int, t: int):
+        """Step k on a handle with a policy table: the policy kernel, the step into scratch, the table's row into obs_in[k+1]."""
+        slab, sim, D = self.slab, self.sim, self.sim.policy_width
+        if self.deterministic:
+            actor_mean(self.blob, D, slab.obs_in[k], self.activation, out=slab.actions[k])
+        elif self.critic:
+            policy_act_asym(sim, slab.obs_in[k], slab.critic_obs_in[k], self.blob, slab.actions[k], self.pol.mean[k],
+                            self.pol.log_prob[k], self.pol.values[k], t)
+        else:
+            policy_act(sim, slab.obs_in[k], self.blob, slab.actions[k], self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t,
+                       self.activation)
+        if self.device_terms:
+            sim.step_terms(slab.actions[k], t, out=self._step_outputs(k), log=self.logs[k], term_log=self.term_logs[k])
+        else:
+            sim.step(slab.actions[k], t, out=self._step_outputs(k), log=self.logs[k])
+        sim.policy_observe(t, out=slab.obs[k])
+        if self.critic:
+            sim.critic_observe(out=slab.critic_obs_in[k + 1])
+
+    def observe0(self, step_counter: int):
+        """The first rollout row (observation_manager.compute at `step_counter`, call 0) into obs0 (and cobs0)."""
+        self.sim.observe_policy_row(step_counter, 0, self.obs0)
+        if self.critic:
+            self.sim.critic_observe(out=self.cobs0)
+
     def _body(self):
         self.slab.obs_in[0].copy_(self.obs0)
         if self.critic:
             self.slab.critic_obs_in[0].copy_(self.cobs0)
         for k in range(self.T):
             t = WheeledSim.device_counter_plus(k)
-            if self.critic:
+            if self.table:
+                self._table_step(k, t)
+            elif self.critic:
                 policy_act_asym(self.sim, self.slab.obs_in[k], self.slab.critic_obs_in[k], self.blob, self.slab.actions[k],
                                 self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t)
                 self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
@@ -349,9 +392,7 @@ class FusedPolicyRollout:
 
     def capture(self, step_counter: int):
         sim = self.sim
-        sim.observe(step_counter, 0, out=self.obs0)
-        if self.critic:
-            sim.critic_observe(out=self.cobs0)
+        self.observe0(step_counter)
         sim.set_step_counter(step_counter)
         self.graph = torch.cuda.CUDAGraph()
         s = self._stream

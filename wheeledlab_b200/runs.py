@@ -30,11 +30,16 @@ def task_activation(task: str) -> str:
     return "relu" if name in ("elevation", "visual", "visual_random") else "elu"
 
 
-def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict) -> str:
+def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict, policy_terms=None) -> str:
+    """`policy_terms`: the env's policy observation table (``(name, library term, noise, clip, scale)`` as
+    ``TaskSpec.policy_terms`` holds it), so that playback observes what the policy was trained on; None: the built-in row."""
     os.makedirs(log_dir, exist_ok=True)
     path = os.path.join(log_dir, RUN_CONFIG)
+    cfg = {"task": task, "num_envs": int(num_envs), "seed": int(seed), "agent_cfg": agent}
+    if policy_terms:
+        cfg["policy_terms"] = [list(t) for t in policy_terms]
     with open(path, "w") as f:
-        json.dump({"task": task, "num_envs": int(num_envs), "seed": int(seed), "agent_cfg": agent}, f, indent=1)
+        json.dump(cfg, f, indent=1)
     return path
 
 

@@ -409,6 +409,64 @@ class WheeledSim:
         check(lib.wl_critic_observe(self._h, C.c_void_p(obs.data_ptr()), _stream_ptr(self.device)), "wl_critic_observe")
         return obs
 
+    def set_policy_terms(self, terms) -> int:
+        """The handle's policy observation table (wl_set_policy_terms): a list of ``(library name, noise, clip, scale)``
+        (``policy_obs.lower_term``'s form; a bare name is a term without noise, clip or scale), concatenated in this order
+        into the policy row; [] clears it.  Returns Dp.  Nothing is launched; a graph captured earlier keeps its table."""
+        terms = [(t, None, None, None) if isinstance(t, str) else tuple(t) + (None,) * (4 - len(t)) for t in terms]
+        arr = (_lib.WlPolicyTerm * max(1, len(terms)))()
+        for k, (name, noise, clip, scale) in enumerate(terms):
+            if name not in _lib.WL_POLICY_TERMS:
+                raise ValueError(f"policy term {name!r} is not in the library {sorted(_lib.WL_POLICY_TERMS)}")
+            if noise is not None and noise[0] not in _lib.WL_NOISE:
+                raise ValueError(f"policy term {name!r}: unknown noise model {noise[0]!r}")
+            d = arr[k]
+            d.kind = _lib.WL_POLICY_TERMS[name][0]
+            if noise is not None:
+                d.noise = _lib.WL_NOISE[noise[0]]
+                d.noise_params[0], d.noise_params[1] = float(noise[1]), float(noise[2])
+            if clip is not None:
+                d.clip = 1
+                d.clip_range[0], d.clip_range[1] = float(clip[0]), float(clip[1])
+            if scale is not None:
+                scale = (float(scale),) if isinstance(scale, (int, float)) else tuple(float(s) for s in scale)
+                d.n_scale = len(scale)
+                for j, s in enumerate(scale[:4]):
+                    d.scale[j] = s
+        check(lib.wl_set_policy_terms(self._h, arr, len(terms)), "wl_set_policy_terms")
+        return self.policy_obs_dim
+
+    @property
+    def policy_obs_dim(self) -> int:
+        """Dp, the width of the policy row of the handle's table (0 without one; sim.obs_dim stays the built-in width)."""
+        return int(lib.wl_policy_obs_dim(self._h))
+
+    @property
+    def policy_width(self) -> int:
+        """The width of the row the policy reads: Dp with a policy table, else obs_dim (the policy kernels read the same)."""
+        return self.policy_obs_dim or self.obs_dim
+
+    def observe_policy_row(self, step_counter: int, call_idx: int, out: torch.Tensor) -> torch.Tensor:
+        """observation_manager.compute()'s policy row into `out` [N, policy_width]: wl_observe, or with a policy table
+        wl_policy_observe at the same call index."""
+        if self.policy_obs_dim:
+            return self.policy_observe(step_counter, call_idx, out=out)
+        return self.observe(step_counter, call_idx, out=out)
+
+    def policy_observe(self, step_counter: int, call_idx: int | None = None, out: torch.Tensor | None = None) -> torch.Tensor:
+        """The policy row [N, Dp] of the table (wl_policy_observe) from the current state: with call_idx None the row of the
+        step just taken at `step_counter` (a host value or WL_DEVICE_COUNTER_PLUS(k)), else the row of
+        observe(step_counter, call_idx).  Capturable."""
+        dp = self.policy_obs_dim
+        obs = out if out is not None else torch.empty((self.num_envs, dp), dtype=torch.float32, device=self.device)
+        if dp and (obs.dtype != torch.float32 or tuple(obs.shape) != (self.num_envs, dp) or not obs.is_contiguous()
+                   or not obs.is_cuda or obs.device.index != self.device.index):
+            raise ValueError(f"out must be a contiguous float32 [{self.num_envs}, {dp}] tensor on {self.device} (the table's row "
+                             f"is {dp} floats wide), not {obs.dtype} {tuple(obs.shape)} on {obs.device}")
+        ci = _lib.WL_POLICY_OBS_AFTER_STEP if call_idx is None else int(call_idx)
+        check(lib.wl_policy_observe(self._h, step_counter, ci, C.c_void_p(obs.data_ptr()), _stream_ptr(self.device)), "wl_policy_observe")
+        return obs
+
     def observe(self, step_counter: int, call_idx: int = 0, out: torch.Tensor | None = None):
         obs = out if out is not None else torch.empty((self.num_envs, self.obs_dim), dtype=torch.float32, device=self.device)
         check(lib.wl_observe(self._h, C.c_void_p(obs.data_ptr()), step_counter, call_idx, _stream_ptr(self.device)),

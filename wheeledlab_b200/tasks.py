@@ -71,6 +71,9 @@ class TaskSpec:
     device_events: list = field(default_factory=list)
     # the critic observation group (privileged.py, wl_critic_observe): [(name, library term, clip)] in row order; [] = none
     critic_terms: list = field(default_factory=list)
+    # a modified policy observation group (policy_obs.py, wl_policy_observe): [(name, library term, noise, clip, scale)] in row
+    # order; [] = the built-in row.  obs_dim stays the built-in row's width; the policy side is sized by the table's
+    policy_terms: list = field(default_factory=list)
     # DR events in IsaacLab's mode="reset" (wl_set_reset_events): names of _lib.WL_RESET_EVENTS; [] = start-up DR only
     reset_events: list = field(default_factory=list)
 
