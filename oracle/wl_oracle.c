@@ -68,6 +68,11 @@ static inline real r_clamp(real x, real lo, real hi) { return r_min(r_max(x, lo)
 #define RNG_CMD 8u
 #define RNG_CAM 10u
 #define RNG_CAM_EXTRA 11u
+#define RNG_RESET_DR 12u
+#define RNG_EVENT 13u
+#define RNG_EVENT_INIT 14u
+#define RNG_DEVICE_EVENT 15u
+#define RNG_POLICY_OBS 16u
 
 static void philox4x32(uint64_t seed, uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t out[4]) {
     uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
@@ -246,6 +251,7 @@ typedef struct wlo_sim {
     uint8_t* vis_map;         /* visual: traversability map [rows, cols] */
     struct wlo_dterms* dt;    /* wlo_set_device_terms: the term table and its per-env state (NULL: none) */
     int32_t dt_run;           /* set by wlo_step_terms: env_step runs the device terms between E and F */
+    uint32_t reset_ev;        /* wlo_set_reset_events: WL_RESET_EV_* events redrawn at every reset (0: start-up only) */
 } wlo_sim;
 
 static inline real dot3(real ax, real ay, real az, real bx, real by, real bz) { return fm(ax, bx, fm(ay, by, az * bz)); }
@@ -1263,6 +1269,35 @@ int wlo_is_double(void) {
 #endif
 }
 
+/* the DR parameters of one env from its four Philox blocks: r0 friction buckets, r1 actuator gains, r2 base mass, r3 wheel
+ * masses (dr_params in wl_reset_dr.cuh, for wl_startup_kernel and wl_reset_dr_kernel) */
+static void dr_params(const wl_config* c, wlo_env* e, const uint32_t r0[4], const uint32_t r1[4], const uint32_t r2[4], const uint32_t r3[4]) {
+    for (int i = 0; i < 4; ++i) {
+        uint32_t bk = 0;
+        if (c->dr_enable && c->dr_num_buckets > 1) bk = (uint32_t)(((uint64_t)r0[i] * (uint64_t)c->dr_num_buckets) >> 32);
+        e->D[i] = (real)c->dr_bucket_D[bk];
+        e->C[i] = (real)c->dr_bucket_C[bk];
+        e->kd[i] = (real)c->dc_damping[i];
+        if (c->dr_enable && ((c->dr_kd_mask >> i) & 1)) e->kd[i] = uniform(r1[i], (real)c->dr_kd_range[0], (real)c->dr_kd_range[1]);
+    }
+    /* randomize_rigid_body_mass [UPSTREAM-RECALL]: "add" -> base_link mass += U; "abs" -> base_link mass := U
+     * (mushr_visual_env_cfg.py:280-288); wheel links := U (:290-299), their inertia rescaled by the mass ratio */
+    e->mass = (real)c->mass_nominal;
+    for (int i = 0; i < 4; ++i) e->inv_Iw[i] = (real)c->d_inv_Iw;
+    if (c->dr_enable) {
+        real u = uniform(r2[0], (real)c->dr_mass_add[0], (real)c->dr_mass_add[1]);
+        if (c->dr_mass_mode == 0) e->mass = e->mass + u;
+        else e->mass = (e->mass - (real)c->dr_base_mass_nominal) + u;
+        if (c->dr_wheel_mass_enable)
+            for (int i = 0; i < 4; ++i) {
+                real mw = uniform(r3[i], (real)c->dr_wheel_mass[0], (real)c->dr_wheel_mass[1]);
+                e->mass = e->mass + (mw - (real)c->wheel_mass_nominal);
+                e->inv_Iw[i] = (real)c->d_inv_Iw * ((real)c->wheel_mass_nominal / mw);
+            }
+    }
+    e->inv_mass = K(1.0) / e->mass;
+}
+
 /* startup events a14: material buckets, actuator gains, base mass; initial interval timers */
 int wlo_startup(wlo_sim* s) {
     const wl_config* c = &s->cfg;
@@ -1274,34 +1309,30 @@ int wlo_startup(wlo_sim* s) {
         philox4x32(c->seed, gid, 0u, RNG_STARTUP, 1u, r1);
         philox4x32(c->seed, gid, 0u, RNG_STARTUP, 2u, r2);
         philox4x32(c->seed, gid, 0u, RNG_STARTUP, 3u, r3);
-        for (int i = 0; i < 4; ++i) {
-            uint32_t bk = 0;
-            if (c->dr_enable && c->dr_num_buckets > 1) bk = (uint32_t)(((uint64_t)r0[i] * (uint64_t)c->dr_num_buckets) >> 32);
-            e->D[i] = (real)c->dr_bucket_D[bk];
-            e->C[i] = (real)c->dr_bucket_C[bk];
-            e->kd[i] = (real)c->dc_damping[i];
-            if (c->dr_enable && ((c->dr_kd_mask >> i) & 1)) e->kd[i] = uniform(r1[i], (real)c->dr_kd_range[0], (real)c->dr_kd_range[1]);
-        }
-        /* randomize_rigid_body_mass [UPSTREAM-RECALL]: "add" -> base_link mass += U; "abs" -> base_link mass := U
-         * (mushr_visual_env_cfg.py:280-288); wheel links := U (:290-299), their inertia rescaled by the mass ratio */
-        e->mass = (real)c->mass_nominal;
-        for (int i = 0; i < 4; ++i) e->inv_Iw[i] = (real)c->d_inv_Iw;
-        if (c->dr_enable) {
-            real u = uniform(r2[0], (real)c->dr_mass_add[0], (real)c->dr_mass_add[1]);
-            if (c->dr_mass_mode == 0) e->mass = e->mass + u;
-            else e->mass = (e->mass - (real)c->dr_base_mass_nominal) + u;
-            if (c->dr_wheel_mass_enable)
-                for (int i = 0; i < 4; ++i) {
-                    real mw = uniform(r3[i], (real)c->dr_wheel_mass[0], (real)c->dr_wheel_mass[1]);
-                    e->mass = e->mass + (mw - (real)c->wheel_mass_nominal);
-                    e->inv_Iw[i] = (real)c->d_inv_Iw * ((real)c->wheel_mass_nominal / mw);
-                }
-        }
-        e->inv_mass = K(1.0) / e->mass;
+        dr_params(c, e, r0, r1, r2, r3);
         sample_interval_timers(c, e, r2[1], r2[2]);
         e->q[0] = K(1.0); e->q[1] = e->q[2] = e->q[3] = K(0.0);
     }
     return 0;
+}
+
+/* wl_reset_dr_kernel for env li reset by the call with counter t: block k from the reset key when event k is in reset mode,
+ * else from the start-up key; only the named events' parameters are written */
+static void redraw_dr(wlo_sim* s, int li, uint32_t t) {
+    const wl_config* c = &s->cfg;
+    const uint32_t m = s->reset_ev, gid = (uint32_t)(c->env_id_offset + li);
+    uint32_t r[4][4];
+    for (uint32_t k = 0; k < 4; ++k) {
+        if ((m >> k) & 1u) philox4x32(c->seed, gid, t, RNG_RESET_DR, k, r[k]);
+        else philox4x32(c->seed, gid, 0u, RNG_STARTUP, k, r[k]);
+    }
+    wlo_env* e = &s->env[li];
+    wlo_env d = *e;
+    dr_params(c, &d, r[0], r[1], r[2], r[3]);
+    if (m & WL_RESET_EV_MATERIAL) for (int i = 0; i < 4; ++i) { e->D[i] = d.D[i]; e->C[i] = d.C[i]; }
+    if (m & WL_RESET_EV_ACTUATOR_GAINS) for (int i = 0; i < 4; ++i) e->kd[i] = d.kd[i];
+    if (m & (WL_RESET_EV_BASE_MASS | WL_RESET_EV_WHEEL_MASS)) { e->mass = d.mass; e->inv_mass = d.inv_mass; e->spare0 = e->spare1 = K(0.0); }
+    if (m & WL_RESET_EV_WHEEL_MASS) for (int i = 0; i < 4; ++i) e->inv_Iw[i] = d.inv_Iw[i];
 }
 
 int wlo_reset(wlo_sim* s, const int64_t* env_ids, int32_t n_ids, int64_t step_counter) {
@@ -1312,6 +1343,7 @@ int wlo_reset(wlo_sim* s, const int64_t* env_ids, int32_t n_ids, int64_t step_co
         if (c->task == WL_TASK_ELEVATION) elev_reset_env(c, &s->env[li], (uint32_t)(c->env_id_offset + li), step_counter);
         else if (c->task == WL_TASK_VISUAL) visual_reset_env(s, &s->env[li], (uint32_t)(c->env_id_offset + li), step_counter);
         else drift_reset_env(c, &s->env[li], (uint32_t)(c->env_id_offset + li), step_counter);
+        if (s->reset_ev) redraw_dr(s, li, (uint32_t)step_counter);
     }
     return 0;
 }
@@ -1362,6 +1394,9 @@ int wlo_step(wlo_sim* s, const float* action, float* obs, float* rew, uint8_t* t
             }
         }
     }
+    if (s->reset_ev)      /* wl_reset_dr_kernel after the step: the envs it reset are those it left at episode length 0 */
+        for (int li = 0; li < c->num_envs; ++li)
+            if (s->env[li].ep_len == 0) redraw_dr(s, li, (uint32_t)step_counter);
     return err;
 }
 
@@ -1383,7 +1418,8 @@ int wlo_set_device_terms(wlo_sim* s, const wl_term_desc* terms, int32_t n_terms)
     s->dt = dt;
     return 0;
 }
-/* wl_step_terms (with a term log): wlo_step with the device terms between E and F; no terms: wlo_step itself */
+/* wl_step_terms (with a term log): wlo_step with the device terms between E and F; no terms: wlo_step itself.  Either way
+ * wlo_step applies the reset-mode DR redraw. */
 int wlo_step_terms(wlo_sim* s, const float* action, float* obs, float* rew, uint8_t* terminated, uint8_t* truncated,
                    int64_t step_counter, int nthreads) {
     if (!s->dt) return wlo_step(s, action, obs, rew, terminated, truncated, step_counter, nthreads);
@@ -1439,6 +1475,166 @@ int wlo_device_terms(const wl_config* c, const uint8_t* map, const wl_term_desc*
     free(contrib); free(ksums);
     return 0;
 }
+
+/* The feature entry points below are compiled only when this file is its own translation unit.  A test file that
+ * #includes this one and defines these entry points itself (with its own helpers of the same names) keeps compiling. */
+#if __INCLUDE_LEVEL__ == 0
+
+/* wl_set_reset_events: the same refusals (WL_EINVAL, the mask unchanged) */
+int wlo_set_reset_events(wlo_sim* s, uint32_t mask) {
+    const wl_config* c = &s->cfg;
+    const uint32_t all = WL_RESET_EV_MATERIAL | WL_RESET_EV_ACTUATOR_GAINS | WL_RESET_EV_BASE_MASS | WL_RESET_EV_WHEEL_MASS;
+    if ((mask & ~all) || (mask && !c->dr_enable) || ((mask & WL_RESET_EV_ACTUATOR_GAINS) && c->dr_kd_mask == 0) ||
+        ((mask & WL_RESET_EV_WHEEL_MASS) && !c->dr_wheel_mass_enable))
+        return WL_EINVAL;
+    s->reset_ev = mask;
+    return 0;
+}
+
+/* ------------------------------------------------------------------------- */
+/* interval timers of host-side event terms (wl_set_event_timers, wl_event_timers_kernel; DESIGN.md 6o)        */
+/* ------------------------------------------------------------------------- */
+/* wlo_event_timers_init is the construction draw, wlo_event_timers one step of every term: redraw where done, subtract
+ * step_dt, fire below 1e-6, redraw where fired -- each fp32 operation in the kernel's order (u * (hi - lo) + lo, no fma) */
+static float event_interval(uint32_t x, float lo, float hi) { return (float)u01(x) * (hi - lo) + lo; }
+
+void wlo_event_timers_init(uint64_t seed, int32_t env_id_offset, int32_t n, int32_t n_terms, const float* lo_hi, float* time_left) {
+    for (int k = 0; k < n_terms; ++k)
+        for (int i = 0; i < n; ++i) {
+            uint32_t r[4];
+            philox4x32(seed, (uint32_t)(env_id_offset + i), 0u, RNG_EVENT_INIT, (uint32_t)k, r);
+            time_left[(size_t)k * n + i] = event_interval(r[0], lo_hi[2 * k], lo_hi[2 * k + 1]);
+        }
+}
+
+void wlo_event_timers(uint64_t seed, int32_t env_id_offset, int32_t n, int32_t n_terms, const float* lo_hi, float step_dt,
+                      const uint8_t* done, float* time_left, uint8_t* fired, int64_t step_counter) {
+    for (int k = 0; k < n_terms; ++k)
+        for (int i = 0; i < n; ++i) {
+            const size_t o = (size_t)k * n + i;
+            const float lo = lo_hi[2 * k], hi = lo_hi[2 * k + 1];
+            uint32_t r[4];
+            philox4x32(seed, (uint32_t)(env_id_offset + i), (uint32_t)step_counter, RNG_EVENT, (uint32_t)k, r);
+            float tl = time_left[o];
+            if (done[i]) tl = event_interval(r[0], lo, hi);
+            tl = tl - step_dt;
+            fired[o] = tl < 1.0e-6f;
+            if (fired[o]) tl = event_interval(r[1], lo, hi);
+            time_left[o] = tl;
+        }
+}
+
+/* ------------------------------------------------------------------------- */
+/* device event terms (wl_set_device_events, wl_device_events_kernel; DESIGN.md 6p)                           */
+/* ------------------------------------------------------------------------- */
+/* IsaacLab's push_by_setting_velocity per term k, in table order: a reset-mode term fires where the env was reset, an
+ * interval-mode term where its timer (wlo_event_timers, on the term's own timer index) ran out; a fired term adds
+ * u * (hi - lo) + lo to each of the six root velocity components, u from the key (seed, env_id_offset + i, t, stream 15, k)
+ * for x, y, z, roll and (..., 8 + k) for pitch, yaw.  Each fp32 operation in the kernel's order (no fma).
+ * vel [n][6] (x, y, z, roll, pitch, yaw) in place; slot[k] the timer index of term k or -1 (reset mode); lo / hi [n_terms][6];
+ * timer_lo_hi [n_timers][2] and time_left [n_timers][n] as wlo_event_timers takes them. */
+void wlo_device_events(uint64_t seed, int32_t env_id_offset, int32_t n, int32_t n_terms, const int32_t* slot, const float* lo,
+                       const float* hi, int32_t n_timers, const float* timer_lo_hi, float step_dt, const uint8_t* done,
+                       float* time_left, float* vel, int64_t step_counter) {
+    uint8_t* fired = (uint8_t*)calloc((size_t)(n_timers > 0 ? n_timers : 1) * n, 1);
+    if (n_timers > 0)
+        wlo_event_timers(seed, env_id_offset, n, n_timers, timer_lo_hi, step_dt, done, time_left, fired, step_counter);
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < n_terms; ++k) {
+            const int f = slot[k] < 0 ? done[i] != 0 : fired[(size_t)slot[k] * n + i] != 0;
+            if (!f) continue;
+            uint32_t a[4], b[4];
+            philox4x32(seed, (uint32_t)(env_id_offset + i), (uint32_t)step_counter, RNG_DEVICE_EVENT, (uint32_t)k, a);
+            philox4x32(seed, (uint32_t)(env_id_offset + i), (uint32_t)step_counter, RNG_DEVICE_EVENT, (uint32_t)(WL_MAX_DEVICE_EVENTS + k), b);
+            const uint32_t r[6] = {a[0], a[1], a[2], a[3], b[0], b[1]};
+            for (int j = 0; j < 6; ++j)
+                vel[(size_t)i * 6 + j] = vel[(size_t)i * 6 + j] + event_interval(r[j], lo[k * 6 + j], hi[k * 6 + j]);
+        }
+    free(fired);
+}
+
+/* ------------------------------------------------------------------------- */
+/* policy observation table (wl_set_policy_terms, wl_policy_observe_kernel; DESIGN.md 6q)                      */
+/* ------------------------------------------------------------------------- */
+/* For every env i and output column j: the library float src[j] of the state groups st [WL_NUM_GROUPS][n][4] (the device
+ * state's layout), then, when corrupt, the column's additive noise keyed as the header documents, then the clip (r_clamp),
+ * then the scale -- each fp32 operation in the kernel's order (no fma). */
+/* the 32 library floats of env i: the critic library's 29 (root_pos_w, root_euler_xyz, base_lin_vel, base_ang_vel,
+ * last_action, joint_vel, joint_pos, wheel_friction, base_mass, motor_damping) then projected_gravity */
+static void pobs_library(const float* st, int32_t n, int i, float o[32]) {
+    const float* g[WL_NUM_GROUPS];
+    for (int k = 0; k < WL_NUM_GROUPS; ++k) g[k] = st + ((size_t)k * n + i) * 4;
+    const real q[4] = {g[WL_G_QUAT][0], g[WL_G_QUAT][1], g[WL_G_QUAT][2], g[WL_G_QUAT][3]};
+    real R[9], eu[3], vb[3], wb[3], gb[3];
+    const real v[3] = {g[WL_G_LINVEL][0], g[WL_G_LINVEL][1], g[WL_G_LINVEL][2]};
+    const real w[3] = {g[WL_G_ANGVEL][0], g[WL_G_ANGVEL][1], g[WL_G_ANGVEL][2]};
+    const real down[3] = {0.0f, 0.0f, -1.0f};
+    rotmat(q, R);
+    euler_xyz(q, eu);
+    rotT(R, v, vb);
+    rotT(R, w, wb);
+    rotT(R, down, gb);
+    for (int k = 0; k < 3; ++k) {
+        o[k] = g[WL_G_POS][k]; o[3 + k] = eu[k]; o[6 + k] = vb[k]; o[9 + k] = wb[k]; o[29 + k] = gb[k];
+    }
+    o[12] = g[WL_G_ACTION][0]; o[13] = g[WL_G_ACTION][1];
+    for (int k = 0; k < 4; ++k) {
+        o[14 + k] = g[WL_G_WHEEL][k]; o[20 + k] = g[WL_G_PMU_D][k]; o[25 + k] = g[WL_G_PKD][k];
+    }
+    o[18] = g[WL_G_STEER][0]; o[19] = g[WL_G_STEER][1];
+    o[24] = g[WL_G_PMASS][0];
+}
+
+/* library [n][32] of every env, for the numpy restatement */
+void wlo_policy_library(const float* st, int32_t n, float* out) {
+    for (int i = 0; i < n; ++i) pobs_library(st, n, i, out + (size_t)i * 32);
+}
+
+/* the noise draw of column j: z ~ N(0, 1) (Gaussian) or u in [0, 1) (uniform), keyed as the header documents */
+float wlo_policy_obs_draw(uint64_t seed, uint32_t gid, uint32_t t, int32_t call_idx, int32_t j, int32_t kind) {
+    uint32_t r[4];
+    if (kind == WL_NOISE_GAUSSIAN && j < 12)
+        philox4x32(seed, gid, t, call_idx < 0 ? RNG_OBS : RNG_OBS_EXTRA, (call_idx < 0 ? 0u : 3u * (uint32_t)call_idx) + (uint32_t)(j / 4), r);
+    else
+        philox4x32(seed, gid, t, RNG_POLICY_OBS, 16u * (uint32_t)(call_idx + 1) + (kind == WL_NOISE_UNIFORM ? 8u : 0u) + (uint32_t)(j / 4), r);
+    const int w = j % 4;
+    if (kind == WL_NOISE_UNIFORM) return u01(r[w]);
+    real z0, z1;
+    box_muller(r[w < 2 ? 0 : 2], r[w < 2 ? 1 : 3], &z0, &z1);
+    return (float)((w & 1) ? z1 : z0);
+}
+
+/* out [n][dp]; per column: src, noise (0 none, 1 Gaussian (na, nb) = (mean, std), 2 uniform (na, nb) = (n_min, n_max - n_min)),
+ * clip flag with [lo, hi], scale flag with scale.  call_idx = -1: the row after the step at t; >= 0: an observe call. */
+void wlo_policy_observe(uint64_t seed, int32_t env_id_offset, int32_t n, const float* st, int32_t dp, const uint8_t* src,
+                        const uint8_t* noise, const float* na, const float* nb, const uint8_t* has_clip, const float* lo,
+                        const float* hi, const uint8_t* has_scale, const float* scale, int32_t corrupt, uint32_t t,
+                        int32_t call_idx, float* out) {
+    for (int i = 0; i < n; ++i) {
+        float lib[32];
+        pobs_library(st, n, i, lib);
+        const uint32_t gid = (uint32_t)(env_id_offset + i);
+        for (int j = 0; j < dp; ++j) {
+            float x = lib[src[j]];
+            if (corrupt && noise[j]) {
+                const float d = wlo_policy_obs_draw(seed, gid, t, call_idx, j, noise[j]);
+                if (noise[j] == WL_NOISE_GAUSSIAN) {
+                    const float v = x + na[j];
+                    const float s = nb[j] * d;
+                    x = v + s;
+                } else {
+                    const float s = d * nb[j];
+                    const float v = x + s;
+                    x = v + na[j];
+                }
+            }
+            if (has_clip[j]) x = r_clamp(x, lo[j], hi[j]);
+            if (has_scale[j]) x = x * scale[j];
+            out[(size_t)i * dp + j] = x;
+        }
+    }
+}
+#endif  /* __INCLUDE_LEVEL__ == 0 */
 
 int wlo_observe(wlo_sim* s, float* obs, int64_t step_counter, int32_t call_idx) {
     const wl_config* c = &s->cfg;

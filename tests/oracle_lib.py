@@ -62,6 +62,14 @@ def _load(path):
     lib.wlo_step_terms.argtypes = [vp, vp, vp, vp, vp, vp, i64, i32]
     lib.wlo_get_device_terms.argtypes = [vp, vp, vp, vp, vp]
     lib.wlo_device_terms.argtypes = [vp, vp, vp, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp]
+    lib.wlo_set_reset_events.argtypes = [vp, u32]
+    lib.wlo_event_timers_init.argtypes = [u64, i32, i32, i32, vp, vp]
+    lib.wlo_event_timers.argtypes = [u64, i32, i32, i32, vp, C.c_float, vp, vp, vp, i64]
+    lib.wlo_device_events.argtypes = [u64, i32, i32, i32, vp, vp, vp, i32, vp, C.c_float, vp, vp, vp, i64]
+    lib.wlo_policy_observe.argtypes = [u64, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, u32, i32, vp]
+    lib.wlo_policy_library.argtypes = [vp, i32, vp]
+    lib.wlo_policy_obs_draw.argtypes = [u64, u32, u32, i32, i32, i32]
+    lib.wlo_policy_obs_draw.restype = C.c_float
     lib.wlo_config_describe.restype = C.c_char_p
     return lib
 
@@ -152,6 +160,116 @@ def device_terms(cfg, terms, state, done, t, vis_map=None, prev=None, sums=None,
     return out
 
 
+def event_timers_init(seed, env_id_offset, n, ranges) -> np.ndarray:
+    """wlo_event_timers_init: the interval timers [n_terms, N] f32 of (lo, hi) ranges as wl_set_event_timers draws them."""
+    lo_hi = np.ascontiguousarray(ranges, dtype=np.float32).reshape(-1)
+    tl = np.zeros((len(ranges), n), dtype=np.float32)
+    get_lib().wlo_event_timers_init(seed, env_id_offset, n, len(ranges), _p(lo_hi), _p(tl))
+    return tl
+
+
+def event_timers_step(seed, env_id_offset, ranges, step_dt, done, time_left, step_counter):
+    """wlo_event_timers: one step in place on time_left; returns fired [n_terms, N] u8."""
+    lo_hi = np.ascontiguousarray(ranges, dtype=np.float32).reshape(-1)
+    n = time_left.shape[1]
+    done = np.ascontiguousarray(done, dtype=np.uint8)
+    fired = np.zeros(time_left.shape, dtype=np.uint8)
+    get_lib().wlo_event_timers(seed, env_id_offset, n, len(ranges), _p(lo_hi), np.float32(step_dt), _p(done), _p(time_left),
+                               _p(fired), step_counter)
+    return fired
+
+
+# A device event table is a list of (mode, interval_range_s or None, six (lo, hi) velocity ranges), as
+# WheeledSim.set_device_events takes it.
+def _timer_ranges(table):
+    return [tuple(r) for mode, r, _ in table if mode == "interval"]
+
+
+def device_events_init(seed, env_id_offset, n, table) -> np.ndarray:
+    """The interval terms' timers as wl_set_device_events draws them: [n_interval_terms, N] f32."""
+    ranges = _timer_ranges(table)
+    return event_timers_init(seed, env_id_offset, n, ranges) if ranges else np.zeros((0, n), np.float32)
+
+
+def device_events_step(seed, env_id_offset, table, step_dt, done, time_left, vel, step_counter):
+    """wlo_device_events: one step of every term, in place on time_left [n_interval_terms, N] f32 and vel [N, 6] f32 (x, y, z,
+    roll, pitch, yaw)."""
+    n = vel.shape[0]
+    slot, j = [], 0
+    for mode, _, _ in table:
+        slot.append(j if mode == "interval" else -1)
+        j += mode == "interval"
+    slot = np.asarray(slot or [0], dtype=np.int32)
+    lo = np.ascontiguousarray([[r[0] for r in rr] for _, _, rr in table] or [[0.0] * 6], dtype=np.float32)
+    hi = np.ascontiguousarray([[r[1] for r in rr] for _, _, rr in table] or [[0.0] * 6], dtype=np.float32)
+    tlh = np.ascontiguousarray(_timer_ranges(table) or [(0.0, 0.0)], dtype=np.float32).reshape(-1)
+    done = np.ascontiguousarray(done, dtype=np.uint8)
+    assert vel.dtype == np.float32 and vel.flags.c_contiguous and time_left.dtype == np.float32 and time_left.flags.c_contiguous
+    get_lib().wlo_device_events(seed, env_id_offset, n, len(table), _p(slot), _p(lo), _p(hi), j, _p(tlh), np.float32(step_dt), _p(done),
+                                _p(time_left), _p(vel), step_counter)
+
+
+# A policy observation table is a list of (library name, noise, clip, scale) as WheeledSim.set_policy_terms takes it; the state
+# is the device state's groups, float32 [NUM_GROUPS, N, 4] (sim.groups).
+# First library float and width of each term (the row the kernel forms per env: the critic library, then gravity).
+LIBRARY = {"root_pos_w": (0, 3), "root_euler_xyz": (3, 3), "base_lin_vel": (6, 3), "base_ang_vel": (9, 3), "last_action": (12, 2),
+           "joint_vel": (14, 4), "joint_pos": (18, 2), "wheel_friction": (20, 4), "base_mass": (24, 1), "motor_damping": (25, 4),
+           "projected_gravity": (29, 3)}
+NOISE = {None: 0, "gaussian": 1, "uniform": 2}
+
+
+def policy_columns(table) -> dict:
+    """Per output column: src, noise kind, (na, nb) = (mean, std) or (n_min, n_max - n_min) with the span formed in double,
+    clip flag and bounds, scale flag and value -- each parameter rounded to fp32."""
+    cols = {k: [] for k in ("src", "noise", "na", "nb", "has_clip", "lo", "hi", "has_scale", "scale")}
+    for name, noise, clip, scale in table:
+        first, width = LIBRARY[name]
+        sc = None if scale is None else ((float(scale),) if isinstance(scale, (int, float)) else tuple(float(s) for s in scale))
+        for k in range(width):
+            cols["src"].append(first + k)
+            cols["noise"].append(NOISE[None if noise is None else noise[0]])
+            a, b = (0.0, 0.0) if noise is None else (float(noise[1]), float(noise[2]))
+            cols["na"].append(a)
+            cols["nb"].append(b - a if noise is not None and noise[0] == "uniform" else b)
+            cols["has_clip"].append(clip is not None)
+            cols["lo"].append(0.0 if clip is None else float(clip[0]))
+            cols["hi"].append(0.0 if clip is None else float(clip[1]))
+            cols["has_scale"].append(sc is not None)
+            cols["scale"].append(1.0 if sc is None else sc[0 if len(sc) == 1 else k])
+    out = {}
+    for k, v in cols.items():
+        dt = np.uint8 if k in ("src", "noise", "has_clip", "has_scale") else np.float32
+        out[k] = np.ascontiguousarray(np.asarray(v or [0], dtype=np.float64 if dt is np.float32 else np.int64).astype(dt))
+    return out
+
+
+def policy_observe(seed, env_id_offset, st, table, corrupt, t, call_idx=-1) -> np.ndarray:
+    """wlo_policy_observe: the policy row [N, Dp] of the state groups st [G, N, 4] for the step at t (call_idx -1) or an
+    observe call."""
+    st = np.ascontiguousarray(st, dtype=np.float32)
+    n = st.shape[1]
+    c = policy_columns(table)
+    dp = sum(LIBRARY[name][1] for name, *_ in table)
+    out = np.zeros((n, max(dp, 1)), dtype=np.float32)
+    get_lib().wlo_policy_observe(seed, env_id_offset, n, _p(st), dp, _p(c["src"]), _p(c["noise"]), _p(c["na"]), _p(c["nb"]),
+                                 _p(c["has_clip"]), _p(c["lo"]), _p(c["hi"]), _p(c["has_scale"]), _p(c["scale"]), int(bool(corrupt)),
+                                 t & 0xFFFFFFFF, call_idx, _p(out))
+    return out[:, :dp]
+
+
+def policy_library(st) -> np.ndarray:
+    """wlo_policy_library: [N, 32] library floats of every env."""
+    st = np.ascontiguousarray(st, dtype=np.float32)
+    out = np.zeros((st.shape[1], 32), dtype=np.float32)
+    get_lib().wlo_policy_library(_p(st), st.shape[1], _p(out))
+    return out
+
+
+def policy_draw(seed, gid, t, call_idx, j, kind) -> np.float32:
+    """wlo_policy_obs_draw: the noise draw of column j, z (kind "gaussian") or u in [0, 1) (kind "uniform")."""
+    return np.float32(get_lib().wlo_policy_obs_draw(seed, gid, t & 0xFFFFFFFF, call_idx, j, NOISE[kind]))
+
+
 class Oracle:
     """One oracle instance; mirrors the wl_* calls with host (numpy) buffers."""
 
@@ -201,6 +319,11 @@ class Oracle:
     def set_device_terms(self, terms):
         """wl_set_device_terms: (kind, role, weight, params) rows; [] clears them."""
         assert self.lib.wlo_set_device_terms(self._h, term_table(terms), len(terms)) == 0
+
+    def set_reset_events(self, mask) -> int:
+        """wl_set_reset_events: the WL_RESET_EV_* bits step, step_terms and reset redraw; 0, or WL_EINVAL with the mask left
+        as it was."""
+        return self.lib.wlo_set_reset_events(self._h, mask)
 
     def step_terms(self, action, step_counter):
         """wl_step_terms: step() with the device terms; returns (obs, rew, term, trunc, fired [N], term_log [8])."""

@@ -212,7 +212,7 @@ def _numpy_events(seed, off, n, table, dt, dones, vel):
 
 
 def test_twin_equals_the_numpy_restatement():
-    import device_events_oracle as deo
+    from oracle_lib import device_events_init, device_events_step
     seed, n, dt = 99, 41, np.float32(0.1)
     rng = np.random.default_rng(2)
     table = [("interval", (0.2, 0.6), RANGES), ("reset", None, [(-1.0, 1.0)] * 6), ("interval", (0.0, 0.0), [(0.0, 0.0)] * 6),
@@ -222,24 +222,25 @@ def test_twin_equals_the_numpy_restatement():
         for tb in (table[:1], table[1:2], table):
             vel0 = rng.standard_normal((n, 6)).astype(np.float32)
             want = _numpy_events(seed, off, n, tb, dt, dones, vel0.copy())
-            tl, vel = deo.init(seed, off, n, tb), vel0.copy()
+            tl, vel = device_events_init(seed, off, n, tb), vel0.copy()
             for t, done in enumerate(dones):
-                deo.step(seed, off, tb, dt, done, tl, vel, t)
+                device_events_step(seed, off, tb, dt, done, tl, vel, t)
                 assert np.array_equal(vel.view(np.uint32), want[t].view(np.uint32)), (off, len(tb), t)
             assert not np.array_equal(vel, vel0)
 
 
 def test_twin_does_not_depend_on_sharding():
-    import device_events_oracle as deo
+    from oracle_lib import device_events_init, device_events_step
     seed, n, dt = 3, 64, np.float32(0.1)
     table = [("interval", (0.1, 0.4), RANGES), ("reset", None, [(-0.1, 0.3)] * 6)]
     rng = np.random.default_rng(4)
     vel = rng.standard_normal((n, 6)).astype(np.float32)
     halves = [vel[:32].copy(), vel[32:].copy()]
-    tl, th = deo.init(seed, 0, n, table), [deo.init(seed, 0, 32, table), deo.init(seed, 32, 32, table)]
+    tl = device_events_init(seed, 0, n, table)
+    th = [device_events_init(seed, 0, 32, table), device_events_init(seed, 32, 32, table)]
     for t in range(30):
         done = (rng.random(n) < 0.1).astype(np.uint8)
-        deo.step(seed, 0, table, dt, done, tl, vel, t)
+        device_events_step(seed, 0, table, dt, done, tl, vel, t)
         for h in (0, 1):
-            deo.step(seed, 32 * h, table, dt, done[32 * h:32 * h + 32], th[h], halves[h], t)
+            device_events_step(seed, 32 * h, table, dt, done[32 * h:32 * h + 32], th[h], halves[h], t)
         assert np.array_equal(vel, np.concatenate(halves)) and np.array_equal(tl, np.concatenate(th, axis=1))

@@ -1,6 +1,6 @@
 """Device event terms (wl_set_device_events / wl_device_events / wl_step_terms, DESIGN 6p) on the GPU:
 
-- wl_device_events equals the CPU twin (tests/device_events_oracle.c) bit for bit on every task at N = 1, 33, 4096, 8192
+- wl_device_events equals the oracle's twin (wlo_device_events) bit for bit on every task at N = 1, 33, 4096, 8192
   with 1 and 8 terms (an interval range of (0, 0), which fires every step; every env reset every tenth step), and two
   shards equal one handle;
 - the whole step with device events equals the step without them plus the twin's push on its state, step after step, on
@@ -86,21 +86,21 @@ def _done(rng, n, t):
 @pytest.mark.parametrize("n", [1, 33, 4096, 8192])
 @pytest.mark.parametrize("table", [TABLE_1, TABLE_8], ids=["1term", "8terms"])
 def test_kernel_equals_the_twin(task, n, table):
-    import device_events_oracle as deo
+    from oracle_lib import device_events_init, device_events_step
     sim = _sim(task, n, table=table)
     gen = torch.Generator(device=DEV).manual_seed(n)
     sim.groups[G_LINVEL, :, 0:3] = torch.randn((n, 3), device=DEV, generator=gen)
     sim.groups[G_ANGVEL, :, 0:3] = torch.randn((n, 3), device=DEV, generator=gen)
     w_before = torch.stack([sim.groups[G_LINVEL, :, 3], sim.groups[G_ANGVEL, :, 3]]).clone()
     seed, dt = int(sim.cfg.seed), _step_dt(sim.cfg)
-    tl, vel = deo.init(seed, 0, n, table), _vel(sim)
+    tl, vel = device_events_init(seed, 0, n, table), _vel(sim)
     rng = np.random.default_rng(7)
     moved = 0
     for t in range(40):
         term, trunc = _done(rng, n, t)
         sim.device_events(torch.from_numpy(term).to(DEV), torch.from_numpy(trunc).to(DEV), t)
         before = vel.copy()
-        deo.step(seed, 0, table, dt, term | trunc, tl, vel, t)
+        device_events_step(seed, 0, table, dt, term | trunc, tl, vel, t)
         got = _vel(sim)
         assert np.array_equal(got.view(np.uint32), vel.view(np.uint32)), f"step {t}"
         moved += int((before != vel).any(axis=1).sum())
@@ -141,7 +141,7 @@ def _add_terms(env):
 def test_the_step_is_the_step_without_events_plus_the_twins_push(task, terms):
     """Each step: B takes A's state, both step (A with the events), and A's state equals B's with the twin's push applied
     for B's done bytes; rewards and dones are equal (the events come after them).  With device terms on both."""
-    import device_events_oracle as deo
+    from oracle_lib import device_events_init, device_events_step
     n = 256
     spec = lambda: wl.make_task(task, num_envs=n, seed=5)
     a, b = ManagerBasedRLEnv(spec(), device=DEV), ManagerBasedRLEnv(spec(), device=DEV)
@@ -153,7 +153,7 @@ def test_the_step_is_the_step_without_events_plus_the_twins_push(task, terms):
     for e in (a, b):
         e.reset()
     seed, dt = int(a.spec.cfg.seed), _step_dt(a.spec.cfg)
-    tl = deo.init(seed, 0, n, table)
+    tl = device_events_init(seed, 0, n, table)
     gen = torch.Generator(device=DEV).manual_seed(2)
     fired = 0
     for t in range(120):
@@ -165,7 +165,7 @@ def test_the_step_is_the_step_without_events_plus_the_twins_push(task, terms):
         assert torch.equal(_bits(ra), _bits(rb)) and torch.equal(ta, tb) and torch.equal(ua, ub), f"step {t}"
         vel = _vel(b.sim)
         before = vel.copy()
-        deo.step(seed, 0, table, dt, (tb | ub).cpu().numpy().astype(np.uint8), tl, vel, t)
+        device_events_step(seed, 0, table, dt, (tb | ub).cpu().numpy().astype(np.uint8), tl, vel, t)
         assert np.array_equal(_vel(a.sim).view(np.uint32), vel.view(np.uint32)), f"step {t}"
         rest = [g for g in range(a.sim.groups.shape[0]) if g not in (G_LINVEL, G_ANGVEL)]
         assert torch.equal(a.sim.groups[rest], b.sim.groups[rest]), f"step {t}"

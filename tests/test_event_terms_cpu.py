@@ -147,7 +147,7 @@ def _numpy_timers(seed, off, n, ranges, dt, dones):
 
 
 def test_twin_equals_the_numpy_restatement():
-    import event_timers_oracle as eo
+    from oracle_lib import event_timers_init, event_timers_step
     seed, n, dt = 1234, 37, np.float32(0.1)
     ranges = [(0.5, 1.0), (0.0, 0.0), (0.1, 0.1), (0.02, 0.05), (2.0, 3.0), (0.3, 0.9), (0.0, 0.05), (1.0, 1.5)]
     rng = np.random.default_rng(0)
@@ -155,28 +155,29 @@ def test_twin_equals_the_numpy_restatement():
     for off in (0, 1000):
         for rr in (ranges[:1], ranges):
             want = _numpy_timers(seed, off, n, rr, dt, dones)
-            tl = eo.init(seed, off, n, rr)
+            tl = event_timers_init(seed, off, n, rr)
             fires = 0
             for t, done in enumerate(dones):
-                fired = eo.step(seed, off, rr, dt, done, tl, t)
+                fired = event_timers_step(seed, off, rr, dt, done, tl, t)
                 assert np.array_equal(fired, want[t][0]), (off, t)
                 assert np.array_equal(tl.view(np.uint32), want[t][1].view(np.uint32)), (off, t)
                 fires += int(fired.sum())
             assert fires > 0
     # the semantics at the edges: lo == hi == 0 fires every step; a fresh timer of hi > step_dt never fires in its reset step
-    tl = eo.init(seed, 0, n, [(0.0, 0.0), (0.5, 1.0)])
-    fired = eo.step(seed, 0, [(0.0, 0.0), (0.5, 1.0)], dt, np.ones(n, np.uint8), tl, 5)
+    tl = event_timers_init(seed, 0, n, [(0.0, 0.0), (0.5, 1.0)])
+    fired = event_timers_step(seed, 0, [(0.0, 0.0), (0.5, 1.0)], dt, np.ones(n, np.uint8), tl, 5)
     assert fired[0].all() and not fired[1].any()
 
 
 def test_twin_does_not_depend_on_sharding():
-    import event_timers_oracle as eo
+    from oracle_lib import event_timers_init, event_timers_step
     seed, n, dt, ranges = 7, 64, np.float32(0.1), [(0.1, 0.4), (0.0, 0.2)]
     rng = np.random.default_rng(1)
-    whole, halves = eo.init(seed, 0, n, ranges), [eo.init(seed, 0, 32, ranges), eo.init(seed, 32, 32, ranges)]
+    whole = event_timers_init(seed, 0, n, ranges)
+    halves = [event_timers_init(seed, 0, 32, ranges), event_timers_init(seed, 32, 32, ranges)]
     assert np.array_equal(whole, np.concatenate(halves, axis=1))
     for t in range(30):
         done = (rng.random(n) < 0.1).astype(np.uint8)
-        f = eo.step(seed, 0, ranges, dt, done, whole, t)
-        fh = [eo.step(seed, 32 * h, ranges, dt, done[32 * h:32 * h + 32], halves[h], t) for h in (0, 1)]
+        f = event_timers_step(seed, 0, ranges, dt, done, whole, t)
+        fh = [event_timers_step(seed, 32 * h, ranges, dt, done[32 * h:32 * h + 32], halves[h], t) for h in (0, 1)]
         assert np.array_equal(f, np.concatenate(fh, axis=1)) and np.array_equal(whole, np.concatenate(halves, axis=1))

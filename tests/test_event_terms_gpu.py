@@ -92,18 +92,18 @@ RANGES8 = [(0.5, 1.0), (0.0, 0.0), (0.1, 0.1), (0.02, 0.05), (2.0, 3.0), (0.3, 0
 @pytest.mark.parametrize("ranges", [RANGES8[:1], RANGES8[1:2], RANGES8], ids=["1 term", "1 term lo == hi == 0", "8 terms"])
 def test_event_timers_equal_the_twin(n, ranges):
     _need_gpu()
-    import event_timers_oracle as eo
+    from oracle_lib import event_timers_init, event_timers_step
     sim = _sim("drift", n)
     seed, dt = int(sim.cfg.seed), _step_dt(sim.cfg)
     sim.set_event_timers(ranges)
-    tl = eo.init(seed, 0, n, ranges)
+    tl = event_timers_init(seed, 0, n, ranges)
     fired = torch.empty((len(ranges), n), dtype=torch.uint8, device=DEV)
     rng = np.random.default_rng(n)
     fires = 0
     for t in range(120):
         done = np.ones(n, np.uint8) if 5 <= t < 15 else (rng.random(n) < 0.02).astype(np.uint8)   # (5..14: every env every step)
         sim.event_timers(torch.from_numpy(done).to(DEV), t, fired)
-        want = eo.step(seed, 0, ranges, dt, done, tl, t)
+        want = event_timers_step(seed, 0, ranges, dt, done, tl, t)
         assert np.array_equal(fired.cpu().numpy(), want), t
         fires += int(want.sum())
     assert fires > 0 or n == 1
@@ -150,7 +150,7 @@ def _env(n=256, task="Isaac-MushrDriftRL-v0", **kw):
 
 def test_reset_startup_and_interval_event_semantics():
     _need_gpu()
-    import event_timers_oracle as eo
+    from oracle_lib import event_timers_init, event_timers_step
     n = 256
     env = _env(n)
     log = {"startup": [], "reset": [], "kick": []}
@@ -173,7 +173,7 @@ def test_reset_startup_and_interval_event_semantics():
     env.add_event_term("spawn", on_reset, "reset", {"x": 50.0})
     ranges = [(0.1, 0.5)]
     env.add_event_term("kick", on_kick, "interval", interval_range_s=ranges[0])
-    tl = eo.init(int(env.spec.cfg.seed), 0, n, ranges)
+    tl = event_timers_init(int(env.spec.cfg.seed), 0, n, ranges)
     dt = _step_dt(env.spec.cfg)
     env.reset()
     _same(log["reset"].pop(), torch.arange(n, device=DEV), "reset() calls the reset events with every env")
@@ -194,7 +194,7 @@ def test_reset_startup_and_interval_event_semantics():
             assert (p[ids[ids % 2 == 1], 0]).abs().le(20.0).all()
             resets += ids.numel()
         assert not log["reset"], f"step {t}: the reset event ran without resets"
-        fired = eo.step(int(env.spec.cfg.seed), 0, ranges, dt, done.to(torch.uint8).cpu().numpy(), tl, t)
+        fired = event_timers_step(int(env.spec.cfg.seed), 0, ranges, dt, done.to(torch.uint8).cpu().numpy(), tl, t)
         want = torch.from_numpy(np.nonzero(fired[0])[0]).to(DEV)
         if want.numel():
             _same(log["kick"].pop(), want, f"step {t}: interval ids")

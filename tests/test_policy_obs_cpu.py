@@ -12,7 +12,7 @@ import pytest
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tests"))
 
-import policy_obs_oracle as po  # noqa: E402
+from oracle_lib import LIBRARY, policy_draw, policy_library, policy_observe  # noqa: E402
 
 G = 16          # WL_NUM_GROUPS
 SEED = 0x5EED1234ABCDEF
@@ -28,14 +28,14 @@ def _random_state(n, rng):
 def _restated(seed, env_id_offset, st, table, corrupt, t, call_idx):
     """ObservationManager.compute for one group, term by term: value, then noise (enable_corruption only), then clip, then
     scale, then the concatenation -- numpy fp32 arithmetic on the twin's library values and draws."""
-    lib = po.library(st)
+    lib = policy_library(st)
     n = st.shape[1]
     blocks, j0 = [], 0
     for name, noise, clip, scale in table:
-        first, width = po.LIBRARY[name]
+        first, width = LIBRARY[name]
         x = lib[:, first:first + width].copy()
         if corrupt and noise is not None:
-            d = np.array([[po.draw(seed, env_id_offset + i, t, call_idx, j0 + k, noise[0]) for k in range(width)] for i in range(n)],
+            d = np.array([[policy_draw(seed, env_id_offset + i, t, call_idx, j0 + k, noise[0]) for k in range(width)] for i in range(n)],
                          dtype=np.float32)
             if noise[0] == "gaussian":                      # data + mean + std * randn_like(data)
                 x = (x + np.float32(noise[1])) + np.float32(noise[2]) * d
@@ -70,8 +70,8 @@ TABLES = {
 
 
 def test_the_tables_cover_the_library():
-    assert {t[0] for tb in TABLES.values() for t in tb} == set(po.LIBRARY)
-    assert sum(po.LIBRARY[t[0]][1] for t in TABLES["wide_32"]) == 32
+    assert {t[0] for tb in TABLES.values() for t in tb} == set(LIBRARY)
+    assert sum(LIBRARY[t[0]][1] for t in TABLES["wide_32"]) == 32
 
 
 @pytest.mark.parametrize("table", sorted(TABLES))
@@ -80,14 +80,14 @@ def test_the_tables_cover_the_library():
 def test_twin_equals_the_restated_observation_manager(table, corrupt, t, call_idx):
     rng = np.random.default_rng([sorted(TABLES).index(table), t, call_idx + 1])
     st = _random_state(37, rng)
-    got = po.observe(SEED, 5, st, TABLES[table], corrupt, t, call_idx)
+    got = policy_observe(SEED, 5, st, TABLES[table], corrupt, t, call_idx)
     want = _restated(SEED, 5, st, TABLES[table], corrupt, t, call_idx)
     assert got.view(np.uint32).tolist() == want.view(np.uint32).tolist()
 
 
 def test_the_draws_follow_the_documented_keys():
     """Gaussian columns below 12 share blind_obs's draws; the others differ across columns, steps and call indices."""
-    g = lambda t, ci, j, k="gaussian": float(po.draw(SEED, 3, t, ci, j, k))
+    g = lambda t, ci, j, k="gaussian": float(policy_draw(SEED, 3, t, ci, j, k))
     assert len({g(9, -1, 12), g(9, -1, 13), g(9, -1, 16), g(10, -1, 12), g(9, 0, 12), g(9, 1, 12)}) == 6
     assert len({g(9, -1, j, "uniform") for j in range(32)} | {g(9, 0, 0, "uniform"), g(10, -1, 0, "uniform")}) == 34
     assert g(9, -1, 0) != g(9, 0, 0) != g(9, 1, 0)
@@ -97,8 +97,8 @@ def test_twin_does_not_depend_on_sharding():
     rng = np.random.default_rng(3)
     st = _random_state(64, rng)
     table = TABLES["wide_32"]
-    whole = po.observe(SEED, 0, st, table, True, 41, -1)
-    halves = np.concatenate([po.observe(SEED, 0, st[:, :32], table, True, 41, -1), po.observe(SEED, 32, st[:, 32:], table, True, 41, -1)])
+    whole = policy_observe(SEED, 0, st, table, True, 41, -1)
+    halves = np.concatenate([policy_observe(SEED, 0, st[:, :32], table, True, 41, -1), policy_observe(SEED, 32, st[:, 32:], table, True, 41, -1)])
     assert whole.view(np.uint32).tolist() == halves.view(np.uint32).tolist()
 
 

@@ -21,11 +21,11 @@ pytestmark = pytest.mark.gpu
 if not torch.cuda.is_available():
     pytest.skip("needs a CUDA device", allow_module_level=True)
 
-import policy_obs_oracle as po                                 # noqa: E402
 import wheeledlab_b200 as wl                                   # noqa: E402
 from wheeledlab_b200 import policy_obs                         # noqa: E402
 from wheeledlab_b200.env import ManagerBasedRLEnv              # noqa: E402
 from wheeledlab_b200.sim import WheeledSim                     # noqa: E402
+from oracle_lib import policy_observe                           # noqa: E402
 
 DEV = "cuda:0"
 NO_POS = [("root_euler_xyz", ("gaussian", 0.0, 0.1), None, None), ("base_lin_vel", ("gaussian", 0.0, 0.5), None, None),
@@ -65,7 +65,7 @@ def _bits(x):
 
 def _twin(sim, table, t, call_idx=-1):
     c = sim.cfg
-    return po.observe(int(c.seed), int(c.env_id_offset), sim.groups.cpu().numpy(), table, bool(c.enable_corruption), t, call_idx)
+    return policy_observe(int(c.seed), int(c.env_id_offset), sim.groups.cpu().numpy(), table, bool(c.enable_corruption), t, call_idx)
 
 
 def _run(sim, steps, t0=0):

@@ -72,21 +72,22 @@ def test_other_modes_and_a_minimum_step_count_are_refused_by_name(ref_registry):
 # ---- the oracle twin ----------------------------------------------------------------------------------------------------------
 
 def _oracle(task, n, mask, seed=3, offset=0):
-    import reset_dr_oracle
+    from oracle_lib import Oracle
     import wheeledlab_b200 as wl
     spec = wl.make_task(task, num_envs=n, seed=seed, env_id_offset=offset)
-    o = reset_dr_oracle.Oracle(spec.cfg, heightfield=spec.heightfield, mask=mask)
+    o = Oracle(spec.cfg, heightfield=spec.heightfield)
+    assert o.set_reset_events(mask) == 0
     o.startup()
     o.reset(None, 0)
     return o
 
 
 def test_oracle_refusals_leave_the_mask_as_it_was():
-    import reset_dr_oracle
+    from oracle_lib import Oracle
     import wheeledlab_b200 as wl
     for task, bad in (("drift", 16), ("drift", WHEEL), ("elevation", GAINS), ("visual", MATERIAL), ("visual_random", GAINS)):
         spec = wl.make_task(task, num_envs=4, seed=1)
-        o = reset_dr_oracle.Oracle(spec.cfg, heightfield=spec.heightfield)
+        o = Oracle(spec.cfg, heightfield=spec.heightfield)
         assert o.set_reset_events(bad) != 0, (task, bad)
     ref, o = _oracle("drift", 64, MATERIAL), _oracle("drift", 64, MATERIAL)
     assert o.set_reset_events(MATERIAL | 32) != 0 and o.set_reset_events(WHEEL) != 0

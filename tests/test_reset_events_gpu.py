@@ -42,10 +42,11 @@ def _sim(task, n, events, seed=3, offset=0, variant=None):
 
 
 def _oracle(task, n, mask, seed=3, offset=0):
-    import reset_dr_oracle
+    from oracle_lib import Oracle
     import wheeledlab_b200 as wl
     spec = wl.make_task(task, num_envs=n, seed=seed, env_id_offset=offset)
-    o = reset_dr_oracle.Oracle(spec.cfg, heightfield=spec.heightfield, mask=mask, threads=os.cpu_count() or 1)
+    o = Oracle(spec.cfg, heightfield=spec.heightfield, threads=os.cpu_count() or 1)
+    assert o.set_reset_events(mask) == 0
     o.startup()
     o.reset(None, 0)
     return o

@@ -1391,7 +1391,6 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
     }
 }
 
-// (wl_reset_dr.cuh restates the DR draw below for its own kernel: this kernel is left as it is, machine code included)
 #include "wl_reset_dr.cuh"
 
 __global__ void wl_startup_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st) {
@@ -1403,39 +1402,13 @@ __global__ void wl_startup_kernel(const __grid_constant__ wl_config c, float4* _
     uint4 r1 = philox4x32(c.seed, gid, 0u, RNG_STARTUP, 1u);
     uint4 r2 = philox4x32(c.seed, gid, 0u, RNG_STARTUP, 2u);
     uint4 r3 = philox4x32(c.seed, gid, 0u, RNG_STARTUP, 3u);
-    const uint32_t rb[4] = {r0.x, r0.y, r0.z, r0.w}, rk[4] = {r1.x, r1.y, r1.z, r1.w}, rm[4] = {r3.x, r3.y, r3.z, r3.w};
-    float D[4], C[4], kd[4];
-#pragma unroll
-    for (int w = 0; w < 4; ++w) {
-        uint32_t bk = 0;
-        if (c.dr_enable && c.dr_num_buckets > 1) bk = __umulhi(rb[w], (uint32_t)c.dr_num_buckets);
-        D[w] = c.dr_bucket_D[bk]; C[w] = c.dr_bucket_C[bk];
-        kd[w] = c.dc_damping[w];
-        if (c.dr_enable && ((c.dr_kd_mask >> w) & 1)) kd[w] = uniform(rk[w], c.dr_kd_range[0], c.dr_kd_range[1]);
-    }
-    // randomize_rigid_body_mass: "add" -> base_link mass += U; "abs" -> base_link mass := U (mushr_visual_env_cfg.py:280-288);
-    // wheel links := U (:290-299), their spin inertia rescaled by the mass ratio
-    float mass = c.mass_nominal;
-    float inv_Iw[4] = {c.d_inv_Iw, c.d_inv_Iw, c.d_inv_Iw, c.d_inv_Iw};
-    if (c.dr_enable) {
-        const float u = uniform(r2.x, c.dr_mass_add[0], c.dr_mass_add[1]);
-        if (c.dr_mass_mode == 0) mass = mass + u;
-        else mass = (mass - c.dr_base_mass_nominal) + u;
-        if (c.dr_wheel_mass_enable) {
-#pragma unroll
-            for (int w = 0; w < 4; ++w) {
-                const float mw = uniform(rm[w], c.dr_wheel_mass[0], c.dr_wheel_mass[1]);
-                mass = mass + (mw - c.wheel_mass_nominal);
-                inv_Iw[w] = c.d_inv_Iw * (c.wheel_mass_nominal / mw);
-            }
-        }
-    }
-    float inv_mass = 1.0f / mass;
-    stg4(st, WL_G_PIW, n, i, make_float4(inv_Iw[0], inv_Iw[1], inv_Iw[2], inv_Iw[3]));
-    stg4(st, WL_G_PMASS, n, i, make_float4(mass, inv_mass, 0.0f, 0.0f));
-    stg4(st, WL_G_PMU_D, n, i, make_float4(D[0], D[1], D[2], D[3]));
-    stg4(st, WL_G_PMU_C, n, i, make_float4(C[0], C[1], C[2], C[3]));
-    stg4(st, WL_G_PKD, n, i, make_float4(kd[0], kd[1], kd[2], kd[3]));
+    DrParams p;
+    dr_params(c, r0, r1, r2, r3, p);
+    stg4(st, WL_G_PIW, n, i, make_float4(p.inv_Iw[0], p.inv_Iw[1], p.inv_Iw[2], p.inv_Iw[3]));
+    stg4(st, WL_G_PMASS, n, i, make_float4(p.mass, p.inv_mass, 0.0f, 0.0f));
+    stg4(st, WL_G_PMU_D, n, i, make_float4(p.D[0], p.D[1], p.D[2], p.D[3]));
+    stg4(st, WL_G_PMU_C, n, i, make_float4(p.C[0], p.C[1], p.C[2], p.C[3]));
+    stg4(st, WL_G_PKD, n, i, make_float4(p.kd[0], p.kd[1], p.kd[2], p.kd[3]));
     float t_hf = uniform(r2.y, c.push_hf_interval[0], c.push_hf_interval[1]);
     float t_lf = uniform(r2.z, c.push_lf_interval[0], c.push_lf_interval[1]);
     float4 g;

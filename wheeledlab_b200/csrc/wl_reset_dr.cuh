@@ -8,8 +8,8 @@
 
 #define WL_RESET_DR_BS 128
 
-// The DR parameters of one env from its four Philox blocks: r0 friction buckets, r1 actuator gains, r2 base mass, r3 wheel
-// masses.  The total mass starts from the nominal mass every time (randomize_rigid_body_mass applies to the default mass):
+// The DR parameters of one env from its four Philox blocks (wl_startup_kernel's and wl_reset_dr_kernel's draw): r0 friction
+// buckets, r1 actuator gains, r2 base mass, r3 wheel masses.  The total mass starts from the nominal mass every time (randomize_rigid_body_mass applies to the default mass):
 // base term first, then the four wheel terms.
 struct DrParams {
     float D[4], C[4], kd[4];
