@@ -787,6 +787,40 @@ int32_t wl_policy_obs_dim(const wl_sim* sim);
  * fan-out is set (only the built-in row carries it). */
 int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float* d_out, void* stream);
 
+/* ---- noise, clip and scale on the Elevation and Visual policy rows (DESIGN.md 6r) ----------------------------------------
+ * The row terms of a handle: one wl_policy_term per term of the task's built-in policy row, in row order, with the term's
+ * kind at that position --
+ *   Elevation (689 floats):  WL_ROW_GOAL_RELATIVE_XYZ (2), WL_CRITIC_ROOT_EULER_XYZ (3), WL_CRITIC_BASE_LIN_VEL (3),
+ *                            WL_CRITIC_BASE_ANG_VEL (3), WL_CRITIC_LAST_ACTION (2), WL_ROW_WORLD_HEIGHT_MAP (676)
+ *   Visual (camera floats, then 8): WL_CRITIC_BASE_LIN_VEL (3), WL_CRITIC_BASE_ANG_VEL (3), WL_CRITIC_LAST_ACTION (2)
+ * With row terms every entry that writes the row forms those columns from the raw values (goal_relative_xyz with its
+ * nan_to_num, the euler angles, the body-frame velocities, the unclipped last action; a ray that misses is +inf), then per
+ * term, as ObservationManager.compute does and with wl_policy_term's arithmetic and rounding (6q): additive noise only when
+ * the config's enable_corruption is set, the clip, the scale.  The camera floats are not touched.  So the registered
+ * group is the row terms {none, none, clip +-obs_clip, clip +-obs_clip, clip +-1, clip +-obs_clip}, and the Visual tail
+ * {none, none, clip +-1}.
+ * Noise keys of row column j (0-based: 0..688 on Elevation, 0..7 in the Visual tail), env global id g, step counter t
+ * (decoded from WL_DEVICE_COUNTER_PLUS(k)):
+ *   Philox (seed, g, t, 17, 512 (call_idx + 1) + 256 u + j / 4), u = 1 for uniform noise, call_idx = -1 for the row a
+ *   step writes and wl_observe's call_idx (0..2^23-2) for an observe call; word j % 4 gives U[0,1) from its top 24 bits,
+ *   lanes (x, y) -> Box-Muller -> columns 4b, 4b + 1 and lanes (z, w) -> 4b + 2, 4b + 3 give N(0, 1)
+ * so no two columns, noise kinds, steps or call indices share a key, and the draws do not depend on launch geometry. */
+#define WL_ROW_GOAL_RELATIVE_XYZ 12
+#define WL_ROW_WORLD_HEIGHT_MAP  13
+#define WL_ROW_TERMS_ELEVATION   6
+#define WL_ROW_TERMS_VISUAL      3
+/* Store the handle's row terms (a host-side set-up call: nothing is launched; every term is checked before anything is
+ * replaced, so a failure leaves the handle as it was).  n_terms = 0 clears them; otherwise it is the task's term count.
+ * WL_EINVAL: a null handle, a null table with n_terms > 0, n_terms neither 0 nor the count, a kind other than the row's term
+ * at that position, an unknown noise model, n_scale not 0, 1 or the width (the map: 0 or 1), a parameter that is not
+ * finite.  WL_EUNSUPPORTED: the Drift family (wl_set_policy_terms), a peer / multicast fan-out set, scan mode 2.
+ * With row terms wl_step, wl_step_terms, wl_step_stage_b / _b2, wl_observe, wl_step_host and wl_step_host_zero_copy write
+ * the modified row; wl_act_step, wl_act_infer_step and wl_rollout return WL_EUNSUPPORTED, and so does wl_set_scan_tma(2).
+ * wl_observe takes call_idx 0..2^23-2 (WL_EINVAL otherwise).  A graph captured with the old terms keeps the old terms. */
+int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms);
+/* the number of row terms (0: none) */
+int32_t wl_row_terms(const wl_sim* sim);
+
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out
  * bootstrap of PPO.process_env_step (rewards += gamma * values * time_outs) folded in when d_time_outs != NULL:

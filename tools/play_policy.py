@@ -11,7 +11,8 @@ and agent cfg come from the run's ``run.json`` (``tools/ppo_train.py --log-dir``
 the activation follows the task.  ``-sd`` saves ``{'observations', 'actions'}`` as ``<playback-dir>/<play-name>-rollouts.pt``,
 the reference's file.  Prints the mean return and length of the episodes that finished during the playback.  A run trained on
 a policy observation table (``policy_terms`` in ``run.json``, DESIGN 6q) plays on an env with the same table, through
-``wl_actor_mean`` on the table's row.
+``wl_actor_mean`` on the table's row.  A run of an Elevation or Visual env with row terms (``row_terms`` in ``run.json``,
+DESIGN 6r) plays with the same terms: their clips and scales change the policy's input even without noise.
 """
 from __future__ import annotations
 
@@ -64,7 +65,7 @@ def resolve(args) -> dict:
     num_envs = args.num_envs if args.num_envs is not None else (run_cfg or {}).get("num_envs")
     seed = args.seed if args.seed is not None else (run_cfg or {}).get("seed")
     return {"task": task, "policy_path": policy_path, "playback_dir": playback_dir, "agent_cfg": agent, "num_envs": num_envs, "seed": seed,
-            "policy_terms": (run_cfg or {}).get("policy_terms")}
+            "policy_terms": (run_cfg or {}).get("policy_terms"), "row_terms": (run_cfg or {}).get("row_terms")}
 
 
 def play(r: dict, steps: int, device: str = "cuda:0"):
@@ -78,6 +79,10 @@ def play(r: dict, steps: int, device: str = "cuda:0"):
     if r.get("policy_terms"):
         env.set_policy_observation([(name, fn, {"noise": tuple(nz) if nz else None, "clip": cl, "scale": sc})
                                     for name, fn, nz, cl, sc in r["policy_terms"]])
+    if r.get("row_terms"):
+        env.set_row_terms([(name, fn, {"noise": tuple(nz) if nz else None, "clip": tuple(cl) if cl else None,
+                                       "scale": tuple(sc) if isinstance(sc, list) else sc})
+                           for name, fn, nz, cl, sc in r["row_terms"]])
     runner = FusedOnPolicyRunner(env, r["agent_cfg"], device=device)
     runner.load(r["policy_path"], load_optimizer=False)
     env.reset()

@@ -98,6 +98,36 @@ def _validate_obs(cfg, expected, c, blind=False, task=None):
             c.noise_std[k] = std
 
 
+def _lower_rows(cfg, spec: T.TaskSpec, c, expected, task: str, device_terms: bool):
+    """``cfg.observations.policy`` of the Elevation / Visual task.  Without ``device_terms``, or when the term list is not
+    the built-in row's, it is validated onto the built-in row as before (a modified term list raises, naming the task).  With
+    ``device_terms`` a group of the row's own terms whose effective noise (a noise with enable_corruption), clips or scales
+    differ from the built-in row's is lowered to ``spec.row_terms`` (row_terms.py, wl_set_row_terms), refusing by term name
+    what the kernels do not do; a group the built-in row restates exactly is validated as before."""
+    group = cfg.observations.policy
+    terms = [(k, t) for k, t in _fields(group) if hasattr(t, "func")]
+    if not device_terms or [_fname(t) for _, t in terms] != expected or getattr(group, "concatenate_terms", True) is not True:
+        _validate_obs(cfg, expected, c, task=task)
+        return
+    from . import row_terms
+    kind = task.lower()
+    corrupt = bool(getattr(group, "enable_corruption", False))
+    table = []
+    for k, (name, t) in enumerate(terms):
+        if kind == "visual" and k == 0:                     # the camera term: its own augmentation, nothing of this path
+            if getattr(t, "clip", None) is not None or getattr(t, "scale", None) not in (None, 1, 1.0) or (corrupt and getattr(t, "noise", None) is not None):
+                raise NotImplementedError(f"{name}: noise, clip or scale on the camera term is not implemented")
+            continue
+        table.append((name,) + row_terms.lower_term(name, t.func, getattr(t, "noise", None) if corrupt else None, getattr(t, "clip", None),
+                                                    getattr(t, "scale", None), getattr(t, "modifiers", None), getattr(t, "history_length", 0)))
+    if row_terms.is_builtin(kind, [t[1:] for t in table]) and not getattr(group, "history_length", None):
+        _validate_obs(cfg, expected, c, task=task)
+        return
+    if getattr(group, "history_length", None):
+        raise NotImplementedError("policy observation group: history_length is not implemented")
+    spec.row_terms = table
+
+
 def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
     """``cfg.observations.critic`` (an ObservationGroupCfg next to ``policy``) -> ``spec.critic_terms``, the term table of
     ``wl_critic_observe``.  Anything the kernels do not do raises NotImplementedError naming the term; no group, no table."""
@@ -429,7 +459,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     spec = T.elevation_task(num_envs=num_envs, seed=seed, env_id_offset=env_id_offset)
     c = spec.cfg
     _lower_common(cfg, spec)
-    _validate_obs(cfg, _OBS_ELEV, c, task="Elevation")
+    _lower_rows(cfg, spec, c, _OBS_ELEV, "Elevation", device_terms)
     for _, t in _fields(cfg.observations.policy):
         if hasattr(t, "func") and _fname(t) == "world_height_map":
             c.scan_offset, c.scan_plane_init = float(t.params["offset"]), float(t.params["plane_init_value"])
@@ -490,7 +520,7 @@ def _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device
     spec = T.visual_task(num_envs=num_envs, seed=seed, env_id_offset=env_id_offset, traversability=trav, camera=cam_mode, randomize=randomize)
     c = spec.cfg
     _lower_common(cfg, spec)
-    _validate_obs(cfg, [funcs[0]] + _OBS_VIS_TAIL, c, task="Visual")
+    _lower_rows(cfg, spec, c, [funcs[0]] + _OBS_VIS_TAIL, "Visual", device_terms)
     # map geometry (VisualTerrainImporterCfg :63-124) and ground material (:126-135)
     c.vis_row_spacing, c.vis_col_spacing = float(terrain.row_spacing), float(terrain.col_spacing)
     c.vis_width, c.vis_height = float(terrain.width), float(terrain.height)

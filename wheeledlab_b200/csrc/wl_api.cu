@@ -16,6 +16,7 @@ using namespace wl;
 
 #include "wl_critic.cuh"
 #include "wl_policy_obs.cuh"
+#include "wl_row_terms.cuh"
 #include "wl_events.cuh"
 
 // ---------------------------------------------------------------------------------------
@@ -53,6 +54,7 @@ struct wl_sim {
     EventTable events;         // wl_set_event_timers: the interval terms' ranges and per-env timers (n = 0: none)
     struct DevEvents* devents; // wl_set_device_events: the device event terms and their timers (null: none)
     PolicyObsTable pobs;       // wl_set_policy_terms: the policy observation's columns (n_cols = 0: none)
+    RowTable rows;             // wl_set_row_terms: noise, clip and scale of the Elevation / Visual row (n_terms = 0: none)
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1257,7 +1259,11 @@ __device__ __forceinline__ ScanPose scan_pose(const wl_config& c, const float4* 
     q.oy = (int)floorf((q.by - reach - c.hf_y0) * inv);
     return q;
 }
-__device__ __forceinline__ void scan_rays(const wl_config& c, const float* __restrict__ tl, const ScanPose& q, float* __restrict__ row, int tid) {
+// ROW (row terms, DESIGN 6r): the raw world_height_map value (a miss is +inf), then the map term's stages, with the draw of
+// ray r at dz[r] (formed before the tile landed)
+template <bool ROW = false>
+__device__ __forceinline__ void scan_rays(const wl_config& c, const float* __restrict__ tl, const ScanPose& q, float* __restrict__ row, int tid,
+                                          const RowStage* __restrict__ ms = nullptr, const float* __restrict__ dz = nullptr) {
     constexpr int ITER = (WL_SCAN_RAYS + WL_SCAN_THREADS - 1) / WL_SCAN_THREADS;
     const float inv = c.d_inv_hf_cell;
     const float fxmax = (float)(c.hf_nx - 1), fymax = (float)(c.hf_ny - 1);
@@ -1294,8 +1300,14 @@ __device__ __forceinline__ void scan_rays(const wl_config& c, const float* __res
         const float za = fm(z10[j] - z00[j], tx[j], z00[j]), zb = fm(z11[j] - z01[j], tx[j], z01[j]);
         const float hit = fm(zb - za, ty[j], za);
         const float hs = q.bz - hit - c.scan_offset;                              // mdp.height_scan
+        if (ROW) {
+            const int r = min(tid + WL_SCAN_THREADS * j, WL_SCAN_RAYS - 1);
+            const float h = -hs + base;
+            v[j] = row_stage(*ms, inside[j] ? h : __int_as_float(0x7f800000), ms->noise != WL_NOISE_NONE ? dz[r] : 0.0f);
+        } else {
         const float hv = r_clamp(-hs + base, -c.obs_clip, c.obs_clip);           // world_height_map, clip
         v[j] = inside[j] ? hv : c.obs_clip;                                       // miss: +inf clipped
+        }
     }
 #pragma unroll
     for (int j = 0; j < ITER; ++j) {
@@ -1389,6 +1401,74 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);                           // this warp is done with the stage
     }
+}
+
+// The ray-caster of a handle with row terms (DESIGN 6r): the whole 689-float row from the state.  Columns 0..12 are the raw
+// proprioceptive terms (elev_proprio without its clips), columns 13..688 the raw world_height_map of the 676 rays, each
+// through its term's noise, clip and scale.  The draws do not depend on the height-field: every thread forms one or two
+// Philox blocks (4 columns each) into shared memory while the tile is in flight, and thread 32 forms the proprioceptive
+// values meanwhile.  Same launch shape, tile staging and ray arithmetic as wl_scan_kernel.
+template <bool USE_TMA>
+__global__ void __launch_bounds__(WL_SCAN_THREADS, 8)
+wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ RowTable rt,
+                   const float4* __restrict__ st, const float* __restrict__ hf, const wl_globals* __restrict__ gl, uint32_t t_arg,
+                   int32_t call_idx, float* __restrict__ obs) {
+    __shared__ __align__(128) float tile[WL_TILE_W * WL_TILE_H];
+    __shared__ __align__(8) uint64_t mbar;
+    __shared__ ScanPose sp;
+    __shared__ __align__(16) float dz[4 * WL_ROW_BLOCKS];  // the noise draw of every column (float4 stores; only when some column is noisy)
+    __shared__ float raw[WL_ROW_PROPRIO];    // the raw proprioceptive columns
+    const int i = blockIdx.x, n = c.num_envs, tid = threadIdx.x;
+    if (tid == 0) {
+        const ScanPose p = scan_pose(c, st, n, i);
+        sp = p;
+        if (USE_TMA) {
+            mbar_init(&mbar, 1);
+            mbar_init_fence();
+            mbar_expect(&mbar, WL_TILE_W * WL_TILE_H * 4);
+            tma_load_2d(tile, &tmap, p.ox, p.oy, &mbar);
+        }
+    } else if (tid == 32) {
+        const float4 p = ldg4(st, WL_G_POS, n, i), q = ldg4(st, WL_G_QUAT, n, i), v = ldg4(st, WL_G_LINVEL, n, i),
+                     w = ldg4(st, WL_G_ANGVEL, n, i), a = ldg4(st, WL_G_ACTION, n, i), cb = ldg4(st, WL_G_CMDB, n, i);
+        const M3 R = rotmat(q.x, q.y, q.z, q.w);
+        const V3 vb = rotT(R, V3{v.x, v.y, v.z}), wb = rotT(R, V3{w.x, w.y, w.z}), eu = euler_xyz(q.x, q.y, q.z, q.w);
+        const float gx = cb.x - p.x, gy = cb.y - p.y;
+        raw[0] = (gx != gx) ? 0.0f : gx; raw[1] = (gy != gy) ? 0.0f : gy;            // nan_to_num(nan=0)
+        raw[2] = eu.x; raw[3] = eu.y; raw[4] = eu.z;
+        raw[5] = vb.x; raw[6] = vb.y; raw[7] = vb.z; raw[8] = wb.x; raw[9] = wb.y; raw[10] = wb.z;
+        raw[11] = a.x; raw[12] = a.y;
+    }
+    if (rt.noisy) {                          // in the TMA's shadow
+        const uint32_t t = decode_step(gl, t_arg), gid = (uint32_t)(c.env_id_offset + i);
+        for (int b = tid; b < WL_ROW_BLOCKS; b += WL_SCAN_THREADS) {
+            float d[4];
+            if (4 * b >= WL_ROW_PROPRIO) {   // map columns only (the last block's padding draws are not read)
+                if (rt.map.noise != WL_NOISE_NONE) row_draws(row_block(c.seed, gid, t, call_idx, rt.map.noise, (uint32_t)b), rt.map.noise, d);
+                else d[0] = d[1] = d[2] = d[3] = 0.0f;
+            } else {
+                int k[4];
+#pragma unroll
+                for (int w = 0; w < 4; ++w) k[w] = 4 * b + w < WL_ROW_PROPRIO ? rt.col[4 * b + w].noise : rt.map.noise;
+                row_mixed_draws(c.seed, gid, t, call_idx, (uint32_t)b, k, d);
+            }
+            *reinterpret_cast<float4*>(dz + 4 * b) = make_float4(d[0], d[1], d[2], d[3]);
+        }
+    }
+    __syncthreads();                         // constants, mbarrier, draws and raw columns visible to everyone
+    const ScanPose q = sp;
+    float* row = obs + (size_t)WL_OBS_DIM_ELEV * i;
+    if (tid < WL_ROW_PROPRIO) row[tid] = row_stage(rt.col[tid], raw[tid], rt.col[tid].noise != WL_NOISE_NONE ? dz[tid] : 0.0f);
+    if (USE_TMA) {
+        mbar_wait_parity(&mbar, 0);
+    } else {
+        for (int k = tid; k < WL_TILE_W * WL_TILE_H; k += WL_SCAN_THREADS) {
+            int tx = k % WL_TILE_W, ty = k / WL_TILE_W, gx = q.ox + tx, gy = q.oy + ty;
+            tile[k] = (gx >= 0 && gy >= 0 && gx < c.hf_nx && gy < c.hf_ny) ? __ldg(hf + (size_t)gy * c.hf_pitch + gx) : 0.0f;
+        }
+        __syncthreads();
+    }
+    scan_rays<true>(c, tile, q, row + WL_ROW_PROPRIO, tid, &rt.map, dz + WL_ROW_PROPRIO);
 }
 
 #include "wl_reset_dr.cuh"
@@ -1715,6 +1795,11 @@ static int refuse_pobs(const wl_sim* sim, const char* fn) {
     return fail(WL_EUNSUPPORTED, std::string(fn) + ": the handle has a policy observation table, whose row wl_policy_observe forms "
                                  "(wl_set_policy_terms(0) first)");
 }
+// a call that writes the built-in Elevation / Visual row in its own kernel refuses a handle with row terms, before any device work
+static int refuse_rows(const wl_sim* sim, const char* fn) {
+    if (sim->rows.n_terms == 0) return WL_OK;
+    return fail(WL_EUNSUPPORTED, std::string(fn) + ": the handle has row terms, which wl_step writes (wl_set_row_terms(0) first)");
+}
 // the width of the row the policy kernels read: the policy table's when the handle has one, else the built-in row's
 static int policy_in_dim(const wl_sim* sim) { return sim->pobs.n_cols ? sim->pobs.n_cols : sim->obs_dim; }
 
@@ -1917,8 +2002,17 @@ static int duo_block(wl_sim* sim, KF kernel, int grid) {
     return sim->duo_threads;
 }
 
-static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
+// t: the step counter (host value or WL_DEVICE_COUNTER_PLUS(k)); call_idx: -1 after a step, wl_observe's otherwise.  Both
+// key the row terms' noise only.
+static int launch_scan(wl_sim* sim, float* d_obs, uint32_t t, int32_t call_idx, cudaStream_t cs) {
     const int n = sim->cfg.num_envs;
+    if (sim->rows.n_terms) {                                 // row terms: the whole row (scan mode 2 is refused with them)
+        if (sim->scan_mode >= 1 && sim->has_tmap)
+            wl_scan_row_kernel<true><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->rows, sim->state, sim->hf, sim->globals, t, call_idx, d_obs);
+        else
+            wl_scan_row_kernel<false><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->rows, sim->state, sim->hf, sim->globals, t, call_idx, d_obs);
+        return launched(sim, "wl_scan_row_kernel");
+    }
     if (sim->scan_mode == 2 && sim->has_tmap) {              // TMA producer/consumer pipeline, persistent CTAs
         static const int per_sm = [] { const char* e = getenv("WL_SCAN_CTAS_PER_SM"); int v = e ? atoi(e) : 6; return v < 1 ? 1 : (v > 12 ? 12 : v); }();
         const int grid = n < WL_NUM_SMS * per_sm ? n : WL_NUM_SMS * per_sm;    // (WL_SCAN_CTAS_PER_SM: tuning experiments only)
@@ -1928,6 +2022,14 @@ static int launch_scan(wl_sim* sim, float* d_obs, cudaStream_t cs) {
     else
         wl_scan_kernel<false><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->state, sim->hf, d_obs);
     return launched(sim, "wl_scan_kernel");
+}
+// the Visual tail through the row terms, after every launch that writes the Visual row (nothing without row terms)
+static int launch_visual_row(wl_sim* sim, float* d_obs, uint32_t t, int32_t call_idx, cudaStream_t cs) {
+    if (!sim->rows.n_terms) return WL_OK;
+    const int n = sim->cfg.num_envs;
+    wl_visual_row_kernel<<<(n + WL_ROW_VIS_BS - 1) / WL_ROW_VIS_BS, WL_ROW_VIS_BS, 0, cs>>>(
+        sim->rows, sim->state, sim->globals, n, vis_cam_floats(sim->cfg), sim->cfg.seed, sim->cfg.env_id_offset, t, call_idx, d_obs);
+    return launched(sim, "wl_visual_row_kernel");
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2165,6 +2267,7 @@ int32_t wl_obs_dim(const wl_sim* sim) { return sim ? sim->obs_dim : 0; }
 int wl_set_scan_tma(wl_sim* sim, int32_t use_tma) {
     if (!sim) return fail(WL_EINVAL, "wl_set_scan_tma: null handle");
     if (use_tma < 0 || use_tma > 2) return fail(WL_EINVAL, "wl_set_scan_tma: 0, 1 or 2");
+    if (use_tma == 2 && sim->rows.n_terms) return fail(WL_EUNSUPPORTED, "wl_set_scan_tma: the pipelined ray-caster (2) has no row-terms variant");
     sim->scan_mode = use_tma;
     return WL_OK;
 }
@@ -2296,8 +2399,9 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     }
     sim->step_variant = variant; sim->step_specialised = specialised; sim->step_threads = cta_threads;
     if (int rc = launched(sim, "wl_step_kernel")) return rc;
-    if (elev) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
+    if (elev) { if (int rc = launch_scan(sim, d_obs, t, -1, cs)) return rc; }
     if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
+    if (vis) { if (int rc = launch_visual_row(sim, d_obs, t, -1, cs)) return rc; }
     if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
     return post_step(sim, step_counter, cs);
 }
@@ -2355,9 +2459,10 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
     if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, (uint32_t)step_counter,
                                  StageIO{const_cast<uint8_t*>(d_term_bits), d_extra_terminated, d_extra_truncated}, (cudaStream_t)stream))
         return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (cudaStream_t)stream)) return rc; }
+    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
+    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
     if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
     return post_step(sim, step_counter, (cudaStream_t)stream);
 }
@@ -2384,9 +2489,10 @@ int wl_step_stage_b2(wl_sim* sim, float* d_obs, int64_t step_counter, void* stre
     if (int rc = launch_stage<4>(sim, nullptr, d_obs, nullptr, nullptr, nullptr, nullptr, (uint32_t)step_counter,
                                  StageIO{nullptr, nullptr, nullptr}, (cudaStream_t)stream))
         return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (cudaStream_t)stream)) return rc; }
+    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
+    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
     return WL_OK;
 }
 
@@ -2589,9 +2695,10 @@ int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew
     } else if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, t, sio, cs)) {
         return rc;
     }
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, cs)) return rc; }
+    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, t, -1, cs)) return rc; }
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
         if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc;   // t may be device-relative
+    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, t, -1, cs)) return rc; }
     if (!de) { if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc; }
     return post_step(sim, step_counter, cs);
 }
@@ -2603,6 +2710,7 @@ int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_
     if (int rc = refuse_fan(sim, "wl_rollout")) return rc;
     if (int rc = refuse_devents(sim, "wl_rollout")) return rc;
     if (int rc = refuse_pobs(sim, "wl_rollout")) return rc;
+    if (int rc = refuse_rows(sim, "wl_rollout")) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, "wl_rollout: the elevation step is two kernels (use wl_step)");
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam) return fail(WL_EUNSUPPORTED, "wl_rollout: the camera term is a second kernel (use wl_step)");
     if (sim->reset_ev) return fail(WL_EUNSUPPORTED, "wl_rollout: the reset-mode DR events are a second kernel after each step (use wl_step)");
@@ -2677,14 +2785,17 @@ int wl_step_host_zero_copy(wl_sim* sim, const float* h_action, float* d_obs, flo
 
 int wl_observe(wl_sim* sim, float* d_obs, int64_t step_counter, int32_t call_idx, void* stream) {
     if (!sim || !d_obs) return fail(WL_EINVAL, "wl_observe: null argument");
+    if (sim->rows.n_terms && (call_idx < 0 || call_idx > WL_ROW_MAX_CALL))
+        return fail(WL_EINVAL, "wl_observe: with row terms call_idx must be in 0..2^23-2 (it keys their noise)");
     ensure_device(sim);
     const int n = sim->cfg.num_envs, bs = 128;
     wl_observe_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, d_obs, (uint32_t)step_counter,
                                                                          (uint32_t)call_idx);
     if (int rc = launched(sim, "wl_observe_kernel")) return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) return launch_scan(sim, d_obs, (cudaStream_t)stream);
+    if (sim->cfg.task == WL_TASK_ELEVATION) return launch_scan(sim, d_obs, (uint32_t)step_counter, call_idx, (cudaStream_t)stream);
     if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
-        return launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM_EXTRA, (uint32_t)call_idx, nullptr, (cudaStream_t)stream);
+        if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM_EXTRA, (uint32_t)call_idx, nullptr, (cudaStream_t)stream)) return rc;
+    if (sim->cfg.task == WL_TASK_VISUAL) return launch_visual_row(sim, d_obs, (uint32_t)step_counter, call_idx, (cudaStream_t)stream);
     return WL_OK;
 }
 
@@ -2821,6 +2932,57 @@ int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float
     return launched(sim, "wl_policy_observe_kernel");
 }
 
+int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) {
+    const std::string fn = "wl_set_row_terms: ";
+    if (!sim) return fail(WL_EINVAL, fn + "null handle");
+    if (n_terms > 0 && !terms) return fail(WL_EINVAL, fn + "null term table");
+    const int task = sim->cfg.task;
+    if (task != WL_TASK_ELEVATION && task != WL_TASK_VISUAL)
+        return fail(WL_EUNSUPPORTED, fn + "row terms are implemented for the Elevation and Visual tasks (the Drift family's groups go through wl_set_policy_terms)");
+    if (fan_set(sim)) return fail(WL_EUNSUPPORTED, fn + "the peer fan-out is set, and only the built-in row carries it");
+    if (sim->scan_mode == 2 && task == WL_TASK_ELEVATION)
+        return fail(WL_EUNSUPPORTED, fn + "the pipelined ray-caster (wl_set_scan_tma(2)) has no row-terms variant");
+    static const int elev[WL_ROW_TERMS_ELEVATION] = {WL_ROW_GOAL_RELATIVE_XYZ, WL_CRITIC_ROOT_EULER_XYZ, WL_CRITIC_BASE_LIN_VEL,
+                                                     WL_CRITIC_BASE_ANG_VEL, WL_CRITIC_LAST_ACTION, WL_ROW_WORLD_HEIGHT_MAP};
+    static const int vis[WL_ROW_TERMS_VISUAL] = {WL_CRITIC_BASE_LIN_VEL, WL_CRITIC_BASE_ANG_VEL, WL_CRITIC_LAST_ACTION};
+    const int* kinds = task == WL_TASK_ELEVATION ? elev : vis;
+    const int count = task == WL_TASK_ELEVATION ? WL_ROW_TERMS_ELEVATION : WL_ROW_TERMS_VISUAL;
+    if (n_terms != 0 && n_terms != count)
+        return fail(WL_EINVAL, fn + "n_terms must be 0 or the task's " + std::to_string(count) + " terms");
+    RowTable tb;
+    memset(&tb, 0, sizeof tb);
+    int col = 0;
+    for (int k = 0; k < n_terms; ++k) {
+        const wl_policy_term& d = terms[k];
+        const std::string at = fn + "term " + std::to_string(k) + ": ";
+        if (d.kind != kinds[k]) return fail(WL_EINVAL, at + "kind " + std::to_string(d.kind) + " is not the row's term " + std::to_string(kinds[k]));
+        if (d.noise < WL_NOISE_NONE || d.noise > WL_NOISE_UNIFORM) return fail(WL_EINVAL, at + "unknown noise model " + std::to_string(d.noise));
+        const bool map = d.kind == WL_ROW_WORLD_HEIGHT_MAP;
+        const int w = map ? WL_SCAN_RAYS : d.kind == WL_ROW_GOAL_RELATIVE_XYZ ? 2 : critic_width(d.kind);
+        if (map ? (d.n_scale != 0 && d.n_scale != 1) : (d.n_scale != 0 && d.n_scale != 1 && d.n_scale != w))
+            return fail(WL_EINVAL, at + (map ? "n_scale must be 0 or 1 on the height map" : "n_scale must be 0, 1 or the term's width"));
+        bool finite = std::isfinite(d.noise_params[0]) && std::isfinite(d.noise_params[1]) && std::isfinite(d.clip_range[0]) &&
+                      std::isfinite(d.clip_range[1]);
+        for (int s = 0; s < 4; ++s) finite = finite && std::isfinite(d.scale[s]);
+        if (!finite) return fail(WL_EINVAL, at + "a noise, clip or scale parameter is not finite");
+        for (int j = 0; j < (map ? 1 : w); ++j) {
+            RowStage& s = map ? tb.map : tb.col[col++];
+            s.noise = sim->cfg.enable_corruption ? d.noise : WL_NOISE_NONE;
+            s.na = (float)d.noise_params[0];
+            s.nb = d.noise == WL_NOISE_UNIFORM ? (float)(d.noise_params[1] - d.noise_params[0]) : (float)d.noise_params[1];
+            s.flags = (d.clip ? WL_ROW_CLIP : 0u) | (d.n_scale ? WL_ROW_SCALE : 0u);
+            s.lo = (float)d.clip_range[0];
+            s.hi = (float)d.clip_range[1];
+            s.sc = d.n_scale ? (float)d.scale[d.n_scale == 1 ? 0 : j] : 1.0f;
+            tb.noisy |= s.noise != WL_NOISE_NONE;
+        }
+    }
+    tb.n_terms = n_terms;
+    sim->rows = tb;
+    return WL_OK;
+}
+int32_t wl_row_terms(const wl_sim* sim) { return sim ? sim->rows.n_terms : 0; }
+
 int wl_set_reset_events(wl_sim* sim, uint32_t mask) {
     if (!sim) return fail(WL_EINVAL, "wl_set_reset_events: null handle");
     const uint32_t all = WL_RESET_EV_MATERIAL | WL_RESET_EV_ACTUATOR_GAINS | WL_RESET_EV_BASE_MASS | WL_RESET_EV_WHEEL_MASS;
@@ -2853,6 +3015,7 @@ static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float*
     if (int rc = refuse_fan(sim, fn)) return rc;
     if (int rc = refuse_devents(sim, fn)) return rc;
     if (int rc = refuse_pobs(sim, fn)) return rc;
+    if (int rc = refuse_rows(sim, fn)) return rc;
     if (sim->cfg.task == WL_TASK_ELEVATION) return fail(WL_EUNSUPPORTED, std::string(fn) + ": blind-observation tasks only (obs_dim <= 16)");
     if (sim->obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16");
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))

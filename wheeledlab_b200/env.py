@@ -318,6 +318,7 @@ class ManagerBasedRLEnv:
         self._critic_terms = []                  # the critic observation group (set_critic_observation)
         self._policy_terms = []                  # a modified policy observation group (set_policy_observation)
         self._policy_ring = None
+        self._row_terms = []                     # noise, clip and scale on the Elevation / Visual row (set_row_terms)
         for name, func, weight, params in self.spec.python_reward_terms:
             self.add_reward_term(name, func, weight, params)
         for name, func, time_out, params in self.spec.python_termination_terms:
@@ -342,6 +343,8 @@ class ManagerBasedRLEnv:
             self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
         if self.spec.policy_terms:
             self.set_policy_observation([(name, fn, {"noise": nz, "clip": cl, "scale": sc}) for name, fn, nz, cl, sc in self.spec.policy_terms])
+        if self.spec.row_terms:
+            self.set_row_terms([(name, fn, {"noise": nz, "clip": cl, "scale": sc}) for name, fn, nz, cl, sc in self.spec.row_terms])
         # event_manager.apply(mode="startup")
         self.sim.startup()
         self._needs_reset = True
@@ -461,6 +464,37 @@ class ManagerBasedRLEnv:
         self.observation_manager.group_obs_dim["policy"] = (d,)
         self.single_observation_space = {"policy": _Box(-math.inf, math.inf, (d,))}
         self.observation_space = {"policy": _Box(-math.inf, math.inf, (self.num_envs, d))}
+
+    # -- noise, clip and scale on the Elevation / Visual row (row_terms.py, wl_set_row_terms; DESIGN 6r) ---------------------
+    def set_row_terms(self, terms):
+        """Noise, clip and scale on the built-in Elevation or Visual ``policy`` row: `terms` is a list of (name, fn, params),
+        one per term of the row in its order (Elevation: ``goal_relative_xyz``, ``root_euler_xyz``, ``base_lin_vel``,
+        ``base_ang_vel``, ``last_action``, ``world_height_map``; Visual after the camera term: ``base_lin_vel``,
+        ``base_ang_vel``, ``last_action``), `fn` the function or its name; `params` may hold ``noise`` (an
+        ``AdditiveGaussianNoiseCfg`` / ``AdditiveUniformNoiseCfg`` or ``("gaussian", mean, std)`` / ``("uniform", n_min,
+        n_max)``, drawn when the config's enable_corruption is set), ``clip=(lo, hi)`` and ``scale``, applied in that order
+        after the raw value, as IsaacLab's ObservationManager does.  A term without a clip is unclipped: the registered
+        group's clips must be restated (``row_terms.registered``).  The row's width does not change.  A term list other
+        than the row's own raises NotImplementedError; ``[]`` restores the built-in row.  Every path that writes the row
+        (``step``, device terms and events, the staged step of host-side Python terms, ``reset`` / ``get_observations``,
+        ``step_host``) writes the modified one."""
+        from . import row_terms
+        from .tasks import TASK_ELEVATION, TASK_VISUAL
+        task = {TASK_ELEVATION: "elevation", TASK_VISUAL: "visual"}.get(self.spec.cfg.task, "drift")
+        terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
+        table = []
+        for name, fn, params in terms:
+            p = dict(params or {})
+            table.append(row_terms.lower_term(name, fn, p.pop("noise", None), p.pop("clip", None), p.pop("scale", None)))
+        if table:
+            row_terms.check_order(task, [t[0] for t in table])
+        self.sim.set_row_terms(table)
+        self._row_terms = [(name,) + t for (name, _, _), t in zip(terms, table)]
+
+    @property
+    def row_terms(self) -> list:
+        """The env's row terms as ``(name, row term, noise, clip, scale)`` (``TaskSpec.row_terms``' form); [] = none."""
+        return list(self._row_terms)
 
     def _obs_groups(self, obs: torch.Tensor) -> dict:
         """The observation dict of the current state: ``policy`` and, with a critic group, a fresh ``critic`` row; the same

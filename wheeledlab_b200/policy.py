@@ -300,6 +300,8 @@ class FusedPolicyRollout:
         if activation == "relu" and (sim.num_envs * sim.obs_dim) % 2:
             raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
         self.table = sim.policy_obs_dim > 0
+        # row terms (DESIGN 6r): the fused act step writes the built-in row, so the policy kernel and wl_step are separate
+        self.rows = sim.row_terms > 0
         D = sim.policy_width
         self.slab = slab or RolloutSlab(T, sim.num_envs, D, 2, sim.device, policy_fields=not self.deterministic,
                                         critic_obs_dim=sim.critic_obs_dim if self.critic else None)
@@ -368,8 +370,8 @@ class FusedPolicyRollout:
                 self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
                 self.sim.critic_observe(out=self.slab.critic_obs_in[k + 1])
             elif self.deterministic:
-                if self.activation == "relu":
-                    actor_mean(self.blob, self.sim.obs_dim, self.slab.obs_in[k], "relu", out=self.slab.actions[k])
+                if self.activation == "relu" or self.rows:
+                    actor_mean(self.blob, self.sim.obs_dim, self.slab.obs_in[k], self.activation, out=self.slab.actions[k])
                     self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
                 else:
                     act_infer_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.slab.step_outputs(k),
@@ -378,9 +380,9 @@ class FusedPolicyRollout:
                 policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
                            self.pol.values[k], t, self.activation)
                 self.sim.step_terms(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k], term_log=self.term_logs[k])
-            elif self.activation == "relu":
+            elif self.activation == "relu" or self.rows:
                 policy_act(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
-                           self.pol.values[k], t)
+                           self.pol.values[k], t, self.activation)
                 self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
             else:
                 act_step(self.sim, self.slab.obs_in[k], self.blob, self.slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],

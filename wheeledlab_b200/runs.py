@@ -30,14 +30,18 @@ def task_activation(task: str) -> str:
     return "relu" if name in ("elevation", "visual", "visual_random") else "elu"
 
 
-def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict, policy_terms=None) -> str:
+def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict, policy_terms=None, row_terms=None) -> str:
     """`policy_terms`: the env's policy observation table (``(name, library term, noise, clip, scale)`` as
-    ``TaskSpec.policy_terms`` holds it), so that playback observes what the policy was trained on; None: the built-in row."""
+    ``TaskSpec.policy_terms`` holds it), so that playback observes what the policy was trained on; None: the built-in row.
+    `row_terms`: the Elevation / Visual env's row terms in the same form (``env.row_terms``, ``TaskSpec.row_terms``): their
+    clips and scales change the policy's input even where playback draws no noise."""
     os.makedirs(log_dir, exist_ok=True)
     path = os.path.join(log_dir, RUN_CONFIG)
     cfg = {"task": task, "num_envs": int(num_envs), "seed": int(seed), "agent_cfg": agent}
     if policy_terms:
         cfg["policy_terms"] = [list(t) for t in policy_terms]
+    if row_terms:
+        cfg["row_terms"] = [list(t) for t in row_terms]
     with open(path, "w") as f:
         json.dump(cfg, f, indent=1)
     return path

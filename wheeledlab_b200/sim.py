@@ -36,6 +36,31 @@ def upload_graph(graph: "torch.cuda.CUDAGraph", stream=None):
     check(lib.wl_graph_upload(C.c_void_p(int(graph.raw_cuda_graph_exec())), C.c_void_p(st.cuda_stream)), "wl_graph_upload")
 
 
+def _policy_term_array(terms, library: dict, what: str):
+    """``[(name, noise, clip, scale)]`` (a bare name: none of them) -> (the normalised list, a wl_policy_term array)."""
+    terms = [(t, None, None, None) if isinstance(t, str) else tuple(t) + (None,) * (4 - len(t)) for t in terms]
+    arr = (_lib.WlPolicyTerm * max(1, len(terms)))()
+    for k, (name, noise, clip, scale) in enumerate(terms):
+        if name not in library:
+            raise ValueError(f"{what} {name!r} is not in the library {sorted(library)}")
+        if noise is not None and noise[0] not in _lib.WL_NOISE:
+            raise ValueError(f"{what} {name!r}: unknown noise model {noise[0]!r}")
+        d = arr[k]
+        d.kind = library[name][0]
+        if noise is not None:
+            d.noise = _lib.WL_NOISE[noise[0]]
+            d.noise_params[0], d.noise_params[1] = float(noise[1]), float(noise[2])
+        if clip is not None:
+            d.clip = 1
+            d.clip_range[0], d.clip_range[1] = float(clip[0]), float(clip[1])
+        if scale is not None:
+            scale = (float(scale),) if isinstance(scale, (int, float)) else tuple(float(s) for s in scale)
+            d.n_scale = len(scale)
+            for j, s in enumerate(scale[:4]):
+                d.scale[j] = s
+    return terms, arr
+
+
 def _device_u8_view(ptr: int, n: int, device) -> torch.Tensor:
     """uint8 [n] tensor over device memory the library owns (through __cuda_array_interface__; torch does not own it)."""
     class _Arr:
@@ -413,28 +438,24 @@ class WheeledSim:
         """The handle's policy observation table (wl_set_policy_terms): a list of ``(library name, noise, clip, scale)``
         (``policy_obs.lower_term``'s form; a bare name is a term without noise, clip or scale), concatenated in this order
         into the policy row; [] clears it.  Returns Dp.  Nothing is launched; a graph captured earlier keeps its table."""
-        terms = [(t, None, None, None) if isinstance(t, str) else tuple(t) + (None,) * (4 - len(t)) for t in terms]
-        arr = (_lib.WlPolicyTerm * max(1, len(terms)))()
-        for k, (name, noise, clip, scale) in enumerate(terms):
-            if name not in _lib.WL_POLICY_TERMS:
-                raise ValueError(f"policy term {name!r} is not in the library {sorted(_lib.WL_POLICY_TERMS)}")
-            if noise is not None and noise[0] not in _lib.WL_NOISE:
-                raise ValueError(f"policy term {name!r}: unknown noise model {noise[0]!r}")
-            d = arr[k]
-            d.kind = _lib.WL_POLICY_TERMS[name][0]
-            if noise is not None:
-                d.noise = _lib.WL_NOISE[noise[0]]
-                d.noise_params[0], d.noise_params[1] = float(noise[1]), float(noise[2])
-            if clip is not None:
-                d.clip = 1
-                d.clip_range[0], d.clip_range[1] = float(clip[0]), float(clip[1])
-            if scale is not None:
-                scale = (float(scale),) if isinstance(scale, (int, float)) else tuple(float(s) for s in scale)
-                d.n_scale = len(scale)
-                for j, s in enumerate(scale[:4]):
-                    d.scale[j] = s
+        terms, arr = _policy_term_array(terms, _lib.WL_POLICY_TERMS, "policy term")
         check(lib.wl_set_policy_terms(self._h, arr, len(terms)), "wl_set_policy_terms")
         return self.policy_obs_dim
+
+    def set_row_terms(self, terms) -> int:
+        """The handle's row terms (wl_set_row_terms, DESIGN 6r): noise, clip and scale on the Elevation or Visual built-in
+        row, one ``(name, noise, clip, scale)`` per term of the row in row order (``row_terms.lower_term``'s form; a bare
+        name has none of them, so it is the raw value); [] clears them.  The names are the row's own
+        (``_lib.WL_ROW_TASK_TERMS``).  Returns the number of terms.  Nothing is launched; a graph captured earlier keeps the
+        terms it was captured with."""
+        terms, arr = _policy_term_array(terms, _lib.WL_ROW_TERMS, "row term")
+        check(lib.wl_set_row_terms(self._h, arr, len(terms)), "wl_set_row_terms")
+        return self.row_terms
+
+    @property
+    def row_terms(self) -> int:
+        """The number of row terms of the handle (0: the built-in row)."""
+        return int(lib.wl_row_terms(self._h))
 
     @property
     def policy_obs_dim(self) -> int:

@@ -74,6 +74,9 @@ class TaskSpec:
     # a modified policy observation group (policy_obs.py, wl_policy_observe): [(name, library term, noise, clip, scale)] in row
     # order; [] = the built-in row.  obs_dim stays the built-in row's width; the policy side is sized by the table's
     policy_terms: list = field(default_factory=list)
+    # noise, clip and scale on the Elevation / Visual row (row_terms.py, wl_set_row_terms): [(name, row term, noise, clip,
+    # scale)], one per term of the built-in row in row order; [] = the built-in row
+    row_terms: list = field(default_factory=list)
     # DR events in IsaacLab's mode="reset" (wl_set_reset_events): names of _lib.WL_RESET_EVENTS; [] = start-up DR only
     reset_events: list = field(default_factory=list)
 
