@@ -136,6 +136,40 @@ def summarize(recs, tag, n_launch_expected):
         "launches whose last env-warp store is from such a late warp": int(sum(last_is_late)),
     })
     out.update(pass_cycles(recs))
+    out.update(tails(recs, L))
+    return out
+
+
+def tails(recs, launches):
+    """Which warp of each CTA stores last, which one ends the launch, and the segments outside the sub-step loop (ns,
+    median over launches of the per-launch median warp): env warp wait -> bar.sync 1 and bar.arrive 2 -> last store, aux
+    warp wait -> bar.arrive 1 and bar.sync 2 -> last store"""
+    import numpy as np
+    aux_last_cta, aux_ends_launch, tail_gap = [], 0, []
+    seg = {"env: griddepcontrol.wait -> bar.sync 1": [], "env: bar.arrive 2 -> last store": [],
+           "aux: griddepcontrol.wait -> bar.arrive 1": [], "aux: bar.sync 2 -> last store": []}
+    for ix in launches:
+        ix = np.asarray(ix)
+        ts = recs["ts"][ix].astype(np.int64)
+        role, cta = recs["role"][ix], recs["cta"][ix]
+        for name, r, a, b in (("env: griddepcontrol.wait -> bar.sync 1", 0, 2, 4), ("env: bar.arrive 2 -> last store", 0, 13, 14),
+                              ("aux: griddepcontrol.wait -> bar.arrive 1", 1, 2, 4), ("aux: bar.sync 2 -> last store", 1, 13, 14)):
+            m = (role == r) & (ts[:, a] > 0) & (ts[:, b] > 0)
+            if m.any():
+                seg[name].append(float(np.median(ts[m, b] - ts[m, a])))
+        env_last = {int(c): int(v) for c, v in zip(cta[role == 0], ts[role == 0, 14])}
+        aux_last = {int(c): int(v) for c, v in zip(cta[role == 1], ts[role == 1, 14])}
+        both = [c for c in env_last if c in aux_last]
+        if both:
+            aux_last_cta.append(sum(aux_last[c] > env_last[c] for c in both) / len(both))
+            tail_gap.append(float(np.median([aux_last[c] - env_last[c] for c in both])))
+        aux_ends_launch += int(role[int(np.argmax(ts[:, 14]))] == 1)
+    out = {k: _median(v) for k, v in seg.items()}
+    out.update({
+        "CTAs whose aux warp stores after its env warp (fraction, median)": _median(aux_last_cta),
+        "aux last store - env last store, same CTA (ns, median)": _median(tail_gap),
+        "launches whose last store is an aux warp's": aux_ends_launch,
+    })
     return out
 
 

@@ -171,14 +171,17 @@ __device__ __forceinline__ bool janitor_cta(const wl_config& c, wl_globals* __re
     }
     return true;
 }
+template <int WIDTH = 32>
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    for (int o = WIDTH / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
 // Finished envs -> this step's accumulator row: warp-shuffle reduce, one RED set per warp (no fence, no ticket: the
 // kernel boundary publishes the row to the next launch).  acc layout: [0..7] episode sums, [8] #reset, [9+j] #envs whose
-// termination term j fired (tmask bit j).
+// termination term j fired (tmask bit j).  WIDTH = 8: only lanes 0..7 can contribute, and the lanes above add zeros to the
+// full butterfly, so three steps give lanes 0..7 the same nonzero sums; lanes 0..15 then issue the 16 REDs side by side.
+template <int WIDTH = 32>
 __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool contrib, uint32_t tmask,
                                                const float sums[WL_MAX_REW_TERMS]) {
     const unsigned any_c = __ballot_sync(0xffffffffu, contrib);
@@ -190,8 +193,16 @@ __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool con
 #pragma unroll
     for (int j = 0; j < WL_MAX_TERM_TERMS; ++j) vals[9 + j] = (contrib && ((tmask >> j) & 1u)) ? 1.0f : 0.0f;
 #pragma unroll
-    for (int k = 0; k < 16; ++k) vals[k] = warp_sum(vals[k]);
-    if ((threadIdx.x & 31) == 0) {
+    for (int k = 0; k < 16; ++k) vals[k] = warp_sum<WIDTH>(vals[k]);
+    if (WIDTH < 32) {
+        const int lane = threadIdx.x & 31, m = lane & 7;
+        float a = vals[0], b = vals[8];
+#pragma unroll
+        for (int k = 1; k < 8; ++k) { a = sel(m == k, vals[k], a); b = sel(m == k, vals[8 + k], b); }
+        a = __shfl_sync(0xffffffffu, a, m); b = __shfl_sync(0xffffffffu, b, m);
+        const float v = (lane < 8) ? a : b;                   // lane k < 16: element k, as lanes 0..7 hold it
+        if (lane < 16 && v != 0.0f) atomicAdd(&acc[lane], v);
+    } else if ((threadIdx.x & 31) == 0) {
 #pragma unroll
         for (int k = 0; k < 16; ++k) if (vals[k] != 0.0f) atomicAdd(&acc[k], vals[k]);
     }
@@ -316,11 +327,19 @@ wl_step_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_
 // chassis is integrated redundantly in the 4 lanes.  Used when N is too small to fill the chip with one thread/env.
 // quad_env_step = sections A..I of ONE env.step() on register-resident state `e` (lane-local view, see load_env_quad).
 // lane w of an env's quad computes ONE of the three euler angles (lane 0 roll, 1 pitch, 2 and 3 yaw), wrapped to [0, 2 pi)
+// SEL: the pitch override, the atan2 zero cases and the wrap as selects, with no lane-divergent region.  The pitch root is
+// needed only for |sin_pitch| < 1, where (1 - s)(1 + s) >= 2^-24 is normal, so the fast-path root is the IEEE one.
+template <bool SEL = false>
 __device__ __forceinline__ float euler_lane(float qw, float qx, float qy, float qz, int w) {
     float sin_roll = 2.0f * fm(qw, qx, qy * qz), cos_roll = fm(-2.0f, fm(qx, qx, qy * qy), 1.0f);
     float sin_pitch = 2.0f * fm(qw, qy, -(qz * qx));
     float sin_yaw = 2.0f * fm(qw, qz, qx * qy), cos_yaw = fm(-2.0f, fm(qy, qy, qz * qz), 1.0f);
     float ay = (w == 0) ? sin_roll : (w == 1) ? sin_pitch : sin_yaw;
+    if (SEL) {
+        const float ax = sel(w == 1, fsqrt_norm((1.0f - sin_pitch) * (1.0f + sin_pitch)), (w == 0) ? cos_roll : cos_yaw);
+        const float ovr = (sin_pitch < 0.0f) ? -1.57079632679489661923f : 1.57079632679489661923f;
+        return wrap_2pi(sel(w == 1 && fabsf(sin_pitch) >= 1.0f, ovr, det_atan2_sel(ay, ax)));
+    }
     float ax = (w == 0) ? cos_roll : (w == 1) ? sqrtf((1.0f - sin_pitch) * (1.0f + sin_pitch)) : cos_yaw;
     float ang = det_atan2(ay, ax);
     if (w == 1 && fabsf(sin_pitch) >= 1.0f) ang = (sin_pitch < 0.0f) ? -1.57079632679489661923f : 1.57079632679489661923f;
@@ -604,7 +623,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             t_hf = fst[((size_t)WL_G_LINVEL * n + ii) * 4 + 3]; t_lf = fst[((size_t)WL_G_ANGVEL * n + ii) * 4 + 3];
         }
         float wts[WL_MAX_REW_TERMS];
-        load_weights(c, gl, t, wts);
+        if (!S::fixed) load_weights(c, gl, t, wts);
         TR(TR_LOADS, __float_as_uint(a.x) ^ __float_as_uint(s1.w) ^ __float_as_uint(t_lf));
         // A. action map -> targets of the whole env step
         if (lane < 8) {
@@ -669,6 +688,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             TR(TR_AUX_ARRIVE3, __float_as_uint(eu));
         }
         bar_arrive(3);
+        // (a fixed spec loads the weights only now, off the way to bar.arrive 1: only the rewards below read them)
+        if (S::fixed) load_weights(c, gl, t, wts);
         // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
         bar_sync(2);
         TR(TR_ARRIVE2, __float_as_uint(sh.fin[j][0]));
@@ -682,9 +703,10 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             const uint32_t raw = __float_as_uint(fi[12]);
             const bool time_out = (raw & 1u) != 0u, oob = (raw & 2u) != 0u;
             float f[WL_MAX_REW_TERMS];
-            drift_reward_terms(c, fi[10], fi[11], det_atan2(vb.y, vb.x), p, vb, wb, fi[9], oob, time_out, f);
+            if (S::fixed) drift_reward_terms<true>(c, fi[10], fi[11], det_atan2_sel(vb.y, vb.x), p, vb, wb, fi[9], oob, time_out, f);
+            else drift_reward_terms(c, fi[10], fi[11], det_atan2(vb.y, vb.x), p, vb, wb, fi[9], oob, time_out, f);
             tmask = raw & (uint32_t)c.term_enable;
-            const float total = weigh_rewards(c, wts, f, sums);
+            const float total = weigh_rewards<S::fixed>(c, wts, f, sums);
             done = tmask != 0u;
             // fan-out active, full CTA, aligned rows: 32 + 8 + 8 contiguous bytes leave as four wide stores (one NVLink /
             // multicast write each instead of 24 small ones); otherwise element by element (without peers the staging round
@@ -698,13 +720,16 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
                 if (lane < 2) fan_store16<FAN == 2>(pf, reinterpret_cast<float4*>(rew + env0) + lane, reinterpret_cast<const float4*>(sh.rewrow)[lane]);
                 else if (lane == 2) fan_store8<FAN == 2>(pf, reinterpret_cast<float2*>(terminated_o + env0), *reinterpret_cast<const float2*>(sh.maskrow[0]));
                 else if (lane == 3) fan_store8<FAN == 2>(pf, reinterpret_cast<float2*>(truncated_o + env0), *reinterpret_cast<const float2*>(sh.maskrow[1]));
+            } else if (S::fixed) {
+                st_global_if(reinterpret_cast<float*>(rew + i), total, live);
+                st_global_if(terminated_o + i, tb, live); st_global_if(truncated_o + i, ub, live);
             } else if (live) {
                 if (FAN == 1) { fan_store(pf, &rew[i], total); fan_store(pf, &terminated_o[i], tb); fan_store(pf, &truncated_o[i], ub); }
                 else { rew[i] = total; terminated_o[i] = tb; truncated_o[i] = ub; }
             }
             if (live && term_bits != nullptr) term_bits[i] = (uint8_t)tmask;
         }
-        log_accumulate(gl->acc[t % 3u], done && live, tmask, sums);
+        log_accumulate<S::fixed ? 8 : 32>(gl->acc[t % 3u], done && live, tmask, sums);
         if (live) {
             if (done) {
 #pragma unroll
@@ -764,12 +789,32 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     // and triggering after the last store was slower on H100 (DESIGN.md 6e).
     pdl_trigger();
     // I'. observation inputs from the post-physics state (an env that resets / gets pushed takes others below)
-    float eu_k = euler_lane(e.qw, e.qx, e.qy, e.qz, w);
+    float eu_k = euler_lane<S::fixed>(e.qw, e.qx, e.qy, e.qz, w);
     V3 wbo = rotT(R, e.w);
     const bool done = (raw_mask & (uint32_t)c.term_enable) != 0u;
     // F. auto-reset and H. interval pushes: the reset outcome, the push draws and the noise come from the aux warp
     bar_sync(3);
-    if (done) {                                                 // (sums and log: aux warp)
+    if (S::fixed) {
+        // as selects over both outcomes, so that a warp with resetting and pushed envs does not split.  The pushed velocities
+        // are rotated whether a push fired or not: unpushed, they are the same values, so the same bits.
+        const float4* ro = reinterpret_cast<const float4*>(sh.rst[q]);
+        const float4 r0 = ro[0], r1 = ro[1], r2 = ro[2];
+        const float eu_r = sh.rst[q][12 + w];
+        EnvState er = e;
+        drift_reset_apply(DriftReset{r0.x, r0.y, r0.z, r0.w, r1.x, r1.y}, er);
+        V3 vbp = vb, wbp = wbo;
+        if (S::push_enable(c)) {
+            const float* pu = sh.push[q];
+            const bool hf = pu[0] != 0.0f, lf = pu[5] != 0.0f;
+            e.v.x = hf ? e.v.x + pu[1] : e.v.x; e.v.y = hf ? e.v.y + pu[2] : e.v.y;
+            e.w.z = hf ? e.w.z + pu[3] : e.w.z; e.w.z = lf ? e.w.z + pu[6] : e.w.z;
+            e.t_hf = pu[4]; e.t_lf = pu[7];
+            vbp = rotT(R, e.v); wbp = rotT(R, e.w);
+        }
+        e = done ? er : e;
+        vb = done ? V3{r1.z, r1.w, r2.x} : vbp; wbo = done ? V3{r2.y, r2.z, r2.w} : wbp;
+        eu_k = done ? eu_r : eu_k;
+    } else if (done) {                                                 // (sums and log: aux warp)
         const float4* ro = reinterpret_cast<const float4*>(sh.rst[q]);
         const float4 r0 = ro[0], r1 = ro[1], r2 = ro[2];
         drift_reset_apply(DriftReset{r0.x, r0.y, r0.z, r0.w, r1.x, r1.y}, e);
@@ -790,7 +835,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     // (full sectors towards HBM, NVLink peers and -- zero-copy host transport -- PCIe, instead of 8-byte pieces)
     float* orow0 = obs + (size_t)WL_OBS_DIM_BLIND * env0;
     if ((FAN == 2) || (env0 + WL_DUO_ENVS <= n && (reinterpret_cast<uintptr_t>(orow0) & 15u) == 0)) {
-        const float4 v = blind_obs_quad_values(c, e, w, eu_k, vb, wbo, zn);
+        const float4 v = blind_obs_quad_values<S::fixed>(c, e, w, eu_k, vb, wbo, zn);
         float* so = sh.obs + WL_OBS_DIM_BLIND * q + 4 * w;
         so[0] = v.x; so[1] = v.y;
         if (w < 3) { so[2] = v.z; so[3] = v.w; }
@@ -804,7 +849,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         if (FAN == 1) blind_obs_quad(c, e, w, eu_k, vb, wbo, zn, obs + (size_t)WL_OBS_DIM_BLIND * ii, live, pf);
         else blind_obs_quad(c, e, w, eu_k, vb, wbo, zn, obs + (size_t)WL_OBS_DIM_BLIND * ii, live);
     }
-    if (live) store_env_quad(st, n, i, w, e, false, false);
+    if (S::fixed) store_env_quad_sel(st, n, i, w, e, live);
+    else if (live) store_env_quad(st, n, i, w, e, false, false);
     TR(TR_LAST, __float_as_uint(e.omega[0]));
     TR_COMMIT(0);
 }

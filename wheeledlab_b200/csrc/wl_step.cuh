@@ -144,6 +144,33 @@ __device__ __forceinline__ void store_env_quad(float4* __restrict__ st, int n, i
         }
     }
 }
+// store_env_quad for the duo kernel's fixed specs (no command, no sums), with no lane-divergent region: the chassis is the
+// same in the quad's four lanes, so lane w writes state group w (position, quaternion, linear, angular velocity), lane 0
+// also the actions and lanes 2 / 3 their steer joint.  Every store is predicated on its lane's condition.
+__device__ __forceinline__ void st_global_if(float* p, float v, bool pred) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.u32 p, %2, 0;\n @p st.global.f32 [%0], %1;\n}" ::"l"(p), "f"(v), "r"((uint32_t)pred) : "memory");
+}
+__device__ __forceinline__ void st_global_if(float4* p, float4 v, bool pred) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.u32 p, %5, 0;\n @p st.global.v4.f32 [%0], {%1, %2, %3, %4};\n}"
+                 ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"((uint32_t)pred) : "memory");
+}
+__device__ __forceinline__ void st_global_if(uint8_t* p, uint32_t v, bool pred) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.u32 p, %2, 0;\n @p st.global.u8 [%0], %1;\n}" ::"l"(p), "r"(v), "r"((uint32_t)pred) : "memory");
+}
+__device__ __forceinline__ void store_env_quad_sel(float4* __restrict__ st, int n, int i, int w, const EnvState& e, bool live) {
+    float* f = reinterpret_cast<float*>(st);
+    const bool w0 = w == 0, w1 = w == 1, w2 = w == 2;
+    const float4 g = make_float4(sel(w0, e.p.x, sel(w1, e.qw, sel(w2, e.v.x, e.w.x))), sel(w0, e.p.y, sel(w1, e.qx, sel(w2, e.v.y, e.w.y))),
+                                 sel(w0, e.p.z, sel(w1, e.qy, sel(w2, e.v.z, e.w.z))),
+                                 sel(w0, __int_as_float(e.ep_len), sel(w1, e.qz, sel(w2, e.t_hf, e.t_lf))));
+    st_global_if(st + (size_t)w * n + i, g, live);                                 // WL_G_POS + w
+    st_global_if(st + (size_t)WL_G_ACTION * n + i, make_float4(e.action[0], e.action[1], e.prev_action[0], e.prev_action[1]),
+                 live && w == 0);
+    st_global_if(f + (size_t)WL_G_WHEEL * n * 4 + (size_t)i * 4 + w, e.omega[0], live);
+    const int js = (w >= 2) ? w - 2 : 0;
+    st_global_if(f + (size_t)WL_G_STEER * n * 4 + (size_t)i * 4 + js, e.steer[0], live && w >= 2);
+    st_global_if(f + (size_t)WL_G_STEER * n * 4 + (size_t)i * 4 + 2 + js, e.steer_vel[0], live && w >= 2);
+}
 
 // ---- step spec: the config fields that pick a branch or set a trip count in the Drift-family step ----------------------
 // A kernel templated on a packed spec key K != 0 reads these fields as constants, so the branches it does not take and the
@@ -280,7 +307,8 @@ __device__ __forceinline__ StepConsts make_step_consts(const wl_config& c, const
 #pragma unroll
     for (int i = 0; i < NW; ++i) {
         k.hI[i] = Spec<K>::wheel_mass(c) ? c.d_h * e.inv_Iw[i] : c.d_hI;
-        k.idk[i] = 1.0f / fm(k.hI[i], e.kd[i], 1.0f);
+        // hI > 0 and the damping kd >= 0, so the divisor is >= 1 and the quotient normal: a fixed spec skips the slow-path check
+        k.idk[i] = Spec<K>::fixed ? fdiv_norm(1.0f, fm(k.hI[i], e.kd[i], 1.0f)) : 1.0f / fm(k.hI[i], e.kd[i], 1.0f);
         // longitudinal stick cap (tire_mx / h) with this wheel's own spin inertia
         k.fxk[i] = Spec<K>::wheel_mass(c) ? c.d_inv_h / fm(c.wheel_radius * c.wheel_radius, e.inv_Iw[i], c.tire_mx_rest) : c.d_fxk;
     }
@@ -498,9 +526,32 @@ __device__ __forceinline__ bool drift_off_track(const wl_config& c, float x, flo
 }
 
 // `slip_atan` = det_atan2(vb.y, vb.x) (computed by the caller so that the quad kernel can batch its atan2 calls)
+// SEL: no divergent region and no slow-path call: the roots through fsqrt_sel, both cross-track cases evaluated and selected.
+template <bool SEL = false>
 __device__ __forceinline__ void drift_reward_terms(const wl_config& c, float steer_l, float steer_r, float slip_atan, V3 p, V3 vb,
                                                    V3 wb, float wz_world, bool out_of_bounds, bool time_out,
                                                    float f[WL_MAX_REW_TERMS]) {
+    if (SEL) {
+        const float slip = fabsf(slip_atan);
+        float valid = (fabsf(vb.x) < c.slip_min_vel_x || slip > c.slip_max_thresh) ? 0.0f : slip;
+        f[WL_DR_SIDE_SLIP] = (valid < c.slip_min_thresh) ? 0.0f : valid;
+        const float dv = fsqrt_sel(vb.x * vb.x + vb.y * vb.y) - c.vel_speed_target;
+        f[WL_DR_VEL] = dv * dv + c.vel_offset;
+        f[WL_DR_PROGRESS] = wz_world;
+        const float sm = (steer_l + steer_r) / 2.0f;
+        const float av = r_clamp(wb.z, -c.tlgr_ang_vel_thresh, c.tlgr_ang_vel_thresh);
+        f[WL_DR_TLGR] = r_max(sm * av * -1.0f, 0.0f);
+        const float sp = fsqrt_sel(vb.x * vb.x + vb.y * vb.y + vb.z * vb.z);
+        f[WL_DR_TURN_ENERGY] = (fabsf(p.y) > c.energy_straight) ? sp * sp : 0.0f;
+        const float st = c.trk_straight, tr = c.ctd_track_radius;
+        const float ds = (p.x > 0.0f) ? (p.x - tr) : (p.x + tr);
+        const float yy = (p.y > 0.0f) ? (p.y - st) : (p.y + st);
+        const float dc = fsqrt_sel(yy * yy + p.x * p.x) - tr;
+        f[WL_DR_CROSS_TRACK] = fsqrt_sel(sel(fabsf(p.y) < st, ds * ds, dc * dc)) + c.ctd_offset;
+        f[WL_DR_TERM_PENS] = (out_of_bounds && !time_out) ? 1.0f : 0.0f;
+        f[7] = 0.0f;
+        return;
+    }
     float slip = fabsf(slip_atan);
     float valid = (fabsf(vb.x) < c.slip_min_vel_x || slip > c.slip_max_thresh) ? 0.0f : slip;
     if (valid < c.slip_min_thresh) valid = 0.0f;
@@ -699,12 +750,18 @@ __device__ __forceinline__ void visual_proprio(const wl_config& c, const EnvStat
 
 // ---- E. reward weighting and done flags ----------------------------------------------------
 // value = f * w * dt per term, terms with w == 0 skipped; adds each value to the episode sums, returns the step reward
+// SEL: every term is weighed and the sums take it by select (the same operations in the same order, so the same bits)
+template <bool SEL = false>
 __device__ __forceinline__ float weigh_rewards(const wl_config& c, const float wts[WL_MAX_REW_TERMS], const float f[WL_MAX_REW_TERMS],
                                                float sums[WL_MAX_REW_TERMS]) {
     float total = 0.0f;
 #pragma unroll
     for (int k = 0; k < WL_MAX_REW_TERMS; ++k) {
-        if (k < c.num_rew_terms) {
+        if (SEL) {
+            const float val = f[k] * wts[k] * c.d_step_dt;
+            const bool on = k < c.num_rew_terms && wts[k] != 0.0f;
+            total = sel(on, total + val, total); sums[k] = sel(on, sums[k] + val, sums[k]);
+        } else if (k < c.num_rew_terms) {
             float w = wts[k];
             if (w != 0.0f) { float val = f[k] * w * c.d_step_dt; total += val; sums[k] += val; }
         }
@@ -850,9 +907,20 @@ __device__ __forceinline__ void quad_obs_noise(const wl_config& c, int w, uint32
     }
 }
 // this lane's slice of the 14-float row: lanes 0..2 four floats (obs[4w..4w+3], noise added), lane 3 the two last-action floats
+// SEL: every lane evaluates the same sums and selects its slice, with no lane-divergent region.
+template <bool SEL = false>
 __device__ __forceinline__ float4 blind_obs_quad_values(const wl_config& c, const EnvState& e, int w, float eu_k, V3 vb, V3 wb, const float z[4]) {
     const unsigned base = (threadIdx.x & 31u) & ~3u;
     float eu1 = __shfl_sync(0xffffffffu, eu_k, base + 1), eu2 = __shfl_sync(0xffffffffu, eu_k, base + 2);
+    if (SEL) {
+        const bool w0 = w == 0, w1 = w == 1;
+        const float n0 = c.noise_std[0], n1 = c.noise_std[1], n2 = c.noise_std[2], n3 = c.noise_std[3];
+        const float4 v = make_float4((w0 ? e.p.x : w1 ? eu1 : vb.z) + (w0 ? n0 : w1 ? n1 : n2) * z[0],
+                                     (w0 ? e.p.y : w1 ? eu2 : wb.x) + (w0 ? n0 : w1 ? n1 : n3) * z[1],
+                                     (w0 ? e.p.z : w1 ? vb.x : wb.y) + (w0 ? n0 : w1 ? n2 : n3) * z[2],
+                                     (w0 ? eu_k : w1 ? vb.y : wb.z) + (w0 ? n1 : w1 ? n2 : n3) * z[3]);
+        return (w == 3) ? make_float4(r_clamp(e.action[0], -1.0f, 1.0f), r_clamp(e.action[1], -1.0f, 1.0f), 0.0f, 0.0f) : v;
+    }
     float b0, b1, b2, b3, s0, s1, s2, s3;
     if (w == 0) { b0 = e.p.x; b1 = e.p.y; b2 = e.p.z; b3 = eu_k; s0 = s1 = s2 = c.noise_std[0]; s3 = c.noise_std[1]; }
     else if (w == 1) { b0 = eu1; b1 = eu2; b2 = vb.x; b3 = vb.y; s0 = s1 = c.noise_std[1]; s2 = s3 = c.noise_std[2]; }
