@@ -74,6 +74,22 @@ static int launched(wl_sim* sim, const char* what, int count = 1) {
     sim->launches += count;
     return cuda_check(cudaGetLastError(), what);
 }
+// the step counter of an entry that does not advance it: a host value below 2^31, or WL_DEVICE_COUNTER_PLUS(k)
+static int check_counter(const std::string& fn, int64_t step_counter) {
+    if (step_counter < ((int64_t)1 << 31) && step_counter >= -((int64_t)1 << 31)) return WL_OK;
+    return fail(WL_EINVAL, fn + ": step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+}
+// Raise KERNEL's dynamic shared-memory limit to `bytes` on device `dev`, once per device.  It must happen before the kernel's
+// first launch and outside any graph capture: every entry calls this before it launches, and the PPO workspace queries reach
+// it before the first update (see ppo_workspace).
+template <auto KERNEL>
+static int raise_smem(int dev, size_t bytes, const char* fn) {
+    static bool done[64] = {false};
+    if (dev < 0 || dev >= 64 || done[dev]) return WL_OK;
+    if (int rc = cuda_check(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes), fn)) return rc;
+    done[dev] = true;
+    return WL_OK;
+}
 // f(std::integral_constant<int, T>{}) for the first listed task T equal to `task`, else for WL_TASK_DRIFT: a caller
 // instantiates its kernel for the tasks it lists only
 template <int... TASKS, typename F>
@@ -2085,6 +2101,17 @@ static int launch_camera(wl_sim* sim, float* d_obs, uint32_t t, uint32_t stream_
     wl_camera_kernel<<<sim->cfg.num_envs, WL_CAM_THREADS, 0, cs>>>(sim->cfg, sim->state, sim->globals, sim->hf, d_obs, t, stream_id, sub, d_aug);
     return launched(sim, "wl_camera_kernel");
 }
+// The row tail: the kernels that finish the Elevation and Visual built-in rows, after every launch that writes one (nothing on
+// the Drift family).  After a step (call_idx -1) the camera draws from RNG_CAM, sub 0; in wl_observe's tail it draws from
+// RNG_CAM_EXTRA, sub call_idx, which without row terms may be any value, -1 included: hence the flag.
+static int launch_row_tail(wl_sim* sim, float* d_obs, uint32_t t, bool after_step, int32_t call_idx, cudaStream_t cs) {
+    if (sim->cfg.task == WL_TASK_ELEVATION) return launch_scan(sim, d_obs, t, call_idx, cs);
+    if (sim->cfg.task != WL_TASK_VISUAL) return WL_OK;
+    if (sim->cfg.vis_cam)        // t may be device-relative
+        if (int rc = launch_camera(sim, d_obs, t, after_step ? RNG_CAM : RNG_CAM_EXTRA, after_step ? 0u : (uint32_t)call_idx, nullptr, cs))
+            return rc;
+    return launch_visual_row(sim, d_obs, t, call_idx, cs);
+}
 
 extern "C" {
 
@@ -2373,6 +2400,12 @@ static int reset_dr(wl_sim* sim, const int64_t* ids, int n_ids, int64_t step_cou
         sim->cfg, sim->state, sim->globals, ids, n_ids, (uint32_t)step_counter, after_step, sim->reset_ev);
     return launched(sim, "wl_reset_dr_kernel");
 }
+// the step epilogue, after the step kernel(s) and the row tail: the reset-mode DR of the envs the step reset, then the
+// curriculum boundary
+static int end_step(wl_sim* sim, int64_t step_counter, cudaStream_t cs) {
+    if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, cs)) return rc;
+    return post_step(sim, step_counter, cs);
+}
 extern "C" {
 
 int wl_startup(wl_sim* sim, void* stream) {
@@ -2410,7 +2443,6 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     cudaStream_t cs = (cudaStream_t)stream;
     const uint32_t t = (uint32_t)step_counter;               // negative (device base + k) stays encoded: see decode_step
     if (int rc = prep_step(sim, step_counter, 1, cs)) return rc;
-    const bool elev = sim->cfg.task == WL_TASK_ELEVATION, vis = sim->cfg.task == WL_TASK_VISUAL;
     StageIO sio0{sim->term_bits, nullptr, nullptr};
     int specialised = 0, cta_threads = 0;
     if (variant == 8) {
@@ -2445,11 +2477,8 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
     }
     sim->step_variant = variant; sim->step_specialised = specialised; sim->step_threads = cta_threads;
     if (int rc = launched(sim, "wl_step_kernel")) return rc;
-    if (elev) { if (int rc = launch_scan(sim, d_obs, t, -1, cs)) return rc; }
-    if (vis && sim->cfg.vis_cam) { if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc; }   // t may be device-relative
-    if (vis) { if (int rc = launch_visual_row(sim, d_obs, t, -1, cs)) return rc; }
-    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
-    return post_step(sim, step_counter, cs);
+    if (int rc = launch_row_tail(sim, d_obs, t, true, -1, cs)) return rc;
+    return end_step(sim, step_counter, cs);
 }
 
 #ifdef WL_DUO_TRACE
@@ -2505,12 +2534,8 @@ int wl_step_stage_b(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_ex
     if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, (uint32_t)step_counter,
                                  StageIO{const_cast<uint8_t*>(d_term_bits), d_extra_terminated, d_extra_truncated}, (cudaStream_t)stream))
         return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
-    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
-        if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
-    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
-    if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
-    return post_step(sim, step_counter, (cudaStream_t)stream);
+    if (int rc = launch_row_tail(sim, d_obs, (uint32_t)step_counter, true, -1, (cudaStream_t)stream)) return rc;
+    return end_step(sim, step_counter, (cudaStream_t)stream);
 }
 
 int wl_step_stage_b1(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_extra_terminated, const uint8_t* d_extra_truncated,
@@ -2522,8 +2547,7 @@ int wl_step_stage_b1(wl_sim* sim, const uint8_t* d_term_bits, const uint8_t* d_e
     if (int rc = launch_stage<3>(sim, nullptr, nullptr, nullptr, d_terminated, d_truncated, d_log, (uint32_t)step_counter,
                                  StageIO{const_cast<uint8_t*>(d_term_bits), d_extra_terminated, d_extra_truncated}, (cudaStream_t)stream))
         return rc;
-    if (int rc = reset_dr(sim, nullptr, sim->cfg.num_envs, step_counter, true, (cudaStream_t)stream)) return rc;
-    return post_step(sim, step_counter, (cudaStream_t)stream);
+    return end_step(sim, step_counter, (cudaStream_t)stream);
 }
 
 int wl_step_stage_b2(wl_sim* sim, float* d_obs, int64_t step_counter, void* stream) {
@@ -2535,11 +2559,7 @@ int wl_step_stage_b2(wl_sim* sim, float* d_obs, int64_t step_counter, void* stre
     if (int rc = launch_stage<4>(sim, nullptr, d_obs, nullptr, nullptr, nullptr, nullptr, (uint32_t)step_counter,
                                  StageIO{nullptr, nullptr, nullptr}, (cudaStream_t)stream))
         return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
-    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
-        if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM, 0u, nullptr, (cudaStream_t)stream)) return rc;
-    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, (uint32_t)step_counter, -1, (cudaStream_t)stream)) return rc; }
-    return WL_OK;
+    return launch_row_tail(sim, d_obs, (uint32_t)step_counter, true, -1, (cudaStream_t)stream);
 }
 
 int wl_set_event_timers(wl_sim* sim, int32_t n_terms, const float* lo_hi) {
@@ -2643,8 +2663,7 @@ int wl_set_device_events(wl_sim* sim, const wl_device_event_desc* table, int32_t
 
 int wl_device_events(wl_sim* sim, const uint8_t* d_terminated, const uint8_t* d_truncated, int64_t step_counter, void* stream) {
     if (!sim || !d_terminated || !d_truncated) return fail(WL_EINVAL, "wl_device_events: null argument");
-    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
-        return fail(WL_EINVAL, "wl_device_events: step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+    if (int rc = check_counter("wl_device_events", step_counter)) return rc;
     if (!sim->devents) return fail(WL_EINVAL, "wl_device_events: no device event terms (wl_set_device_events)");
     if (fan_set(sim)) return fail(WL_EINVAL, "wl_device_events: the peer fan-out is set, and device events run with wl_step_terms only");
     ensure_device(sim);
@@ -2741,12 +2760,8 @@ int wl_step_terms(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew
     } else if (int rc = launch_stage<2>(sim, nullptr, d_obs, nullptr, d_terminated, d_truncated, d_log, t, sio, cs)) {
         return rc;
     }
-    if (sim->cfg.task == WL_TASK_ELEVATION) { if (int rc = launch_scan(sim, d_obs, t, -1, cs)) return rc; }
-    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
-        if (int rc = launch_camera(sim, d_obs, t, RNG_CAM, 0u, nullptr, cs)) return rc;   // t may be device-relative
-    if (sim->cfg.task == WL_TASK_VISUAL) { if (int rc = launch_visual_row(sim, d_obs, t, -1, cs)) return rc; }
-    if (!de) { if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc; }
-    return post_step(sim, step_counter, cs);
+    if (int rc = launch_row_tail(sim, d_obs, t, true, -1, cs)) return rc;
+    return de ? post_step(sim, step_counter, cs) : end_step(sim, step_counter, cs);     // (with device events reset_dr ran above)
 }
 
 int wl_rollout(wl_sim* sim, int32_t K, const float* d_actions, float* d_actions_out, float* d_obs, float* d_rew,
@@ -2838,11 +2853,7 @@ int wl_observe(wl_sim* sim, float* d_obs, int64_t step_counter, int32_t call_idx
     wl_observe_kernel<<<(n + bs - 1) / bs, bs, 0, (cudaStream_t)stream>>>(sim->cfg, sim->state, d_obs, (uint32_t)step_counter,
                                                                          (uint32_t)call_idx);
     if (int rc = launched(sim, "wl_observe_kernel")) return rc;
-    if (sim->cfg.task == WL_TASK_ELEVATION) return launch_scan(sim, d_obs, (uint32_t)step_counter, call_idx, (cudaStream_t)stream);
-    if (sim->cfg.task == WL_TASK_VISUAL && sim->cfg.vis_cam)
-        if (int rc = launch_camera(sim, d_obs, (uint32_t)step_counter, RNG_CAM_EXTRA, (uint32_t)call_idx, nullptr, (cudaStream_t)stream)) return rc;
-    if (sim->cfg.task == WL_TASK_VISUAL) return launch_visual_row(sim, d_obs, (uint32_t)step_counter, call_idx, (cudaStream_t)stream);
-    return WL_OK;
+    return launch_row_tail(sim, d_obs, (uint32_t)step_counter, false, call_idx, (cudaStream_t)stream);
 }
 
 int wl_camera(wl_sim* sim, float* d_obs, int64_t step_counter, const float* d_aug, void* stream) {
@@ -3073,22 +3084,18 @@ static int act_step_launch(bool infer, const char* fn, wl_sim* sim, const float*
     Terrain T{sim->hf};
     cudaStream_t cs = (cudaStream_t)stream;
     if (int rc = prep_step(sim, step_counter, 1, cs)) return rc;
-    static bool attr_set[64] = {false};                       // the attribute is per device
-    if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
-        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_VISUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_DRIFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_VISUAL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        cudaFuncSetAttribute(wl_act_step_quad_kernel<WL_TASK_DRIFT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        attr_set[sim->device] = true;
-    }
+    // all four forms on the first call (prep_step made sim->device current), as the other entry may next run inside a capture
+    if (int rc = raise_smem<wl_act_step_quad_kernel<WL_TASK_VISUAL>>(sim->device, 96 * 1024, fn)) return rc;
+    if (int rc = raise_smem<wl_act_step_quad_kernel<WL_TASK_DRIFT>>(sim->device, 96 * 1024, fn)) return rc;
+    if (int rc = raise_smem<wl_act_step_quad_kernel<WL_TASK_VISUAL, true>>(sim->device, 96 * 1024, fn)) return rc;
+    if (int rc = raise_smem<wl_act_step_quad_kernel<WL_TASK_DRIFT, true>>(sim->device, 96 * 1024, fn)) return rc;
     with_task<WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
         launch_k(infer ? wl_act_step_quad_kernel<task, true> : wl_act_step_quad_kernel<task, false>, grid, WL_ACT_THREADS, smem, cs, g_pdl,
                  sim->cfg, sim->state, sim->globals, T, d_obs_in, d_policy_blob, blob_floats, po, out, d_obs, d_rew, d_terminated,
                  d_truncated, d_log, (uint32_t)step_counter, sim->obs_dim);
     });
     if (int rc = launched(sim, infer ? "wl_act_step_quad_kernel<infer>" : "wl_act_step_quad_kernel")) return rc;
-    if (int rc = reset_dr(sim, nullptr, n, step_counter, true, cs)) return rc;
-    return post_step(sim, step_counter, cs);
+    return end_step(sim, step_counter, cs);
 }
 
 int wl_act_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, float* d_obs, float* d_rew,
@@ -3109,63 +3116,47 @@ int wl_act_infer_step(wl_sim* sim, const float* d_obs_in, const float* d_policy_
                            step_counter, stream);
 }
 
-int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
-                       const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
-    const char* fn = "wl_policy_act_asym";
-    if (!sim || !d_obs_in || !d_critic_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
-        return fail(WL_EINVAL, std::string(fn) + ": null argument");
+// wl_policy_act_elu and wl_policy_act_asym (asym: the critic reads d_critic_obs_in, critic_obs_dim wide) after their null
+// checks: the same checks, blob and shared-memory sizing, and grid
+static int policy_act_narrow(bool asym, const char* fn, wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in,
+                             int32_t critic_obs_dim, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
     if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u) || ((uintptr_t)d_obs_in & 3u) ||
         ((uintptr_t)d_critic_obs_in & 3u) || ((uintptr_t)out.log_prob & 3u) || ((uintptr_t)out.value & 3u))
-        return fail(WL_EINVAL, std::string(fn) + ": policy blob must be 16-byte aligned, actions/mean 8-byte aligned, obs_in/critic_obs_in/log_prob/value 4-byte aligned");
-    if (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
-    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
-        return fail(WL_EINVAL, std::string(fn) + ": step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
+        return fail(WL_EINVAL, std::string(fn) + ": policy blob must be 16-byte aligned, actions/mean 8-byte aligned, " +
+                                   (asym ? "obs_in/critic_obs_in/log_prob/value" : "obs_in/log_prob/value") + " 4-byte aligned");
+    if (asym && (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS)) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
+    if (int rc = check_counter(fn, step_counter)) return rc;
+    // no step rows are written, but the step that consumes these actions refuses the fan-out: refuse it here already
     if (int rc = refuse_fan(sim, fn)) return rc;
     const int D = policy_in_dim(sim);
     if (D < 1 || D > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
     ensure_device(sim);
     PolicyOffsets po;
     const int blob_floats = policy_offsets(D, po.o, critic_obs_dim);
-    const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS + WL_ACT_XC));
-    static bool attr_set[64] = {false};                       // the attribute is per device
-    if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_asym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024), fn))
-            return rc;
-        attr_set[sim->device] = true;
-    }
-    const int n = sim->cfg.num_envs;
-    wl_policy_act_asym_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
-        sim->cfg, sim->globals, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
-    return launched(sim, "wl_policy_act_asym_kernel");
+    const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS + (asym ? WL_ACT_XC : 0)));
+    if (int rc = asym ? raise_smem<wl_policy_act_asym_kernel>(sim->device, 96 * 1024, fn) : raise_smem<wl_policy_act_elu_kernel>(sim->device, 96 * 1024, fn))
+        return rc;
+    const int n = sim->cfg.num_envs, grid = (n + WL_ACT_ENVS - 1) / WL_ACT_ENVS;
+    if (asym)
+        wl_policy_act_asym_kernel<<<grid, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
+            sim->cfg, sim->globals, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
+    else
+        wl_policy_act_elu_kernel<<<grid, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
+            sim->cfg, sim->globals, d_obs_in, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
+    return launched(sim, asym ? "wl_policy_act_asym_kernel" : "wl_policy_act_elu_kernel");
+}
+
+int wl_policy_act_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
+                       const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
+    if (!sim || !d_obs_in || !d_critic_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
+        return fail(WL_EINVAL, "wl_policy_act_asym: null argument");
+    return policy_act_narrow(true, "wl_policy_act_asym", sim, d_obs_in, d_critic_obs_in, critic_obs_dim, d_policy_blob, out, step_counter, stream);
 }
 
 int wl_policy_act_elu(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
     if (!sim || !d_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
         return fail(WL_EINVAL, "wl_policy_act_elu: null argument");
-    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u) || ((uintptr_t)d_obs_in & 3u) ||
-        ((uintptr_t)out.log_prob & 3u) || ((uintptr_t)out.value & 3u))
-        return fail(WL_EINVAL, "wl_policy_act_elu: policy blob must be 16-byte aligned, actions/mean 8-byte aligned, obs_in/log_prob/value 4-byte aligned");
-    if (step_counter >= ((int64_t)1 << 31) || step_counter < -((int64_t)1 << 31))
-        return fail(WL_EINVAL, "wl_policy_act_elu: step counter out of range (< 2^31, or WL_DEVICE_COUNTER_PLUS(k))");
-    // no step rows are written, but the step that consumes these actions refuses the fan-out: refuse it here already
-    if (int rc = refuse_fan(sim, "wl_policy_act_elu")) return rc;
-    const int D = policy_in_dim(sim);
-    if (D < 1 || D > 16) return fail(WL_EUNSUPPORTED, "wl_policy_act_elu: obs_dim > 16 (the network wl_act_step runs)");
-    ensure_device(sim);
-    PolicyOffsets po;
-    const int blob_floats = policy_offsets(D, po.o);
-    const size_t smem = sizeof(float) * ((size_t)blob_floats + WL_ACT_ENVS * (WL_ACT_XS + WL_ACT_HS));
-    static bool attr_set[64] = {false};                       // the attribute is per device
-    if (sim->device >= 0 && sim->device < 64 && !attr_set[sim->device]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_elu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024),
-                                "wl_policy_act_elu"))
-            return rc;
-        attr_set[sim->device] = true;
-    }
-    const int n = sim->cfg.num_envs;
-    wl_policy_act_elu_kernel<<<(n + WL_ACT_ENVS - 1) / WL_ACT_ENVS, WL_ACT_THREADS, smem, (cudaStream_t)stream>>>(
-        sim->cfg, sim->globals, d_obs_in, d_policy_blob, blob_floats, po, out, (uint32_t)step_counter, D);
-    return launched(sim, "wl_policy_act_elu_kernel");
+    return policy_act_narrow(false, "wl_policy_act_elu", sim, d_obs_in, nullptr, 0, d_policy_blob, out, step_counter, stream);
 }
 
 int wl_gae(const float* d_rewards, const float* d_values, const float* d_last_values, const uint8_t* d_dones,
@@ -3247,31 +3238,46 @@ static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_bat
     w.rows_off = align256(w.norm_off + sizeof(double) * w.norm_parts);
     w.bytes = w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas;
 }
-static int ppo_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
+// the network an update trains: wl_ppo_update's ELU network, wl_ppo_update_wide's ReLU network, wl_ppo_update_asym's ELU
+// network with a critic row of its own
+enum PpoNet { PPO_NARROW, PPO_WIDE, PPO_ASYM };
+static size_t ppo_grad_asym_smem(int obs_dim, int critic_obs_dim);
+static int wide_attributes(int dev, const char* fn);
+// The shape checks and the workspace layout of an update of `net` (critic_obs_dim: PPO_ASYM only).  The gradient kernels'
+// shared-memory limits are per-device attributes: raised once to what the widest network needs, so updates of any obs_dim
+// share them in one process.  The workspace query reaches here before the first update, so callers that query outside a
+// graph capture (FusedPPO, PPOIteration.start) never set them inside one.
+static int ppo_workspace(const char* fn, PpoNet net, int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches,
+                         PpoWideWorkspace& x) {
     if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
-    if (obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    if (net == PPO_WIDE && obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
+    if (net != PPO_WIDE && obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    if (net == PPO_ASYM && (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS))
+        return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
     if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
     int dev = 0, sms = 0;
     if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
     if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
-    // the grad kernel's shared-memory limit is a per-device attribute: raised once to what the widest obs_dim needs, so
-    // updates of any obs_dim share it in one process.  The workspace query reaches here before the first update, so
-    // callers that query outside a graph capture (FusedPPO, PPOIteration.start) never set it inside one.
-    static bool attr_set[64] = {false};
-    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_grad_smem(16)), fn))
-            return rc;
-        attr_set[dev] = true;
+    if (int rc = net == PPO_WIDE ? wide_attributes(dev, fn)
+                 : net == PPO_ASYM ? raise_smem<wl_ppo_grad_asym_kernel>(dev, ppo_grad_asym_smem(16, WL_MAX_CRITIC_OBS), fn)
+                                   : raise_smem<wl_ppo_grad_kernel>(dev, ppo_grad_smem(16), fn))
+        return rc;
+    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, x.w, net == PPO_ASYM ? critic_obs_dim : 0);
+    x.bytes = x.w.bytes;
+    if (net == PPO_WIDE) {      // then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
+        const size_t hb = sizeof(float) * 2 * WL_HID * (size_t)WL_PPO_TILE * ((batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE);
+        x.h1_off = align256(x.w.bytes);
+        x.dz_off = align256(x.h1_off + hb);
+        x.bytes = x.dz_off + hb;
     }
-    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, w);
     return WL_OK;
 }
 
 int32_t wl_ppo_state_floats(void) { return 10 + 2 * WL_PPO_MAX_UPDATES; }
 
 size_t wl_ppo_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches) {
-    PpoWorkspace w;
-    return ppo_workspace("wl_ppo_workspace_bytes", obs_dim, batch, num_mini_batches, w) ? 0 : w.bytes;
+    PpoWideWorkspace x;
+    return ppo_workspace("wl_ppo_workspace_bytes", PPO_NARROW, obs_dim, 0, batch, num_mini_batches, x) ? 0 : x.bytes;
 }
 
 // the host-side checks of one rank's arguments to a PPO update entry (fn names the entry in the message)
@@ -3286,25 +3292,18 @@ static int ppo_check_args(const char* fn, const wl_ppo_params* p, const wl_ppo_b
     return WL_OK;
 }
 
-static int ppo_wide_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWideWorkspace& x);
-
-// the workspace layout of the update (narrow: wl_ppo_update's, wide: wl_ppo_update_wide's) and the checks against it
-static int ppo_check_layout(const char* fn, bool wide, const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_blob,
-                            const float* d_adam_m, const float* d_adam_v, const void* d_workspace, size_t workspace_bytes,
-                            PpoWideWorkspace& x) {
-    if (wide) {
-        if (int rc = ppo_wide_workspace(fn, p->obs_dim, p->batch, p->num_mini_batches, x)) return rc;
-    } else {
-        if (int rc = ppo_workspace(fn, p->obs_dim, p->batch, p->num_mini_batches, x.w)) return rc;
-        x.bytes = x.w.bytes;
-    }
+// the workspace layout of an update of `net` and the checks against it
+static int ppo_check_layout(const char* fn, PpoNet net, int32_t critic_obs_dim, const wl_ppo_params* p, const wl_ppo_batch* b,
+                            const float* d_blob, const float* d_adam_m, const float* d_adam_v, const void* d_workspace,
+                            size_t workspace_bytes, PpoWideWorkspace& x) {
+    if (int rc = ppo_workspace(fn, net, p->obs_dim, critic_obs_dim, p->batch, p->num_mini_batches, x)) return rc;
     if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
         return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
     if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
         return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
+    static const char* const query[] = {"wl_ppo_workspace_bytes", "wl_ppo_wide_workspace_bytes", "wl_ppo_asym_workspace_bytes"};
     if (workspace_bytes < x.bytes)
-        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (" + (wide ? "wl_ppo_wide_workspace_bytes" : "wl_ppo_workspace_bytes") +
-                                   " gives " + std::to_string(x.bytes) + ")");
+        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (" + query[net] + " gives " + std::to_string(x.bytes) + ")");
     return WL_OK;
 }
 
@@ -3339,14 +3338,21 @@ static void ppo_launch_args(const wl_ppo_params* p, const wl_ppo_batch* b, PpoAr
     sa = PpoStepArgs{p->max_grad_norm, p->desired_kl, a.inv_B, p->adaptive != 0, 0};
 }
 
-int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
-                  void* d_workspace, size_t workspace_bytes, void* stream) {
-    if (int rc = ppo_check_args("wl_ppo_update", p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
+static int wide_compact_offsets(const PolicyOffsets& po, int blob_floats, PolicyOffsets& pc);
+
+// wl_ppo_update (wide false) and wl_ppo_update_wide: rsl_rl's update, epochs x mini-batches of the gradient phase, the
+// reduction and the Adam step
+static int ppo_update(const char* fn, bool wide, const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m,
+                      float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = ppo_check_args(fn, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
     PpoWideWorkspace x;
-    if (int rc = ppo_check_layout("wl_ppo_update", false, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x)) return rc;
+    if (int rc = ppo_check_layout(fn, wide ? PPO_WIDE : PPO_NARROW, 0, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x))
+        return rc;
     const PpoWorkspace& w = x.w;
-    PolicyOffsets po;
+    PolicyOffsets po, pc;
     policy_offsets(p->obs_dim, po.o);
+    if (wide) wide_compact_offsets(po, w.blob_floats, pc);
+    else pc = po;
     cudaStream_t cs = (cudaStream_t)stream;
     char* ws = (char*)d_workspace;
     float* red = (float*)ws;
@@ -3361,15 +3367,21 @@ int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, 
         for (int i = 0; i < p->num_mini_batches; ++i) {
             a.row0 = (int64_t)i * a.B;
             sa.update_index = e * p->num_mini_batches + i;
-            ppo_grad_phase(false, x, po, po, a, d_blob, d_state, ws, cs);
+            ppo_grad_phase(wide, x, po, pc, a, d_blob, d_state, ws, cs);
             wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
                                                                p->entropy_coef, red, norm_part);
             wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
                                                                         w.blob_floats, po, p->obs_dim, sa, nullptr);
-            if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel")) return rc;
+            if (int rc = cuda_check(cudaGetLastError(), wide ? "wl_ppo_update_wide kernels" : "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel"))
+                return rc;
         }
     }
     return WL_OK;
+}
+
+int wl_ppo_update(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
+                  void* d_workspace, size_t workspace_bytes, void* stream) {
+    return ppo_update("wl_ppo_update", false, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace, workspace_bytes, stream);
 }
 
 // ---- the asymmetric update (DESIGN 6m): wl_ppo_update's loop over wl_ppo_grad_asym_kernel and the asymmetric blob layout ----
@@ -3378,28 +3390,9 @@ static size_t ppo_grad_asym_smem(int obs_dim, int critic_obs_dim) {
     return sizeof(float) * ((size_t)policy_offsets(obs_dim, off, critic_obs_dim) + 2 * WL_HID * WL_HID + WL_HID + 2 * WL_PPO_TILE * WL_PPO_XA +
                             4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
 }
-static int ppo_asym_workspace(const char* fn, int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches, PpoWorkspace& w) {
-    if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
-    if (obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
-    if (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
-    if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
-    int dev = 0, sms = 0;
-    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
-    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
-    static bool attr_set[64] = {false};                       // per device, raised once to the widest network (see ppo_workspace)
-    if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_grad_asym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                     (int)ppo_grad_asym_smem(16, WL_MAX_CRITIC_OBS)), fn))
-            return rc;
-        attr_set[dev] = true;
-    }
-    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, w, critic_obs_dim);
-    return WL_OK;
-}
-
 size_t wl_ppo_asym_workspace_bytes(int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches) {
-    PpoWorkspace w;
-    return ppo_asym_workspace("wl_ppo_asym_workspace_bytes", obs_dim, critic_obs_dim, batch, num_mini_batches, w) ? 0 : w.bytes;
+    PpoWideWorkspace x;
+    return ppo_workspace("wl_ppo_asym_workspace_bytes", PPO_ASYM, obs_dim, critic_obs_dim, batch, num_mini_batches, x) ? 0 : x.bytes;
 }
 
 int wl_ppo_update_asym(const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_critic_obs, int32_t critic_obs_dim, float* d_blob,
@@ -3407,14 +3400,9 @@ int wl_ppo_update_asym(const wl_ppo_params* p, const wl_ppo_batch* b, const floa
     const char* fn = "wl_ppo_update_asym";
     if (int rc = ppo_check_args(fn, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
     if (!d_critic_obs || ((uintptr_t)d_critic_obs & 3u)) return fail(WL_EINVAL, std::string(fn) + ": d_critic_obs is null or not 4-byte aligned");
-    PpoWorkspace w;
-    if (int rc = ppo_asym_workspace(fn, p->obs_dim, critic_obs_dim, p->batch, p->num_mini_batches, w)) return rc;
-    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
-        return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
-    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
-        return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
-    if (workspace_bytes < w.bytes)
-        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (wl_ppo_asym_workspace_bytes gives " + std::to_string(w.bytes) + ")");
+    PpoWideWorkspace x;
+    if (int rc = ppo_check_layout(fn, PPO_ASYM, critic_obs_dim, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x)) return rc;
+    const PpoWorkspace& w = x.w;
     PolicyOffsets po;
     policy_offsets(p->obs_dim, po.o, critic_obs_dim);
     cudaStream_t cs = (cudaStream_t)stream;
@@ -3462,15 +3450,11 @@ static size_t ppo_wide_grad_smem() {
 }
 static size_t ppo_wide_dw1_smem() { return sizeof(float) * 2 * WL_PPO_TILE * (WL_DW1_K + 2 * WL_HID); }
 
-// the dynamic shared-memory limits of the wide kernels, raised once per device (the sizes do not depend on obs_dim)
+// the dynamic shared-memory limits of the wide kernels, raised together (the sizes do not depend on obs_dim)
 static int wide_attributes(int dev, const char* fn) {
-    static bool attr_set[64] = {false};
-    if (dev < 0 || dev >= 64 || attr_set[dev]) return WL_OK;
-    if (int rc = cuda_check(cudaFuncSetAttribute(wl_policy_act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)policy_act_smem()), fn)) return rc;
-    if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_wide_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_wide_grad_smem()), fn)) return rc;
-    if (int rc = cuda_check(cudaFuncSetAttribute(wl_ppo_wide_dw1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ppo_wide_dw1_smem()), fn)) return rc;
-    attr_set[dev] = true;
-    return WL_OK;
+    if (int rc = raise_smem<wl_policy_act_kernel>(dev, policy_act_smem(), fn)) return rc;
+    if (int rc = raise_smem<wl_ppo_wide_grad_kernel>(dev, ppo_wide_grad_smem(), fn)) return rc;
+    return raise_smem<wl_ppo_wide_dw1_kernel>(dev, ppo_wide_dw1_smem(), fn);
 }
 
 int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
@@ -3508,12 +3492,8 @@ int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d
     int cur = -1;
     if (cudaGetDevice(&cur) == cudaSuccess && cur != pa.device) cudaSetDevice(pa.device);
     const size_t smem = actor_mean_smem();
-    static bool attr_set[64] = {false};
-    if (pa.device >= 0 && pa.device < 64 && !attr_set[pa.device]) {
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_actor_mean_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_actor_mean")) return rc;
-        if (int rc = cuda_check(cudaFuncSetAttribute(wl_actor_mean_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "wl_actor_mean")) return rc;
-        attr_set[pa.device] = true;
-    }
+    if (int rc = raise_smem<wl_actor_mean_kernel<false>>(pa.device, smem, "wl_actor_mean")) return rc;
+    if (int rc = raise_smem<wl_actor_mean_kernel<true>>(pa.device, smem, "wl_actor_mean")) return rc;
     PolicyOffsets po;
     policy_offsets(obs_dim, po.o);
     const int grid = (n + WL_AM_ROWS - 1) / WL_AM_ROWS;
@@ -3524,60 +3504,14 @@ int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d
     return cuda_check(cudaGetLastError(), "wl_actor_mean_kernel");
 }
 
-// workspace of wl_ppo_update_wide: wl_ppo_update's, then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
-static int ppo_wide_workspace(const char* fn, int32_t obs_dim, int32_t batch, int32_t num_mini_batches, PpoWideWorkspace& x) {
-    if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
-    if (obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
-    if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
-    int dev = 0, sms = 0;
-    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
-    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
-    if (int rc = wide_attributes(dev, fn)) return rc;       // (the workspace query comes first, outside any graph capture)
-    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, x.w);
-    const size_t hb = sizeof(float) * 2 * WL_HID * (size_t)WL_PPO_TILE * ((batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE);
-    x.h1_off = align256(x.w.bytes);
-    x.dz_off = align256(x.h1_off + hb);
-    x.bytes = x.dz_off + hb;
-    return WL_OK;
-}
-
 size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches) {
     PpoWideWorkspace x;
-    return ppo_wide_workspace("wl_ppo_wide_workspace_bytes", obs_dim, batch, num_mini_batches, x) ? 0 : x.bytes;
+    return ppo_workspace("wl_ppo_wide_workspace_bytes", PPO_WIDE, obs_dim, 0, batch, num_mini_batches, x) ? 0 : x.bytes;
 }
 
 int wl_ppo_update_wide(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
                        void* d_workspace, size_t workspace_bytes, void* stream) {
-    if (int rc = ppo_check_args("wl_ppo_update_wide", p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
-    PpoWideWorkspace x;
-    if (int rc = ppo_check_layout("wl_ppo_update_wide", true, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x)) return rc;
-    const PpoWorkspace& w = x.w;
-    PolicyOffsets po, pc;
-    policy_offsets(p->obs_dim, po.o);
-    wide_compact_offsets(po, w.blob_floats, pc);
-    cudaStream_t cs = (cudaStream_t)stream;
-    char* ws = (char*)d_workspace;
-    float* red = (float*)ws;
-    double* norm_part = (double*)(ws + w.norm_off);
-    float* rows = (float*)(ws + w.rows_off);
-    wl_ppo_begin_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(b->advantages, p->batch, d_blob, po.o[12], d_state);
-    if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_begin_kernel")) return rc;
-    PpoArgs a;
-    PpoStepArgs sa;
-    ppo_launch_args(p, b, a, sa);
-    for (int e = 0; e < p->num_learning_epochs; ++e) {
-        for (int i = 0; i < p->num_mini_batches; ++i) {
-            a.row0 = (int64_t)i * a.B;
-            sa.update_index = e * p->num_mini_batches + i;
-            ppo_grad_phase(true, x, po, pc, a, d_blob, d_state, ws, cs);
-            wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
-                                                               p->entropy_coef, red, norm_part);
-            wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
-                                                                        w.blob_floats, po, p->obs_dim, sa, nullptr);
-            if (int rc = cuda_check(cudaGetLastError(), "wl_ppo_update_wide kernels")) return rc;
-        }
-    }
-    return WL_OK;
+    return ppo_update("wl_ppo_update_wide", true, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace, workspace_bytes, stream);
 }
 
 // ---- the data-parallel update (DESIGN 6j) ---------------------------------------------------------------------------
@@ -3634,7 +3568,7 @@ int wl_ppo_update_dp(const wl_ppo_params* p, int32_t activation, int32_t n_ranks
     const bool wide = activation == WL_ACTIVATION_RELU;
     PpoWideWorkspace x;
     for (int l = 0; l < n_local; ++l)
-        if (int rc = ppo_check_layout(fn, wide, p, &batches[l], d_blob[l], d_adam_m[l], d_adam_v[l], d_workspace[l], workspace_bytes, x)) return rc;
+        if (int rc = ppo_check_layout(fn, wide ? PPO_WIDE : PPO_NARROW, 0, p, &batches[l], d_blob[l], d_adam_m[l], d_adam_v[l], d_workspace[l], workspace_bytes, x)) return rc;
     const PpoWorkspace& w = x.w;
     PolicyOffsets po, pc;
     policy_offsets(p->obs_dim, po.o);
