@@ -692,7 +692,7 @@ typedef struct wl_critic_term {
  * with n_terms > 0, an unknown kind, a negative or non-finite clip, a total width above WL_MAX_CRITIC_OBS;
  * WL_EUNSUPPORTED: a task other than the Drift family.  A graph captured with the old table keeps the old table. */
 int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_terms);
-/* Dc: the width of the critic row (0 with no table) */
+/* Dc: the width of the critic row (0 with no table; a row critic's 689 + extra width) */
 int32_t wl_critic_obs_dim(const wl_sim* sim);
 
 /* ---- reset-mode domain randomisation (IsaacLab EventTermCfg mode="reset", DESIGN.md 6n) --------------------------------
@@ -820,6 +820,18 @@ int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float
 int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms);
 /* the number of row terms (0: none) */
 int32_t wl_row_terms(const wl_sim* sim);
+/* The row critic of an Elevation handle (DESIGN.md 6s): a critic row of Dc = 689 + (extra width) floats -- the Elevation
+ * row's six terms in row order (row_terms, as for wl_set_row_terms), noise-free, each with its own clip and scale, then
+ * the critic-library terms `extra` (WL_CRITIC_*, as wl_set_critic_terms, at most WL_MAX_CRITIC_OBS floats), so Dc is in
+ * 689..721.  wl_critic_obs_dim gives Dc and wl_critic_observe writes [N, Dc]: the ray-cast again, from the state the most
+ * recent step / reset left, with no draw; a ray that misses is +inf before the map term's clip, as in the policy row.  The
+ * policy row (built-in or row terms, noisy or not) is not touched.  A host-side set-up call: everything is checked before
+ * anything is replaced.  n_row_terms = 0 (and n_extra = 0) clears it.  WL_EINVAL: a null handle, a null table with a count
+ * above 0, wl_set_row_terms's refusals, a term with noise, a height-map term without a clip, extra columns without the row
+ * terms, more than WL_MAX_CRITIC_TERMS extra terms, an unknown extra kind, a negative or non-finite extra clip, extra columns
+ * wider than WL_MAX_CRITIC_OBS.  WL_EUNSUPPORTED: a task other than Elevation.  A handle without a row critic behaves as
+ * before; one with both a row critic and a wl_set_critic_terms table cannot exist (that call refuses Elevation). */
+int wl_set_row_critic(wl_sim* sim, const wl_policy_term* row_terms, int32_t n_row_terms, const wl_critic_term* extra, int32_t n_extra);
 
 /* ---- the step after the rollout: returns / advantages over the [T, N] slab (SURVEY 8f-2) ---------------------------
  * rsl_rl RolloutStorage.compute_returns as called at modified_rsl_rl_runner.py:116 [UPSTREAM-RECALL], with the time-out
@@ -957,6 +969,26 @@ int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d
 size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_mini_batches);
 int wl_ppo_update_wide(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
                        float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* ---- the wide asymmetric actor-critic: a critic input of its own (DESIGN.md 6s) ------------------------------------------
+ * The network above with the critic's first layer fed from a second row, d_critic_obs_in [N, critic_obs_dim], and a blob
+ * laid out by wl_policy_blob_floats_asym(obs_dim, critic_obs_dim); obs_dim and critic_obs_dim in 1..4096.
+ * Each net's layer 1 keeps wl_policy_act's K chunks (32 inputs from 0, each summed alone, then added to the running sum
+ * from the bias); a net that has run out of chunks adds nothing.  So actions, mean and log-prob equal wl_policy_act's for
+ * the same d_obs_in and actor blocks bit for bit whatever the critic input is, and with critic_obs_dim == obs_dim and
+ * d_critic_obs_in == d_obs_in the value does too.  Returns before any launch as wl_policy_act does, plus WL_EINVAL for a
+ * null / misaligned d_critic_obs_in or critic_obs_dim outside 1..4096. */
+int wl_policy_act_wide_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
+                            const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream);
+/* wl_ppo_update_wide for that network: the critic's layer-1 forward and its dW1 are taken over d_critic_obs [batch,
+ * critic_obs_dim] (slab order, gathered through the same perm); the layers 2-3 kernel is wl_ppo_update_wide's; the
+ * reduction and Adam step skip the padding rows of both W1t blocks.  No float atomics, a fixed sum order.  With
+ * critic_obs_dim == obs_dim and d_critic_obs == batch->obs it leaves blob, moments and state equal to wl_ppo_update_wide's,
+ * bit for bit.  d_critic_obs 4-byte aligned; otherwise wl_ppo_update_wide's checks. */
+size_t wl_ppo_wide_asym_workspace_bytes(int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches);
+int wl_ppo_update_wide_asym(const wl_ppo_params* params, const wl_ppo_batch* batch, const float* d_critic_obs, int32_t critic_obs_dim,
+                            float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes,
+                            void* stream);
 
 /* ---- the data-parallel PPO update: rsl_rl's multi-GPU PPO.update() [UPSTREAM-RECALL] ------------------------------------
  * n_ranks replicas of the update above (activation WL_ACTIVATION_ELU: wl_ppo_update's network; WL_ACTIVATION_RELU:

@@ -194,6 +194,7 @@ WL_ROW_TASK_TERMS = {"elevation": ("goal_relative_xyz", "root_euler_xyz", "base_
 lib.wl_set_row_terms.argtypes = [_vp, _vp, _i32]
 lib.wl_row_terms.restype = _i32
 lib.wl_row_terms.argtypes = [_vp]
+lib.wl_set_row_critic.argtypes = [_vp, _vp, _i32, _vp, _i32]
 # WL_RESET_EV_*: the DR events wl_set_reset_events can redraw at every reset (name -> bit)
 WL_RESET_EVENTS = {"material": 1, "actuator_gains": 2, "base_mass": 4, "wheel_mass": 8}
 lib.wl_set_reset_events.argtypes = [_vp, _u32]
@@ -239,6 +240,10 @@ lib.wl_ppo_update_asym.argtypes = [C.POINTER(WlPpoParams), C.POINTER(WlPpoBatch)
 lib.wl_ppo_wide_workspace_bytes.restype = _sz
 lib.wl_ppo_wide_workspace_bytes.argtypes = [_i32, _i32, _i32]
 lib.wl_ppo_update_wide.argtypes = [C.POINTER(WlPpoParams), C.POINTER(WlPpoBatch), _vp, _vp, _vp, _vp, _vp, _sz, _vp]
+lib.wl_policy_act_wide_asym.argtypes = [_vp, _vp, _vp, _i32, _vp, WlPolicyOut, _i64, _vp]
+lib.wl_ppo_wide_asym_workspace_bytes.restype = _sz
+lib.wl_ppo_wide_asym_workspace_bytes.argtypes = [_i32, _i32, _i32, _i32]
+lib.wl_ppo_update_wide_asym.argtypes = [C.POINTER(WlPpoParams), C.POINTER(WlPpoBatch), _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]
 lib.wl_ppo_dp_exchange_bytes.restype = _sz
 lib.wl_ppo_dp_exchange_bytes.argtypes = [_i32]
 lib.wl_ppo_update_dp.argtypes = [C.POINTER(WlPpoParams), _i32, _i32, C.POINTER(_vp), _i32, C.POINTER(_i32), C.POINTER(WlPpoBatch),
@@ -253,7 +258,7 @@ lib.wl_graph_upload.argtypes = [_vp, _vp]
 EXPORTED_SYMBOLS = [
     "wl_config_describe", "wl_config_sizeof", "wl_config_finalize", "wl_set_step_counter", "wl_advance_counter", "wl_note_device_counter", "wl_log_flush", "wl_reward_weights", "wl_set_seed", "wl_set_term_bits", "wl_set_peer_fanout", "wl_set_multicast_fanout", "wl_state_bytes", "wl_globals_offset", "wl_create", "wl_destroy",
     "wl_last_error", "wl_build_info", "wl_startup", "wl_reset", "wl_step", "wl_step_host", "wl_step_host_zero_copy", "wl_rollout", "wl_result_bytes", "wl_observe", "wl_curriculum",
-    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_step_stage_b1", "wl_step_stage_b2", "wl_set_event_timers", "wl_event_timers", "wl_set_device_terms", "wl_step_terms", "wl_device_term_masks", "wl_set_device_events", "wl_device_events", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_policy_act", "wl_ppo_wide_workspace_bytes", "wl_ppo_update_wide", "wl_ppo_dp_exchange_bytes", "wl_ppo_update_dp", "wl_episode_stats_workspace_bytes", "wl_episode_stats", "wl_act_infer_step", "wl_policy_act_elu", "wl_actor_mean", "wl_set_critic_terms", "wl_critic_obs_dim", "wl_critic_observe", "wl_set_policy_terms", "wl_policy_obs_dim", "wl_policy_observe", "wl_set_row_terms", "wl_row_terms", "wl_set_reset_events", "wl_reset_events", "wl_policy_blob_floats_asym", "wl_policy_act_asym", "wl_ppo_asym_workspace_bytes", "wl_ppo_update_asym", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_device_terms", "wl_test_null", "wl_test_null_cfg",
+    "wl_synth_actions", "wl_derive_suspension", "wl_set_kernel_variant", "wl_set_scan_tma", "wl_obs_dim", "wl_launch_count", "wl_step_launch_info", "wl_policy_blob_floats", "wl_act_step", "wl_step_stage_a", "wl_step_stage_b", "wl_step_stage_b1", "wl_step_stage_b2", "wl_set_event_timers", "wl_event_timers", "wl_set_device_terms", "wl_step_terms", "wl_device_term_masks", "wl_set_device_events", "wl_device_events", "wl_camera", "wl_gae", "wl_dp_adam_step", "wl_ppo_state_floats", "wl_ppo_workspace_bytes", "wl_ppo_update", "wl_policy_act", "wl_ppo_wide_workspace_bytes", "wl_ppo_update_wide", "wl_ppo_dp_exchange_bytes", "wl_ppo_update_dp", "wl_episode_stats_workspace_bytes", "wl_episode_stats", "wl_act_infer_step", "wl_policy_act_elu", "wl_actor_mean", "wl_set_critic_terms", "wl_critic_obs_dim", "wl_critic_observe", "wl_set_policy_terms", "wl_policy_obs_dim", "wl_policy_observe", "wl_set_row_terms", "wl_row_terms", "wl_set_reset_events", "wl_reset_events", "wl_policy_blob_floats_asym", "wl_policy_act_asym", "wl_ppo_asym_workspace_bytes", "wl_ppo_update_asym", "wl_set_row_critic", "wl_policy_act_wide_asym", "wl_ppo_wide_asym_workspace_bytes", "wl_ppo_update_wide_asym", "wl_graph_upload", "wl_test_detmath", "wl_test_philox", "wl_test_device_terms", "wl_test_null", "wl_test_null_cfg",
 ]
 
 

@@ -153,6 +153,47 @@ def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
     spec.critic_terms = table
 
 
+def _lower_row_critic(cfg, spec: T.TaskSpec):
+    """An Elevation ``cfg.observations.critic`` (``device_terms=True`` only) -> ``spec.row_critic``: the policy row's six
+    terms in row order, noise-free with their own clips and scales, then terms of the critic library (DESIGN 6s).  Anything
+    else raises NotImplementedError naming the term: noise, history or modifiers, a per-element map scale, a map without a
+    clip, row terms out of order, a term after them outside the library; a group that does not open with the row terms
+    keeps the library path's refusal on Elevation."""
+    group = getattr(cfg.observations, "critic", None)
+    if group is None:
+        return
+    from . import privileged, row_terms
+    if getattr(group, "concatenate_terms", True) is not True:
+        raise NotImplementedError("critic observation group: concatenate_terms=False is not implemented")
+    terms = [(name, t) for name, t in _fields(group) if hasattr(t, "func")]
+    head = row_terms.task_terms("elevation")
+    fns = [_fname(t) for _, t in terms]
+    if not fns or fns[0] not in head:
+        _lower_critic(cfg, None, "elevation")               # a library-only group: refused as before
+    for k, ((name, t), fn) in enumerate(zip(terms, fns)):
+        if k < len(head) and fn != head[k]:
+            raise NotImplementedError(f"critic term {name}: {fn} at position {k}; a row critic opens with the Elevation row's "
+                                      f"terms {list(head)} in row order")
+    if len(terms) < len(head):
+        raise NotImplementedError(f"critic observation group {[n for n, _ in terms]}: a row critic opens with all six row terms {list(head)}")
+    out, lib = [], []
+    for k, (name, t) in enumerate(terms):
+        nz = getattr(t, "noise", None)
+        if k < len(head):
+            row_terms.lower_critic_term(name, t.func, nz, getattr(t, "clip", None), getattr(t, "scale", None),
+                                        getattr(t, "modifiers", None), getattr(t, "history_length", 0))
+            params = {k2: v for k2, v in (("clip", getattr(t, "clip", None)), ("scale", getattr(t, "scale", None))) if v is not None}
+            out.append((name, fns[k], params))
+        else:
+            if getattr(t, "modifiers", None) or getattr(t, "history_length", 0):
+                raise NotImplementedError(f"critic term {name}: history_length / modifiers are not implemented")
+            fn, clip = privileged.lower_term(name, t.func, getattr(t, "params", None), getattr(t, "clip", None), nz, getattr(t, "scale", None))
+            lib.append((fn, clip))
+            out.append((name, fn, {"clip": (-clip, clip)} if clip else {}))
+    privileged.check_width(lib, "critic observation group " + ", ".join(n for n, _ in terms[len(head):]))
+    spec.row_critic = out
+
+
 def _lower_policy(cfg, spec: T.TaskSpec, c, device_terms: bool):
     """``cfg.observations.policy`` of the Drift family: BlindObsCfg's group is validated onto the built-in row as before;
     with ``device_terms`` any other group is lowered to ``spec.policy_terms``, the term table of ``wl_policy_observe``
@@ -384,7 +425,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     num_envs = int(cfg.scene.num_envs)
     seed = int(cfg.seed) if getattr(cfg, "seed", None) is not None else 42
     kind = _task_kind(cfg)
-    if getattr(cfg.observations, "critic", None) is not None and kind != "drift":
+    if getattr(cfg.observations, "critic", None) is not None and kind != "drift" and not (kind == "elevation" and device_terms):
         _lower_critic(cfg, None, kind)                      # (refused by name before anything is lowered)
     if kind == "visual":
         return _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device_terms)
@@ -460,6 +501,8 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     c = spec.cfg
     _lower_common(cfg, spec)
     _lower_rows(cfg, spec, c, _OBS_ELEV, "Elevation", device_terms)
+    if device_terms:
+        _lower_row_critic(cfg, spec)
     for _, t in _fields(cfg.observations.policy):
         if hasattr(t, "func") and _fname(t) == "world_height_map":
             c.scan_offset, c.scan_plane_init = float(t.params["offset"]), float(t.params["plane_init_value"])

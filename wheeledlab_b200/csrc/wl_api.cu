@@ -55,6 +55,8 @@ struct wl_sim {
     struct DevEvents* devents; // wl_set_device_events: the device event terms and their timers (null: none)
     PolicyObsTable pobs;       // wl_set_policy_terms: the policy observation's columns (n_cols = 0: none)
     RowTable rows;             // wl_set_row_terms: noise, clip and scale of the Elevation / Visual row (n_terms = 0: none)
+    RowTable crit_rows;        // wl_set_row_critic: clip and scale of the critic's copy of the Elevation row (n_terms = 0: none)
+    CriticTable crit_extra;    // wl_set_row_critic: the critic-library columns after it
 };
 
 // SMs of the H100 SXM the launch geometry is sized for
@@ -1470,16 +1472,19 @@ wl_scan_pipe_kernel(const __grid_constant__ wl_config c, const __grid_constant__
 // through its term's noise, clip and scale.  The draws do not depend on the height-field: every thread forms one or two
 // Philox blocks (4 columns each) into shared memory while the tile is in flight, and thread 32 forms the proprioceptive
 // values meanwhile.  Same launch shape, tile staging and ray arithmetic as wl_scan_kernel.
-template <bool USE_TMA>
-__global__ void __launch_bounds__(WL_SCAN_THREADS, 8)
-wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ RowTable rt,
-                   const float4* __restrict__ st, const float* __restrict__ hf, const wl_globals* __restrict__ gl, uint32_t t_arg,
-                   int32_t call_idx, float* __restrict__ obs) {
+// CRITIC (wl_critic_observe on a row critic, DESIGN 6s): the same row through the critic's clips and scales, with no draw
+// formed (the critic's stages have no noise), in rows of Dc floats, followed by the extra critic-library columns `ex`; thread 32,
+// which loads the state groups, forms their library floats too.
+template <bool USE_TMA, bool CRITIC>
+__device__ __forceinline__ void scan_row_body(const wl_config& c, const CUtensorMap& tmap, const RowTable& rt, const float4* __restrict__ st,
+                                              const float* __restrict__ hf, const wl_globals* __restrict__ gl, uint32_t t_arg,
+                                              int32_t call_idx, float* __restrict__ obs, const CriticTable* ex, int Dc) {
     __shared__ __align__(128) float tile[WL_TILE_W * WL_TILE_H];
     __shared__ __align__(8) uint64_t mbar;
     __shared__ ScanPose sp;
-    __shared__ __align__(16) float dz[4 * WL_ROW_BLOCKS];  // the noise draw of every column (float4 stores; only when some column is noisy)
+    __shared__ __align__(16) float dz[CRITIC ? 4 : 4 * WL_ROW_BLOCKS];  // the noise draw of every column (float4 stores; only when some column is noisy; CRITIC: unused)
     __shared__ float raw[WL_ROW_PROPRIO];    // the raw proprioceptive columns
+    __shared__ float lib[CRITIC ? WL_CRITIC_LIB_FLOATS : 1];            // CRITIC: the critic library floats of the extra columns
     const int i = blockIdx.x, n = c.num_envs, tid = threadIdx.x;
     if (tid == 0) {
         const ScanPose p = scan_pose(c, st, n, i);
@@ -1500,8 +1505,21 @@ wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ 
         raw[2] = eu.x; raw[3] = eu.y; raw[4] = eu.z;
         raw[5] = vb.x; raw[6] = vb.y; raw[7] = vb.z; raw[8] = wb.x; raw[9] = wb.y; raw[10] = wb.z;
         raw[11] = a.x; raw[12] = a.y;
+        if constexpr (CRITIC) {                                // wl_critic_observe_kernel's library floats (critic_first order)
+            const uint32_t G = ex->groups;
+            lib[0] = p.x; lib[1] = p.y; lib[2] = p.z;
+            lib[3] = eu.x; lib[4] = eu.y; lib[5] = eu.z;
+            lib[6] = vb.x; lib[7] = vb.y; lib[8] = vb.z; lib[9] = wb.x; lib[10] = wb.y; lib[11] = wb.z;
+            lib[12] = a.x; lib[13] = a.y;
+            float4 g;
+            if (G & (1u << WL_G_WHEEL)) { g = ldg4(st, WL_G_WHEEL, n, i); lib[14] = g.x; lib[15] = g.y; lib[16] = g.z; lib[17] = g.w; }
+            if (G & (1u << WL_G_STEER)) { g = ldg4(st, WL_G_STEER, n, i); lib[18] = g.x; lib[19] = g.y; }
+            if (G & (1u << WL_G_PMU_D)) { g = ldg4(st, WL_G_PMU_D, n, i); lib[20] = g.x; lib[21] = g.y; lib[22] = g.z; lib[23] = g.w; }
+            if (G & (1u << WL_G_PMASS)) { g = ldg4(st, WL_G_PMASS, n, i); lib[24] = g.x; }
+            if (G & (1u << WL_G_PKD)) { g = ldg4(st, WL_G_PKD, n, i); lib[25] = g.x; lib[26] = g.y; lib[27] = g.z; lib[28] = g.w; }
+        }
     }
-    if (rt.noisy) {                          // in the TMA's shadow
+    if (!CRITIC && rt.noisy) {               // in the TMA's shadow
         const uint32_t t = decode_step(gl, t_arg), gid = (uint32_t)(c.env_id_offset + i);
         for (int b = tid; b < WL_ROW_BLOCKS; b += WL_SCAN_THREADS) {
             float d[4];
@@ -1519,8 +1537,16 @@ wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ 
     }
     __syncthreads();                         // constants, mbarrier, draws and raw columns visible to everyone
     const ScanPose q = sp;
-    float* row = obs + (size_t)WL_OBS_DIM_ELEV * i;
-    if (tid < WL_ROW_PROPRIO) row[tid] = row_stage(rt.col[tid], raw[tid], rt.col[tid].noise != WL_NOISE_NONE ? dz[tid] : 0.0f);
+    float* row = obs + (size_t)(CRITIC ? Dc : WL_OBS_DIM_ELEV) * i;
+    if constexpr (CRITIC) {                  // (wl_set_row_critic refuses noise: every stage is clip and scale)
+        if (tid < WL_ROW_PROPRIO) row[tid] = row_stage(rt.col[tid], raw[tid], 0.0f);
+        if (tid < ex->n_cols) {
+            const float x = lib[ex->src[tid]], cl = ex->clip[tid];
+            row[WL_OBS_DIM_ELEV + tid] = cl > 0.0f ? r_clamp(x, -cl, cl) : x;
+        }
+    } else {
+        if (tid < WL_ROW_PROPRIO) row[tid] = row_stage(rt.col[tid], raw[tid], rt.col[tid].noise != WL_NOISE_NONE ? dz[tid] : 0.0f);
+    }
     if (USE_TMA) {
         mbar_wait_parity(&mbar, 0);
     } else {
@@ -1530,7 +1556,22 @@ wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ 
         }
         __syncthreads();
     }
-    scan_rays<true>(c, tile, q, row + WL_ROW_PROPRIO, tid, &rt.map, dz + WL_ROW_PROPRIO);
+    scan_rays<true>(c, tile, q, row + WL_ROW_PROPRIO, tid, &rt.map, CRITIC ? nullptr : dz + WL_ROW_PROPRIO);
+}
+template <bool USE_TMA>
+__global__ void __launch_bounds__(WL_SCAN_THREADS, 8)
+wl_scan_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ RowTable rt,
+                   const float4* __restrict__ st, const float* __restrict__ hf, const wl_globals* __restrict__ gl, uint32_t t_arg,
+                   int32_t call_idx, float* __restrict__ obs) {
+    scan_row_body<USE_TMA, false>(c, tmap, rt, st, hf, gl, t_arg, call_idx, obs, nullptr, 0);
+}
+// the critic row [N, Dc] of a row critic (rt: the critic's stages, ex: its extra columns)
+template <bool USE_TMA>
+__global__ void __launch_bounds__(WL_SCAN_THREADS, 8)
+wl_scan_critic_row_kernel(const __grid_constant__ wl_config c, const __grid_constant__ CUtensorMap tmap, const __grid_constant__ RowTable rt,
+                          const __grid_constant__ CriticTable ex, const float4* __restrict__ st, const float* __restrict__ hf, int Dc,
+                          float* __restrict__ obs) {
+    scan_row_body<USE_TMA, true>(c, tmap, rt, st, hf, nullptr, 0u, 0, obs, &ex, Dc);
 }
 
 #include "wl_reset_dr.cuh"
@@ -2932,7 +2973,10 @@ int wl_set_critic_terms(wl_sim* sim, const wl_critic_term* terms, int32_t n_term
     sim->critic = tb;
     return WL_OK;
 }
-int32_t wl_critic_obs_dim(const wl_sim* sim) { return sim ? sim->critic.n_cols : 0; }
+int32_t wl_critic_obs_dim(const wl_sim* sim) {
+    if (!sim) return 0;
+    return sim->crit_rows.n_terms ? WL_OBS_DIM_ELEV + sim->crit_extra.n_cols : sim->critic.n_cols;
+}
 
 int wl_set_policy_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) {
     const std::string fn = "wl_set_policy_terms: ";
@@ -2989,16 +3033,9 @@ int wl_policy_observe(wl_sim* sim, int64_t step_counter, int32_t call_idx, float
     return launched(sim, "wl_policy_observe_kernel");
 }
 
-int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) {
-    const std::string fn = "wl_set_row_terms: ";
-    if (!sim) return fail(WL_EINVAL, fn + "null handle");
-    if (n_terms > 0 && !terms) return fail(WL_EINVAL, fn + "null term table");
-    const int task = sim->cfg.task;
-    if (task != WL_TASK_ELEVATION && task != WL_TASK_VISUAL)
-        return fail(WL_EUNSUPPORTED, fn + "row terms are implemented for the Elevation and Visual tasks (the Drift family's groups go through wl_set_policy_terms)");
-    if (fan_set(sim)) return fail(WL_EUNSUPPORTED, fn + "the peer fan-out is set, and only the built-in row carries it");
-    if (sim->scan_mode == 2 && task == WL_TASK_ELEVATION)
-        return fail(WL_EUNSUPPORTED, fn + "the pipelined ray-caster (wl_set_scan_tma(2)) has no row-terms variant");
+// The row table of the Elevation / Visual terms `terms` (n_terms: 0 or the task's count), every term checked before `tb` is
+// written; noise kept only when `corrupt`.  Error messages start with fn.
+static int row_table(const std::string& fn, int task, const wl_policy_term* terms, int32_t n_terms, bool corrupt, RowTable& out) {
     static const int elev[WL_ROW_TERMS_ELEVATION] = {WL_ROW_GOAL_RELATIVE_XYZ, WL_CRITIC_ROOT_EULER_XYZ, WL_CRITIC_BASE_LIN_VEL,
                                                      WL_CRITIC_BASE_ANG_VEL, WL_CRITIC_LAST_ACTION, WL_ROW_WORLD_HEIGHT_MAP};
     static const int vis[WL_ROW_TERMS_VISUAL] = {WL_CRITIC_BASE_LIN_VEL, WL_CRITIC_BASE_ANG_VEL, WL_CRITIC_LAST_ACTION};
@@ -3024,7 +3061,7 @@ int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) 
         if (!finite) return fail(WL_EINVAL, at + "a noise, clip or scale parameter is not finite");
         for (int j = 0; j < (map ? 1 : w); ++j) {
             RowStage& s = map ? tb.map : tb.col[col++];
-            s.noise = sim->cfg.enable_corruption ? d.noise : WL_NOISE_NONE;
+            s.noise = corrupt ? d.noise : WL_NOISE_NONE;
             s.na = (float)d.noise_params[0];
             s.nb = d.noise == WL_NOISE_UNIFORM ? (float)(d.noise_params[1] - d.noise_params[0]) : (float)d.noise_params[1];
             s.flags = (d.clip ? WL_ROW_CLIP : 0u) | (d.n_scale ? WL_ROW_SCALE : 0u);
@@ -3035,7 +3072,56 @@ int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) 
         }
     }
     tb.n_terms = n_terms;
-    sim->rows = tb;
+    out = tb;
+    return WL_OK;
+}
+
+int wl_set_row_terms(wl_sim* sim, const wl_policy_term* terms, int32_t n_terms) {
+    const std::string fn = "wl_set_row_terms: ";
+    if (!sim) return fail(WL_EINVAL, fn + "null handle");
+    if (n_terms > 0 && !terms) return fail(WL_EINVAL, fn + "null term table");
+    const int task = sim->cfg.task;
+    if (task != WL_TASK_ELEVATION && task != WL_TASK_VISUAL)
+        return fail(WL_EUNSUPPORTED, fn + "row terms are implemented for the Elevation and Visual tasks (the Drift family's groups go through wl_set_policy_terms)");
+    if (fan_set(sim)) return fail(WL_EUNSUPPORTED, fn + "the peer fan-out is set, and only the built-in row carries it");
+    if (sim->scan_mode == 2 && task == WL_TASK_ELEVATION)
+        return fail(WL_EUNSUPPORTED, fn + "the pipelined ray-caster (wl_set_scan_tma(2)) has no row-terms variant");
+    return row_table(fn, task, terms, n_terms, sim->cfg.enable_corruption != 0, sim->rows);
+}
+
+int wl_set_row_critic(wl_sim* sim, const wl_policy_term* row_terms, int32_t n_row_terms, const wl_critic_term* extra, int32_t n_extra) {
+    const std::string fn = "wl_set_row_critic: ";
+    if (!sim) return fail(WL_EINVAL, fn + "null handle");
+    if ((n_row_terms > 0 && !row_terms) || (n_extra > 0 && !extra)) return fail(WL_EINVAL, fn + "null term table");
+    if (sim->cfg.task != WL_TASK_ELEVATION)
+        return fail(WL_EUNSUPPORTED, fn + "a row critic is implemented for the Elevation task only (the Drift family's critic: wl_set_critic_terms)");
+    if (n_row_terms == 0 && n_extra != 0) return fail(WL_EINVAL, fn + "extra columns need the row terms");
+    if (n_extra < 0 || n_extra > WL_MAX_CRITIC_TERMS) return fail(WL_EINVAL, fn + "at most 16 extra critic terms");
+    RowTable rt;
+    if (int rc = row_table(fn, WL_TASK_ELEVATION, row_terms, n_row_terms, false, rt)) return rc;
+    static const char* const names[WL_ROW_TERMS_ELEVATION] = {"goal_relative_xyz", "root_euler_xyz", "base_lin_vel", "base_ang_vel",
+                                                              "last_action", "world_height_map"};
+    for (int k = 0; k < n_row_terms; ++k) {
+        const std::string at = fn + "term " + std::to_string(k) + " (" + names[k] + "): ";
+        if (row_terms[k].noise != WL_NOISE_NONE) return fail(WL_EINVAL, at + "the critic row is noise-free (noise must be WL_NOISE_NONE)");
+        if (k == 5 && !row_terms[k].clip) return fail(WL_EINVAL, at + "the critic's height map needs a finite clip (a miss is +inf)");
+    }
+    CriticTable ex;
+    memset(&ex, 0, sizeof ex);
+    for (int k = 0; k < n_extra; ++k) {
+        const wl_critic_term& d = extra[k];
+        const std::string at = fn + "extra term " + std::to_string(k) + ": ";
+        if (d.kind < 1 || d.kind >= WL_CRITIC_KINDS) return fail(WL_EINVAL, at + "unknown term kind " + std::to_string(d.kind));
+        if (!std::isfinite(d.clip) || d.clip < 0.0f) return fail(WL_EINVAL, at + "clip must be finite and >= 0");
+        if (ex.n_cols + critic_width(d.kind) > WL_MAX_CRITIC_OBS) return fail(WL_EINVAL, fn + "the extra columns are wider than 32 floats");
+        for (int j = 0; j < critic_width(d.kind); ++j) {
+            ex.src[ex.n_cols] = (uint8_t)(critic_first(d.kind) + j);
+            ex.clip[ex.n_cols++] = d.clip;
+        }
+        ex.groups |= critic_groups(d.kind);
+    }
+    sim->crit_rows = rt;
+    sim->crit_extra = ex;
     return WL_OK;
 }
 int32_t wl_row_terms(const wl_sim* sim) { return sim ? sim->rows.n_terms : 0; }
@@ -3057,9 +3143,19 @@ uint32_t wl_reset_events(const wl_sim* sim) { return sim ? sim->reset_ev : 0u; }
 int wl_critic_observe(wl_sim* sim, float* d_critic_obs, void* stream) {
     if (!sim || !d_critic_obs) return fail(WL_EINVAL, "wl_critic_observe: null argument");
     if ((uintptr_t)d_critic_obs & 3u) return fail(WL_EINVAL, "wl_critic_observe: d_critic_obs must be 4-byte aligned");
-    if (sim->critic.n_cols < 1) return fail(WL_EINVAL, "wl_critic_observe: no critic table (wl_set_critic_terms)");
+    if (sim->critic.n_cols < 1 && !sim->crit_rows.n_terms)
+        return fail(WL_EINVAL, "wl_critic_observe: no critic table (wl_set_critic_terms / wl_set_row_critic)");
     ensure_device(sim);
     const int n = sim->cfg.num_envs;
+    if (sim->crit_rows.n_terms) {                            // the row critic: the ray-caster again, noise-free (DESIGN 6s)
+        const int Dc = WL_OBS_DIM_ELEV + sim->crit_extra.n_cols;
+        cudaStream_t cs = (cudaStream_t)stream;
+        if (sim->scan_mode >= 1 && sim->has_tmap)
+            wl_scan_critic_row_kernel<true><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->crit_rows, sim->crit_extra, sim->state, sim->hf, Dc, d_critic_obs);
+        else
+            wl_scan_critic_row_kernel<false><<<n, WL_SCAN_THREADS, 0, cs>>>(sim->cfg, sim->tmap, sim->crit_rows, sim->crit_extra, sim->state, sim->hf, Dc, d_critic_obs);
+        return launched(sim, "wl_scan_critic_row_kernel");
+    }
     wl_critic_observe_kernel<<<(n + WL_CRITIC_BS - 1) / WL_CRITIC_BS, WL_CRITIC_BS, 0, (cudaStream_t)stream>>>(sim->critic, sim->state, n, d_critic_obs);
     return launched(sim, "wl_critic_observe_kernel");
 }
@@ -3239,10 +3335,11 @@ static void ppo_rows_layout(int32_t obs_dim, int32_t batch, int32_t num_mini_bat
     w.bytes = w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas;
 }
 // the network an update trains: wl_ppo_update's ELU network, wl_ppo_update_wide's ReLU network, wl_ppo_update_asym's ELU
-// network with a critic row of its own
-enum PpoNet { PPO_NARROW, PPO_WIDE, PPO_ASYM };
+// network with a critic row of its own, wl_ppo_update_wide_asym's ReLU network with one
+enum PpoNet { PPO_NARROW, PPO_WIDE, PPO_ASYM, PPO_WIDE_ASYM };
 static size_t ppo_grad_asym_smem(int obs_dim, int critic_obs_dim);
 static int wide_attributes(int dev, const char* fn);
+static int wide_asym_attributes(int dev, const char* fn);
 // The shape checks and the workspace layout of an update of `net` (critic_obs_dim: PPO_ASYM only).  The gradient kernels'
 // shared-memory limits are per-device attributes: raised once to what the widest network needs, so updates of any obs_dim
 // share them in one process.  The workspace query reaches here before the first update, so callers that query outside a
@@ -3250,21 +3347,25 @@ static int wide_attributes(int dev, const char* fn);
 static int ppo_workspace(const char* fn, PpoNet net, int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches,
                          PpoWideWorkspace& x) {
     if (obs_dim < 1 || batch < 1 || num_mini_batches < 1) return fail(WL_EINVAL, std::string(fn) + ": obs_dim, batch and num_mini_batches must be >= 1");
-    if (net == PPO_WIDE && obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
-    if (net != PPO_WIDE && obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
+    const bool wide = net == PPO_WIDE || net == PPO_WIDE_ASYM;
+    if (wide && obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 4096");
+    if (!wide && obs_dim > 16) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim > 16 (the network wl_act_step runs)");
     if (net == PPO_ASYM && (critic_obs_dim < 1 || critic_obs_dim > WL_MAX_CRITIC_OBS))
         return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..32");
+    if (net == PPO_WIDE_ASYM && (critic_obs_dim < 1 || critic_obs_dim > WL_WIDE_MAX_OBS))
+        return fail(WL_EUNSUPPORTED, std::string(fn) + ": critic_obs_dim must be in 1..4096");
     if (batch % num_mini_batches != 0) return fail(WL_EINVAL, std::string(fn) + ": batch must be a multiple of num_mini_batches");
     int dev = 0, sms = 0;
     if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
     if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
     if (int rc = net == PPO_WIDE ? wide_attributes(dev, fn)
+                 : net == PPO_WIDE_ASYM ? wide_asym_attributes(dev, fn)
                  : net == PPO_ASYM ? raise_smem<wl_ppo_grad_asym_kernel>(dev, ppo_grad_asym_smem(16, WL_MAX_CRITIC_OBS), fn)
                                    : raise_smem<wl_ppo_grad_kernel>(dev, ppo_grad_smem(16), fn))
         return rc;
-    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, x.w, net == PPO_ASYM ? critic_obs_dim : 0);
+    ppo_rows_layout(obs_dim, batch, num_mini_batches, sms, x.w, net == PPO_ASYM || net == PPO_WIDE_ASYM ? critic_obs_dim : 0);
     x.bytes = x.w.bytes;
-    if (net == PPO_WIDE) {      // then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
+    if (wide) {                 // then H1 and dZ1 of a mini-batch ([tiles * 32][128] fp32 each)
         const size_t hb = sizeof(float) * 2 * WL_HID * (size_t)WL_PPO_TILE * ((batch / num_mini_batches + WL_PPO_TILE - 1) / WL_PPO_TILE);
         x.h1_off = align256(x.w.bytes);
         x.dz_off = align256(x.h1_off + hb);
@@ -3301,7 +3402,8 @@ static int ppo_check_layout(const char* fn, PpoNet net, int32_t critic_obs_dim, 
         return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
     if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)b->actions & 7u) || ((uintptr_t)b->mean & 7u))
         return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, actions / mean 8-byte aligned");
-    static const char* const query[] = {"wl_ppo_workspace_bytes", "wl_ppo_wide_workspace_bytes", "wl_ppo_asym_workspace_bytes"};
+    static const char* const query[] = {"wl_ppo_workspace_bytes", "wl_ppo_wide_workspace_bytes", "wl_ppo_asym_workspace_bytes",
+                                        "wl_ppo_wide_asym_workspace_bytes"};
     if (workspace_bytes < x.bytes)
         return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (" + query[net] + " gives " + std::to_string(x.bytes) + ")");
     return WL_OK;
@@ -3310,11 +3412,13 @@ static int ppo_check_layout(const char* fn, PpoNet net, int32_t critic_obs_dim, 
 static size_t ppo_grad_smem(int obs_dim);
 static size_t ppo_wide_grad_smem();
 static size_t ppo_wide_dw1_smem();
+static size_t ppo_wide_dw1_asym_smem();
 
 // The gradient phase of one mini-batch (a.row0): one gradient row per CTA in the workspace.  Narrow: wl_ppo_grad_kernel;
-// wide: the gathered layer-1 forward, the layers 2-3 gradient kernel and the split-K dW1.
+// wide: the gathered layer-1 forward, the layers 2-3 gradient kernel and the split-K dW1 -- with xc, the critic's layer 1
+// over xc [batch, Dc] (the asymmetric forward and dW1 kernels; the layers 2-3 kernel is the same).
 static void ppo_grad_phase(bool wide, const PpoWideWorkspace& x, const PolicyOffsets& po, const PolicyOffsets& pc, const PpoArgs& a,
-                           const float* d_blob, const float* d_state, char* ws, cudaStream_t cs) {
+                           const float* d_blob, const float* d_state, char* ws, cudaStream_t cs, const float* xc = nullptr, int Dc = 0) {
     const PpoWorkspace& w = x.w;
     float* rows = (float*)(ws + w.rows_off);
     if (!wide) {
@@ -3323,11 +3427,14 @@ static void ppo_grad_phase(bool wide, const PpoWideWorkspace& x, const PolicyOff
     }
     float* H1 = (float*)(ws + x.h1_off);
     float* dZ1 = (float*)(ws + x.dz_off);
-    const dim3 dw1_grid((unsigned)((a.obs_dim + WL_DW1_K - 1) / WL_DW1_K), (unsigned)w.ctas);
-    wl_ppo_wide_fwd_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE, cs>>>(d_blob, po, a, H1);
+    const int K = xc && Dc > a.obs_dim ? Dc : a.obs_dim;
+    const dim3 dw1_grid((unsigned)((K + WL_DW1_K - 1) / WL_DW1_K), (unsigned)w.ctas);
+    if (xc) wl_ppo_wide_fwd_asym_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE_ASYM, cs>>>(d_blob, po, a, xc, Dc, H1);
+    else wl_ppo_wide_fwd_kernel<<<a.tiles, WL_WIDE_THREADS, sizeof(float) * 2 * WL_WIDE_STAGE, cs>>>(d_blob, po, a, H1);
     wl_ppo_wide_grad_kernel<<<w.ctas, WL_PPO_THREADS, ppo_wide_grad_smem(), cs>>>(d_blob, w.blob_floats, po, pc, a, d_state, H1, dZ1,
                                                                                  rows, w.rowlen);
-    wl_ppo_wide_dw1_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
+    if (xc) wl_ppo_wide_dw1_asym_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_asym_smem(), cs>>>(po, a, dZ1, rows, w.rowlen, xc, Dc);
+    else wl_ppo_wide_dw1_kernel<<<dw1_grid, WL_WIDE_THREADS, ppo_wide_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
 }
 
 // the per-mini-batch arguments of every update entry
@@ -3340,17 +3447,19 @@ static void ppo_launch_args(const wl_ppo_params* p, const wl_ppo_batch* b, PpoAr
 
 static int wide_compact_offsets(const PolicyOffsets& po, int blob_floats, PolicyOffsets& pc);
 
-// wl_ppo_update (wide false) and wl_ppo_update_wide: rsl_rl's update, epochs x mini-batches of the gradient phase, the
-// reduction and the Adam step
+// wl_ppo_update (wide false), wl_ppo_update_wide and wl_ppo_update_wide_asym (xc: the critic's rows, Dc wide): rsl_rl's
+// update, epochs x mini-batches of the gradient phase, the reduction and the Adam step
 static int ppo_update(const char* fn, bool wide, const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m,
-                      float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes, void* stream) {
+                      float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes, void* stream,
+                      const float* xc = nullptr, int Dc = 0) {
     if (int rc = ppo_check_args(fn, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace)) return rc;
     PpoWideWorkspace x;
-    if (int rc = ppo_check_layout(fn, wide ? PPO_WIDE : PPO_NARROW, 0, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x))
+    const PpoNet net = !wide ? PPO_NARROW : xc ? PPO_WIDE_ASYM : PPO_WIDE;
+    if (int rc = ppo_check_layout(fn, net, Dc, p, b, d_blob, d_adam_m, d_adam_v, d_workspace, workspace_bytes, x))
         return rc;
     const PpoWorkspace& w = x.w;
     PolicyOffsets po, pc;
-    policy_offsets(p->obs_dim, po.o);
+    policy_offsets(p->obs_dim, po.o, Dc);
     if (wide) wide_compact_offsets(po, w.blob_floats, pc);
     else pc = po;
     cudaStream_t cs = (cudaStream_t)stream;
@@ -3367,11 +3476,18 @@ static int ppo_update(const char* fn, bool wide, const wl_ppo_params* p, const w
         for (int i = 0; i < p->num_mini_batches; ++i) {
             a.row0 = (int64_t)i * a.B;
             sa.update_index = e * p->num_mini_batches + i;
-            ppo_grad_phase(wide, x, po, pc, a, d_blob, d_state, ws, cs);
-            wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
-                                                               p->entropy_coef, red, norm_part);
-            wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
-                                                                        w.blob_floats, po, p->obs_dim, sa, nullptr);
+            ppo_grad_phase(wide, x, po, pc, a, d_blob, d_state, ws, cs, xc, Dc);
+            if (xc) {                                        // the asymmetric parameter lengths (ppo_is_param's critic_dim)
+                wl_ppo_reduce_asym_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, Dc,
+                                                                        d_blob, p->entropy_coef, red, norm_part);
+                wl_ppo_step_asym_kernel<<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                          w.blob_floats, po, p->obs_dim, Dc, sa);
+            } else {
+                wl_ppo_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, w.ctas, w.rowlen, w.blob_floats, po, p->obs_dim, d_blob,
+                                                                   p->entropy_coef, red, norm_part);
+                wl_ppo_step_kernel<false><<<1, WL_PPO_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts,
+                                                                            w.blob_floats, po, p->obs_dim, sa, nullptr);
+            }
             if (int rc = cuda_check(cudaGetLastError(), wide ? "wl_ppo_update_wide kernels" : "wl_ppo_grad_kernel / wl_ppo_reduce_kernel / wl_ppo_step_kernel"))
                 return rc;
         }
@@ -3449,12 +3565,21 @@ static size_t ppo_wide_grad_smem() {
     return wide_compact_bytes() + sizeof(float) * (2 * WL_HID * WL_HID + WL_HID + 4 * WL_PPO_TILE * WL_PPO_HS + WL_PPO_TILE * WL_PPO_SD);
 }
 static size_t ppo_wide_dw1_smem() { return sizeof(float) * 2 * WL_PPO_TILE * (WL_DW1_K + 2 * WL_HID); }
+static size_t policy_act_asym_smem() { return sizeof(float) * (2 * WL_WIDE_STAGE_ASYM + WL_WIDE_ROWS * WL_PPO_HS) + wide_compact_bytes(); }
+static size_t ppo_wide_dw1_asym_smem() { return sizeof(float) * 2 * WL_PPO_TILE * (2 * WL_DW1_K + 2 * WL_HID); }
 
 // the dynamic shared-memory limits of the wide kernels, raised together (the sizes do not depend on obs_dim)
 static int wide_attributes(int dev, const char* fn) {
     if (int rc = raise_smem<wl_policy_act_kernel>(dev, policy_act_smem(), fn)) return rc;
     if (int rc = raise_smem<wl_ppo_wide_grad_kernel>(dev, ppo_wide_grad_smem(), fn)) return rc;
     return raise_smem<wl_ppo_wide_dw1_kernel>(dev, ppo_wide_dw1_smem(), fn);
+}
+// the same for the asymmetric kernels (and the wide grad kernel they share)
+static int wide_asym_attributes(int dev, const char* fn) {
+    if (int rc = wide_attributes(dev, fn)) return rc;
+    if (int rc = raise_smem<wl_policy_act_wide_asym_kernel>(dev, policy_act_asym_smem(), fn)) return rc;
+    if (int rc = raise_smem<wl_ppo_wide_fwd_asym_kernel>(dev, sizeof(float) * 2 * WL_WIDE_STAGE_ASYM, fn)) return rc;
+    return raise_smem<wl_ppo_wide_dw1_asym_kernel>(dev, ppo_wide_dw1_asym_smem(), fn);
 }
 
 int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
@@ -3472,6 +3597,29 @@ int wl_policy_act(wl_sim* sim, const float* d_obs_in, const float* d_policy_blob
     wl_policy_act_kernel<<<(n + WL_WIDE_ROWS - 1) / WL_WIDE_ROWS, WL_WIDE_THREADS, policy_act_smem(), (cudaStream_t)stream>>>(
         d_obs_in, n, D, d_policy_blob, blob_floats, po, pc, out, sim->globals, sim->cfg.seed, sim->cfg.env_id_offset, (uint32_t)step_counter);
     return launched(sim, "wl_policy_act_kernel");
+}
+
+int wl_policy_act_wide_asym(wl_sim* sim, const float* d_obs_in, const float* d_critic_obs_in, int32_t critic_obs_dim,
+                            const float* d_policy_blob, wl_policy_out out, int64_t step_counter, void* stream) {
+    const char* fn = "wl_policy_act_wide_asym";
+    if (!sim || !d_obs_in || !d_critic_obs_in || !d_policy_blob || !out.actions || !out.mean || !out.log_prob || !out.value)
+        return fail(WL_EINVAL, std::string(fn) + ": null argument");
+    const int D = policy_in_dim(sim), n = sim->cfg.num_envs;
+    if (D < 1 || D > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim must be in 1..4096");
+    if (critic_obs_dim < 1 || critic_obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EINVAL, std::string(fn) + ": critic_obs_dim must be in 1..4096");
+    if (((uintptr_t)d_policy_blob & 15u) || ((uintptr_t)out.actions & 7u) || ((uintptr_t)out.mean & 7u))
+        return fail(WL_EINVAL, std::string(fn) + ": policy blob must be 16-byte aligned, actions/mean 8-byte aligned");
+    if (((uintptr_t)d_obs_in & 3u) || ((uintptr_t)d_critic_obs_in & 3u))
+        return fail(WL_EINVAL, std::string(fn) + ": obs_in / critic_obs_in must be 4-byte aligned");
+    ensure_device(sim);
+    if (int rc = wide_asym_attributes(sim->device, fn)) return rc;
+    PolicyOffsets po, pc;
+    const int blob_floats = policy_offsets(D, po.o, critic_obs_dim);
+    wide_compact_offsets(po, blob_floats, pc);
+    wl_policy_act_wide_asym_kernel<<<(n + WL_WIDE_ROWS - 1) / WL_WIDE_ROWS, WL_WIDE_THREADS, policy_act_asym_smem(), (cudaStream_t)stream>>>(
+        d_obs_in, n, D, d_critic_obs_in, critic_obs_dim, d_policy_blob, blob_floats, po, pc, out, sim->globals, sim->cfg.seed,
+        sim->cfg.env_id_offset, (uint32_t)step_counter);
+    return launched(sim, "wl_policy_act_wide_asym_kernel");
 }
 
 int wl_actor_mean(const float* d_obs, int32_t n, int32_t obs_dim, const float* d_policy_blob, int32_t activation, float* d_mean,
@@ -3512,6 +3660,18 @@ size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_m
 int wl_ppo_update_wide(const wl_ppo_params* p, const wl_ppo_batch* b, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state,
                        void* d_workspace, size_t workspace_bytes, void* stream) {
     return ppo_update("wl_ppo_update_wide", true, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace, workspace_bytes, stream);
+}
+
+size_t wl_ppo_wide_asym_workspace_bytes(int32_t obs_dim, int32_t critic_obs_dim, int32_t batch, int32_t num_mini_batches) {
+    PpoWideWorkspace x;
+    return ppo_workspace("wl_ppo_wide_asym_workspace_bytes", PPO_WIDE_ASYM, obs_dim, critic_obs_dim, batch, num_mini_batches, x) ? 0 : x.bytes;
+}
+
+int wl_ppo_update_wide_asym(const wl_ppo_params* p, const wl_ppo_batch* b, const float* d_critic_obs, int32_t critic_obs_dim, float* d_blob,
+                            float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace, size_t workspace_bytes, void* stream) {
+    const char* fn = "wl_ppo_update_wide_asym";
+    if (!d_critic_obs || ((uintptr_t)d_critic_obs & 3u)) return fail(WL_EINVAL, std::string(fn) + ": d_critic_obs is null or not 4-byte aligned");
+    return ppo_update(fn, true, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace, workspace_bytes, stream, d_critic_obs, critic_obs_dim);
 }
 
 // ---- the data-parallel update (DESIGN 6j) ---------------------------------------------------------------------------

@@ -12,12 +12,16 @@
 //                              heads, db1, dsigma and the loss sums in registers (one gradient row per CTA, as 6f)
 //   wl_ppo_wide_dw1_kernel     PPO: dW1 = X[perm]^T dZ1, split over samples: split s writes gradient row s
 // then wl_ppo_reduce_kernel and wl_ppo_step_kernel as for the narrow network.  No float atomics: every sum has a fixed order.
+// The asymmetric network (DESIGN 6s) has the critic's layer 1 over a row of its own: wl_policy_act_wide_asym_kernel,
+// wl_ppo_wide_fwd_asym_kernel and wl_ppo_wide_dw1_asym_kernel are the kernels above with that second input (the grad
+// kernel is shared), followed by the asymmetric reduce and step kernels.
 #pragma once
 
 #define WL_WIDE_ROWS 32                           // rows per layer-1 tile (8 warps x 4 rows in the mlp_tile_layer geometry)
 #define WL_WIDE_KC 32                             // inputs per staged chunk of layer 1
 #define WL_WIDE_XS (WL_WIDE_KC + 4)               // padded staged observation row
 #define WL_WIDE_STAGE (WL_WIDE_ROWS * WL_WIDE_XS + 2 * WL_WIDE_KC * WL_HID)     // floats per stage: x rows | W1t actor | W1t critic
+#define WL_WIDE_STAGE_ASYM (2 * WL_WIDE_ROWS * WL_WIDE_XS + 2 * WL_WIDE_KC * WL_HID)   // actor rows | critic rows | W1t actor | W1t critic
 #define WL_WIDE_THREADS 256
 #define WL_WIDE_MAX_OBS 4096
 #define WL_DW1_K 64                               // W1t rows per dW1 tile (x 128 columns of both nets)
@@ -50,40 +54,76 @@ __device__ __forceinline__ void wide_stage(float* sb, const float* __restrict__ 
         cp_async16(sw + net * WL_WIDE_KC * WL_HID + q * 4, blob + (net ? oWc : oWa) + (size_t)k0 * WL_HID + q * 4);
     }
 }
+// the asymmetric stage (WL_WIDE_STAGE_ASYM floats: actor rows | critic rows | W1t actor | W1t critic): net `net` stages its
+// rows and kn[net] W1t rows from its own input; a net with kn <= 0 (past its last chunk) stages nothing
+__device__ __forceinline__ void wide_stage_asym(float* sb, const float* __restrict__ x, int D, const float* __restrict__ xc, int Dc,
+                                                const int64_t* srow, const float* __restrict__ blob, int oWa, int oWc, int k0,
+                                                int kna, int knc) {
+#pragma unroll
+    for (int net = 0; net < 2; ++net) {
+        const float* xs = net ? xc : x;
+        const int Dn = net ? Dc : D, kn = net ? knc : kna;
+        if (kn <= 0) continue;
+        for (int k = threadIdx.x; k < WL_WIDE_ROWS * WL_WIDE_KC; k += WL_WIDE_THREADS) {
+            const int r = k / WL_WIDE_KC, j = k % WL_WIDE_KC, col = k0 + j;
+            const int64_t row = srow[r];
+            const bool ok = row >= 0 && col < Dn;
+            cp_async4(sb + (net * WL_WIDE_ROWS + r) * WL_WIDE_XS + j, ok ? xs + row * Dn + col : xs, ok);
+        }
+        float* sw = sb + 2 * WL_WIDE_ROWS * WL_WIDE_XS + net * WL_WIDE_KC * WL_HID;
+        const float* w = blob + (net ? oWc : oWa) + (size_t)k0 * WL_HID;
+        for (int q = threadIdx.x; q < kn * (WL_HID / 4); q += WL_WIDE_THREADS) cp_async16(sw + q * 4, w + q * 4);
+    }
+}
 
 // layer 1 (pre-activation) of both nets for the 32 rows srow[] of x (-1: a zero row), in the mlp_tile_layer geometry: warp w
 // takes rows 4w..4w+3, lane = (net, 4 units).  Each K chunk is summed on its own (inputs ascending) and added to the running
 // sum, which starts at the bias: two-level summation keeps the rounding error of a 689-long (3208-long) dot product near
-// that of torch's blocked sums.  `stage`: 2 * WL_WIDE_STAGE floats of shared memory.  Ends with a __syncthreads.
+// that of torch's blocked sums.  `stage`: 2 * WL_WIDE_STAGE floats of shared memory (ASYM: 2 * WL_WIDE_STAGE_ASYM).  Ends
+// with a __syncthreads.
+// ASYM (DESIGN 6s): the critic's inputs are xc [.., Dc] instead of x.  Each net keeps its own chunks of 32 from input 0,
+// so a net's sums are those of the symmetric layer on its own input; a net that has run out of chunks adds nothing (not
+// zeros: -0 + 0 is +0).
+template <bool ASYM = false>
 __device__ __forceinline__ void wide_layer1(const float* __restrict__ x, int D, const int64_t* srow, const float* __restrict__ blob,
-                                            const PolicyOffsets& po, float* stage, float acc[4][4]) {
+                                            const PolicyOffsets& po, float* stage, float acc[4][4],
+                                            const float* __restrict__ xc = nullptr, int Dc = 0) {
+    constexpr int STAGE = ASYM ? WL_WIDE_STAGE_ASYM : WL_WIDE_STAGE;
     const int lane = threadIdx.x & 31, net = lane >> 4, ucol = (lane & 15) * 4, env0 = (threadIdx.x >> 5) * 4;
-    const int nin1 = (D + 3) & ~3, nch = (nin1 + WL_WIDE_KC - 1) / WL_WIDE_KC;
+    const int nina = (D + 3) & ~3, ninc = ASYM ? (Dc + 3) & ~3 : nina;
+    const int nin1 = max(nina, ninc), nch = (nin1 + WL_WIDE_KC - 1) / WL_WIDE_KC, ninn = net ? ninc : nina;
     const float4 b0 = *reinterpret_cast<const float4*>(blob + (net ? po.o[7] : po.o[1]) + ucol);
 #pragma unroll
     for (int e = 0; e < 4; ++e) { acc[e][0] = b0.x; acc[e][1] = b0.y; acc[e][2] = b0.z; acc[e][3] = b0.w; }
-    wide_stage(stage, x, D, srow, blob, po.o[0], po.o[6], 0, min(WL_WIDE_KC, nin1));
+    if (ASYM) wide_stage_asym(stage, x, D, xc, Dc, srow, blob, po.o[0], po.o[6], 0, min(WL_WIDE_KC, nina), min(WL_WIDE_KC, ninc));
+    else wide_stage(stage, x, D, srow, blob, po.o[0], po.o[6], 0, min(WL_WIDE_KC, nin1));
     cp_async_commit();
     for (int c = 0; c < nch; ++c) {
         if (c + 1 < nch) {
             const int k1 = (c + 1) * WL_WIDE_KC;
-            wide_stage(stage + ((c + 1) & 1) * WL_WIDE_STAGE, x, D, srow, blob, po.o[0], po.o[6], k1, min(WL_WIDE_KC, nin1 - k1));
+            if (ASYM) wide_stage_asym(stage + ((c + 1) & 1) * STAGE, x, D, xc, Dc, srow, blob, po.o[0], po.o[6], k1,
+                                      min(WL_WIDE_KC, nina - k1), min(WL_WIDE_KC, ninc - k1));
+            else wide_stage(stage + ((c + 1) & 1) * STAGE, x, D, srow, blob, po.o[0], po.o[6], k1, min(WL_WIDE_KC, nin1 - k1));
             cp_async_commit();
             cp_async_wait<1>();
         } else {
             cp_async_wait<0>();
         }
         __syncthreads();                                     // chunk c is in shared memory for every thread
-        const float* sb = stage + (c & 1) * WL_WIDE_STAGE;
-        float part[4][4];
+        const float* sb = stage + (c & 1) * STAGE;
+        const int kn = min(WL_WIDE_KC, ninn - c * WL_WIDE_KC);
+        if (!ASYM || kn > 0) {
+            const int xoff = ASYM ? (net * WL_WIDE_ROWS + env0) * WL_WIDE_XS : env0 * WL_WIDE_XS;
+            float part[4][4];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { part[e][0] = 0.0f; part[e][1] = 0.0f; part[e][2] = 0.0f; part[e][3] = 0.0f; }
-        mlp_tile_accum(sb + WL_WIDE_ROWS * WL_WIDE_XS + net * WL_WIDE_KC * WL_HID + ucol, sb + env0 * WL_WIDE_XS, WL_WIDE_XS,
-                       min(WL_WIDE_KC, nin1 - c * WL_WIDE_KC), part);
+            for (int e = 0; e < 4; ++e) { part[e][0] = 0.0f; part[e][1] = 0.0f; part[e][2] = 0.0f; part[e][3] = 0.0f; }
+            mlp_tile_accum(sb + (ASYM ? 2 : 1) * WL_WIDE_ROWS * WL_WIDE_XS + net * WL_WIDE_KC * WL_HID + ucol, sb + xoff, WL_WIDE_XS,
+                           kn, part);
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
+            for (int e = 0; e < 4; ++e)
 #pragma unroll
-            for (int q = 0; q < 4; ++q) acc[e][q] += part[e][q];
+                for (int q = 0; q < 4; ++q) acc[e][q] += part[e][q];
+        }
         __syncthreads();                                     // every thread is done with the buffer the next chunk refills
     }
 }
@@ -107,16 +147,18 @@ __device__ __forceinline__ void store_relu(float* h0, int hstride, const float a
 
 // ---- the rollout's policy ------------------------------------------------------------------------------------------
 // One CTA per 32 envs.  po: blob offsets; pc: the compact offsets of the shared-memory copy.  Does not step the env and
-// does not trigger dependents early: a step launched after it with PDL waits for every action.
-__global__ void __launch_bounds__(WL_WIDE_THREADS)
-wl_policy_act_kernel(const float* __restrict__ obs_in, int n, int D, const float* __restrict__ blob, int blob_floats, PolicyOffsets po,
-                     PolicyOffsets pc, wl_policy_out out, const wl_globals* __restrict__ gl, uint64_t seed, int env_id_offset,
-                     uint32_t t_arg) {
+// does not trigger dependents early: a step launched after it with PDL waits for every action.  ASYM (wl_policy_act_wide_asym):
+// the critic's layer 1 reads critic_in [n, Dc]; everything after layer 1 is the same code.
+template <bool ASYM>
+__device__ __forceinline__ void policy_act_wide_body(const float* __restrict__ obs_in, int n, int D, const float* __restrict__ blob,
+                                                     int blob_floats, const PolicyOffsets& po, const PolicyOffsets& pc,
+                                                     const wl_policy_out& out, const wl_globals* __restrict__ gl, uint64_t seed,
+                                                     int env_id_offset, uint32_t t_arg, const float* __restrict__ critic_in, int Dc) {
     extern __shared__ __align__(128) float smem[];
     __shared__ __align__(8) uint64_t mbar;
     __shared__ int64_t srow[WL_WIDE_ROWS];
     float* stage = smem;
-    float* sw = stage + 2 * WL_WIDE_STAGE;                               // compact blob
+    float* sw = stage + 2 * (ASYM ? WL_WIDE_STAGE_ASYM : WL_WIDE_STAGE);   // compact blob
     float* sh = sw + (po.o[6] - po.o[1]) + (blob_floats - po.o[7]);     // [32][WL_PPO_HS]
     const int tid = threadIdx.x, r0 = blockIdx.x * WL_WIDE_ROWS;
     if (tid == 0) wide_load_compact(sw, blob, blob_floats, po, &mbar);
@@ -124,7 +166,7 @@ wl_policy_act_kernel(const float* __restrict__ obs_in, int n, int D, const float
     __syncthreads();
     const int lane = tid & 31, net = lane >> 4, ucol = (lane & 15) * 4, env0 = (tid >> 5) * 4;
     float acc[4][4];
-    wide_layer1(obs_in, D, srow, blob, po, stage, acc);
+    wide_layer1<ASYM>(obs_in, D, srow, blob, po, stage, acc, critic_in, Dc);
     float* h0 = sh + env0 * WL_PPO_HS + net * WL_HID;
     store_relu(h0 + ucol, WL_PPO_HS, acc);
     mbar_wait_parity(&mbar, 0);
@@ -161,6 +203,18 @@ wl_policy_act_kernel(const float* __restrict__ obs_in, int n, int D, const float
         out.value[i] = vv;
     }
 }
+__global__ void __launch_bounds__(WL_WIDE_THREADS)
+wl_policy_act_kernel(const float* __restrict__ obs_in, int n, int D, const float* __restrict__ blob, int blob_floats, PolicyOffsets po,
+                     PolicyOffsets pc, wl_policy_out out, const wl_globals* __restrict__ gl, uint64_t seed, int env_id_offset,
+                     uint32_t t_arg) {
+    policy_act_wide_body<false>(obs_in, n, D, blob, blob_floats, po, pc, out, gl, seed, env_id_offset, t_arg, nullptr, 0);
+}
+__global__ void __launch_bounds__(WL_WIDE_THREADS)
+wl_policy_act_wide_asym_kernel(const float* __restrict__ obs_in, int n, int D, const float* __restrict__ critic_in, int Dc,
+                               const float* __restrict__ blob, int blob_floats, PolicyOffsets po, PolicyOffsets pc, wl_policy_out out,
+                               const wl_globals* __restrict__ gl, uint64_t seed, int env_id_offset, uint32_t t_arg) {
+    policy_act_wide_body<true>(obs_in, n, D, blob, blob_floats, po, pc, out, gl, seed, env_id_offset, t_arg, critic_in, Dc);
+}
 
 // ---- PPO update ------------------------------------------------------------------------------------------------------
 // H1[row] = relu(layer 1 of X[perm[row0 + row]]) for the mini-batch, [tiles * 32][128] (rows past B: relu(b1), never used)
@@ -173,6 +227,20 @@ wl_ppo_wide_fwd_kernel(const float* __restrict__ blob, PolicyOffsets po, const _
     __syncthreads();
     float acc[4][4];
     wide_layer1(a.b.obs, a.obs_dim, srow, blob, po, smem, acc);
+    const int lane = tid & 31, net = lane >> 4, ucol = (lane & 15) * 4, env0 = (tid >> 5) * 4;
+    store_relu(H1 + (size_t)(s0 + env0) * (2 * WL_HID) + net * WL_HID + ucol, 2 * WL_HID, acc);
+}
+// the same with the critic's layer 1 over xc [batch, Dc] (slab order, gathered through the same perm)
+__global__ void __launch_bounds__(WL_WIDE_THREADS)
+wl_ppo_wide_fwd_asym_kernel(const float* __restrict__ blob, PolicyOffsets po, const __grid_constant__ PpoArgs a, const float* __restrict__ xc,
+                            int Dc, float* __restrict__ H1) {
+    extern __shared__ __align__(128) float smem[];
+    __shared__ int64_t srow[WL_WIDE_ROWS];
+    const int tid = threadIdx.x, s0 = blockIdx.x * WL_WIDE_ROWS;
+    if (tid < WL_WIDE_ROWS) srow[tid] = s0 + tid < a.B ? a.b.perm[a.row0 + s0 + tid] : -1;
+    __syncthreads();
+    float acc[4][4];
+    wide_layer1<true>(a.b.obs, a.obs_dim, srow, blob, po, smem, acc, xc, Dc);
     const int lane = tid & 31, net = lane >> 4, ucol = (lane & 15) * 4, env0 = (tid >> 5) * 4;
     store_relu(H1 + (size_t)(s0 + env0) * (2 * WL_HID) + net * WL_HID + ucol, 2 * WL_HID, acc);
 }
@@ -319,23 +387,29 @@ wl_ppo_wide_grad_kernel(const float* __restrict__ blob, int blob_floats, PolicyO
 // dW1t[k][u] (both nets: u < 64 actor, u >= 64 critic) = sum over samples of X[perm[row0 + s]][k] dZ1[s][u].  Block
 // (kt, split) owns W1t rows 64 kt .. 64 kt + 63 and the samples of tiles split, split + gridDim.y, ... (the grad kernel's
 // tiles), summed in sample order; it writes its partial into gradient row `split`.  Thread: 4 rows x 8 columns.
-__global__ void __launch_bounds__(WL_WIDE_THREADS)
-wl_ppo_wide_dw1_kernel(PolicyOffsets po, const __grid_constant__ PpoArgs a, const float* __restrict__ dZ1, float* __restrict__ rows, int rowlen) {
-    extern __shared__ __align__(128) float smem[];           // 2 stages of [32][64] X | [32][128] dZ1
-    constexpr int XF = WL_PPO_TILE * WL_DW1_K, SF = XF + WL_PPO_TILE * 2 * WL_HID;
+// ASYM: the critic's columns take their rows from xc [batch, Dc] (staged beside X); gridDim.x covers max(D, Dc).
+template <bool ASYM>
+__device__ __forceinline__ void ppo_wide_dw1_body(const PolicyOffsets& po, const PpoArgs& a, const float* __restrict__ dZ1,
+                                                  float* __restrict__ rows, int rowlen, const float* __restrict__ xc, int Dc) {
+    extern __shared__ __align__(128) float smem[];           // 2 stages of [32][64] X (ASYM: and [32][64] Xc) | [32][128] dZ1
+    constexpr int XF = WL_PPO_TILE * WL_DW1_K, NX = ASYM ? 2 : 1, SF = NX * XF + WL_PPO_TILE * 2 * WL_HID;
     const int tid = threadIdx.x, D = a.obs_dim, k0 = blockIdx.x * WL_DW1_K;
     const int tk = (tid >> 4) * 4, tu = (tid & 15) * 8;
     auto stage = [&](float* sb, int tile) {
         const int s0 = tile * WL_PPO_TILE;
-        for (int k = tid; k < XF; k += WL_WIDE_THREADS) {
-            const int s = k / WL_DW1_K, j = k % WL_DW1_K, col = k0 + j;
-            const bool ok = s0 + s < a.B && col < D;
-            const float* src = a.b.obs;
-            if (ok) src += (size_t)a.b.perm[a.row0 + s0 + s] * D + col;
-            cp_async4(sb + k, src, ok);
+#pragma unroll
+        for (int net = 0; net < NX; ++net) {
+            const int Dn = net ? Dc : D;
+            for (int k = tid; k < XF; k += WL_WIDE_THREADS) {
+                const int s = k / WL_DW1_K, j = k % WL_DW1_K, col = k0 + j;
+                const bool ok = s0 + s < a.B && col < Dn;
+                const float* src = net ? xc : a.b.obs;
+                if (ok) src += (size_t)a.b.perm[a.row0 + s0 + s] * Dn + col;
+                cp_async4(sb + net * XF + k, src, ok);
+            }
         }
         for (int k = tid; k < WL_PPO_TILE * 32; k += WL_WIDE_THREADS)
-            cp_async16(sb + XF + 4 * k, dZ1 + (size_t)s0 * (2 * WL_HID) + 4 * k);
+            cp_async16(sb + NX * XF + 4 * k, dZ1 + (size_t)s0 * (2 * WL_HID) + 4 * k);
     };
     float g[4][8];
 #pragma unroll
@@ -354,8 +428,8 @@ wl_ppo_wide_dw1_kernel(PolicyOffsets po, const __grid_constant__ PpoArgs a, cons
             cp_async_wait<0>();
         }
         __syncthreads();
-        const float* sx = smem + (it & 1) * SF;
-        const float* sz = sx + XF;
+        const float* sx = smem + (it & 1) * SF + (ASYM && tu >= WL_HID ? XF : 0);
+        const float* sz = smem + (it & 1) * SF + NX * XF;
         for (int s = 0; s < WL_PPO_TILE; ++s) {
             const float4 xv = *reinterpret_cast<const float4*>(sx + s * WL_DW1_K + tk);
             const float4 za = *reinterpret_cast<const float4*>(sz + s * 2 * WL_HID + tu), zb = *reinterpret_cast<const float4*>(sz + s * 2 * WL_HID + tu + 4);
@@ -367,11 +441,21 @@ wl_ppo_wide_dw1_kernel(PolicyOffsets po, const __grid_constant__ PpoArgs a, cons
         }
         __syncthreads();
     }
+    const int Dn = ASYM && tu >= WL_HID ? Dc : D;
     float* row = rows + (size_t)blockIdx.y * rowlen + (tu < WL_HID ? po.o[0] : po.o[6]) + (tu & (WL_HID - 1));
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-        if (k0 + tk + k < D) {
+        if (k0 + tk + k < Dn) {
             *reinterpret_cast<float4*>(row + (size_t)(k0 + tk + k) * WL_HID) = make_float4(g[k][0], g[k][1], g[k][2], g[k][3]);
             *reinterpret_cast<float4*>(row + (size_t)(k0 + tk + k) * WL_HID + 4) = make_float4(g[k][4], g[k][5], g[k][6], g[k][7]);
         }
+}
+__global__ void __launch_bounds__(WL_WIDE_THREADS)
+wl_ppo_wide_dw1_kernel(PolicyOffsets po, const __grid_constant__ PpoArgs a, const float* __restrict__ dZ1, float* __restrict__ rows, int rowlen) {
+    ppo_wide_dw1_body<false>(po, a, dZ1, rows, rowlen, nullptr, 0);
+}
+__global__ void __launch_bounds__(WL_WIDE_THREADS)
+wl_ppo_wide_dw1_asym_kernel(PolicyOffsets po, const __grid_constant__ PpoArgs a, const float* __restrict__ dZ1, float* __restrict__ rows,
+                            int rowlen, const float* __restrict__ xc, int Dc) {
+    ppo_wide_dw1_body<true>(po, a, dZ1, rows, rowlen, xc, Dc);
 }

@@ -341,6 +341,8 @@ class ManagerBasedRLEnv:
             self.sim.set_reset_events(**{name: True for name in self.spec.reset_events})
         if self.spec.critic_terms:
             self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
+        if self.spec.row_critic:
+            self.set_critic_observation(self.spec.row_critic)
         if self.spec.policy_terms:
             self.set_policy_observation([(name, fn, {"noise": nz, "clip": cl, "scale": sc}) for name, fn, nz, cl, sc in self.spec.policy_terms])
         if self.spec.row_terms:
@@ -415,20 +417,33 @@ class ManagerBasedRLEnv:
         by name) or its name, `params` optionally holding ``clip=(-c, c)``.  The row is their concatenation, noise-free,
         at most 32 floats, formed on the device.  From then on ``step`` / ``reset`` / ``get_observations`` put a fresh
         ``[N, Dc]`` tensor at ``extras["observations"]["critic"]`` (and in the returned observation dict) and
-        ``observation_manager.group_obs_dim["critic"]`` is ``(Dc,)``; ``[]`` removes the group.  Drift family only, and not
-        together with host-side Python terms or device terms."""
-        from . import privileged
+        ``observation_manager.group_obs_dim["critic"]`` is ``(Dc,)``; ``[]`` removes the group.  Drift family, and not
+        together with host-side Python terms or device terms.
+
+        On Elevation a list that opens with the policy row's six terms in row order (``goal_relative_xyz``,
+        ``root_euler_xyz``, ``base_lin_vel``, ``base_ang_vel``, ``last_action``, ``world_height_map``) is a row critic
+        (``sim.set_row_critic``, DESIGN 6s): those six with their own ``clip`` and ``scale`` -- no noise, and the map with a
+        clip -- then terms of the critic library, 689..721 floats.  Any other list goes to the library path above."""
+        from . import privileged, row_terms
         terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
         if terms and (self._py_rewards or self._py_terms or self._py_obs or self._py_events):
             raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
         if terms and (self._dev_terms or self._dev_events):
             raise NotImplementedError("a critic observation group together with device terms is not implemented")
-        table = []
-        for name, fn, params in terms:
+        fns = [fn if isinstance(fn, str) else getattr(fn, "__name__", "") for _, fn, _ in terms]
+        row = tuple(fns[:6]) == row_terms.task_terms("elevation")
+        table, head = [], []
+        for k, (name, fn, params) in enumerate(terms):
             p = dict(params or {})
-            table.append(privileged.lower_term(name, fn, p, clip=p.pop("clip", None)))
+            if row and k < 6:
+                head.append(row_terms.lower_critic_term(name, fn, p.pop("noise", None), p.pop("clip", None), p.pop("scale", None)))
+            else:
+                table.append(privileged.lower_term(name, fn, p, clip=p.pop("clip", None)))
         privileged.check_width(table)
-        dc = self.sim.set_critic_terms(table)     # (refuses a task outside the Drift family)
+        if row:
+            dc = self.sim.set_row_critic(head, table)     # (refuses a task other than Elevation)
+        else:
+            dc = self.sim.set_critic_terms(table)     # (refuses a task outside the Drift family)
         self._critic_terms = terms
         if dc:
             self.observation_manager.group_obs_dim["critic"] = (dc,)

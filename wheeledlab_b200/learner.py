@@ -239,13 +239,16 @@ class FusedPPO:
 
     ``critic_obs_dim`` (None: the critic reads the policy row) trains the asymmetric network (``wl_ppo_update_asym``, DESIGN
     6m): the blob is laid out by ``blob_layout(obs_dim, critic_obs_dim)`` and the slab carries ``critic_obs_in``
-    [T + 1, N, critic_obs_dim].  "elu" only, and not with an exchange (its buffers are sized by one obs_dim)."""
+    [T + 1, N, critic_obs_dim].  "elu" for the Drift family (obs_dim <= 16, critic_obs_dim <= 32); "relu" for the wide
+    network (obs_dim > 16: the Elevation row critic, ``wl_ppo_update_wide_asym``, DESIGN 6s, critic_obs_dim <= 4096).
+    Not with an exchange (its buffers are sized by one obs_dim)."""
 
     def __init__(self, blob: torch.Tensor, obs_dim: int, cfg: PPOConfig | None = None, activation: str = "elu",
                  exchange: "PPOExchange | None" = None, critic_obs_dim: int | None = None):
         from .policy import check_activation
-        if critic_obs_dim is not None and activation != "elu":
-            raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+        if critic_obs_dim is not None and activation != "elu" and obs_dim <= 16:
+            raise NotImplementedError('a critic observation group with activation="relu" is not implemented for the Drift family '
+                                      '(obs_dim <= 16: ELU only)')
         if critic_obs_dim is not None and exchange is not None:
             raise NotImplementedError("a critic observation group in a data-parallel world is not implemented "
                                       "(the exchange buffer is sized by one obs_dim)")
@@ -258,6 +261,8 @@ class FusedPPO:
         self.exchange = exchange
         self.activation = check_activation(activation)
         wide = self.activation == "relu"
+        self._asym_ws = lib.wl_ppo_wide_asym_workspace_bytes if wide else lib.wl_ppo_asym_workspace_bytes
+        self._asym_update = lib.wl_ppo_update_wide_asym if wide else lib.wl_ppo_update_asym
         self._ws_query = lib.wl_ppo_wide_workspace_bytes if wide else lib.wl_ppo_workspace_bytes
         self._update = lib.wl_ppo_update_wide if wide else lib.wl_ppo_update
         self.m = torch.zeros_like(blob)
@@ -270,7 +275,7 @@ class FusedPPO:
     def _workspace(self, batch: int) -> torch.Tensor:
         with torch.cuda.device(self.device):
             if self.critic_obs_dim is not None:
-                need = lib.wl_ppo_asym_workspace_bytes(self.obs_dim, self.critic_obs_dim, batch, self.cfg.num_mini_batches)
+                need = self._asym_ws(self.obs_dim, self.critic_obs_dim, batch, self.cfg.num_mini_batches)
             else:
                 need = self._ws_query(self.obs_dim, batch, self.cfg.num_mini_batches)
         if need == 0:
@@ -319,10 +324,10 @@ class FusedPPO:
         p, batch, ws = self._prepare(slab, returns, advantages, perm)
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         if self.critic_obs_dim is not None:
-            check(lib.wl_ppo_update_asym(C.byref(p), C.byref(batch), C.c_void_p(slab.critic_obs_in.data_ptr()), self.critic_obs_dim,
-                                         C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()), C.c_void_p(self.v.data_ptr()),
-                                         C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), stream),
-                  "wl_ppo_update_asym")
+            check(self._asym_update(C.byref(p), C.byref(batch), C.c_void_p(slab.critic_obs_in.data_ptr()), self.critic_obs_dim,
+                                    C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()), C.c_void_p(self.v.data_ptr()),
+                                    C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), stream),
+                  self._asym_update.__name__)
             return self._stats()
         check(self._update(C.byref(p), C.byref(batch), C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
                            C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(ws.data_ptr()),
@@ -493,7 +498,8 @@ class PPOIteration:
 
     ``critic=True`` (a handle with a critic table, ``sim.set_critic_terms``) runs the asymmetric iteration, still one graph:
     the rollout with ``critic=True``, the bootstrap value from the critic row ``critic_obs_in[T]``, and
-    ``wl_ppo_update_asym``; the blob is laid out by ``blob_layout(obs_dim, sim.critic_obs_dim)``."""
+    ``wl_ppo_update_asym``; the blob is laid out by ``blob_layout(obs_dim, sim.critic_obs_dim)``.  With "relu" (an Elevation
+    handle with a row critic, ``sim.set_row_critic``, DESIGN 6s) the update is ``wl_ppo_update_wide_asym``."""
 
     SUMMARY = ("Loss/value_function", "Loss/surrogate", "Loss/entropy", "Loss/learning_rate", "Policy/mean_noise_std")
 
@@ -526,7 +532,7 @@ class PPOIteration:
     def _bootstrap(self) -> torch.Tensor:
         from .policy import critic_value
         if self.critic_obs_dim is not None:                    # cobs0 = critic_obs_in[T] once the rollout has run
-            return critic_value(self.blob, self.sim.policy_width, self.roll.cobs0, "elu", self.critic_obs_dim)
+            return critic_value(self.blob, self.sim.policy_width, self.roll.cobs0, self.ppo.activation, self.critic_obs_dim)
         return critic_value(self.blob, self.sim.policy_width, self.roll.obs0, self.ppo.activation)
 
     def _returns(self):
@@ -765,8 +771,10 @@ class FusedOnPolicyRunner:
     An env with a ``critic`` observation group (``env.set_critic_observation``, or a reference cfg with
     ``observations.critic``) trains the asymmetric network (DESIGN 6m): the critic is ``Linear(Dc, 64)``-first and reads the
     critic row, the iteration is ``PPOIteration(critic=True)`` -- still one graph -- and checkpoints keep rsl_rl's keys with
-    ``critic.0.weight`` ``[64, Dc]``, as ``ActorCritic(num_actor_obs, num_critic_obs, ...)`` has it.  On one GPU with the ELU
-    network; with Python terms, device terms, ``activation="relu"`` or a data-parallel world it raises ``NotImplementedError``.
+    ``critic.0.weight`` ``[64, Dc]``, as ``ActorCritic(num_actor_obs, num_critic_obs, ...)`` has it.  On one GPU: the ELU
+    network on the Drift family, the ReLU network on Elevation with a row critic (DESIGN 6s, noisy row terms included); with
+    Python terms, device terms, ``activation="relu"`` on the Drift family or a data-parallel world it raises
+    ``NotImplementedError``.
 
     An env with a policy observation table (``env.set_policy_observation``, or a reference cfg whose ``observations.policy``
     was lowered with ``device_terms=True``; DESIGN 6q) trains its policy on the table's row: the actor (and, without a critic
@@ -809,8 +817,9 @@ class FusedOnPolicyRunner:
                 raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
             if dev_step:
                 raise NotImplementedError("a critic observation group together with device terms is not implemented")
-            if s.activation != "elu":
-                raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+            if s.activation != "elu" and sim.policy_width <= 16:
+                raise NotImplementedError('a critic observation group with activation="relu" is not implemented for the Drift family '
+                                          '(ELU only)')
             if _world_size() > 1:                           # (before anything initialises NCCL)
                 raise NotImplementedError("a critic observation group in a data-parallel world (WORLD_SIZE > 1) is not implemented: "
                                           "the exchange buffer is sized by one obs_dim")
@@ -829,7 +838,7 @@ class FusedOnPolicyRunner:
         std = torch.full((2,), s.init_noise_std)
         self.blob = pack_actor_critic(mk(2), mk(1, self.critic_obs_dim or D), std, D, sim.device, critic_obs_dim=self.critic_obs_dim)
         if self.critic_obs_dim is not None:
-            self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, "elu", episode_stats=True, critic=True)
+            self.it = PPOIteration(sim, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation, episode_stats=True, critic=True)
         elif self.staged:
             self.it = StagedPPOIteration(e, self.blob, self.alg_cfg, self.num_steps_per_env, self.activation)
         else:

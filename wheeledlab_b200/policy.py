@@ -249,6 +249,25 @@ def policy_act_asym(sim: WheeledSim, obs_in: torch.Tensor, critic_obs_in: torch.
                                  C.c_void_p(blob.data_ptr()), po, step_counter, _stream_ptr(sim.device)), "wl_policy_act_asym")
 
 
+def policy_act_wide_asym(sim: WheeledSim, obs_in: torch.Tensor, critic_obs_in: torch.Tensor, blob: torch.Tensor, actions: torch.Tensor,
+                         mean: torch.Tensor, log_prob: torch.Tensor, value: torch.Tensor, step_counter: int):
+    """policy_act(..., "relu") for the asymmetric network (wl_policy_act_wide_asym, DESIGN 6s): the critic reads
+    `critic_obs_in` [N, Dc] (Dc <= 4096, e.g. an Elevation row critic's) and the blob is laid out by blob_layout(obs_dim, Dc);
+    actions / mean / log-prob are wl_policy_act's bit for bit."""
+    n = sim.num_envs
+    if critic_obs_in.dim() != 2 or not 1 <= critic_obs_in.shape[1] <= 4096:
+        raise ValueError(f"critic_obs_in must have shape [N, Dc] with Dc in 1..4096, not {tuple(critic_obs_in.shape)}")
+    _device_tensor("obs_in", obs_in, sim.device, shape=(n, sim.policy_width))
+    _device_tensor("critic_obs_in", critic_obs_in, sim.device, shape=(n, critic_obs_in.shape[1]))
+    _device_tensor("blob", blob, sim.device, shape=(blob_layout(sim.policy_width, critic_obs_in.shape[1])[1],))
+    for name, t, shape in (("actions", actions, (n, 2)), ("mean", mean, (n, 2)), ("log_prob", log_prob, (n,)), ("value", value, (n,))):
+        _device_tensor(name, t, sim.device, shape=shape)
+    po = WlPolicyOut(actions.data_ptr(), mean.data_ptr(), log_prob.data_ptr(), value.data_ptr())
+    check(lib.wl_policy_act_wide_asym(sim._h, C.c_void_p(obs_in.data_ptr()), C.c_void_p(critic_obs_in.data_ptr()),
+                                      critic_obs_in.shape[-1], C.c_void_p(blob.data_ptr()), po, step_counter, _stream_ptr(sim.device)),
+          "wl_policy_act_wide_asym")
+
+
 class FusedPolicyRollout:
     """T policy-and-step launches captured as ONE CUDA graph: the reference's whole collection loop
     (modified_rsl_rl_runner.py:70-109).  activation "elu" (the Drift family): T x wl_act_step, the policy fused into the
@@ -267,7 +286,9 @@ class FusedPolicyRollout:
     ``critic=True`` rolls out the asymmetric network on a handle that has a critic table (``sim.set_critic_terms``): T x
     (``policy_act_asym``, ``wl_step``, ``wl_critic_observe`` into row k + 1) on device counters, one graph.
     ``slab.critic_obs_in`` [T + 1, N, Dc] holds the critic rows: row k is what ``values[k]`` was computed from, row T the
-    bootstrap row.  The blob is laid out by ``blob_layout(obs_dim, Dc)``.  "elu" only, and not with device terms.
+    bootstrap row.  The blob is laid out by ``blob_layout(obs_dim, Dc)``.  Not with device terms.  "elu" for the Drift
+    family; "relu" for an Elevation handle with a row critic (``sim.set_row_critic``, DESIGN 6s), with or without row
+    terms: T x (``policy_act_wide_asym``, ``wl_step``, ``wl_critic_observe``).
 
     On a handle with a policy observation table (``sim.set_policy_terms``, DESIGN 6q) every step is the policy kernel of the
     network on ``slab.obs_in[k]`` (``wl_policy_act_elu`` / ``wl_policy_act`` / ``wl_policy_act_asym``, or ``wl_actor_mean``
@@ -286,8 +307,9 @@ class FusedPolicyRollout:
                 raise ValueError("critic: the training rollout only (playback reads the actor alone)")
             if self.device_terms:
                 raise NotImplementedError("a critic observation group together with device terms is not implemented")
-            if activation != "elu":
-                raise NotImplementedError('a critic observation group with activation="relu" is not implemented (Drift family, ELU only)')
+            if activation != "elu" and sim.policy_width <= 16:
+                raise NotImplementedError('a critic observation group with activation="relu" is not implemented for the Drift '
+                                          'family (ELU only)')
             if sim.critic_obs_dim < 1:
                 raise ValueError("critic=True needs a critic table on the handle (sim.set_critic_terms)")
             if (sim.num_envs * sim.obs_dim) % 2:
@@ -337,8 +359,9 @@ class FusedPolicyRollout:
         if self.deterministic:
             actor_mean(self.blob, D, slab.obs_in[k], self.activation, out=slab.actions[k])
         elif self.critic:
-            policy_act_asym(sim, slab.obs_in[k], slab.critic_obs_in[k], self.blob, slab.actions[k], self.pol.mean[k],
-                            self.pol.log_prob[k], self.pol.values[k], t)
+            act = policy_act_wide_asym if self.activation == "relu" else policy_act_asym
+            act(sim, slab.obs_in[k], slab.critic_obs_in[k], self.blob, slab.actions[k], self.pol.mean[k], self.pol.log_prob[k],
+                self.pol.values[k], t)
         else:
             policy_act(sim, slab.obs_in[k], self.blob, slab.actions[k], self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t,
                        self.activation)
@@ -365,8 +388,9 @@ class FusedPolicyRollout:
             if self.table:
                 self._table_step(k, t)
             elif self.critic:
-                policy_act_asym(self.sim, self.slab.obs_in[k], self.slab.critic_obs_in[k], self.blob, self.slab.actions[k],
-                                self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t)
+                act = policy_act_wide_asym if self.activation == "relu" else policy_act_asym
+                act(self.sim, self.slab.obs_in[k], self.slab.critic_obs_in[k], self.blob, self.slab.actions[k],
+                    self.pol.mean[k], self.pol.log_prob[k], self.pol.values[k], t)
                 self.sim.step(self.slab.actions[k], t, out=self.slab.step_outputs(k), log=self.logs[k])
                 self.sim.critic_observe(out=self.slab.critic_obs_in[k + 1])
             elif self.deterministic:

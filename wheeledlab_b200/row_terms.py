@@ -50,6 +50,17 @@ def lower_term(name: str, func, noise=None, clip=None, scale=None, modifiers=Non
     return fn, nz, cl, sc
 
 
+def lower_critic_term(name: str, func, noise=None, clip=None, scale=None, modifiers=None, history_length=0) -> tuple:
+    """``lower_term`` for one of the six row terms that open an Elevation row critic (DESIGN 6s): the critic row is
+    noise-free, and a height map without a clip would hand a miss (+inf) to the critic, so both are refused by name."""
+    if noise is not None:
+        raise NotImplementedError(f"critic term {name}: noise on a critic term is not implemented (the critic row is noise-free)")
+    t = lower_term(name, func, None, clip, scale, modifiers, history_length)
+    if t[0] == "world_height_map" and t[2] is None:
+        raise NotImplementedError(f"critic term {name}: the critic's height map needs a finite clip (a ray that misses is +inf)")
+    return t
+
+
 def check_order(task: str, fns) -> None:
     """Row terms name the row's own terms in its order: anything else is a modified term list, which is not implemented."""
     expected = task_terms(task)

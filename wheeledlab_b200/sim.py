@@ -452,6 +452,23 @@ class WheeledSim:
         check(lib.wl_set_row_terms(self._h, arr, len(terms)), "wl_set_row_terms")
         return self.row_terms
 
+    def set_row_critic(self, row_terms, extra=()) -> int:
+        """The handle's row critic (wl_set_row_critic, DESIGN 6s; Elevation only): the critic row is the Elevation row's six
+        terms in row order, noise-free, each with its own clip and scale (``set_row_terms``'s form; a term with noise or a
+        height map without a clip is refused), then the critic-library terms ``extra`` (``set_critic_terms``'s form).
+        ``critic_observe`` writes it; [] clears it.  Returns Dc (689..721).  Nothing is launched; a graph captured earlier
+        keeps the critic it was captured with."""
+        row_terms, arr = _policy_term_array(row_terms, _lib.WL_ROW_TERMS, "row term")
+        pairs = [(t, 0.0) if isinstance(t, str) else (t[0], t[1] or 0.0) for t in extra]
+        for name, _ in pairs:
+            if name not in _lib.WL_CRITIC_TERMS:
+                raise ValueError(f"critic term {name!r} is not in the library {sorted(_lib.WL_CRITIC_TERMS)}")
+        ex = (_lib.WlCriticTerm * max(1, len(pairs)))()
+        for k, (name, clip) in enumerate(pairs):
+            ex[k] = _lib.WlCriticTerm(_lib.WL_CRITIC_TERMS[name][0], float(clip))
+        check(lib.wl_set_row_critic(self._h, arr, len(row_terms), ex, len(pairs)), "wl_set_row_critic")
+        return self.critic_obs_dim
+
     @property
     def row_terms(self) -> int:
         """The number of row terms of the handle (0: the built-in row)."""
