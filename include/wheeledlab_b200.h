@@ -477,6 +477,10 @@ int wl_set_scan_tma(wl_sim* sim, int32_t use_tma);
 int32_t wl_obs_dim(const wl_sim* sim);
 /* number of kernel launches issued through this handle since creation */
 int64_t wl_launch_count(const wl_sim* sim);
+/* number of wl_step launches through this handle that ran chained: the single-GPU duo kernel started without waiting for the
+ * previous grid, because the stream's previous launch of a kernel that triggers its dependents was another env set's duo
+ * step with disjoint buffers (DESIGN.md 6e) */
+int64_t wl_chained_step_count(const wl_sim* sim);
 /* what the most recent wl_step on this handle launched (read-only; launches nothing): the kernel variant actually used (1, 4
  * or 8 after the automatic choice; 0 before the first wl_step), the handle's step-spec key, whether the Drift-family duo
  * kernel (variant 8) ran an instantiation specialised on that key (1) or its generic body (0), and the threads per CTA of the

@@ -6,7 +6,8 @@
 
 `run` steps M independent env sets round-robin inside one CUDA graph, as bench.py does, so that the working set is larger
 than L2 and every launch starts cold.  Every warp that owns envs stamps %globaltimer at its hand-offs and records %smid and
-%warpid (csrc/wl_api.cu, WL_DUO_TRACE).  Times are ns after the launch's first warp entry, median over launches of the
+%warpid (csrc/wl_api.cu, WL_DUO_TRACE); in a chained launch (one whose predecessor is another env set's duo step) the
+aux warp also stamps when its deferred griddepcontrol.wait returns.  Times are ns after the launch's first warp entry, median over launches of the
 per-launch median warp, except where a row says otherwise.  "pass k cycles" rows are SM clock cycles (%clock) of the env
 warp's sub-step pass k (pass 0 from bar.sync 1), median over env warps, split by whether an aux warp on the same SM
 scheduler (%warpid % 4) was between its bar.arrive 1 and bar.arrive 3 (issuing the noise, push and reset draws) at any time
@@ -25,7 +26,8 @@ ROOT = Path(__file__).resolve().parent.parent
 
 # DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64; ck[6] u32
 TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
-     [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3"]
+     [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3",
+                                                        "aux: griddepcontrol.wait, chained launch"]
 
 
 def build(out: Path, defines):
@@ -80,7 +82,8 @@ def summarize(recs, tag, n_launch_expected):
         launches.setdefault(kk, []).append(idx)
     L = sorted(launches.values(), key=lambda ix: int(recs["ts"][ix, 0].min()))
     rows = {name: [] for name in TR}
-    aux_rows = {"aux: state loads landed": 3, "aux: bar.arrive 1": 4, "aux: bar.arrive 3": 15, "aux: bar.sync 2": 13, "aux: last store": 14}
+    aux_rows = {"aux: state loads landed": 3, "aux: bar.arrive 1": 4, "aux: bar.arrive 3": 15,
+                "aux: griddepcontrol.wait, chained launch": 16, "aux: bar.sync 2": 13, "aux: last store": 14}
     aux = {k: [] for k in aux_rows}
     launch_last, gap_med_last, starts, ends, shared, own, late_cta, last_is_late = [], [], [], [], [], [], [], []
     prev_end = None
@@ -121,7 +124,7 @@ def summarize(recs, tag, n_launch_expected):
     period = [b - a for a, b in zip(starts, starts[1:])]
     gap = [s - e for e, s in zip(ends, starts[1:])]
     out = {"tag": tag, "launches": len(L), "launches expected": n_launch_expected, "records": int(len(recs))}
-    for name in TR[:-1]:
+    for name in TR[:-2]:                                       # (the last two are aux-warp stamps)
         if rows[name]:
             out[name] = _median(rows[name])
     out.update({k: _median(v) for k, v in aux.items()})
@@ -209,7 +212,7 @@ def run(args):
     per_launch = 2 * ((E + 7) // 8)
     dtype = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
                       ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
-    assert dtype.itemsize == 192
+    assert dtype.itemsize == 40 + 8 * len(TR) + 24
     cap = per_launch * R
     buf = torch.zeros(cap * dtype.itemsize, dtype=torch.uint8, device=dev)
     lib.wl_duo_trace_arm.argtypes = [C.c_void_p, C.c_uint32]

@@ -4,9 +4,15 @@
 #include <cstdlib>
 #include <cmath>
 #include <cstring>
+#include <functional>
+#include <map>
+#include <mutex>
 #include <new>
 #include <string>
+#include <thread>
+#include <tuple>
 #include <type_traits>
+#include <utility>
 
 #include <cuda.h>
 
@@ -29,6 +35,7 @@ struct wl_sim {
     const float* hf;        // device height-field or null
     size_t state_bytes;
     int64_t launches;
+    int64_t chained_steps;  // wl_step launches of the duo kernel that ran chained (wl_chained_step_count)
     int64_t last_t;         // counter of the most recent step launched through this handle (-1: none); host mirror
     int64_t base_host;      // host mirror of wl_globals.step_base
     uint8_t* term_bits;     // optional per-env termination-term bits output of wl_step (wl_set_term_bits)
@@ -530,7 +537,7 @@ __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64
 // record.  A stamp takes a value as `dep` and is predicated on it, so it is issued only once that value has arrived.
 #ifdef WL_DUO_TRACE
 // (the aux warp stamps TR_BAR1 at its bar.arrive 1 and TR_ARRIVE2 once it passes bar.sync 2)
-enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 = TR_PASS0 + 8, TR_LAST, TR_AUX_ARRIVE3, TR_N };
+enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 = TR_PASS0 + 8, TR_LAST, TR_AUX_ARRIVE3, TR_AUX_WAITED, TR_N };
 struct DuoTraceRec {
     unsigned long long st;          // the env set (state buffer) of the launch
     uint32_t t, cta, smid, warpid;  // step counter, blockIdx.x, %smid, %warpid
@@ -606,7 +613,7 @@ __global__ void __launch_bounds__(WL_DUO_THREADS, 4)
 wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
                    const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
                    uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
-                   uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf) {
+                   uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf, int chained) {
     using S = Spec<K>;
     __shared__ DuoShared sh;
     TR_DECL;
@@ -619,7 +626,13 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     // Launched with PDL, this prologue runs while the previous step's tail is still running: up to the wait it reads only
     // kernel parameters and requests into L2 the lines both warps load first (the janitor CTA owns no envs).
     if (warp == 0 && env0 < n) duo_prefetch_l2(st, action, n, env0, lane, S::wheel_mass(c));
-    pdl_wait();
+    // chained (FAN = 0 only): the previous PDL launch on the stream is a duo step of another env set, and its CTAs
+    // triggered only once ITS predecessor had completed, so all that may still run beside this grid is that step, which
+    // touches none of this launch's buffers (the host checks).  The env CTAs then start on entry.  The aux warp waits before
+    // the weights and the episode log (wl_globals: janitor t-1) and before its trigger, which keeps the same true for the
+    // next launch, and the CTA cannot complete before its predecessor.  The janitor CTA always waits here.  DESIGN.md 6e.
+    const bool early = FAN == 0 && chained != 0 && blockIdx.x != gridDim.x - 1;
+    if (!early) pdl_wait();
     TR(TR_WAITED, n);
     const uint32_t t = decode_step(gl, t_arg);
     if (janitor_cta(c, gl, t, d_log)) return;
@@ -641,7 +654,13 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             t_hf = fst[((size_t)WL_G_LINVEL * n + ii) * 4 + 3]; t_lf = fst[((size_t)WL_G_ANGVEL * n + ii) * 4 + 3];
         }
         float wts[WL_MAX_REW_TERMS];
-        if (!S::fixed) load_weights(c, gl, t, wts);
+        if (!S::fixed) {
+            if (early) {
+                pdl_wait();
+                TR(TR_AUX_WAITED, n);
+            }
+            load_weights(c, gl, t, wts);
+        }
         TR(TR_LOADS, __float_as_uint(a.x) ^ __float_as_uint(s1.w) ^ __float_as_uint(t_lf));
         // A. action map -> targets of the whole env step
         if (lane < 8) {
@@ -707,7 +726,14 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         }
         bar_arrive(3);
         // (a fixed spec loads the weights only now, off the way to bar.arrive 1: only the rewards below read them)
-        if (S::fixed) load_weights(c, gl, t, wts);
+        if (S::fixed) {
+            if (early) {
+                pdl_wait();
+                TR(TR_AUX_WAITED, n);
+                pdl_trigger();                                  // (chained: the CTA's trigger, as early as it may be)
+            }
+            load_weights(c, gl, t, wts);
+        }
         // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
         bar_sync(2);
         TR(TR_ARRIVE2, __float_as_uint(sh.fin[j][0]));
@@ -804,8 +830,9 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     TR(TR_ARRIVE2, raw_mask);
     // The next step's launch may begin once every CTA is here (the aux warp triggers after bar.sync 2; the spacer warp and
     // the janitor CTA have exited).  Triggering at entry instead let each grid launch the next while only partly resident,
-    // and triggering after the last store was slower on H100 (DESIGN.md 6e).
-    pdl_trigger();
+    // and triggering after the last store was slower on H100 (DESIGN.md 6e).  Chained, only the aux warp triggers: the
+    // next launch relies on every trigger following a wait.
+    if (!early) pdl_trigger();
     // I'. observation inputs from the post-physics state (an env that resets / gets pushed takes others below)
     float eu_k = euler_lane<S::fixed>(e.qw, e.qx, e.qy, e.qz, w);
     V3 wbo = rotT(R, e.w);
@@ -2068,8 +2095,58 @@ wl_camera_kernel(const __grid_constant__ wl_config c, const float4* __restrict__
 // written.  The single-GPU duo kernel is always launched with it (DESIGN.md 6e); the fan-out forms of the duo kernel share
 // its code but are launched without it; the thread, quad and act-step kernels use it only with WL_PDL=1.)
 static bool g_pdl = (getenv("WL_PDL") != nullptr) && (atoi(getenv("WL_PDL")) != 0);
+
+// The buffers a single-GPU duo step reads or writes, by stream: what the most recent launch of a kernel that triggers its
+// dependents (griddepcontrol.launch_dependents) was, when it was such a step (n_spans = 0: anything else).  A kernel that
+// triggers releases a PDL-launched successor early, whether it was itself launched with the attribute or not; all of them
+// (the step, quad, act-step and duo kernels) are launched through launch_k, which clears the entry, and the FAN = 0 duo
+// launch then records itself.  Any other kernel lets its successor start only once it has completed, and does so only
+// after its own predecessor has, so it leaves nothing running that this record would have to describe.  An entry holds
+// the id of the graph capture it was made in (0: none): launches captured into a graph never ran on the stream, and the
+// first node of a graph starts only once the work before the graph launch has completed.
+struct Span { uintptr_t lo, hi; };
+struct DuoFootprint { Span w[6]; int n_spans; Span act; };
+struct DuoPrev { unsigned long long capture; DuoFootprint fp; };
+// (stream handle, device, host thread for cudaStreamPerThread: each host thread's per-thread stream is a stream of its own)
+using StreamKey = std::tuple<uintptr_t, int, size_t>;
+struct DuoKey { StreamKey stream; unsigned long long capture; };
+static std::mutex g_duo_mu;
+static std::map<StreamKey, DuoPrev> g_duo_prev;       // one entry per stream ever used (a destroyed stream's entry stays)
+static DuoKey duo_key(cudaStream_t cs) {
+    int dev = 0;
+    cudaGetDevice(&dev);                       // (stream 0 names a different stream on each device)
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    unsigned long long id = 0;
+    if (cudaStreamGetCaptureInfo(cs, &st, &id) != cudaSuccess || st != cudaStreamCaptureStatusActive) id = 0;
+    const size_t thr = (cs == cudaStreamPerThread) ? std::hash<std::thread::id>{}(std::this_thread::get_id()) : 0;
+    return DuoKey{StreamKey{reinterpret_cast<uintptr_t>(cs), dev, thr}, id};
+}
+static bool spans_meet(Span a, Span b) { return a.lo < b.hi && b.lo < a.hi; }
+// true when the footprints are disjoint, reads of the actions by both excepted
+static bool footprints_apart(const DuoFootprint& a, const DuoFootprint& b) {
+    for (int i = 0; i < a.n_spans; ++i) {
+        if (spans_meet(a.w[i], b.act)) return false;
+        for (int k = 0; k < b.n_spans; ++k) if (spans_meet(a.w[i], b.w[k])) return false;
+    }
+    for (int k = 0; k < b.n_spans; ++k) if (spans_meet(b.w[k], a.act)) return false;
+    return true;
+}
+// whether a duo step with footprint `fp` may run chained (wl_step_duo_kernel): the previous triggering launch on the
+// stream, in the same capture or outside any, was a FAN = 0 duo step that touches none of the buffers this one touches,
+// the actions both read excepted
+static bool duo_chained(const DuoKey& key, const DuoFootprint& fp) {
+    std::lock_guard<std::mutex> lk(g_duo_mu);
+    auto it = g_duo_prev.find(key.stream);
+    return it != g_duo_prev.end() && it->second.capture == key.capture && it->second.fp.n_spans > 0 && footprints_apart(it->second.fp, fp);
+}
+static void set_duo_prev(const DuoKey& key, const DuoFootprint& fp) {
+    std::lock_guard<std::mutex> lk(g_duo_mu);
+    g_duo_prev[key.stream] = DuoPrev{key.capture, fp};
+}
+
 template <typename... KArgs, typename... Args>
 static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t cs, bool pdl, const Args&... args) {
+    set_duo_prev(duo_key(cs), DuoFootprint{});
     static_assert(sizeof...(KArgs) == sizeof...(Args), "argument count");
     cudaLaunchConfig_t lc;
     memset(&lc, 0, sizeof lc);
@@ -2331,6 +2408,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     s->hf = d_heightfield;
     s->state_bytes = state_bytes;
     s->launches = 0;
+    s->chained_steps = 0;
     s->last_t = -1;
     s->base_host = 0;
     s->term_bits = nullptr;
@@ -2393,6 +2471,7 @@ int wl_set_kernel_variant(wl_sim* sim, int32_t lanes_per_env) {
     return WL_OK;
 }
 int64_t wl_launch_count(const wl_sim* sim) { return sim ? sim->launches : 0; }
+int64_t wl_chained_step_count(const wl_sim* sim) { return sim ? sim->chained_steps : 0; }
 int wl_step_launch_info(const wl_sim* sim, int32_t* variant, uint32_t* spec_key, int32_t* specialised, int32_t* threads_per_cta) {
     if (!sim) return fail(WL_EINVAL, "wl_step_launch_info: null handle");
     if (variant) *variant = sim->step_variant;
@@ -2490,15 +2569,26 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
         const int grid = (n + WL_DUO_ENVS - 1) / WL_DUO_ENVS + 1;                            // + the janitor CTA
         const bool rows_ok = (n % WL_DUO_ENVS) == 0 && (((uintptr_t)d_obs | (uintptr_t)d_rew) & 15u) == 0 &&
                              (((uintptr_t)d_terminated | (uintptr_t)d_truncated) & 7u) == 0;
+        const int unchained = 0;
         if (sim->fan.mc && rows_ok)
-            launch_k(wl_step_duo_kernel<2, 0u>, grid, duo_block(sim, wl_step_duo_kernel<2, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+            launch_k(wl_step_duo_kernel<2, 0u>, grid, duo_block(sim, wl_step_duo_kernel<2, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan, unchained);
         else if (fan_set(sim))
-            launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
-        else
+            launch_k(wl_step_duo_kernel<1, 0u>, grid, duo_block(sim, wl_step_duo_kernel<1, 0u>, grid), 0, cs, false, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan, unchained);
+        else {
+            auto span = [](const void* p, size_t bytes) { const uintptr_t a = reinterpret_cast<uintptr_t>(p); return Span{a, a + bytes}; };
+            const size_t un = (size_t)n;
+            DuoFootprint fp{{span(sim->state, sim->state_bytes), span(d_obs, un * WL_OBS_DIM_BLIND * sizeof(float)), span(d_rew, un * sizeof(float)),
+                             span(d_terminated, un), span(d_truncated, un), span(sim->term_bits, sim->term_bits ? un : 0)},
+                            6, span(act, un * sizeof(float2))};
+            const DuoKey key = duo_key(cs);
+            const int chained = duo_chained(key, fp) ? 1 : 0;
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
                 specialised = k.value != 0u;
-                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan, chained);
             });
+            set_duo_prev(key, fp);
+            sim->chained_steps += chained;
+        }
         cta_threads = sim->duo_threads;
     } else if (variant == 4) {
 #ifndef WL_QUAD_BS
@@ -2543,7 +2633,7 @@ static int launch_stage(wl_sim* sim, const float2* act, float* d_obs, float* d_r
     const int n = sim->cfg.num_envs, bs = pick_block(n), grid = (n + bs - 1) / bs + (jan ? 1 : 0);
     Terrain T{sim->hf};
     with_task<WL_TASK_ELEVATION, WL_TASK_VISUAL>(sim->cfg.task, [&](auto task) {
-        wl_step_kernel<task, STAGE><<<grid, bs, 0, cs>>>(sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
+        launch_k(wl_step_kernel<task, STAGE>, grid, bs, 0, cs, false, sim->cfg, sim->state, sim->globals, T, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sio);
     });
     static const char* const names[] = {"wl_step_kernel", "wl_step_kernel<stage a>", "wl_step_kernel<stage b>", "wl_step_kernel<stage b1>",
                                         "wl_step_kernel<stage b2>"};

@@ -59,7 +59,8 @@ __device__ __forceinline__ uint4 dr_block(const wl_config& c, uint32_t gid, uint
 // are those whose episode_length_buf it left at 0 (every step kernel counts an env up by one, then a reset sets it to 0), and
 // t is that step's counter, decoded as the step decoded it; after wl_reset t is wl_reset's counter as wl_reset_kernel uses it.
 // Launched without the PDL attribute and without an early trigger: it starts once the step has finished, and a step launched
-// after it with PDL passes its griddepcontrol.wait only when these stores are complete.
+// after it with PDL starts only when it has completed (a chained duo step, which skips its griddepcontrol.wait, included:
+// DESIGN.md 6e).
 __global__ void __launch_bounds__(WL_RESET_DR_BS)
 wl_reset_dr_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, const wl_globals* __restrict__ gl,
                    const int64_t* __restrict__ ids, int n_ids, uint32_t t_arg, bool after_step, uint32_t mask) {

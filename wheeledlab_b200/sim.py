@@ -560,6 +560,11 @@ class WheeledSim:
     def launch_count(self) -> int:
         return int(lib.wl_launch_count(self._h))
 
+    @property
+    def chained_step_count(self) -> int:
+        """wl_step launches of the duo kernel that ran chained after another env set's step (DESIGN.md 6e)."""
+        return int(lib.wl_chained_step_count(self._h))
+
     # -- zero-copy state views (IsaacLab ArticulationData names) -------------------------------------
     @property
     def root_pos_w(self):
