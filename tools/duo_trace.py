@@ -11,8 +11,10 @@ aux warp also stamps when its deferred griddepcontrol.wait returns.  Times are n
 per-launch median warp, except where a row says otherwise.  "pass k cycles" rows are SM clock cycles (%clock) of the env
 warp's sub-step pass k (pass 0 from bar.sync 1), median over env warps, split by whether an aux warp on the same SM
 scheduler (%warpid % 4) was between its bar.arrive 1 and bar.arrive 3 (issuing the noise, push and reset draws) at any time
-during the pass.  The traced build is a diagnostic build: its stamps and
-records cost time of their own, so compare traces with traces, and bench.py figures with bench.py figures."""
+during the pass.  The residency rows (residency()) give when each CTA entered after its launch's first entry, how long
+late and on-time CTAs ran, and how the CTAs of consecutive launches shared the SMs.  The traced build is a diagnostic
+build: its stamps and records cost time of their own, so compare traces with traces, and bench.py figures with bench.py
+figures."""
 import argparse
 import json
 import math
@@ -28,6 +30,14 @@ ROOT = Path(__file__).resolve().parent.parent
 TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
      [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3",
                                                         "aux: griddepcontrol.wait, chained launch"]
+
+
+def record_dtype():
+    import numpy as np
+    dt = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
+                   ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
+    assert dt.itemsize == 40 + 8 * len(TR) + 24
+    return dt
 
 
 def build(out: Path, defines):
@@ -140,7 +150,67 @@ def summarize(recs, tag, n_launch_expected):
     })
     out.update(pass_cycles(recs))
     out.update(tails(recs, L))
+    out.update(residency(recs, L))
     return out
+
+
+def residency(recs, launches, late_ns=1000):
+    """When each CTA of a launch entered and how the CTAs of consecutive launches shared the SMs.  A CTA's entry is its
+    first warp's entry, its end its last store; "late" CTAs entered more than `late_ns` after the launch's first entry
+    (a CTA that waits for a slot enters late).  Per SM: how many CTAs of launch k and of launch k+1 ran there, and
+    the most CTAs of the two launches resident there at one time."""
+    import numpy as np
+    frac, spread50, spread90, spread_max, life_late, life_rest, late_end, n_late, n_all = [], [], [], [], [], [], 0, 0, 0
+    per_launch = []
+    for ix in launches:
+        ix = np.asarray(ix)
+        ts = recs["ts"][ix].astype(np.int64)
+        cta, sm = recs["cta"][ix], recs["smid"][ix]
+        t0 = int(ts[:, 0].min())
+        ctas = {}
+        for c, s, e, l in zip(cta.tolist(), sm.tolist(), ts[:, 0].tolist(), ts[:, 14].tolist()):
+            r = ctas.setdefault(c, [s, e, l])
+            r[1], r[2] = min(r[1], e), max(r[2], l)
+        a = np.array(list(ctas.values()), dtype=np.int64)          # smid, entry, end
+        ent = a[:, 1] - t0
+        late = ent > late_ns
+        frac.append(float(late.mean()))
+        n_late += int(late.sum()); n_all += len(late)
+        spread50.append(float(np.median(ent))); spread90.append(float(np.percentile(ent, 90))); spread_max.append(float(ent.max()))
+        life = a[:, 2] - a[:, 1]
+        if late.any():
+            life_late.append(float(np.median(life[late])))
+        if (~late).any():
+            life_rest.append(float(np.median(life[~late])))
+        late_end += int(late[int(np.argmax(a[:, 2]))])
+        per_launch.append(a)
+    pair_counts, peak = {}, {}
+    for a, b in zip(per_launch, per_launch[1:]):
+        for s in np.union1d(a[:, 0], b[:, 0]).tolist():
+            x, y = a[a[:, 0] == s], b[b[:, 0] == s]
+            key = f"{len(x)}+{len(y)}"
+            pair_counts[key] = pair_counts.get(key, 0) + 1
+            ev = sorted([(e, 1) for e in np.concatenate([x[:, 1], y[:, 1]]).tolist()] +
+                        [(l, -1) for l in np.concatenate([x[:, 2], y[:, 2]]).tolist()])
+            cur = hi = 0
+            for _, d in ev:
+                cur += d; hi = max(hi, cur)
+            peak[hi] = peak.get(hi, 0) + 1
+    npairs = max(1, len(per_launch) - 1)
+    return {
+        f"env CTAs entering > {late_ns} ns after the launch's first entry (fraction, median)": _median(frac),
+        f"env CTAs entering > {late_ns} ns after the launch's first entry (fraction of all launches' CTAs / most in one launch)":
+            [n_late / max(1, n_all), max(frac, default=None)],
+        "CTA entry after the launch's first entry: median / p90 / max (ns, median over launches)":
+            [_median(spread50), _median(spread90), _median(spread_max)],
+        "CTA last store - CTA entry, late CTAs (ns, median)": _median(life_late),
+        "CTA last store - CTA entry, other CTAs (ns, median)": _median(life_rest),
+        "launches whose last store is a late CTA's": late_end,
+        "SMs by CTAs of launch k + launch k+1 (mean SMs per launch pair)":
+            {k: round(v / npairs, 1) for k, v in sorted(pair_counts.items(), key=lambda kv: -kv[1])[:12]},
+        "SMs by most CTAs of launches k and k+1 resident at once (mean SMs per launch pair)":
+            {str(k): round(v / npairs, 1) for k, v in sorted(peak.items())},
+    }
 
 
 def tails(recs, launches):
@@ -210,9 +280,7 @@ def run(args):
     torch.cuda.current_stream().wait_stream(cs)
     g.replay(); torch.cuda.synchronize()
     per_launch = 2 * ((E + 7) // 8)
-    dtype = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
-                      ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
-    assert dtype.itemsize == 40 + 8 * len(TR) + 24
+    dtype = record_dtype()
     cap = per_launch * R
     buf = torch.zeros(cap * dtype.itemsize, dtype=torch.uint8, device=dev)
     lib.wl_duo_trace_arm.argtypes = [C.c_void_p, C.c_uint32]

@@ -703,6 +703,14 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             sh.push[j][0] = hf; sh.push[j][1] = dvx; sh.push[j][2] = dvy; sh.push[j][3] = dwh; sh.push[j][4] = t_hf;
             sh.push[j][5] = lf; sh.push[j][6] = dwl; sh.push[j][7] = t_lf;
         }
+        // chained, fixed spec: the wait on the previous grid and the CTA's trigger come before the reset draw, the aux warp's
+        // longest draw, rather than after it (Drift measured 7 % faster on H100, DESIGN.md 6e).  Nothing the draw reads is
+        // written by another launch; the weights are still loaded after the wait.
+        if (S::fixed && early) {
+            pdl_wait();
+            TR(TR_AUX_WAITED, n);
+            pdl_trigger();
+        }
         // Z. the auto-reset outcome of every env, whether it resets or not: lane = (env, wheel) as in the env warp, which
         // only selects it after bar.sync 3.  A reset env is not pushed: its fresh timers exceed step_dt and only count down.
         // (Drawn before the action map, in the shadow of the loads, it delayed bar.arrive 1 and the step took longer.)
@@ -726,14 +734,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         }
         bar_arrive(3);
         // (a fixed spec loads the weights only now, off the way to bar.arrive 1: only the rewards below read them)
-        if (S::fixed) {
-            if (early) {
-                pdl_wait();
-                TR(TR_AUX_WAITED, n);
-                pdl_trigger();                                  // (chained: the CTA's trigger, as early as it may be)
-            }
-            load_weights(c, gl, t, wts);
-        }
+        if (S::fixed) load_weights(c, gl, t, wts);
         // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
         bar_sync(2);
         TR(TR_ARRIVE2, __float_as_uint(sh.fin[j][0]));
