@@ -974,6 +974,34 @@ size_t wl_ppo_wide_workspace_bytes(int32_t obs_dim, int32_t batch, int32_t num_m
 int wl_ppo_update_wide(const wl_ppo_params* params, const wl_ppo_batch* batch, float* d_blob, float* d_adam_m, float* d_adam_v,
                        float* d_state, void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* ---- behaviour cloning: rsl_rl's Distillation.update() on the student actor (DESIGN.md 6t) -------------------------------
+ * The student is the actor of a blob laid out by wl_policy_blob_floats(obs_dim) (its critic blocks unused), trained to the
+ * teacher's actions: d_obs [T, N, obs_dim] and d_teacher_actions [T, N, 2] (slab order, row = t*N + n).  The loss of step
+ * t is mse(actor(obs_t), teacher_actions_t), the mean over N x 2 elements.  The epochs walk the T steps in order, counting
+ * across epochs; after every gradient_length-th step the summed loss of those steps is back-propagated through the actor,
+ * clip_grad_norm_(max_grad_norm) is applied when max_grad_norm > 0, and Adam (0.9, 0.999, 1e-8, the fixed learning rate
+ * d_state[0]) steps the actor's parameters.  Steps after the last full chunk are evaluated but not stepped.  The critic
+ * blocks, the std and every padding float of the blob and the moments are never written.  activation WL_ACTIVATION_ELU:
+ * obs_dim 1..16; WL_ACTIVATION_RELU: obs_dim 1..4096.  One call enqueues the whole update, never syncs the host and is
+ * graph-capturable; no float atomics, so results are bit-identical run to run for a given (N, gradient_length, SM count).
+ * d_state[wl_distill_state_floats(T, num_learning_epochs)] (fp32; the caller sets [0] = learning rate, [1] = 0):
+ *   [0] learning rate  [1] Adam step count  [2] the mean of this update's per-step losses (rsl_rl's Loss/behavior)
+ *   [3] the number of Adam steps this update took  [4 + i] the loss of the i-th step walked (i < T * epochs)
+ * Bad arguments (T < gradient_length, ELU with obs_dim > 16, a null or misaligned pointer, a short workspace) return
+ * WL_EINVAL / WL_EUNSUPPORTED before any launch. */
+typedef struct wl_distill_params {
+    int32_t obs_dim;                /* the student's input width */
+    int32_t num_learning_epochs;
+    int32_t gradient_length;        /* stored steps per Adam step */
+    float max_grad_norm;            /* > 0: clip the actor's gradient norm; <= 0: no clip (rsl_rl's None) */
+} wl_distill_params;
+int32_t wl_distill_state_floats(int32_t T, int32_t num_learning_epochs);
+/* workspace for wl_distill_update on the current device (0 and wl_last_error() on error) */
+size_t wl_distill_workspace_bytes(int32_t obs_dim, int32_t n_envs, int32_t gradient_length);
+int wl_distill_update(const wl_distill_params* params, const float* d_obs, const float* d_teacher_actions, int32_t T, int32_t N,
+                      int32_t activation, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* ---- the wide asymmetric actor-critic: a critic input of its own (DESIGN.md 6s) ------------------------------------------
  * The network above with the critic's first layer fed from a second row, d_critic_obs_in [N, critic_obs_dim], and a blob
  * laid out by wl_policy_blob_floats_asym(obs_dim, critic_obs_dim); obs_dim and critic_obs_dim in 1..4096.

@@ -12,7 +12,9 @@ the activation follows the task.  ``-sd`` saves ``{'observations', 'actions'}`` 
 the reference's file.  Prints the mean return and length of the episodes that finished during the playback.  A run trained on
 a policy observation table (``policy_terms`` in ``run.json``, DESIGN 6q) plays on an env with the same table, through
 ``wl_actor_mean`` on the table's row.  A run of an Elevation or Visual env with row terms (``row_terms`` in ``run.json``,
-DESIGN 6r) plays with the same terms: their clips and scales change the policy's input even without noise.
+DESIGN 6r) plays with the same terms: their clips and scales change the policy's input even without noise.  A distillation
+run (``teacher_terms`` in ``run.json``, DESIGN 6t) plays its student: the env gets the teacher group its runner needs, and
+the student's mean is played on the student's row.
 """
 from __future__ import annotations
 
@@ -65,7 +67,8 @@ def resolve(args) -> dict:
     num_envs = args.num_envs if args.num_envs is not None else (run_cfg or {}).get("num_envs")
     seed = args.seed if args.seed is not None else (run_cfg or {}).get("seed")
     return {"task": task, "policy_path": policy_path, "playback_dir": playback_dir, "agent_cfg": agent, "num_envs": num_envs, "seed": seed,
-            "policy_terms": (run_cfg or {}).get("policy_terms"), "row_terms": (run_cfg or {}).get("row_terms")}
+            "policy_terms": (run_cfg or {}).get("policy_terms"), "row_terms": (run_cfg or {}).get("row_terms"),
+            "teacher_terms": (run_cfg or {}).get("teacher_terms")}
 
 
 def play(r: dict, steps: int, device: str = "cuda:0"):
@@ -83,6 +86,9 @@ def play(r: dict, steps: int, device: str = "cuda:0"):
         env.set_row_terms([(name, fn, {"noise": tuple(nz) if nz else None, "clip": tuple(cl) if cl else None,
                                        "scale": tuple(sc) if isinstance(sc, list) else sc})
                            for name, fn, nz, cl, sc in r["row_terms"]])
+    if r.get("teacher_terms"):
+        env.set_teacher_observation([(name, fn, {k: tuple(v) if isinstance(v, list) else v for k, v in params.items()})
+                                     for name, fn, params in r["teacher_terms"]])
     runner = FusedOnPolicyRunner(env, r["agent_cfg"], device=device)
     runner.load(r["policy_path"], load_optimizer=False)
     env.reset()

@@ -128,18 +128,18 @@ def _lower_rows(cfg, spec: T.TaskSpec, c, expected, task: str, device_terms: boo
     spec.row_terms = table
 
 
-def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
+def _lower_critic(cfg, spec: T.TaskSpec, kind: str, group_name: str = "critic"):
     """``cfg.observations.critic`` (an ObservationGroupCfg next to ``policy``) -> ``spec.critic_terms``, the term table of
     ``wl_critic_observe``.  Anything the kernels do not do raises NotImplementedError naming the term; no group, no table."""
-    group = getattr(cfg.observations, "critic", None)
+    group = getattr(cfg.observations, group_name, None)
     if group is None:
         return
     from . import privileged
     if kind != "drift":
-        raise NotImplementedError(f"a critic observation group on the {kind.capitalize()} task is not implemented "
+        raise NotImplementedError(f"a {group_name} observation group on the {kind.capitalize()} task is not implemented "
                                   "(the asymmetric actor-critic covers the Drift family)")
     if getattr(group, "concatenate_terms", True) is not True:
-        raise NotImplementedError("critic observation group: concatenate_terms=False is not implemented")
+        raise NotImplementedError(f"{group_name} observation group: concatenate_terms=False is not implemented")
     table = []
     for name, t in _fields(group):
         if not hasattr(t, "func"):
@@ -148,34 +148,34 @@ def _lower_critic(cfg, spec: T.TaskSpec, kind: str):
         fn, clip = privileged.lower_term(name, t.func, getattr(t, "params", None), getattr(t, "clip", None), noise, getattr(t, "scale", None))
         table.append((name, fn, clip))
     if not table:
-        raise NotImplementedError("critic observation group: no terms")
-    privileged.check_width([(fn, c) for _, fn, c in table], "critic observation group " + ", ".join(n for n, _, _ in table))
-    spec.critic_terms = table
+        raise NotImplementedError(f"{group_name} observation group: no terms")
+    privileged.check_width([(fn, c) for _, fn, c in table], f"{group_name} observation group " + ", ".join(n for n, _, _ in table))
+    setattr(spec, "critic_terms" if group_name == "critic" else "teacher_terms", table)
 
 
-def _lower_row_critic(cfg, spec: T.TaskSpec):
+def _lower_row_critic(cfg, spec: T.TaskSpec, group_name: str = "critic"):
     """An Elevation ``cfg.observations.critic`` (``device_terms=True`` only) -> ``spec.row_critic``: the policy row's six
     terms in row order, noise-free with their own clips and scales, then terms of the critic library (DESIGN 6s).  Anything
     else raises NotImplementedError naming the term: noise, history or modifiers, a per-element map scale, a map without a
     clip, row terms out of order, a term after them outside the library; a group that does not open with the row terms
     keeps the library path's refusal on Elevation."""
-    group = getattr(cfg.observations, "critic", None)
+    group = getattr(cfg.observations, group_name, None)
     if group is None:
         return
     from . import privileged, row_terms
     if getattr(group, "concatenate_terms", True) is not True:
-        raise NotImplementedError("critic observation group: concatenate_terms=False is not implemented")
+        raise NotImplementedError(f"{group_name} observation group: concatenate_terms=False is not implemented")
     terms = [(name, t) for name, t in _fields(group) if hasattr(t, "func")]
     head = row_terms.task_terms("elevation")
     fns = [_fname(t) for _, t in terms]
     if not fns or fns[0] not in head:
-        _lower_critic(cfg, None, "elevation")               # a library-only group: refused as before
+        _lower_critic(cfg, None, "elevation", group_name)   # a library-only group: refused as before
     for k, ((name, t), fn) in enumerate(zip(terms, fns)):
         if k < len(head) and fn != head[k]:
-            raise NotImplementedError(f"critic term {name}: {fn} at position {k}; a row critic opens with the Elevation row's "
+            raise NotImplementedError(f"{group_name} term {name}: {fn} at position {k}; a row critic opens with the Elevation row's "
                                       f"terms {list(head)} in row order")
     if len(terms) < len(head):
-        raise NotImplementedError(f"critic observation group {[n for n, _ in terms]}: a row critic opens with all six row terms {list(head)}")
+        raise NotImplementedError(f"{group_name} observation group {[n for n, _ in terms]}: a row critic opens with all six row terms {list(head)}")
     out, lib = [], []
     for k, (name, t) in enumerate(terms):
         nz = getattr(t, "noise", None)
@@ -186,12 +186,12 @@ def _lower_row_critic(cfg, spec: T.TaskSpec):
             out.append((name, fns[k], params))
         else:
             if getattr(t, "modifiers", None) or getattr(t, "history_length", 0):
-                raise NotImplementedError(f"critic term {name}: history_length / modifiers are not implemented")
+                raise NotImplementedError(f"{group_name} term {name}: history_length / modifiers are not implemented")
             fn, clip = privileged.lower_term(name, t.func, getattr(t, "params", None), getattr(t, "clip", None), nz, getattr(t, "scale", None))
             lib.append((fn, clip))
             out.append((name, fn, {"clip": (-clip, clip)} if clip else {}))
-    privileged.check_width(lib, "critic observation group " + ", ".join(n for n, _ in terms[len(head):]))
-    spec.row_critic = out
+    privileged.check_width(lib, f"{group_name} observation group " + ", ".join(n for n, _ in terms[len(head):]))
+    setattr(spec, "row_critic" if group_name == "critic" else "row_teacher", out)
 
 
 def _lower_policy(cfg, spec: T.TaskSpec, c, device_terms: bool):
@@ -427,6 +427,11 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     kind = _task_kind(cfg)
     if getattr(cfg.observations, "critic", None) is not None and kind != "drift" and not (kind == "elevation" and device_terms):
         _lower_critic(cfg, None, kind)                      # (refused by name before anything is lowered)
+    if device_terms and getattr(cfg.observations, "teacher", None) is not None:
+        if getattr(cfg.observations, "critic", None) is not None:
+            raise NotImplementedError("an env has a critic observation group or a teacher observation group, not both")
+        if kind == "visual":
+            _lower_critic(cfg, None, kind, "teacher")       # (refused by name, as a Visual critic group)
     if kind == "visual":
         return _lower_visual(cfg, num_envs, seed, env_id_offset, allow_python_terms, device_terms)
     if kind == "drift":
@@ -440,6 +445,8 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
         _lower_common(cfg, spec)
         _lower_policy(cfg, spec, c, device_terms)
         _lower_critic(cfg, spec, kind)
+        if device_terms:
+            _lower_critic(cfg, spec, kind, "teacher")
 
         def h_slip(p):
             c.slip_min_thresh, c.slip_max_thresh = p["min_thresh"], p["max_thresh"]
@@ -503,6 +510,7 @@ def spec_from_reference_cfg(cfg, env_id_offset: int = 0, allow_python_terms: boo
     _lower_rows(cfg, spec, c, _OBS_ELEV, "Elevation", device_terms)
     if device_terms:
         _lower_row_critic(cfg, spec)
+        _lower_row_critic(cfg, spec, "teacher")
     for _, t in _fields(cfg.observations.policy):
         if hasattr(t, "func") and _fname(t) == "world_height_map":
             c.scan_offset, c.scan_plane_init = float(t.params["offset"]), float(t.params["plane_init_value"])

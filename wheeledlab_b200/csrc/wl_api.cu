@@ -1885,6 +1885,7 @@ __global__ void wl_dp_adam_kernel(float* __restrict__ param, float* __restrict__
 #include "wl_episode.cuh"
 #include "wl_terms.cuh"
 #include "wl_dev_events.cuh"
+#include "wl_distill.cuh"
 
 // the handle's device terms: the kernel's table and one device allocation holding the per-env state
 struct DevTerms {
@@ -3763,6 +3764,132 @@ int wl_ppo_update_wide_asym(const wl_ppo_params* p, const wl_ppo_batch* b, const
     const char* fn = "wl_ppo_update_wide_asym";
     if (!d_critic_obs || ((uintptr_t)d_critic_obs & 3u)) return fail(WL_EINVAL, std::string(fn) + ": d_critic_obs is null or not 4-byte aligned");
     return ppo_update(fn, true, p, b, d_blob, d_adam_m, d_adam_v, d_state, d_workspace, workspace_bytes, stream, d_critic_obs, critic_obs_dim);
+}
+
+// ---- behaviour cloning: rsl_rl's Distillation.update() on the student actor (DESIGN 6t) ------------------------------
+// workspace: [reduced row][fp64 block sums of squares][one gradient row per CTA][per-row squared errors of a chunk]
+// [H1 of a chunk][dZ1 of a chunk] (the last two are the ReLU network's), each 256-byte aligned.  A row covers the actor,
+// blob [0, o6).
+struct DistillWorkspace { int rowlen, ctas, tiles, norm_parts; size_t norm_off, rows_off, sq_off, h1_off, dz_off, bytes; };
+static size_t distill_grad_smem(bool relu) {
+    int32_t off[13];
+    policy_offsets(16, off);
+    const int nact = relu ? off[6] - off[1] : off[6];
+    return sizeof(float) * ((size_t)nact + WL_HID * WL_HID + WL_HID + (relu ? 0 : WL_DS_TILE * WL_DS_XS) + 4 * WL_DS_TILE * WL_DS_HS +
+                            WL_DS_TILE * WL_DS_SD);
+}
+static size_t distill_dw1_smem() { return sizeof(float) * 2 * WL_DS_TILE * (WL_DW1_K + WL_HID); }
+static size_t distill_fwd_smem() { return sizeof(float) * 2 * WL_DS_FWD_STAGE; }
+static int distill_workspace(const char* fn, int32_t obs_dim, int32_t n_envs, int32_t gradient_length, DistillWorkspace& w) {
+    if (obs_dim < 1 || obs_dim > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim must be in 1..4096");
+    if (n_envs < 1 || gradient_length < 1) return fail(WL_EINVAL, std::string(fn) + ": n_envs and gradient_length must be >= 1");
+    const int64_t B = (int64_t)n_envs * gradient_length;
+    if (B > (int64_t)1 << 30) return fail(WL_EINVAL, std::string(fn) + ": n_envs * gradient_length must be <= 2^30");
+    int dev = 0, sms = 0;
+    if (int rc = cuda_check(cudaGetDevice(&dev), fn)) return rc;
+    if (int rc = cuda_check(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), fn)) return rc;
+    if (int rc = raise_smem<wl_distill_grad_kernel<false>>(dev, distill_grad_smem(false), fn)) return rc;
+    if (int rc = raise_smem<wl_distill_grad_kernel<true>>(dev, distill_grad_smem(true), fn)) return rc;
+    if (int rc = raise_smem<wl_distill_fwd_kernel>(dev, distill_fwd_smem(), fn)) return rc;
+    if (int rc = raise_smem<wl_distill_dw1_kernel>(dev, distill_dw1_smem(), fn)) return rc;
+    int32_t off[13];
+    policy_offsets(obs_dim, off);
+    w.rowlen = off[6];
+    w.tiles = (int)((B + WL_DS_TILE - 1) / WL_DS_TILE);
+    w.ctas = w.tiles < sms ? w.tiles : sms;
+    w.norm_parts = (w.rowlen + 255) / 256;
+    w.norm_off = align256(sizeof(float) * w.rowlen);
+    w.rows_off = align256(w.norm_off + sizeof(double) * w.norm_parts);
+    w.sq_off = align256(w.rows_off + sizeof(float) * (size_t)w.rowlen * w.ctas);
+    w.h1_off = align256(w.sq_off + sizeof(float) * (size_t)B);
+    const size_t hb = sizeof(float) * WL_HID * (size_t)w.tiles * WL_DS_TILE;
+    w.dz_off = align256(w.h1_off + hb);
+    w.bytes = w.dz_off + hb;
+    return WL_OK;
+}
+
+int32_t wl_distill_state_floats(int32_t T, int32_t num_learning_epochs) {
+    if (T < 1 || num_learning_epochs < 1 || (int64_t)T * num_learning_epochs > (1 << 24)) {
+        fail(WL_EINVAL, "wl_distill_state_floats: T and num_learning_epochs must be >= 1 (T * epochs <= 2^24)");
+        return 0;
+    }
+    return WL_DS_STATE_HEAD + T * num_learning_epochs;
+}
+
+size_t wl_distill_workspace_bytes(int32_t obs_dim, int32_t n_envs, int32_t gradient_length) {
+    DistillWorkspace w;
+    return distill_workspace("wl_distill_workspace_bytes", obs_dim, n_envs, gradient_length, w) ? 0 : w.bytes;
+}
+
+int wl_distill_update(const wl_distill_params* p, const float* d_obs, const float* d_teacher_actions, int32_t T, int32_t N,
+                      int32_t activation, float* d_blob, float* d_adam_m, float* d_adam_v, float* d_state, void* d_workspace,
+                      size_t workspace_bytes, void* stream) {
+    const char* fn = "wl_distill_update";
+    if (!p) return fail(WL_EINVAL, std::string(fn) + ": null params");
+    if (!d_obs || !d_teacher_actions || !d_blob || !d_adam_m || !d_adam_v || !d_state || !d_workspace)
+        return fail(WL_EINVAL, std::string(fn) + ": null d_obs / d_teacher_actions / d_blob / d_adam_m / d_adam_v / d_state / d_workspace");
+    if (activation != WL_ACTIVATION_ELU && activation != WL_ACTIVATION_RELU)
+        return fail(WL_EINVAL, std::string(fn) + ": activation must be WL_ACTIVATION_ELU or WL_ACTIVATION_RELU");
+    const int D = p->obs_dim;
+    if (D < 1 || D > WL_WIDE_MAX_OBS) return fail(WL_EUNSUPPORTED, std::string(fn) + ": obs_dim must be in 1..4096");
+    if (activation == WL_ACTIVATION_ELU && D > 16)
+        return fail(WL_EUNSUPPORTED, std::string(fn) + ": the ELU network (wl_act_step's) takes obs_dim <= 16");
+    if (p->num_learning_epochs < 1) return fail(WL_EINVAL, std::string(fn) + ": num_learning_epochs must be >= 1");
+    if (p->gradient_length < 1) return fail(WL_EINVAL, std::string(fn) + ": gradient_length must be >= 1");
+    if (T < 1 || N < 1) return fail(WL_EINVAL, std::string(fn) + ": T and N must be >= 1");
+    if (T < p->gradient_length) return fail(WL_EINVAL, std::string(fn) + ": T must be >= gradient_length (no step would cover a chunk)");
+    if (wl_distill_state_floats(T, p->num_learning_epochs) == 0) return fail(WL_EINVAL, std::string(fn) + ": T * num_learning_epochs > 2^24");
+    if (((uintptr_t)d_blob & 15u) || ((uintptr_t)d_adam_m & 15u) || ((uintptr_t)d_adam_v & 15u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_blob / d_adam_m / d_adam_v must be 16-byte aligned");
+    if (((uintptr_t)d_workspace & 255u) || ((uintptr_t)d_teacher_actions & 7u) || ((uintptr_t)d_obs & 3u) || ((uintptr_t)d_state & 3u))
+        return fail(WL_EINVAL, std::string(fn) + ": d_workspace must be 256-byte aligned, d_teacher_actions 8-byte, d_obs / d_state 4-byte");
+    DistillWorkspace w;
+    if (int rc = distill_workspace(fn, D, N, p->gradient_length, w)) return rc;
+    if (workspace_bytes < w.bytes)
+        return fail(WL_EINVAL, std::string(fn) + ": workspace_bytes too small (wl_distill_workspace_bytes gives " + std::to_string(w.bytes) + ")");
+    const bool relu = activation == WL_ACTIVATION_RELU;
+    PolicyOffsets po;
+    policy_offsets(D, po.o);
+    cudaStream_t cs = (cudaStream_t)stream;
+    char* ws = (char*)d_workspace;
+    float* red = (float*)ws;
+    double* norm_part = (double*)(ws + w.norm_off);
+    float* rows = (float*)(ws + w.rows_off);
+    float* H1 = (float*)(ws + w.h1_off);
+    float* dZ1 = (float*)(ws + w.dz_off);
+    DistillArgs a;
+    a.obs = d_obs; a.target = d_teacher_actions; a.sqerr = (float*)(ws + w.sq_off);
+    a.D = D; a.N = N; a.T = T; a.inv_N = (float)(1.0 / N);
+    // rsl_rl counts the stored steps across epochs: Adam steps after every gradient_length-th step of the E * T, and the
+    // steps after the last one are evaluated (their losses are logged) but not stepped
+    const int total = T * p->num_learning_epochs, G = p->gradient_length;
+    int n_steps = 0;
+    for (int k0 = 0; k0 < total; k0 += G) {
+        const int g = total - k0 < G ? total - k0 : G;
+        const bool step = g == G;
+        a.step0 = k0 % T; a.B = g * N; a.tiles = (a.B + WL_DS_TILE - 1) / WL_DS_TILE;
+        const int ctas = a.tiles < w.ctas ? a.tiles : w.ctas;
+        if (relu) {
+            wl_distill_fwd_kernel<<<2 * a.tiles, WL_DS_FWD_THREADS, distill_fwd_smem(), cs>>>(d_blob, po, a, H1);
+            wl_distill_grad_kernel<true><<<ctas, WL_DS_THREADS, distill_grad_smem(true), cs>>>(d_blob, po, a, H1, dZ1, rows, w.rowlen);
+            if (step) {
+                const dim3 grid((unsigned)((D + WL_DW1_K - 1) / WL_DW1_K), (unsigned)ctas);
+                wl_distill_dw1_kernel<<<grid, WL_DS_THREADS, distill_dw1_smem(), cs>>>(po, a, dZ1, rows, w.rowlen);
+            }
+        } else {
+            wl_distill_grad_kernel<false><<<ctas, WL_DS_THREADS, distill_grad_smem(false), cs>>>(d_blob, po, a, nullptr, nullptr, rows, w.rowlen);
+        }
+        wl_distill_loss_kernel<<<g, 256, 0, cs>>>(a.sqerr, N, k0, d_state);
+        if (step) {
+            wl_distill_reduce_kernel<<<w.norm_parts, 256, 0, cs>>>(rows, ctas, w.rowlen, po, D, red, norm_part);
+            wl_distill_step_kernel<<<1, WL_DS_FIN_THREADS, 0, cs>>>(d_blob, d_adam_m, d_adam_v, d_state, red, norm_part, w.norm_parts, po, D,
+                                                                   p->max_grad_norm);
+            ++n_steps;
+        }
+        if (int rc = cuda_check(cudaGetLastError(), "wl_distill_update kernels")) return rc;
+    }
+    wl_distill_finish_kernel<<<1, 1, 0, cs>>>(d_state, total, n_steps);
+    return cuda_check(cudaGetLastError(), "wl_distill_finish_kernel");
 }
 
 // ---- the data-parallel update (DESIGN 6j) ---------------------------------------------------------------------------

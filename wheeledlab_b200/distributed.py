@@ -29,12 +29,17 @@ class RolloutSlab:
 
     ``critic_obs_dim`` (the asymmetric actor-critic, one GPU) adds ``critic_obs_in`` [T+1, N, Dc], the critic rows: row k is
     what ``values[k]`` was computed from, row T the bootstrap row.  It is a tensor of its own, NOT part of ``flat``: the
-    asymmetric network is refused in a data-parallel world, so no gather has to carry it; ``critic_obs_in`` is None otherwise."""
+    asymmetric network is refused in a data-parallel world, so no gather has to carry it; ``critic_obs_in`` is None otherwise.
+
+    ``teacher_actions=True`` (distillation, one GPU) adds ``teacher_actions`` [T, N, A], the teacher's action for the
+    observation of step k (rsl_rl RolloutStorage.privileged_actions), likewise a tensor of its own; None otherwise."""
 
     def __init__(self, T: int, n_local: int, obs_dim: int, act_dim: int, device, policy_fields: bool = False, flat: torch.Tensor | None = None,
-                 critic_obs_dim: int | None = None):
+                 critic_obs_dim: int | None = None, teacher_actions: bool = False):
         self.T, self.n, self.obs_dim, self.act_dim = T, n_local, obs_dim, act_dim
         self.device = torch.device(device)
+        self.teacher_actions = (torch.zeros((T, n_local, act_dim), dtype=torch.float32, device=self.device)
+                                if teacher_actions else None)
         self.critic_obs_in = (torch.zeros((T + 1, n_local, critic_obs_dim), dtype=torch.float32, device=self.device)
                               if critic_obs_dim else None)
         # name -> (dtype, trailing shape)

@@ -316,6 +316,7 @@ class ManagerBasedRLEnv:
         self._dev_events = []                    # device event terms (add_device_event_term): applied by wl_step_terms
         self._term_log_ring = None
         self._critic_terms = []                  # the critic observation group (set_critic_observation)
+        self._teacher_terms = []                 # the teacher observation group (set_teacher_observation)
         self._policy_terms = []                  # a modified policy observation group (set_policy_observation)
         self._policy_ring = None
         self._row_terms = []                     # noise, clip and scale on the Elevation / Visual row (set_row_terms)
@@ -343,6 +344,10 @@ class ManagerBasedRLEnv:
             self.set_critic_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.critic_terms])
         if self.spec.row_critic:
             self.set_critic_observation(self.spec.row_critic)
+        if self.spec.teacher_terms:
+            self.set_teacher_observation([(name, fn, {"clip": (-clip, clip)} if clip else {}) for name, fn, clip in self.spec.teacher_terms])
+        if self.spec.row_teacher:
+            self.set_teacher_observation(self.spec.row_teacher)
         if self.spec.policy_terms:
             self.set_policy_observation([(name, fn, {"noise": nz, "clip": cl, "scale": sc}) for name, fn, nz, cl, sc in self.spec.policy_terms])
         if self.spec.row_terms:
@@ -424,12 +429,34 @@ class ManagerBasedRLEnv:
         ``root_euler_xyz``, ``base_lin_vel``, ``base_ang_vel``, ``last_action``, ``world_height_map``) is a row critic
         (``sim.set_row_critic``, DESIGN 6s): those six with their own ``clip`` and ``scale`` -- no noise, and the map with a
         clip -- then terms of the critic library, 689..721 floats.  Any other list goes to the library path above."""
+        self._set_privileged_group("critic", terms)
+
+    def set_teacher_observation(self, terms):
+        """Give the env a ``teacher`` observation group next to ``policy``: the row a distillation teacher reads (rsl_rl's
+        StudentTeacher, DESIGN 6t), lowered exactly as ``set_critic_observation`` lowers a critic group -- a table of the
+        critic library on the Drift family, a row critic on Elevation -- and put at ``extras["observations"]["teacher"]``
+        by ``step``, ``reset`` and ``get_observations``.  An env has a critic group or a teacher group, not both; the
+        Visual task has neither."""
+        from .tasks import TASK_VISUAL
+        if terms and self.spec.cfg.task == TASK_VISUAL:
+            raise NotImplementedError("a teacher observation group on the Visual task is not implemented: the critic library and the "
+                                      "row critic cover the Drift family and Elevation only")
+        self._set_privileged_group("teacher", terms)
+
+    def _set_privileged_group(self, group: str, terms):
+        """The lowering shared by the critic and teacher groups: both are the handle's critic table (wl_critic_observe)."""
         from . import privileged, row_terms
+        other = "teacher" if group == "critic" else "critic"
         terms = [(t, t, {}) if isinstance(t, str) else tuple(t) + ({},) * (3 - len(t)) for t in terms]
+        if getattr(self, f"_{other}_terms", None):
+            if not terms:
+                return                                  # (nothing of this group to clear; the table is the other group's)
+            raise NotImplementedError(f"an env has a critic observation group or a teacher observation group, not both "
+                                      f"(it already has a {other} group)")
         if terms and (self._py_rewards or self._py_terms or self._py_obs or self._py_events):
-            raise NotImplementedError("a critic observation group together with host-side Python terms is not implemented")
+            raise NotImplementedError(f"a {group} observation group together with host-side Python terms is not implemented")
         if terms and (self._dev_terms or self._dev_events):
-            raise NotImplementedError("a critic observation group together with device terms is not implemented")
+            raise NotImplementedError(f"a {group} observation group together with device terms is not implemented")
         fns = [fn if isinstance(fn, str) else getattr(fn, "__name__", "") for _, fn, _ in terms]
         row = tuple(fns[:6]) == row_terms.task_terms("elevation")
         table, head = [], []
@@ -444,11 +471,11 @@ class ManagerBasedRLEnv:
             dc = self.sim.set_row_critic(head, table)     # (refuses a task other than Elevation)
         else:
             dc = self.sim.set_critic_terms(table)     # (refuses a task outside the Drift family)
-        self._critic_terms = terms
+        setattr(self, f"_{group}_terms", terms)
         if dc:
-            self.observation_manager.group_obs_dim["critic"] = (dc,)
+            self.observation_manager.group_obs_dim[group] = (dc,)
         else:
-            self.observation_manager.group_obs_dim.pop("critic", None)
+            self.observation_manager.group_obs_dim.pop(group, None)
             self.extras.pop("observations", None)
 
     # -- a modified policy observation group (policy_obs.py, wl_policy_observe; DESIGN 6q) ------------------------------------
@@ -515,9 +542,10 @@ class ManagerBasedRLEnv:
         """The observation dict of the current state: ``policy`` and, with a critic group, a fresh ``critic`` row; the same
         dict is what ``extras["observations"]`` holds then (RslRlVecEnvWrapper's convention, read by the reference's runner)."""
         groups = {"policy": self._append_py_obs(obs)}
-        if self._critic_terms:
-            groups["critic"] = self.sim.critic_observe()
-            self.extras["observations"] = groups
+        for group in ("critic", "teacher"):
+            if getattr(self, f"_{group}_terms"):
+                groups[group] = self.sim.critic_observe()
+                self.extras["observations"] = groups
         return groups
 
     def _curriculum_fire_mask(self) -> int:
@@ -597,9 +625,10 @@ class ManagerBasedRLEnv:
     def _refuse_mixing(self, device: bool = False):
         if getattr(self, "_policy_terms", None) and not device:
             raise NotImplementedError("a policy observation table together with host-side Python terms is not implemented")
-        if getattr(self, "_critic_terms", None):
-            raise NotImplementedError("a critic observation group together with " + ("device terms" if device else "host-side Python terms")
-                                      + " is not implemented")
+        for group in ("critic", "teacher"):
+            if getattr(self, f"_{group}_terms", None):
+                raise NotImplementedError(f"a {group} observation group together with " + ("device terms" if device else "host-side Python terms")
+                                          + " is not implemented")
         if (self._py_rewards or self._py_terms or getattr(self, "_py_events", None)) if device else \
                 (self._dev_terms or getattr(self, "_dev_events", None)):
             raise NotImplementedError("an env runs either device terms or host-side Python reward / termination terms, not both")

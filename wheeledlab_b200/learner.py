@@ -8,6 +8,9 @@ rollout-slab layout (``distributed.RolloutSlab``); advantage normalisation is le
 
 ``EpisodeStatistics`` is the runner's episode bookkeeping (``:55-63, :99-109``) and ``FusedOnPolicyRunner`` the runner
 itself (``learn`` / ``save`` / ``load`` in rsl_rl's checkpoint format) over ``PPOIteration`` (DESIGN 6h).
+
+``FusedDistillation`` / ``DistillationIteration`` are rsl_rl's ``Distillation`` algorithm on the device (DESIGN 6t), which
+the runner runs for a ``StudentTeacher`` + ``Distillation`` agent cfg.
 """
 from __future__ import annotations
 
@@ -19,7 +22,7 @@ from types import SimpleNamespace
 
 import torch
 
-from ._lib import WL_ACTIVATION, WlEpisodeStatsState, WlError, WlPpoBatch, WlPpoParams, check, lib
+from ._lib import WL_ACTIVATION, WlDistillParams, WlEpisodeStatsState, WlError, WlPpoBatch, WlPpoParams, check, lib
 
 
 def compute_returns(rewards: torch.Tensor, values: torch.Tensor, last_values: torch.Tensor, dones: torch.Tensor,
@@ -705,6 +708,223 @@ class LocalRanksIteration:
         return self.stats
 
 
+@dataclass
+class DistillationConfig:
+    """rsl_rl Distillation's algorithm settings [UPSTREAM-RECALL]: defaults are rsl-rl-lib 2.3's.  ``max_grad_norm`` None
+    (or 0) clips nothing; Adam runs over the student's parameters at the fixed ``learning_rate``."""
+    num_learning_epochs: int = 1
+    gradient_length: int = 15
+    learning_rate: float = 1.0e-3
+    max_grad_norm: float | None = None
+    loss_type: str = "mse"
+
+    @classmethod
+    def from_rsl_rl(cls, alg_cfg) -> "DistillationConfig":
+        return cls(**{f.name: getattr(alg_cfg, f.name) for f in fields(cls) if hasattr(alg_cfg, f.name)})
+
+
+STUDENT_KEYS = [f"student.{k}.{w}" for k in (0, 2, 4) for w in ("weight", "bias")]
+
+
+class FusedDistillation:
+    """rsl_rl ``Distillation.update()`` [UPSTREAM-RECALL] on the device (``wl_distill_update``, DESIGN 6t): behaviour cloning
+    of the teacher's actions by the actor of ``blob`` (laid out by ``blob_layout(obs_dim)``; its critic blocks and std are
+    never written), over a slab of T steps of N envs.  Owns the Adam moments, the device state (learning rate, Adam step,
+    the update's losses) and the workspace; nothing syncs the host, so an update can be captured into a CUDA graph.
+    "elu": the Drift family's network (obs_dim <= 16); "relu": Elevation (obs_dim <= 4096)."""
+
+    def __init__(self, blob: torch.Tensor, obs_dim: int, T: int, N: int, cfg: DistillationConfig | None = None, activation: str = "elu"):
+        from .policy import blob_layout, check_activation
+        cfg = cfg or DistillationConfig()
+        if cfg.loss_type != "mse":
+            raise NotImplementedError(f"loss_type={cfg.loss_type!r}: the fused distillation update implements rsl_rl's 'mse' loss only")
+        if T < cfg.gradient_length:
+            raise ValueError(f"num_steps_per_env {T} < gradient_length {cfg.gradient_length}: no Adam step would cover a chunk")
+        self.activation = check_activation(activation)
+        if self.activation == "elu" and obs_dim > 16:
+            raise NotImplementedError(f"the ELU student takes a row of at most 16 floats, not {obs_dim}")
+        if tuple(blob.shape) != (blob_layout(obs_dim)[1],):
+            raise ValueError(f"the student blob must be laid out by blob_layout({obs_dim})")
+        self.blob, self.obs_dim, self.T, self.N, self.cfg, self.device = blob, obs_dim, T, N, cfg, blob.device
+        self.m = torch.zeros_like(blob)
+        self.v = torch.zeros_like(blob)
+        n_state = lib.wl_distill_state_floats(T, cfg.num_learning_epochs)
+        if n_state == 0:
+            raise WlError(lib.wl_last_error().decode())
+        self.state = torch.zeros(n_state, dtype=torch.float32, device=blob.device)
+        self.state[0] = cfg.learning_rate
+        with torch.cuda.device(self.device):
+            need = lib.wl_distill_workspace_bytes(obs_dim, N, cfg.gradient_length)
+        if need == 0:
+            raise WlError(f"wl_distill_workspace_bytes failed: {lib.wl_last_error().decode()}")
+        self.workspace = torch.empty(need, dtype=torch.uint8, device=blob.device)
+        self._params = WlDistillParams(obs_dim, cfg.num_learning_epochs, cfg.gradient_length, float(cfg.max_grad_norm or 0.0))
+
+    def update(self, obs: torch.Tensor, teacher_actions: torch.Tensor) -> dict:
+        """One update over obs [T, N, obs_dim] (what the student saw) and teacher_actions [T, N, 2].  Returns device tensors:
+        ``behavior`` (the mean of the per-step losses) and ``learning_rate``."""
+        for name, x, shape in (("obs", obs, (self.T, self.N, self.obs_dim)), ("teacher_actions", teacher_actions, (self.T, self.N, 2))):
+            if tuple(x.shape) != shape or x.dtype != torch.float32 or not (x.is_cuda and x.is_contiguous()) or x.device != self.device:
+                raise ValueError(f"FusedDistillation.update: {name} must be a contiguous float32 tensor {list(shape)} on {self.device}")
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        check(lib.wl_distill_update(C.byref(self._params), C.c_void_p(obs.data_ptr()), C.c_void_p(teacher_actions.data_ptr()), self.T,
+                                    self.N, WL_ACTIVATION[self.activation], C.c_void_p(self.blob.data_ptr()), C.c_void_p(self.m.data_ptr()),
+                                    C.c_void_p(self.v.data_ptr()), C.c_void_p(self.state.data_ptr()), C.c_void_p(self.workspace.data_ptr()),
+                                    self.workspace.numel(), stream), "wl_distill_update")
+        return {"behavior": self.state[2], "learning_rate": self.state[0]}
+
+    @property
+    def losses(self) -> torch.Tensor:
+        """The last update's per-step losses, in the order the epochs walked them [epochs * T] (device view)."""
+        return self.state[4:]
+
+    def last_gradient(self) -> torch.Tensor:
+        """The last Adam step's reduced gradient (before clipping), blob layout over the actor, blob[:o6] (device view)."""
+        from .policy import blob_layout
+        return self.workspace[:4 * blob_layout(self.obs_dim)[0][6]].view(torch.float32)
+
+    def optimizer_state_dict(self) -> dict:
+        """``torch.optim.Adam(student.parameters()).state_dict()``: params 0..5 in student order (student.0/2/4 weight|bias),
+        the moments transposed out of the blob layout, one param group with the learning rate (one sync)."""
+        from .policy import actor_critic_state_dict
+        lr, step = (float(x) for x in self.state[:2].tolist())
+        m, v = (actor_critic_state_dict(x, self.obs_dim) for x in (self.m, self.v))
+        keys = [k.replace("student.", "actor.") for k in STUDENT_KEYS]
+        state = {} if step == 0 else {i: {"step": torch.tensor(step), "exp_avg": m[k], "exp_avg_sq": v[k]} for i, k in enumerate(keys)}
+        group = dict(_adam_param_group(lr), params=list(range(len(keys))))
+        return {"state": state, "param_groups": [group]}
+
+    def load_optimizer_state_dict(self, sd: dict):
+        """Inverse of ``optimizer_state_dict``: the moments and the step count in place (a captured iteration keeps
+        working); malformed states raise ``ValueError`` before anything is written."""
+        from .policy import load_actor_critic_state_dict
+        if not isinstance(sd, dict) or not isinstance(sd.get("state"), dict) or not isinstance(sd.get("param_groups"), (list, tuple)):
+            raise ValueError("optimizer state dict must have 'state' (dict) and 'param_groups' (list)")
+        groups = sd["param_groups"]
+        if len(groups) != 1 or list(groups[0].get("params", ())) != list(range(6)):
+            raise ValueError("optimizer state dict must have one param group over the 6 student parameters 0..5")
+        m, v, step = torch.zeros_like(self.m), torch.zeros_like(self.v), 0.0
+        if sd["state"]:
+            st = sd["state"]
+            if sorted(st) != list(range(6)):
+                raise ValueError(f"optimizer state must cover params 0..5, not {sorted(st)}")
+            try:
+                steps = {float(st[i]["step"]) for i in range(6)}
+                for out, key in ((m, "exp_avg"), (v, "exp_avg_sq")):
+                    part = {k.replace("student.", "actor."): st[i][key] for i, k in enumerate(STUDENT_KEYS)}
+                    load_actor_critic_state_dict(dict(part, std=torch.zeros(2)), self.obs_dim, out=out, actor_only=True)
+            except (KeyError, TypeError, RuntimeError) as e:
+                raise ValueError(f"malformed optimizer state: {e!r}") from None
+            if len(steps) != 1:
+                raise ValueError(f"the 6 parameters have different Adam step counts {sorted(steps)}")
+            step = steps.pop()
+        self.m.copy_(m)
+        self.v.copy_(v)
+        self.state[1] = step
+        self.state[0] = self.cfg.learning_rate
+
+
+class DistillationIteration:
+    """One rsl_rl distillation iteration on one GPU [UPSTREAM-RECALL], ONE CUDA graph with ``capture=True``: T x (the
+    teacher's action on the teacher row -- ``wl_actor_mean`` into ``slab.teacher_actions[k]`` --, the student's sampled
+    action -- ``policy_act`` --, ``wl_step``, the next teacher row -- ``wl_critic_observe``), then ``wl_episode_stats`` and
+    ``wl_distill_update``, on device counters.  The handle's critic table is the teacher row (``env.set_teacher_observation``).
+    ``readback`` is one device block, as ``PPOIteration``'s: the episode statistics' state, ``SUMMARY`` and the rollout's T
+    episode-log rows."""
+
+    SUMMARY = ("Loss/behavior", "Loss/learning_rate", "Policy/mean_noise_std")
+
+    def __init__(self, sim, blob: torch.Tensor, teacher_blob: torch.Tensor, cfg: DistillationConfig | None = None, T: int = 128,
+                 activation: str = "elu"):
+        from .distributed import RolloutSlab
+        from .policy import blob_layout
+        if sim.critic_obs_dim < 1:
+            raise ValueError("distillation needs a teacher row on the handle (env.set_teacher_observation)")
+        D, Dt, N = sim.policy_width, sim.critic_obs_dim, sim.num_envs
+        if (N * sim.obs_dim) % 2:
+            raise ValueError("wl_step writes each slab observation row pair-wise: num_envs * obs_dim must be even")
+        if activation == "elu" and Dt > 16:
+            raise NotImplementedError(f"the ELU teacher takes a row of at most 16 floats (wl_actor_mean), not {Dt}")
+        if tuple(teacher_blob.shape) != (blob_layout(Dt)[1],):
+            raise ValueError(f"the teacher blob must be laid out by blob_layout({Dt})")
+        self.sim, self.blob, self.teacher_blob, self.T, self.activation = sim, blob, teacher_blob, T, activation
+        self.alg = FusedDistillation(blob, D, T, N, cfg, activation)
+        self.slab = RolloutSlab(T, N, D, 2, sim.device, policy_fields=True, teacher_actions=True)
+        self.table = sim.policy_obs_dim > 0
+        self._scratch = torch.empty((N, sim.obs_dim), dtype=torch.float32, device=sim.device) if self.table else None
+        self.obs0 = torch.empty((N, D), dtype=torch.float32, device=sim.device)
+        self.tobs = torch.empty((N, Dt), dtype=torch.float32, device=sim.device)     # the teacher row of the next step
+        ns = C.sizeof(WlEpisodeStatsState)
+        end_logs = ns + 4 * len(self.SUMMARY) + 4 * 16 * T
+        self.readback = torch.zeros(end_logs, dtype=torch.uint8, device=sim.device)
+        self.episodes = EpisodeStatistics(N, T, sim.device, state=self.readback[:ns])
+        self.summary = self.readback[ns:ns + 4 * len(self.SUMMARY)].view(torch.float32)
+        self.logs = self.readback[ns + 4 * len(self.SUMMARY):end_logs].view(torch.float32).view(T, 16)
+        self.o_std = blob_layout(D)[0][12]
+        self.graph = self.stats = None
+        self._base = 0
+        self._stream = torch.cuda.Stream(device=sim.device)
+
+    def observe0(self, step_counter: int):
+        self.sim.observe_policy_row(step_counter, 0, self.obs0)
+        self.sim.critic_observe(out=self.tobs)
+
+    def _rollout(self):
+        from .policy import actor_mean, policy_act
+        from .sim import WheeledSim
+        sim, slab, Dt = self.sim, self.slab, self.sim.critic_obs_dim
+        slab.obs_in[0].copy_(self.obs0)
+        for k in range(self.T):
+            t = WheeledSim.device_counter_plus(k)
+            actor_mean(self.teacher_blob, Dt, self.tobs, self.activation, out=slab.teacher_actions[k])
+            policy_act(sim, slab.obs_in[k], self.blob, slab.actions[k], slab.mean[k], slab.log_prob[k], slab.values[k], t, self.activation)
+            out = slab.step_outputs(k)
+            sim.step(slab.actions[k], t, out=(self._scratch,) + out[1:] if self.table else out, log=self.logs[k])
+            if self.table:
+                sim.policy_observe(t, out=slab.obs[k])
+            sim.critic_observe(out=self.tobs)
+        sim.advance_counter(self.T)
+        self.obs0.copy_(slab.obs[self.T - 1])
+
+    def _learn(self):
+        slab = self.slab
+        self.episodes.update(slab.rewards, slab.terminated, slab.truncated)
+        stats = self.alg.update(slab.obs_in, slab.teacher_actions)
+        self.summary.copy_(torch.stack([stats["behavior"], stats["learning_rate"], self.blob[self.o_std:self.o_std + 2].mean()]))
+        return stats
+
+    def _body(self):
+        self._rollout()
+        return self._learn()
+
+    def start(self, step_counter: int = 0, capture: bool = True):
+        sim = self.sim
+        self.observe0(step_counter)
+        sim.set_step_counter(step_counter)
+        self._base = step_counter
+        if not capture:
+            return self
+        self.graph = torch.cuda.CUDAGraph()
+        s = self._stream
+        s.wait_stream(torch.cuda.current_stream(sim.device))
+        with torch.cuda.stream(s):
+            with torch.cuda.graph(self.graph, stream=s):
+                self.stats = self._body()
+        torch.cuda.current_stream(sim.device).wait_stream(s)
+        sim.set_step_counter(step_counter)                     # (the captured advance_counter moved the host mirror)
+        return self
+
+    def run(self) -> dict:
+        if self.graph is None:
+            self.stats = self._body()
+            self._base += self.T
+            return self.stats
+        self.graph.replay()
+        self._base += self.T
+        self.sim.note_device_counter(self._base)
+        return self.stats
+
+
 def _world_size() -> int:
     """The runner's world size, without initialising anything: the process group's, else ``WORLD_SIZE`` (default 1)."""
     import torch.distributed as dist
@@ -780,7 +1000,12 @@ class FusedOnPolicyRunner:
     was lowered with ``device_terms=True``; DESIGN 6q) trains its policy on the table's row: the actor (and, without a critic
     group, the critic) is ``Linear(Dp, 64)``-first, the rollout runs the policy kernel on the slab row, the step, then
     ``wl_policy_observe`` into the next slab row, one graph, with device terms, a critic group or data-parallel, and
-    checkpoints keep rsl_rl's keys with ``actor.0.weight`` ``[64, Dp]``."""
+    checkpoints keep rsl_rl's keys with ``actor.0.weight`` ``[64, Dp]``.
+
+    An agent cfg with ``policy.class_name == "StudentTeacher"`` and ``algorithm.class_name == "Distillation"`` distils (DESIGN
+    6t) on an env with a teacher group (``env.set_teacher_observation``): ``load`` of a PPO checkpoint takes its actor as the
+    teacher, ``learn`` runs ``DistillationIteration`` (one graph) and logs ``Loss/behavior``, checkpoints are StudentTeacher's,
+    and ``get_inference_policy`` plays the student.  One GPU, no Python or device terms."""
 
     @staticmethod
     def settings(train_cfg) -> SimpleNamespace:
@@ -791,11 +1016,31 @@ class FusedOnPolicyRunner:
             raise NotImplementedError("empirical_normalization=True: the fused policy reads raw observations (every reference "
                                       "agent cfg sets it to False)")
         pol, alg = dict(cfg["policy"]), dict(cfg["algorithm"])
-        if pol.get("class_name", "ActorCritic") != "ActorCritic" or alg.get("class_name", "PPO") != "PPO":
-            raise NotImplementedError(f"the fused learner runs rsl_rl's ActorCritic + PPO, not {pol.get('class_name')} + {alg.get('class_name')}")
+        pair = (pol.get("class_name", "ActorCritic"), alg.get("class_name", "PPO"))
+        if pair == ("StudentTeacher", "Distillation"):
+            return FusedOnPolicyRunner._distillation_settings(cfg, pol, alg)
+        if pair != ("ActorCritic", "PPO"):
+            raise NotImplementedError(f"the fused learner runs rsl_rl's ActorCritic + PPO or StudentTeacher + Distillation, not "
+                                      f"{pol.get('class_name')} + {alg.get('class_name')}")
         return SimpleNamespace(cfg=cfg, num_steps_per_env=int(cfg["num_steps_per_env"]), save_interval=int(cfg["save_interval"]),
                                activation=activation_from_rsl_rl(SimpleNamespace(**pol)),
-                               init_noise_std=float(pol.get("init_noise_std", 1.0)), alg_cfg=PPOConfig.from_rsl_rl(SimpleNamespace(**alg)))
+                               init_noise_std=float(pol.get("init_noise_std", 1.0)), alg_cfg=PPOConfig.from_rsl_rl(SimpleNamespace(**alg)),
+                               distillation=False)
+
+    @staticmethod
+    def _distillation_settings(cfg: dict, pol: dict, alg: dict) -> SimpleNamespace:
+        """StudentTeacher + Distillation [UPSTREAM-RECALL]: [64, 64] student and teacher with one activation, a scalar std."""
+        from .policy import check_activation
+        dims = [list(pol.get(k, [])) for k in ("student_hidden_dims", "teacher_hidden_dims")]
+        if dims != [[64, 64], [64, 64]]:
+            raise NotImplementedError(f"the fused student and teacher are [64, 64], not {dims[0]} / {dims[1]}")
+        if pol.get("noise_std_type", "scalar") != "scalar":
+            raise NotImplementedError(f"noise_std_type={pol['noise_std_type']!r}: the fused policy keeps a scalar std per action")
+        if alg.get("loss_type", "mse") != "mse":
+            raise NotImplementedError(f"loss_type={alg['loss_type']!r}: the fused distillation update implements rsl_rl's 'mse' loss only")
+        return SimpleNamespace(cfg=cfg, num_steps_per_env=int(cfg["num_steps_per_env"]), save_interval=int(cfg["save_interval"]),
+                               activation=check_activation(pol.get("activation", "elu")), init_noise_std=float(pol.get("init_noise_std", 1.0)),
+                               alg_cfg=DistillationConfig.from_rsl_rl(SimpleNamespace(**alg)), distillation=True)
 
     def __init__(self, env, train_cfg, log_dir: str | None = None, device="cuda:0"):
         from .policy import pack_actor_critic
@@ -811,6 +1056,10 @@ class FusedOnPolicyRunner:
         sim = e.sim
         if torch.device(device) != torch.device(sim.device):
             raise ValueError(f"device {device} is not the env's device {sim.device}")
+        self.distillation = s.distillation
+        if s.distillation:
+            self._init_distillation(e, s, log_dir, dev_step)
+            return
         self.critic_obs_dim = sim.critic_obs_dim if getattr(e, "_critic_terms", None) else None
         if self.critic_obs_dim is not None:
             if self.staged:
@@ -851,12 +1100,48 @@ class FusedOnPolicyRunner:
         self.callback = None
         self.last_log = None
 
+    def _init_distillation(self, e, s, log_dir, dev_step: bool):
+        """The StudentTeacher + Distillation runner (DESIGN 6t): the student is the actor of ``self.blob`` (blob_layout(D),
+        critic blocks zero), the teacher the actor of ``self.teacher_blob`` (blob_layout(Dt)) over the env's teacher row."""
+        from .policy import blob_layout, pack_actor_critic
+        sim = e.sim
+        if not getattr(e, "_teacher_terms", None):
+            raise ValueError("StudentTeacher + Distillation needs a teacher observation group (env.set_teacher_observation, or a "
+                             "reference cfg with observations.teacher)")
+        if self.staged or dev_step:
+            raise NotImplementedError("distillation together with host-side Python terms or device terms is not implemented")
+        if _world_size() > 1:
+            raise NotImplementedError("distillation in a data-parallel world (WORLD_SIZE > 1) is not implemented")
+        self.world, self.rank = 1, 0
+        self.cfg, self.device, self.log_dir = s.cfg, sim.device, log_dir
+        self.num_steps_per_env, self.save_interval, self.activation, self.alg_cfg = s.num_steps_per_env, s.save_interval, s.activation, s.alg_cfg
+        self.critic_obs_dim = None
+        D, Dt = sim.policy_width, sim.critic_obs_dim
+        if self.activation == "elu" and max(D, Dt) > 16:
+            raise NotImplementedError(f"the ELU student and teacher take rows of at most 16 floats, not {D} / {Dt}")
+        act = torch.nn.ELU if self.activation == "elu" else torch.nn.ReLU
+        mk = lambda out, nin: torch.nn.Sequential(torch.nn.Linear(nin, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, out))
+        zero = torch.nn.Sequential(torch.nn.Linear(D, 64), act(), torch.nn.Linear(64, 64), act(), torch.nn.Linear(64, 1))
+        with torch.no_grad():
+            for p in zero.parameters():
+                p.zero_()
+        self.blob = pack_actor_critic(mk(2, D), zero, torch.full((2,), s.init_noise_std), D, sim.device)
+        self.teacher_blob = torch.zeros(blob_layout(Dt)[1], dtype=torch.float32, device=sim.device)
+        self.loaded_teacher = False
+        self.it = DistillationIteration(sim, self.blob, self.teacher_blob, self.alg_cfg, self.num_steps_per_env, self.activation)
+        self.alg = self.it.alg
+        self.current_learning_iteration = 0
+        self.callback = None
+        self.last_log = None
+
     def learn(self, num_learning_iterations: int, init_at_random_ep_len: bool = False):
         """modified_rsl_rl_runner.py:34-127: iterations current_learning_iteration .. + num_learning_iterations - 1.  The
         episode carries and deques start empty (the runner's locals), the step counter continues from
         ``env.common_step_counter`` and is written back after every iteration; ``model_{it}.pt`` goes to
         ``log_dir/models/`` when ``it % save_interval == 0``."""
         env, it, T = self.env, self.it, self.num_steps_per_env
+        if self.distillation and not self.loaded_teacher:
+            raise ValueError("Teacher model parameters not loaded. Please load a teacher model to distill.")
         if getattr(env, "_needs_reset", False):
             env.reset()
         if init_at_random_ep_len:
@@ -875,16 +1160,17 @@ class FusedOnPolicyRunner:
             env.sim.flush_log()                       # publish the rollout's last episode-log row into the read-back block
             rb = it.readback.cpu()
             elapsed = time.perf_counter() - t0
-            if it.ppo.exchange is not None:
+            if not self.distillation and it.ppo.exchange is not None:
                 it.ppo.exchange.check()
             if not self.staged:                       # (the staged step advances the env's counter itself, once per step)
                 env.common_step_counter += T
             self.current_learning_iteration = k
             st = WlEpisodeStatsState.from_buffer_copy(bytes(rb[:ns].numpy()))
-            summary = rb[ns:ns + 4 * len(PPOIteration.SUMMARY)].view(torch.float32).tolist()
-            o_logs = ns + 4 * len(PPOIteration.SUMMARY)
+            keys = it.SUMMARY
+            summary = rb[ns:ns + 4 * len(keys)].view(torch.float32).tolist()
+            o_logs = ns + 4 * len(keys)
             logs = rb[o_logs:o_logs + 4 * 16 * T].view(torch.float32).view(T, 16).double().mean(0).tolist()
-            log = dict(zip(PPOIteration.SUMMARY, summary))
+            log = dict(zip(keys, summary))
             if st.fill > 0:
                 log["Train/mean_reward"] = st.mean_return
                 log["Train/mean_episode_length"] = st.mean_length
@@ -918,10 +1204,14 @@ class FusedOnPolicyRunner:
         return InferencePolicy(self.blob, self.env.sim.policy_width, self.activation, self.critic_obs_dim)
 
     def save(self, path: str, infos=None):
-        """rsl_rl's checkpoint: {"model_state_dict", "optimizer_state_dict", "iter", "infos"}."""
-        from .policy import actor_critic_state_dict
+        """rsl_rl's checkpoint: {"model_state_dict", "optimizer_state_dict", "iter", "infos"} (a distillation run's model
+        state is StudentTeacher's, its optimizer Adam over the student)."""
+        from .policy import actor_critic_state_dict, student_teacher_state_dict
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-        torch.save({"model_state_dict": actor_critic_state_dict(self.blob, self.env.sim.policy_width, self.critic_obs_dim),
+        sim = self.env.sim
+        model = (student_teacher_state_dict(self.blob, sim.policy_width, self.teacher_blob, sim.critic_obs_dim) if self.distillation
+                 else actor_critic_state_dict(self.blob, sim.policy_width, self.critic_obs_dim))
+        torch.save({"model_state_dict": model,
                     "optimizer_state_dict": self.alg.optimizer_state_dict(),
                     "iter": self.current_learning_iteration, "infos": infos}, path)
 
@@ -935,6 +1225,8 @@ class FusedOnPolicyRunner:
         if not isinstance(d, dict) or not {"model_state_dict", "iter"} <= set(d) or (load_optimizer and "optimizer_state_dict" not in d):
             raise ValueError(f"{path}: not an rsl_rl checkpoint (model_state_dict, optimizer_state_dict, iter, infos)")
         D = self.env.sim.policy_width
+        if self.distillation:
+            return self._load_distillation(path, d, load_optimizer)
         try:
             w1 = d["model_state_dict"]["critic.0.weight"]
             # playback of an asymmetric checkpoint on an env without the critic group (play_policy.py loads weights only):
@@ -948,4 +1240,22 @@ class FusedOnPolicyRunner:
             self.alg.load_optimizer_state_dict(d["optimizer_state_dict"])
         self.blob.copy_(blob)
         self.current_learning_iteration = int(d["iter"])
+        return d.get("infos")
+
+    def _load_distillation(self, path: str, d: dict, load_optimizer: bool):
+        """rsl_rl's load for distillation [UPSTREAM-RECALL]: a PPO checkpoint loads its actor as the teacher (not resumed:
+        neither optimizer nor ``iter``); a distillation checkpoint resumes student, teacher, optimizer and ``iter``."""
+        from .policy import load_student_teacher_state_dict
+        sim = self.env.sim
+        if not isinstance(d["model_state_dict"], dict):
+            raise ValueError(f"{path}: malformed model_state_dict")
+        student, teacher = self.blob.clone(), self.teacher_blob.clone()
+        resumed = load_student_teacher_state_dict(d["model_state_dict"], sim.policy_width, sim.critic_obs_dim, student, teacher)
+        if resumed and load_optimizer:
+            self.alg.load_optimizer_state_dict(d["optimizer_state_dict"])
+        self.blob.copy_(student)
+        self.teacher_blob.copy_(teacher)
+        self.loaded_teacher = True
+        if resumed:
+            self.current_learning_iteration = int(d["iter"])
         return d.get("infos")

@@ -114,6 +114,49 @@ def load_actor_critic_state_dict(sd: dict, obs_dim: int, out: torch.Tensor | Non
     return out
 
 
+def student_teacher_state_dict(student: torch.Tensor, obs_dim: int, teacher: torch.Tensor, teacher_obs_dim: int) -> dict:
+    """rsl_rl StudentTeacher's state dict [UPSTREAM-RECALL] (student.0/2/4.weight|bias, teacher.0/2/4.weight|bias, std) of
+    the student blob (``blob_layout(obs_dim)``, its actor and std) and the teacher blob (``blob_layout(teacher_obs_dim)``, its
+    actor).  Tensors are copies."""
+    s, t = (actor_critic_state_dict(b, d) for b, d in ((student, obs_dim), (teacher, teacher_obs_dim)))
+    sd = {f"student.{k[len('actor.'):]}": v for k, v in s.items() if k.startswith("actor.")}
+    sd.update({f"teacher.{k[len('actor.'):]}": v for k, v in t.items() if k.startswith("actor.")})
+    sd["std"] = s["std"]
+    return sd
+
+
+def load_student_teacher_state_dict(sd: dict, obs_dim: int, teacher_obs_dim: int, student: torch.Tensor,
+                                    teacher: torch.Tensor) -> bool:
+    """StudentTeacher.load_state_dict [UPSTREAM-RECALL] into the two blobs, in place.  A PPO checkpoint (``actor.*`` keys)
+    loads its actor into the teacher alone, drops the critic and returns False (not resumed: the runner then loads neither
+    optimizer nor ``iter``); a distillation checkpoint (``student.*`` keys) loads student, teacher and std and returns True.
+    Every shape is checked before anything is written: an ``actor.0.weight`` whose width is not ``teacher_obs_dim`` raises
+    ``ValueError`` and leaves both blobs as they were."""
+    def actor_sd(prefix, with_std):
+        out = {f"actor.{k}.{w}": sd[f"{prefix}.{k}.{w}"] for k in (0, 2, 4) for w in ("weight", "bias")}
+        out["std"] = sd["std"] if with_std else torch.zeros(2)
+        return out
+
+    try:
+        if any(k.startswith("actor.") for k in sd):
+            w1 = sd["actor.0.weight"]
+            if w1.dim() != 2 or w1.shape[1] != teacher_obs_dim:
+                raise ValueError(f"the teacher checkpoint's actor.0.weight is {tuple(w1.shape)}: its actor does not read the teacher "
+                                 f"row of {teacher_obs_dim} floats")
+            t = load_actor_critic_state_dict(actor_sd("actor", False), teacher_obs_dim, out=teacher.clone(), actor_only=True)
+            teacher.copy_(t)
+            return False
+        if any(k.startswith("student.") for k in sd):
+            s = load_actor_critic_state_dict(actor_sd("student", True), obs_dim, out=student.clone(), actor_only=True)
+            t = load_actor_critic_state_dict(actor_sd("teacher", False), teacher_obs_dim, out=teacher.clone(), actor_only=True)
+            student.copy_(s)
+            teacher.copy_(t)
+            return True
+    except (KeyError, TypeError, RuntimeError) as e:
+        raise ValueError(f"malformed StudentTeacher state dict: {e!r}") from None
+    raise ValueError("neither a PPO checkpoint (actor.* keys) nor a distillation checkpoint (student.* keys)")
+
+
 ACTIVATIONS = {"elu": torch.nn.functional.elu, "relu": torch.nn.functional.relu}
 
 

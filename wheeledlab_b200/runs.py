@@ -23,6 +23,17 @@ def agent_cfg(activation: str, steps: int = 128, save_interval: int = 50) -> dic
             "algorithm": {"class_name": "PPO", **asdict(PPOConfig())}}
 
 
+def distillation_agent_cfg(activation: str, steps: int = 128, save_interval: int = 50) -> dict:
+    """rsl_rl's StudentTeacher + Distillation agent cfg [UPSTREAM-RECALL] with rsl-rl-lib 2.3's defaults and the task's
+    activation: the agent cfg of a run that distils a teacher (``tools/ppo_train.py --teacher``)."""
+    from dataclasses import asdict
+    from .learner import DistillationConfig
+    return {"num_steps_per_env": steps, "save_interval": save_interval, "empirical_normalization": False,
+            "policy": {"class_name": "StudentTeacher", "init_noise_std": 0.1, "noise_std_type": "scalar",
+                       "student_hidden_dims": [64, 64], "teacher_hidden_dims": [64, 64], "activation": activation},
+            "algorithm": {"class_name": "Distillation", **asdict(DistillationConfig())}}
+
+
 def task_activation(task: str) -> str:
     """The hidden activation of the reference's agent cfg for `task` (a gym id or task name): ReLU for Elevation and Visual,
     ELU for the Drift family."""
@@ -30,11 +41,13 @@ def task_activation(task: str) -> str:
     return "relu" if name in ("elevation", "visual", "visual_random") else "elu"
 
 
-def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict, policy_terms=None, row_terms=None) -> str:
+def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: dict, policy_terms=None, row_terms=None,
+                    teacher_terms=None) -> str:
     """`policy_terms`: the env's policy observation table (``(name, library term, noise, clip, scale)`` as
     ``TaskSpec.policy_terms`` holds it), so that playback observes what the policy was trained on; None: the built-in row.
     `row_terms`: the Elevation / Visual env's row terms in the same form (``env.row_terms``, ``TaskSpec.row_terms``): their
-    clips and scales change the policy's input even where playback draws no noise."""
+    clips and scales change the policy's input even where playback draws no noise.  `teacher_terms`: a distillation run's
+    teacher group (``env.set_teacher_observation``'s ``(name, term, params)`` list), which its runner needs to load."""
     os.makedirs(log_dir, exist_ok=True)
     path = os.path.join(log_dir, RUN_CONFIG)
     cfg = {"task": task, "num_envs": int(num_envs), "seed": int(seed), "agent_cfg": agent}
@@ -42,6 +55,8 @@ def save_run_config(log_dir: str, task: str, num_envs: int, seed: int, agent: di
         cfg["policy_terms"] = [list(t) for t in policy_terms]
     if row_terms:
         cfg["row_terms"] = [list(t) for t in row_terms]
+    if teacher_terms:
+        cfg["teacher_terms"] = [[name, fn, dict(params)] for name, fn, params in teacher_terms]
     with open(path, "w") as f:
         json.dump(cfg, f, indent=1)
     return path

@@ -74,6 +74,9 @@ class TaskSpec:
     # an Elevation row critic (DESIGN 6s, env.set_critic_observation's form): [(name, term, {"clip": .., "scale": ..})], the
     # policy row's six terms then critic-library terms; [] = none
     row_critic: list = field(default_factory=list)
+    # the teacher observation group of a distillation run (DESIGN 6t): critic_terms' / row_critic's forms; [] = none
+    teacher_terms: list = field(default_factory=list)
+    row_teacher: list = field(default_factory=list)
     # a modified policy observation group (policy_obs.py, wl_policy_observe): [(name, library term, noise, clip, scale)] in row
     # order; [] = the built-in row.  obs_dim stays the built-in row's width; the policy side is sized by the table's
     policy_terms: list = field(default_factory=list)
