@@ -481,6 +481,9 @@ int64_t wl_launch_count(const wl_sim* sim);
  * previous grid, because the stream's previous launch of a kernel that triggers its dependents was another env set's duo
  * step with disjoint buffers (DESIGN.md 6e) */
 int64_t wl_chained_step_count(const wl_sim* sim);
+/* of those, the ones that ran deep: every CTA triggered the next launch at entry and waited for the previous grid only before
+ * it exited, so more than two steps of different env sets could run at once (DESIGN.md 6e) */
+int64_t wl_deep_step_count(const wl_sim* sim);
 /* what the most recent wl_step on this handle launched (read-only; launches nothing): the kernel variant actually used (1, 4
  * or 8 after the automatic choice; 0 before the first wl_step), the handle's step-spec key, whether the Drift-family duo
  * kernel (variant 8) ran an instantiation specialised on that key (1) or its generic body (0), and the threads per CTA of the

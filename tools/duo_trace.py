@@ -12,7 +12,9 @@ per-launch median warp, except where a row says otherwise.  "pass k cycles" rows
 warp's sub-step pass k (pass 0 from bar.sync 1), median over env warps, split by whether an aux warp on the same SM
 scheduler (%warpid % 4) was between its bar.arrive 1 and bar.arrive 3 (issuing the noise, push and reset draws) at any time
 during the pass.  The residency rows (residency()) give when each CTA entered after its launch's first entry, how long
-late and on-time CTAs ran, and how the CTAs of consecutive launches shared the SMs.  The traced build is a diagnostic
+late and on-time CTAs ran, and how the CTAs of consecutive launches shared the SMs.  The in-flight rows (in_flight())
+give how many launches run at each launch's first entry and how long a deep launch's aux warps sit in the wait before they
+exit.  The traced build is a diagnostic
 build: its stamps and records cost time of their own, so compare traces with traces, and bench.py figures with bench.py
 figures."""
 import argparse
@@ -29,7 +31,8 @@ ROOT = Path(__file__).resolve().parent.parent
 # DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64; ck[6] u32
 TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
      [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3",
-                                                        "aux: griddepcontrol.wait, chained launch"]
+                                                        "aux: griddepcontrol.wait, chained launch", "exit wait returned"]
+LAST, EXIT = TR.index("last store"), TR.index("exit wait returned")
 
 
 def record_dtype():
@@ -134,7 +137,7 @@ def summarize(recs, tag, n_launch_expected):
     period = [b - a for a, b in zip(starts, starts[1:])]
     gap = [s - e for e, s in zip(ends, starts[1:])]
     out = {"tag": tag, "launches": len(L), "launches expected": n_launch_expected, "records": int(len(recs))}
-    for name in TR[:-2]:                                       # (the last two are aux-warp stamps)
+    for name in TR[:-3]:                                       # (the last three are aux-warp stamps)
         if rows[name]:
             out[name] = _median(rows[name])
     out.update({k: _median(v) for k, v in aux.items()})
@@ -151,7 +154,38 @@ def summarize(recs, tag, n_launch_expected):
     out.update(pass_cycles(recs))
     out.update(tails(recs, L))
     out.update(residency(recs, L))
+    out.update(in_flight(recs, L))
     return out
+
+
+def in_flight(recs, launches):
+    """How many launches run at once.  A launch runs from its first warp entry to its last warp's end: the exit wait's
+    return where a deep launch stamps it, else the last store.  Depth at launch k's first entry = the launches before it
+    still running, plus k itself.  Also: how often launch k+2 enters before launch k's last store (more than two grids
+    in flight), and how long a deep launch's aux warps and janitor sit in the exit wait after their last store."""
+    import numpy as np
+    ent, end, last = [], [], []
+    waits = []
+    for ix in launches:
+        ts = recs["ts"][np.asarray(ix)].astype(np.int64)
+        ent.append(int(ts[:, 0].min()))
+        last.append(int(ts[:, LAST].max()))
+        ex = ts[:, EXIT]
+        end.append(int(max(ts[:, LAST].max(), ex.max())))
+        m = (ex > 0) & (ts[:, LAST] > 0)
+        if m.any():
+            waits.append(ex[m] - ts[m, LAST])
+    depth = [sum(1 for j in range(k) if end[j] > ent[k]) + 1 for k in range(len(ent))]
+    k2 = [ent[k + 2] < last[k] for k in range(len(ent) - 2)]
+    w = np.concatenate(waits) if waits else np.zeros(0, dtype=np.int64)
+    return {
+        "launches running at a launch's first entry: median / max": [_median(depth), max(depth, default=None)],
+        "launches running at a launch's first entry (launches by depth)":
+            {str(d): depth.count(d) for d in sorted(set(depth))},
+        "launch k+2 enters before launch k's last store (fraction of launches)": (sum(k2) / len(k2)) if k2 else None,
+        "exit wait: return - last store, warps that wait before exit (ns, median / p90 / max)":
+            [float(np.median(w)), float(np.percentile(w, 90)), float(w.max())] if len(w) else None,
+    }
 
 
 def residency(recs, launches, late_ns=1000):

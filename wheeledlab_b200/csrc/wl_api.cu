@@ -13,6 +13,7 @@
 #include <tuple>
 #include <type_traits>
 #include <utility>
+#include <vector>
 
 #include <cuda.h>
 
@@ -36,6 +37,7 @@ struct wl_sim {
     size_t state_bytes;
     int64_t launches;
     int64_t chained_steps;  // wl_step launches of the duo kernel that ran chained (wl_chained_step_count)
+    int64_t deep_steps;     // (of those, the ones that ran deep: wl_deep_step_count)
     int64_t last_t;         // counter of the most recent step launched through this handle (-1: none); host mirror
     int64_t base_host;      // host mirror of wl_globals.step_base
     uint8_t* term_bits;     // optional per-env termination-term bits output of wl_step (wl_set_term_bits)
@@ -519,6 +521,9 @@ wl_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st
 // each env warp has a scheduler of its own (measured with %warpid on H100, DESIGN.md 6e).  The spacer warp holds
 // registers, so at 8192 envs it would leave CTAs waiting for a second wave: there the CTA stays at 2 warps.
 #define WL_DUO_THREADS 96
+// how a single-GPU duo step runs (duo_chain_mode, DESIGN.md 6e): wl_step_duo_kernel waiting at entry / chained (skips
+// that wait; the aux warp waits, then triggers) / wl_step_duo_deep_kernel (triggers at entry, waits before exit)
+enum { WL_CHAIN_NONE = 0, WL_CHAIN_SHALLOW = 1, WL_CHAIN_DEEP = 2 };
 struct DuoShared {
     float tgt[WL_DUO_ENVS][8];      // wheel_target[4], steer_target[2]
     float noise[WL_DUO_ENVS][12];   // observation noise normals (Philox blocks 0..2)
@@ -537,7 +542,7 @@ __device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64
 // record.  A stamp takes a value as `dep` and is predicated on it, so it is issued only once that value has arrived.
 #ifdef WL_DUO_TRACE
 // (the aux warp stamps TR_BAR1 at its bar.arrive 1 and TR_ARRIVE2 once it passes bar.sync 2)
-enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 = TR_PASS0 + 8, TR_LAST, TR_AUX_ARRIVE3, TR_AUX_WAITED, TR_N };
+enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 = TR_PASS0 + 8, TR_LAST, TR_AUX_ARRIVE3, TR_AUX_WAITED, TR_EXIT, TR_N };
 struct DuoTraceRec {
     unsigned long long st;          // the env set (state buffer) of the launch
     uint32_t t, cta, smid, warpid;  // step counter, blockIdx.x, %smid, %warpid
@@ -608,12 +613,12 @@ __device__ __forceinline__ void duo_prefetch_l2(const float4* st, const float2* 
 // K = 0 reads the config at run time (every other config, and FAN = 1 / 2).
 // Launch bounds: 4 CTAs per SM hold the 4096-env grid with the spacer warp (duo_block); without the minimum, ptxas traded
 // a register spill in the env warp for an occupancy no launch here needs.
-template <int FAN, uint32_t K>
-__global__ void __launch_bounds__(WL_DUO_THREADS, 4)
-wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
-                   const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
-                   uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
-                   uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf, int chained) {
+// DEEP: the deep-chained form (wl_step_duo_deep_kernel, FAN = 0 only).
+template <int FAN, uint32_t K, bool DEEP>
+__device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict__ st, wl_globals* __restrict__ gl,
+                                         const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
+                                         uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log,
+                                         uint32_t t_arg, uint8_t* __restrict__ term_bits, const PeerFan& pf, int chained) {
     using S = Spec<K>;
     __shared__ DuoShared sh;
     TR_DECL;
@@ -626,16 +631,23 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     // Launched with PDL, this prologue runs while the previous step's tail is still running: up to the wait it reads only
     // kernel parameters and requests into L2 the lines both warps load first (the janitor CTA owns no envs).
     if (warp == 0 && env0 < n) duo_prefetch_l2(st, action, n, env0, lane, S::wheel_mass(c));
-    // chained (FAN = 0 only): the previous PDL launch on the stream is a duo step of another env set, and its CTAs
-    // triggered only once ITS predecessor had completed, so all that may still run beside this grid is that step, which
-    // touches none of this launch's buffers (the host checks).  The env CTAs then start on entry.  The aux warp waits before
-    // the weights and the episode log (wl_globals: janitor t-1) and before its trigger, which keeps the same true for the
-    // next launch, and the CTA cannot complete before its predecessor.  The janitor CTA always waits here.  DESIGN.md 6e.
-    const bool early = FAN == 0 && chained != 0 && blockIdx.x != gridDim.x - 1;
-    if (!early) pdl_wait();
+    // chained (FAN = 0 only; duo_chain_mode): every launch that may still run beside this grid is a duo step of another env
+    // set that touches none of this launch's buffers, and this set's previous step has completed (the host checks).  The
+    // env CTAs then start on entry.  Shallow (chained != 0): the aux warp waits before the weights and the episode log
+    // (wl_globals: janitor t-1) and before its trigger, and the janitor CTA waits here, so every CTA triggers only once the
+    // grid before has completed.  Deep: every CTA, the janitor's included, triggers here and nothing waits until the aux
+    // warp's and the janitor's last instruction, so the next grid launches once this one is resident; the wait before exit
+    // keeps a grid from completing before its predecessor.  DESIGN.md 6e.
+    constexpr bool deep = DEEP;
+    const bool early = FAN == 0 && (deep || chained != 0) && blockIdx.x != gridDim.x - 1;
+    if (deep) pdl_trigger();
+    else if (!early) pdl_wait();
     TR(TR_WAITED, n);
     const uint32_t t = decode_step(gl, t_arg);
-    if (janitor_cta(c, gl, t, d_log)) return;
+    if (janitor_cta(c, gl, t, d_log)) {
+        if (deep) pdl_wait();
+        return;
+    }
     const Terrain T{nullptr};
     if (warp == 1) {
         // ================= aux warp: lane j < 8 <-> env env0 + j =================
@@ -655,7 +667,7 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
         }
         float wts[WL_MAX_REW_TERMS];
         if (!S::fixed) {
-            if (early) {
+            if (early && !deep) {
                 pdl_wait();
                 TR(TR_AUX_WAITED, n);
             }
@@ -703,10 +715,10 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             sh.push[j][0] = hf; sh.push[j][1] = dvx; sh.push[j][2] = dvy; sh.push[j][3] = dwh; sh.push[j][4] = t_hf;
             sh.push[j][5] = lf; sh.push[j][6] = dwl; sh.push[j][7] = t_lf;
         }
-        // chained, fixed spec: the wait on the previous grid and the CTA's trigger come before the reset draw, the aux warp's
+        // shallow, fixed spec: the wait on the previous grid and the CTA's trigger come before the reset draw, the aux warp's
         // longest draw, rather than after it (Drift measured 7 % faster on H100, DESIGN.md 6e).  Nothing the draw reads is
         // written by another launch; the weights are still loaded after the wait.
-        if (S::fixed && early) {
+        if (S::fixed && early && !deep) {
             pdl_wait();
             TR(TR_AUX_WAITED, n);
             pdl_trigger();
@@ -775,7 +787,12 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             if (live && term_bits != nullptr) term_bits[i] = (uint8_t)tmask;
         }
         log_accumulate<S::fixed ? 8 : 32>(gl->acc[t % 3u], done && live, tmask, sums);
-        if (live) {
+        if (deep && S::fixed) {                                 // (predicated: no branch ahead of the exit wait below)
+#pragma unroll
+            for (int k = 0; k < WL_MAX_REW_TERMS; ++k) sums[k] = done ? 0.0f : sums[k];
+            st_global_if(st + (size_t)WL_G_SUM0 * n + i, make_float4(sums[0], sums[1], sums[2], sums[3]), live);
+            st_global_if(st + (size_t)WL_G_SUM1 * n + i, make_float4(sums[4], sums[5], sums[6], sums[7]), live);
+        } else if (live) {
             if (done) {
 #pragma unroll
                 for (int k = 0; k < WL_MAX_REW_TERMS; ++k) sums[k] = 0.0f;
@@ -784,6 +801,10 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
             stg4(st, WL_G_SUM1, n, i, make_float4(sums[4], sums[5], sums[6], sums[7]));
         }
         TR(TR_LAST, __float_as_uint(sums[7]));
+        if (deep) {
+            pdl_wait();
+            TR(TR_EXIT, n);
+        }
         TR_COMMIT(1);
         return;
     }
@@ -831,8 +852,8 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     TR(TR_ARRIVE2, raw_mask);
     // The next step's launch may begin once every CTA is here (the aux warp triggers after bar.sync 2; the spacer warp and
     // the janitor CTA have exited).  Triggering at entry instead let each grid launch the next while only partly resident,
-    // and triggering after the last store was slower on H100 (DESIGN.md 6e).  Chained, only the aux warp triggers: the
-    // next launch relies on every trigger following a wait.
+    // and triggering after the last store was slower on H100 (DESIGN.md 6e).  Chained, the env warp does not trigger: a
+    // shallow launch's successor relies on every trigger following a wait, and a deep launch has triggered at entry.
     if (!early) pdl_trigger();
     // I'. observation inputs from the post-physics state (an env that resets / gets pushed takes others below)
     float eu_k = euler_lane<S::fixed>(e.qw, e.qx, e.qy, e.qz, w);
@@ -899,6 +920,24 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     else if (live) store_env_quad(st, n, i, w, e, false, false);
     TR(TR_LAST, __float_as_uint(e.omega[0]));
     TR_COMMIT(0);
+}
+template <int FAN, uint32_t K>
+__global__ void __launch_bounds__(WL_DUO_THREADS, 4)
+wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
+                   const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
+                   uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
+                   uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf, int chained) {
+    duo_step<FAN, K, false>(c, st, gl, action, obs, rew, terminated_o, truncated_o, d_log, t_arg, term_bits, pf, chained);
+}
+// The deep-chained step (FAN = 0) is an entry of its own, so that the machine code of the unchained and shallow steps, which
+// single-set rollouts run, carries none of its branches.
+template <uint32_t K>
+__global__ void __launch_bounds__(WL_DUO_THREADS, 4)
+wl_step_duo_deep_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
+                        const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
+                        uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
+                        uint8_t* __restrict__ term_bits, const __grid_constant__ PeerFan pf) {
+    duo_step<0, K, true>(c, st, gl, action, obs, rew, terminated_o, truncated_o, d_log, t_arg, term_bits, pf, 1);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2098,17 +2137,34 @@ wl_camera_kernel(const __grid_constant__ wl_config c, const float4* __restrict__
 // its code but are launched without it; the thread, quad and act-step kernels use it only with WL_PDL=1.)
 static bool g_pdl = (getenv("WL_PDL") != nullptr) && (atoi(getenv("WL_PDL")) != 0);
 
-// The buffers a single-GPU duo step reads or writes, by stream: what the most recent launch of a kernel that triggers its
-// dependents (griddepcontrol.launch_dependents) was, when it was such a step (n_spans = 0: anything else).  A kernel that
-// triggers releases a PDL-launched successor early, whether it was itself launched with the attribute or not; all of them
-// (the step, quad, act-step and duo kernels) are launched through launch_k, which clears the entry, and the FAN = 0 duo
-// launch then records itself.  Any other kernel lets its successor start only once it has completed, and does so only
-// after its own predecessor has, so it leaves nothing running that this record would have to describe.  An entry holds
-// the id of the graph capture it was made in (0: none): launches captured into a graph never ran on the stream, and the
-// first node of a graph starts only once the work before the graph launch has completed.
+// What may still run on a stream, for the single-GPU duo step (DESIGN.md 6e).  A kernel that triggers its dependents
+// (griddepcontrol.launch_dependents) releases a PDL-launched successor early, whether it was itself launched with the
+// attribute or not; all of them (the step, quad, act-step and duo kernels) are launched through launch_k, which clears the
+// record, and the FAN = 0 duo launch then records itself.  Any other kernel lets its successor start only once it has
+// completed, and does so only after its own predecessor has, so it leaves nothing running that the record would have to
+// describe.  The record holds:
+// * the in-flight suffix: the footprints (buffers read or written) of the duo steps since, and including, the most recent
+//   one that triggered only after its wait (unchained or shallow).  Such a step's trigger follows the completion of every
+//   launch before it, and a deep step triggers at entry, so only the steps of the suffix can run beside the next launch;
+// * the env sets (state buffers) of the last WL_DEEP_DISTINCT duo steps;
+// * the id of the graph capture it was made in (0: none): launches captured into a graph never ran on the stream, and the
+//   first node of a graph starts only once the work before the graph launch has completed.
+// Deep chains need the H = WL_DEEP_DISTINCT most recent steps and this one to be of distinct env sets, so that a set that
+// recurs within H steps keeps the two-grid protocol (a deep step lengthens the suffix, and a set that recurs inside the
+// suffix must wait at entry); the suffix stays shorter than C = WL_DEEP_CAP, which bounds the host's disjointness check.
+#ifndef WL_DEEP_DISTINCT
+#define WL_DEEP_DISTINCT 4
+#endif
+#ifndef WL_DEEP_CAP
+#define WL_DEEP_CAP 32
+#endif
 struct Span { uintptr_t lo, hi; };
 struct DuoFootprint { Span w[6]; int n_spans; Span act; };
-struct DuoPrev { unsigned long long capture; DuoFootprint fp; };
+struct DuoPrev {
+    unsigned long long capture = 0;
+    std::vector<DuoFootprint> suffix;
+    uintptr_t recent[WL_DEEP_DISTINCT] = {};       // state buffers of the last duo steps, most recent at [0]; 0: none
+};
 // (stream handle, device, host thread for cudaStreamPerThread: each host thread's per-thread stream is a stream of its own)
 using StreamKey = std::tuple<uintptr_t, int, size_t>;
 struct DuoKey { StreamKey stream; unsigned long long capture; };
@@ -2133,22 +2189,42 @@ static bool footprints_apart(const DuoFootprint& a, const DuoFootprint& b) {
     for (int k = 0; k < b.n_spans; ++k) if (spans_meet(b.w[k], a.act)) return false;
     return true;
 }
-// whether a duo step with footprint `fp` may run chained (wl_step_duo_kernel): the previous triggering launch on the
-// stream, in the same capture or outside any, was a FAN = 0 duo step that touches none of the buffers this one touches,
-// the actions both read excepted
-static bool duo_chained(const DuoKey& key, const DuoFootprint& fp) {
-    std::lock_guard<std::mutex> lk(g_duo_mu);
-    auto it = g_duo_prev.find(key.stream);
-    return it != g_duo_prev.end() && it->second.capture == key.capture && it->second.fp.n_spans > 0 && footprints_apart(it->second.fp, fp);
+// how a duo step with footprint `fp` runs (wl_step_duo_kernel's `chained`), and the record after it.  Chained: the stream's
+// record, in the same capture or outside any, has a suffix and this step touches none of the buffers of any step in it,
+// the actions they read excepted; otherwise unchained, and the suffix restarts with this step.  Deep: chained, the last
+// WL_DEEP_DISTINCT duo steps and this one are of distinct env sets, and the suffix with this step is shorter than
+// WL_DEEP_CAP; otherwise a chained step is shallow and the suffix restarts with it.
+static int duo_chain_mode(const DuoKey& key, const DuoFootprint& fp, DuoPrev& next) {
+    {
+        std::lock_guard<std::mutex> lk(g_duo_mu);
+        auto it = g_duo_prev.find(key.stream);
+        if (it != g_duo_prev.end() && it->second.capture == key.capture) next = it->second;
+    }
+    next.capture = key.capture;
+    bool apart = !next.suffix.empty();
+    for (const DuoFootprint& f : next.suffix) apart = apart && footprints_apart(f, fp);
+    const uintptr_t set = fp.w[0].lo;
+    bool distinct = true;
+    for (int i = 0; i < WL_DEEP_DISTINCT; ++i) {
+        if (next.recent[i] == 0) break;
+        for (int k = 0; k < i; ++k) distinct = distinct && next.recent[k] != next.recent[i];
+        distinct = distinct && next.recent[i] != set;
+    }
+    const int mode = !apart ? WL_CHAIN_NONE : (distinct && (int)next.suffix.size() + 1 < WL_DEEP_CAP) ? WL_CHAIN_DEEP : WL_CHAIN_SHALLOW;
+    if (mode != WL_CHAIN_DEEP) next.suffix.clear();
+    next.suffix.push_back(fp);
+    for (int i = WL_DEEP_DISTINCT - 1; i > 0; --i) next.recent[i] = next.recent[i - 1];
+    next.recent[0] = set;
+    return mode;
 }
-static void set_duo_prev(const DuoKey& key, const DuoFootprint& fp) {
+static void set_duo_prev(const DuoKey& key, DuoPrev rec) {
     std::lock_guard<std::mutex> lk(g_duo_mu);
-    g_duo_prev[key.stream] = DuoPrev{key.capture, fp};
+    g_duo_prev[key.stream] = std::move(rec);
 }
 
 template <typename... KArgs, typename... Args>
 static void launch_k(void (*kernel)(KArgs...), int grid, int block, size_t smem, cudaStream_t cs, bool pdl, const Args&... args) {
-    set_duo_prev(duo_key(cs), DuoFootprint{});
+    set_duo_prev(duo_key(cs), DuoPrev{});
     static_assert(sizeof...(KArgs) == sizeof...(Args), "argument count");
     cudaLaunchConfig_t lc;
     memset(&lc, 0, sizeof lc);
@@ -2170,9 +2246,12 @@ static inline int pick_block(int n) {
     return 32;
 }
 
-// block size of a duo-kernel launch of `grid` CTAs: with the spacer warp when every CTA is resident at once with it, else 64
+// block size of a duo-kernel launch of `grid` CTAs: with the spacer warp when every CTA is resident at once with it, else 64.
+// A deep-chained launch shares the SMs with the grids before it, so CTA slots count more than a scheduler per env warp:
+// it runs without the spacer (10 instead of 6 CTAs per SM on H100; Drift measured faster without it, DESIGN.md 6e).
 template <typename KF>
-static int duo_block(wl_sim* sim, KF kernel, int grid) {
+static int duo_block(wl_sim* sim, KF kernel, int grid, bool deep = false) {
+    if (deep) return 64;
     const void* kp = reinterpret_cast<const void*>(kernel);
     if (sim->duo_kernel != kp) {
         int per_sm = 0, sms = 0;
@@ -2411,6 +2490,7 @@ int wl_create(const wl_config* cfg, void* d_state, size_t state_bytes, const flo
     s->state_bytes = state_bytes;
     s->launches = 0;
     s->chained_steps = 0;
+    s->deep_steps = 0;
     s->last_t = -1;
     s->base_host = 0;
     s->term_bits = nullptr;
@@ -2474,6 +2554,7 @@ int wl_set_kernel_variant(wl_sim* sim, int32_t lanes_per_env) {
 }
 int64_t wl_launch_count(const wl_sim* sim) { return sim ? sim->launches : 0; }
 int64_t wl_chained_step_count(const wl_sim* sim) { return sim ? sim->chained_steps : 0; }
+int64_t wl_deep_step_count(const wl_sim* sim) { return sim ? sim->deep_steps : 0; }
 int wl_step_launch_info(const wl_sim* sim, int32_t* variant, uint32_t* spec_key, int32_t* specialised, int32_t* threads_per_cta) {
     if (!sim) return fail(WL_EINVAL, "wl_step_launch_info: null handle");
     if (variant) *variant = sim->step_variant;
@@ -2583,15 +2664,24 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
                              span(d_terminated, un), span(d_truncated, un), span(sim->term_bits, sim->term_bits ? un : 0)},
                             6, span(act, un * sizeof(float2))};
             const DuoKey key = duo_key(cs);
-            const int chained = duo_chained(key, fp) ? 1 : 0;
+            DuoPrev next;
+            const int chained = duo_chain_mode(key, fp, next);
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
                 specialised = k.value != 0u;
-                launch_k(wl_step_duo_kernel<0, k>, grid, duo_block(sim, wl_step_duo_kernel<0, k>, grid), 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan, chained);
+                if (chained == WL_CHAIN_DEEP) {
+                    cta_threads = duo_block(sim, wl_step_duo_deep_kernel<k>, grid, true);
+                    launch_k(wl_step_duo_deep_kernel<k>, grid, cta_threads, 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+                } else {
+                    const int shallow = chained == WL_CHAIN_SHALLOW;
+                    cta_threads = duo_block(sim, wl_step_duo_kernel<0, k>, grid);
+                    launch_k(wl_step_duo_kernel<0, k>, grid, cta_threads, 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan, shallow);
+                }
             });
-            set_duo_prev(key, fp);
-            sim->chained_steps += chained;
+            set_duo_prev(key, std::move(next));
+            sim->chained_steps += chained != WL_CHAIN_NONE;
+            sim->deep_steps += chained == WL_CHAIN_DEEP;
         }
-        cta_threads = sim->duo_threads;
+        if (cta_threads == 0) cta_threads = sim->duo_threads;
     } else if (variant == 4) {
 #ifndef WL_QUAD_BS
 #define WL_QUAD_BS 32

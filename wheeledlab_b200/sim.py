@@ -565,6 +565,11 @@ class WheeledSim:
         """wl_step launches of the duo kernel that ran chained after another env set's step (DESIGN.md 6e)."""
         return int(lib.wl_chained_step_count(self._h))
 
+    @property
+    def deep_step_count(self) -> int:
+        """Of the chained steps, the ones that ran deep: triggered the next launch at entry (DESIGN.md 6e)."""
+        return int(lib.wl_deep_step_count(self._h))
+
     # -- zero-copy state views (IsaacLab ArticulationData names) -------------------------------------
     @property
     def root_pos_w(self):
