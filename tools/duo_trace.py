@@ -28,7 +28,8 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 
-# DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, pad[2] u32; ts[TR_N] u64; ck[6] u32
+# DuoTraceRec (wl_api.cu): st u64; t, cta, smid, warpid, role, passes, warp, pad u32; ts[TR_N] u64; ck[6] u32.  warp: the
+# warp's index in its CTA (a deep launch's CTA: env warps 0..3, aux warp 4; otherwise env warp 0, aux warp 1)
 TR = ["entry", "params ready", "after griddepcontrol.wait", "state loads landed", "bar.sync 1"] + \
      [f"end of sub-step pass {k}" for k in range(8)] + ["bar.arrive 2", "last store", "aux: bar.arrive 3",
                                                         "aux: griddepcontrol.wait, chained launch", "exit wait returned"]
@@ -38,7 +39,7 @@ LAST, EXIT = TR.index("last store"), TR.index("exit wait returned")
 def record_dtype():
     import numpy as np
     dt = np.dtype([("st", "<u8"), ("t", "<u4"), ("cta", "<u4"), ("smid", "<u4"), ("warpid", "<u4"), ("role", "<u4"),
-                   ("passes", "<u4"), ("pad", "<u4", 2), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
+                   ("passes", "<u4"), ("warp", "<u4"), ("pad", "<u4"), ("ts", "<u8", len(TR)), ("ck", "<u4", 6)])
     assert dt.itemsize == 40 + 8 * len(TR) + 24
     return dt
 
@@ -248,7 +249,8 @@ def residency(recs, launches, late_ns=1000):
 
 
 def tails(recs, launches):
-    """Which warp of each CTA stores last, which one ends the launch, and the segments outside the sub-step loop (ns,
+    """Which warp of each CTA stores last (the aux warp or the last of its env warps), which one ends the launch, and the
+    segments outside the sub-step loop (ns,
     median over launches of the per-launch median warp): env warp wait -> bar.sync 1 and bar.arrive 2 -> last store, aux
     warp wait -> bar.arrive 1 and bar.sync 2 -> last store"""
     import numpy as np
@@ -264,8 +266,10 @@ def tails(recs, launches):
             m = (role == r) & (ts[:, a] > 0) & (ts[:, b] > 0)
             if m.any():
                 seg[name].append(float(np.median(ts[m, b] - ts[m, a])))
-        env_last = {int(c): int(v) for c, v in zip(cta[role == 0], ts[role == 0, 14])}
-        aux_last = {int(c): int(v) for c, v in zip(cta[role == 1], ts[role == 1, 14])}
+        env_last, aux_last = {}, {}                          # per CTA: its env warps' (aux warp's) last store
+        for r, d in ((0, env_last), (1, aux_last)):
+            for c, v in zip(cta[role == r].tolist(), ts[role == r, 14].tolist()):
+                d[c] = max(d.get(c, 0), int(v))
         both = [c for c in env_last if c in aux_last]
         if both:
             aux_last_cta.append(sum(aux_last[c] > env_last[c] for c in both) / len(both))
@@ -278,6 +282,34 @@ def tails(recs, launches):
         "launches whose last store is an aux warp's": aux_ends_launch,
     })
     return out
+
+
+def occupancy(lib: Path):
+    """{deep-kernel spec key (hex): [registers, warps per SM]} of a library's wl_step_duo_deep_kernel instantiations, from
+    cuobjdump -res-usage.  Warps per SM by the register bound: a scheduler holds 16384 registers, allocated per thread in
+    steps of 8; CTAs per SM = warps per SM // warps per CTA.  (A traced build's stamps cost registers: its occupancy can
+    differ from the shipped build's.)"""
+    import re
+    import shutil
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    try:
+        txt = subprocess.run([cuobjdump, "-res-usage", str(lib)], check=True, capture_output=True, text=True).stdout
+    except (OSError, subprocess.CalledProcessError):
+        return None
+    out = {}
+    for m in re.finditer(r"Function _Z23wl_step_duo_deep_kernelILj(\d+)E\S*:\s*\n\s*.*?REG:(\d+)", txt):
+        reg = int(m.group(2))
+        per_sched = min(16, 16384 // (((reg + 7) // 8) * 8 * 32))
+        out[f"0x{int(m.group(1)):08x}"] = [reg, 4 * per_sched]
+    return out
+
+
+def warps_per_cta(recs):
+    """median number of records per CTA of a launch: the warps that own envs (2 shallow, 5 deep)"""
+    per = {}
+    for k in zip(recs["st"].tolist(), recs["t"].tolist(), recs["cta"].tolist()):
+        per[k] = per.get(k, 0) + 1
+    return _median(list(per.values()))
 
 
 def run(args):
@@ -313,7 +345,7 @@ def run(args):
             steps()
     torch.cuda.current_stream().wait_stream(cs)
     g.replay(); torch.cuda.synchronize()
-    per_launch = 2 * ((E + 7) // 8)
+    per_launch = 2 * ((E + 7) // 8)                             # (a deep launch records 5 warps per 32 envs: fewer)
     dtype = record_dtype()
     cap = per_launch * R
     buf = torch.zeros(cap * dtype.itemsize, dtype=torch.uint8, device=dev)
@@ -325,7 +357,10 @@ def run(args):
     n = lib.wl_duo_trace_arm(None, 0)
     recs = np.frombuffer(buf.cpu().numpy().tobytes(), dtype=dtype)[:min(n, cap)]
     out = summarize(recs, args.tag, R)
-    out.update({"task": args.task, "envs": E, "env sets": M, "gpu": torch.cuda.get_device_name(0)})
+    out.update({"task": args.task, "envs": E, "env sets": M, "gpu": torch.cuda.get_device_name(0),
+                "deep kernel registers / warps per SM, traced build": occupancy(Path(args.lib)),
+                "deep kernel registers / warps per SM, shipped build": occupancy(ROOT / "wheeledlab_b200" / "libwheeledlab_b200.so"),
+                "warps recorded per CTA (median)": warps_per_cta(recs)})
     s = json.dumps(out, indent=1)
     print(s)
     if args.json:

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Static report on the segments of wl_step_duo_kernel outside its sub-step loop (CPU only: nvcc + cuobjdump).
+"""Static report on the segments of the duo kernels (wl_step_duo_kernel, wl_step_duo_deep_kernel) outside their sub-step
+loop (CPU only: nvcc + cuobjdump).
 
     python tools/phase_sass.py [--src DIR | --cubin FILE] [--json OUT]
 
@@ -41,8 +42,8 @@ def segments(ins):
 
 def report(cubin: Path):
     rows = []
-    for (fan, key), ins in sorted(ss.kernel_sass(cubin).items()):
-        row = {"kernel": f"wl_step_duo_kernel<{fan}, 0x{key:08x}>", "fan": fan, "spec": key}
+    for (fan, key), ins in ss.sorted_kernels(ss.kernel_sass(cubin)):
+        row = {"kernel": ss.kernel_name(fan, key), "fan": fan, "spec": key}
         for name, (a, b) in segments(ins).items():
             body = ins[a:b + 1]
             row[name] = {"instructions": len(body), "bssy": sum(o == "BSSY" for _, _, o, _ in body),

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Static report on the integrator sub-step loop of every wl_step_duo_kernel instantiation (CPU only: nvcc + cuobjdump).
+"""Static report on the integrator sub-step loop of every wl_step_duo_kernel and wl_step_duo_deep_kernel instantiation (CPU
+only: nvcc + cuobjdump).
 
     python tools/substep_sass.py [--src DIR | --cubin FILE] [--json OUT]
 
@@ -34,6 +35,8 @@ NO_DEST = {"ST", "STS", "STG", "STL", "BRA", "BSSY", "BSYNC", "BAR", "EXIT", "NO
 _LINE = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P[0-9T]\s+)?([A-Z][A-Z0-9_.]*)\s*(.*?)\s*;")
 _REG = re.compile(r"(?<![\w.])(U?R\d+|U?P\d)(?![\w])")
 _KERNEL = re.compile(r"_Z18wl_step_duo_kernelILi(\d)ELj(\d+)E")
+_DEEP_KERNEL = re.compile(r"_Z23wl_step_duo_deep_kernelILj(\d+)E")
+DEEP = "deep"                                               # the FAN field of a wl_step_duo_deep_kernel<K> key
 
 
 def _build_module():
@@ -60,14 +63,24 @@ def compile_cubin(src_root: Path, out: Path) -> Path:
     return out
 
 
+def kernel_name(fan, k) -> str:
+    return f"wl_step_duo_deep_kernel<0x{k:08x}>" if fan == DEEP else f"wl_step_duo_kernel<{fan}, 0x{k:08x}>"
+
+
+def sorted_kernels(sass: dict):
+    """the items of kernel_sass(), wl_step_duo_kernel instantiations first"""
+    return sorted(sass.items(), key=lambda kv: (kv[0][0] == DEEP, str(kv[0][0]), kv[0][1]))
+
+
 def kernel_sass(cubin: Path):
-    """{(FAN, K): [(addr, pred, opcode, operands)]} for every duo kernel in the cubin"""
+    """{(FAN, K): [(addr, pred, opcode, operands)]} for every duo kernel in the cubin; FAN = DEEP for
+    wl_step_duo_deep_kernel<K>"""
     txt = subprocess.run([tools()[1], "-sass", str(cubin)], check=True, capture_output=True, text=True).stdout
     out, cur = {}, None
     for line in txt.splitlines():
         if "Function :" in line:
-            m = _KERNEL.search(line)
-            cur = (int(m.group(1)), int(m.group(2))) if m else None
+            m, d = _KERNEL.search(line), _DEEP_KERNEL.search(line)
+            cur = (int(m.group(1)), int(m.group(2))) if m else (DEEP, int(d.group(1))) if d else None
             if cur is not None:
                 out[cur] = []
             continue
@@ -146,9 +159,9 @@ def chain(body, passes: int = 2) -> int:
 
 def report(cubin: Path):
     rows = []
-    for (fan, k), ins in sorted(kernel_sass(cubin).items()):
+    for (fan, k), ins in sorted_kernels(kernel_sass(cubin)):
         loop = find_loop(ins)
-        row = {"kernel": f"wl_step_duo_kernel<{fan}, 0x{k:08x}>", "fan": fan, "spec": k}
+        row = {"kernel": kernel_name(fan, k), "fan": fan, "spec": k}
         if loop is None:
             row["error"] = "no sub-step loop found"
             rows.append(row); continue

@@ -208,7 +208,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 // kernel boundary publishes the row to the next launch).  acc layout: [0..7] episode sums, [8] #reset, [9+j] #envs whose
 // termination term j fired (tmask bit j).  WIDTH = 8: only lanes 0..7 can contribute, and the lanes above add zeros to the
 // full butterfly, so three steps give lanes 0..7 the same nonzero sums; lanes 0..15 then issue the 16 REDs side by side.
-template <int WIDTH = 32>
+// SPREAD (WIDTH = 32): likewise lanes 0..15 issue the REDs, by select and predicate rather than 16 branches in lane 0.
+template <int WIDTH = 32, bool SPREAD = false>
 __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool contrib, uint32_t tmask,
                                                const float sums[WL_MAX_REW_TERMS]) {
     const unsigned any_c = __ballot_sync(0xffffffffu, contrib);
@@ -228,6 +229,12 @@ __device__ __forceinline__ bool log_accumulate(float* __restrict__ acc, bool con
         for (int k = 1; k < 8; ++k) { a = sel(m == k, vals[k], a); b = sel(m == k, vals[8 + k], b); }
         a = __shfl_sync(0xffffffffu, a, m); b = __shfl_sync(0xffffffffu, b, m);
         const float v = (lane < 8) ? a : b;                   // lane k < 16: element k, as lanes 0..7 hold it
+        if (lane < 16 && v != 0.0f) atomicAdd(&acc[lane], v);
+    } else if (SPREAD) {
+        const int lane = threadIdx.x & 31;
+        float v = vals[0];
+#pragma unroll
+        for (int k = 1; k < 16; ++k) v = sel(lane == k, vals[k], v);
         if (lane < 16 && v != 0.0f) atomicAdd(&acc[lane], v);
     } else if ((threadIdx.x & 31) == 0) {
 #pragma unroll
@@ -521,21 +528,32 @@ wl_step_quad_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st
 // each env warp has a scheduler of its own (measured with %warpid on H100, DESIGN.md 6e).  The spacer warp holds
 // registers, so at 8192 envs it would leave CTAs waiting for a second wave: there the CTA stays at 2 warps.
 #define WL_DUO_THREADS 96
+// The deep-chained step's CTA: four env warps (warps 0..3, 8 envs each) and one aux warp (warp 4, lane = env) for 32 envs.
+// Its grids share the SMs with the grids before them, so CTA slots and registers per env bound how many are in flight:
+// one aux warp per 32 envs instead of per 8 holds 440 instead of 704 registers per env (DESIGN.md 6e).
+#define WL_DEEP_ENV_WARPS 4
+#define WL_DEEP_ENVS (WL_DUO_ENVS * WL_DEEP_ENV_WARPS)
+#define WL_DEEP_THREADS (32 * (WL_DEEP_ENV_WARPS + 1))
 // how a single-GPU duo step runs (duo_chain_mode, DESIGN.md 6e): wl_step_duo_kernel waiting at entry / chained (skips
 // that wait; the aux warp waits, then triggers) / wl_step_duo_deep_kernel (triggers at entry, waits before exit)
 enum { WL_CHAIN_NONE = 0, WL_CHAIN_SHALLOW = 1, WL_CHAIN_DEEP = 2 };
+// the staging of a CTA of E envs: row q0 + q belongs to quad q of the env warp whose first row is q0
+template <int E>
 struct DuoShared {
-    float tgt[WL_DUO_ENVS][8];      // wheel_target[4], steer_target[2]
-    float noise[WL_DUO_ENVS][12];   // observation noise normals (Philox blocks 0..2)
-    float push[WL_DUO_ENVS][8];     // hf fired, dvx, dvy, dwz_hf, t_hf_new, lf fired, dwz_lf, t_lf_new
-    float fin[WL_DUO_ENVS][16];     // post-physics: p(3) vb(3) wb(3) wz_world steer_l steer_r raw-tmask(bits)
-    __align__(16) float rst[WL_DUO_ENVS][16];   // reset outcome: px py qw qz t_hf t_lf (DriftReset, timers after this step) vb(3) wbo(3) euler[wheel lane]
-    __align__(16) float obs[WL_DUO_ENVS * WL_OBS_DIM_BLIND];   // the 8 observation rows of the CTA, staged for 128-bit stores
-    __align__(16) float rewrow[WL_DUO_ENVS];                    // the CTA's 8 rewards and 2 x 8 done bytes, staged the same way
-    __align__(8) uint8_t maskrow[2][WL_DUO_ENVS];
+    float tgt[E][8];                // wheel_target[4], steer_target[2]
+    float noise[E][12];             // observation noise normals (Philox blocks 0..2)
+    float push[E][8];               // hf fired, dvx, dvy, dwz_hf, t_hf_new, lf fired, dwz_lf, t_lf_new
+    float fin[E][16];               // post-physics: p(3) vb(3) wb(3) wz_world steer_l steer_r raw-tmask(bits)
+    __align__(16) float rst[E][16];             // reset outcome: px py qw qz t_hf t_lf (DriftReset, timers after this step) vb(3) wbo(3) euler[wheel lane]
+    __align__(16) float obs[E * WL_OBS_DIM_BLIND];              // the observation rows of the CTA, staged for 128-bit stores
+    __align__(16) float rewrow[E];                              // the CTA's rewards and done bytes, staged the same way
+    __align__(8) uint8_t maskrow[2][E];
 };
-__device__ __forceinline__ void bar_arrive(int id) { asm volatile("bar.arrive %0, 64;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
+// NT: the threads that meet at the barrier (every warp of the CTA but the spacer)
+template <int NT>
+__device__ __forceinline__ void bar_arrive(int id) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(NT) : "memory"); }
+template <int NT>
+__device__ __forceinline__ void bar_sync(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(NT) : "memory"); }
 
 // ---- phase trace of the duo kernel (diagnostic build only: -DWL_DUO_TRACE, tools/duo_trace.py; without the macro the
 // kernel's machine code is unchanged).  Every warp that owns envs stamps %globaltimer at its hand-offs and appends one
@@ -546,7 +564,7 @@ enum { TR_ENTRY, TR_PARAMS, TR_WAITED, TR_LOADS, TR_BAR1, TR_PASS0, TR_ARRIVE2 =
 struct DuoTraceRec {
     unsigned long long st;          // the env set (state buffer) of the launch
     uint32_t t, cta, smid, warpid;  // step counter, blockIdx.x, %smid, %warpid
-    uint32_t role, passes, pad[2];  // 0 env warp, 1 aux warp; sub-step passes stamped
+    uint32_t role, passes, warp, pad;   // 0 env warp, 1 aux warp; sub-step passes stamped; warp index in the CTA
     unsigned long long ts[TR_N];    // %globaltimer, ns (0: not stamped)
     uint32_t ck[6];                 // env warp: %clock (SM cycles) at bar.sync 1 and at the end of sub-step passes 0..3; pad
 };
@@ -580,7 +598,7 @@ __device__ __forceinline__ void tr_commit(const unsigned long long* ts, uint32_t
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
     asm volatile("mov.u32 %0, %%warpid;" : "=r"(warpid));
     r.st = reinterpret_cast<unsigned long long>(st); r.t = t; r.cta = blockIdx.x; r.smid = smid; r.warpid = warpid;
-    r.role = role; r.passes = passes;
+    r.role = role; r.passes = passes; r.warp = threadIdx.x >> 5;
     for (int i = 0; i < TR_N; ++i) r.ts[i] = ts[i];
     for (int i = 0; i < 6; ++i) r.ck[i] = ck[i];
 }
@@ -613,24 +631,28 @@ __device__ __forceinline__ void duo_prefetch_l2(const float4* st, const float2* 
 // K = 0 reads the config at run time (every other config, and FAN = 1 / 2).
 // Launch bounds: 4 CTAs per SM hold the 4096-env grid with the spacer warp (duo_block); without the minimum, ptxas traded
 // a register spill in the env warp for an occupancy no launch here needs.
-// DEEP: the deep-chained form (wl_step_duo_deep_kernel, FAN = 0 only).
+// DEEP: the deep-chained form (wl_step_duo_deep_kernel, FAN = 0 only), in CTAs of WL_DEEP_ENV_WARPS env warps and one aux
+// warp; otherwise warp 0 is the env warp and warp 1 the aux warp.
 template <int FAN, uint32_t K, bool DEEP>
 __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict__ st, wl_globals* __restrict__ gl,
                                          const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
                                          uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log,
                                          uint32_t t_arg, uint8_t* __restrict__ term_bits, const PeerFan& pf, int chained) {
     using S = Spec<K>;
-    __shared__ DuoShared sh;
+    constexpr int EW = DEEP ? WL_DEEP_ENV_WARPS : 1;            // env warps; the aux warp is warp EW
+    constexpr int ENVS = WL_DUO_ENVS * EW, NT = 32 * (EW + 1);
+    __shared__ DuoShared<ENVS> sh;
     TR_DECL;
     TR(TR_ENTRY, 0);
-    if (threadIdx.x >= 64) return;                              // the spacer warp
+    if (!DEEP && threadIdx.x >= 64) return;                     // the spacer warp
     const int n = c.num_envs;
     TR(TR_PARAMS, n);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int env0 = blockIdx.x * WL_DUO_ENVS;
+    const int env0 = blockIdx.x * ENVS;
+    const int q0 = DEEP ? WL_DUO_ENVS * warp : 0;               // an env warp's first env in the CTA (and staging row)
     // Launched with PDL, this prologue runs while the previous step's tail is still running: up to the wait it reads only
     // kernel parameters and requests into L2 the lines both warps load first (the janitor CTA owns no envs).
-    if (warp == 0 && env0 < n) duo_prefetch_l2(st, action, n, env0, lane, S::wheel_mass(c));
+    if ((DEEP ? warp < EW : warp == 0) && env0 + q0 < n) duo_prefetch_l2(st, action, n, env0 + q0, lane, S::wheel_mass(c));
     // chained (FAN = 0 only; duo_chain_mode): every launch that may still run beside this grid is a duo step of another env
     // set that touches none of this launch's buffers, and this set's previous step has completed (the host checks).  The
     // env CTAs then start on entry.  Shallow (chained != 0): the aux warp waits before the weights and the episode log
@@ -649,17 +671,17 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         return;
     }
     const Terrain T{nullptr};
-    if (warp == 1) {
-        // ================= aux warp: lane j < 8 <-> env env0 + j =================
-        const int j = lane & 7;
+    if (warp == EW) {
+        // ================= aux warp: lane j < ENVS <-> env env0 + j =================
+        const int j = DEEP ? lane : lane & 7;
         const int i = env0 + j;
-        const bool live = (lane < 8) && (i < n);
+        const bool live = (lane < ENVS) && (i < n);
         const int ii = (i < n) ? i : n - 1;
         const uint32_t gid = (uint32_t)(c.env_id_offset + ii);
         float2 a = make_float2(0.0f, 0.0f);
         float4 s0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), s1 = s0;
         float t_hf = 0.0f, t_lf = 0.0f;
-        if (lane < 8) {
+        if (lane < ENVS) {
             a = action[ii];
             s0 = ldg4(st, WL_G_SUM0, n, ii); s1 = ldg4(st, WL_G_SUM1, n, ii);
             const float* fst = reinterpret_cast<const float*>(st);
@@ -675,16 +697,23 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         }
         TR(TR_LOADS, __float_as_uint(a.x) ^ __float_as_uint(s1.w) ^ __float_as_uint(t_lf));
         // A. action map -> targets of the whole env step
-        if (lane < 8) {
+        if (lane < ENVS) {
             float wt[4], stt[2];
             process_action<K>(c, a.x, a.y, wt, stt);
             sh.tgt[j][0] = wt[0]; sh.tgt[j][1] = wt[1]; sh.tgt[j][2] = wt[2]; sh.tgt[j][3] = wt[3];
             sh.tgt[j][4] = stt[0]; sh.tgt[j][5] = stt[1];
         }
-        bar_arrive(1);
+        bar_arrive<NT>(1);
         TR(TR_BAR1, __float_as_uint(sh.tgt[j][0]));
-        // N. observation noise: lane = (env, Philox block)
-        if (lane < 24) {
+        // N. observation noise: lane = (env, Philox block); deep, lane = env and its three blocks as independent chains
+        if (DEEP) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                float z[4];
+                quad_obs_noise<K>(c, k, gid, t, RNG_OBS, 0u, z);
+                sh.noise[j][4 * k + 0] = z[0]; sh.noise[j][4 * k + 1] = z[1]; sh.noise[j][4 * k + 2] = z[2]; sh.noise[j][4 * k + 3] = z[3];
+            }
+        } else if (lane < 24) {
             const int jn = lane / 3, k = lane - 3 * jn;
             const int in_ = (env0 + jn < n) ? env0 + jn : n - 1;
             float z[4];
@@ -692,7 +721,7 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
             sh.noise[jn][4 * k + 0] = z[0]; sh.noise[jn][4 * k + 1] = z[1]; sh.noise[jn][4 * k + 2] = z[2]; sh.noise[jn][4 * k + 3] = z[3];
         }
         // P. interval pushes of an env that does NOT reset this step (the env warp ignores them otherwise)
-        if (lane < 8) {
+        if (lane < ENVS) {
             float hf = 0.0f, dvx = 0.0f, dvy = 0.0f, dwh = 0.0f, lf = 0.0f, dwl = 0.0f;
             if (S::push_enable(c)) {
                 t_hf = t_hf - c.d_step_dt;
@@ -726,7 +755,24 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         // Z. the auto-reset outcome of every env, whether it resets or not: lane = (env, wheel) as in the env warp, which
         // only selects it after bar.sync 3.  A reset env is not pushed: its fresh timers exceed step_dt and only count down.
         // (Drawn before the action map, in the shadow of the loads, it delayed bar.arrive 1 and the step took longer.)
-        {
+        // Deep, lane = env: one draw per env, and the euler angle of each wheel lane.
+        if (DEEP) {
+            DriftReset d = drift_reset_draw(c, gid, t);
+            EnvState z;
+            drift_reset_apply(d, z);
+            const M3 R = rotmat(z.qw, z.qx, z.qy, z.qz);
+            const V3 vb = rotT(R, z.v), wbo = rotT(R, z.w);
+            if (S::push_enable(c)) { d.t_hf = d.t_hf - c.d_step_dt; d.t_lf = d.t_lf - c.d_step_dt; }
+            float* ro = sh.rst[j];
+            reinterpret_cast<float4*>(ro)[0] = make_float4(d.px, d.py, d.qw, d.qz);
+            reinterpret_cast<float4*>(ro)[1] = make_float4(d.t_hf, d.t_lf, vb.x, vb.y);
+            reinterpret_cast<float4*>(ro)[2] = make_float4(vb.z, wbo.x, wbo.y, wbo.z);
+            float eu[4];
+#pragma unroll
+            for (int w = 0; w < 4; ++w) eu[w] = euler_lane(z.qw, z.qx, z.qy, z.qz, w);
+            reinterpret_cast<float4*>(ro)[3] = make_float4(eu[0], eu[1], eu[2], eu[3]);
+            TR(TR_AUX_ARRIVE3, __float_as_uint(eu[3]));
+        } else {
             const QuadLane Lz = quad_lane(c, n, env0 + (lane >> 2), lane & 3);
             DriftReset d = drift_reset_draw(c, Lz.gid, t);
             EnvState z;
@@ -744,17 +790,17 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
             ro[12 + Lz.w] = eu;
             TR(TR_AUX_ARRIVE3, __float_as_uint(eu));
         }
-        bar_arrive(3);
+        bar_arrive<NT>(3);
         // (a fixed spec loads the weights only now, off the way to bar.arrive 1: only the rewards below read them)
         if (S::fixed) load_weights(c, gl, t, wts);
-        // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warp publishes
-        bar_sync(2);
+        // R. rewards, episode sums, reward / done stores, episode log -- on the post-physics state the env warps publish
+        bar_sync<NT>(2);
         TR(TR_ARRIVE2, __float_as_uint(sh.fin[j][0]));
         pdl_trigger();                                          // (see the env warp's trigger)
         uint32_t tmask = 0u;
         float sums[WL_MAX_REW_TERMS] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
         bool done = false;
-        if (lane < 8) {
+        if (lane < ENVS) {
             const float* fi = sh.fin[j];
             const V3 p{fi[0], fi[1], fi[2]}, vb{fi[3], fi[4], fi[5]}, wb{fi[6], fi[7], fi[8]};
             const uint32_t raw = __float_as_uint(fi[12]);
@@ -786,7 +832,8 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
             }
             if (live && term_bits != nullptr) term_bits[i] = (uint8_t)tmask;
         }
-        log_accumulate<S::fixed ? 8 : 32>(gl->acc[t % 3u], done && live, tmask, sums);
+        if (DEEP) log_accumulate<32, S::fixed>(gl->acc[t % 3u], done && live, tmask, sums);
+        else log_accumulate<S::fixed ? 8 : 32>(gl->acc[t % 3u], done && live, tmask, sums);
         if (deep && S::fixed) {                                 // (predicated: no branch ahead of the exit wait below)
 #pragma unroll
             for (int k = 0; k < WL_MAX_REW_TERMS; ++k) sums[k] = done ? 0.0f : sums[k];
@@ -808,9 +855,10 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         TR_COMMIT(1);
         return;
     }
-    // ================= env warp: the quad (lane = wheel), 8 envs =================
-    const int q = lane >> 2;
-    const QuadLane L = quad_lane(c, n, env0 + q, lane & 3);
+    // ================= env warp: the quad (lane = wheel), 8 envs from env0 + q0 =================
+    const int q = lane >> 2, qs = q0 + q;                       // qs: the quad's staging row
+    const int env8 = env0 + q0;
+    const QuadLane L = quad_lane(c, n, env8 + q, lane & 3);
     const int i = L.i, w = L.w, ii = L.ii;
     const bool live = L.live;
     const bool wm = S::wheel_mass(c);
@@ -827,9 +875,9 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
     // B. decimation x (actuators -> integrator)
     Chassis b = chassis_from_env(c, e);
     StepConsts kc = make_step_consts<1, K>(c, e);
-    bar_sync(1);
-    const float my_targets[4] = {sh.tgt[q][w], 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
-    const float my_steer_target[2] = {sh.tgt[q][(w == 3) ? 5 : 4], 0.0f};
+    bar_sync<NT>(1);
+    const float my_targets[4] = {sh.tgt[qs][w], 0.0f, 0.0f, 0.0f}, my_efforts[4] = {my_effort, 0.0f, 0.0f, 0.0f};
+    const float my_steer_target[2] = {sh.tgt[qs][(w == 3) ? 5 : 4], 0.0f};
     TR(TR_BAR1, __float_as_uint(my_targets[0]));
     TR_CK_BAR1(__float_as_uint(my_targets[0]));
     // with a fixed spec the pass is free of divergent regions (measured faster on H100, DESIGN.md 6e)
@@ -843,12 +891,12 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
     const bool oob = drift_off_track(c, e.p.x, e.p.y);
     const uint32_t raw_mask = drift_term_mask(time_out, oob);
     if (w == 0) {
-        float* fo = sh.fin[q];
+        float* fo = sh.fin[qs];
         fo[0] = e.p.x; fo[1] = e.p.y; fo[2] = e.p.z; fo[3] = vb.x; fo[4] = vb.y; fo[5] = vb.z;
         fo[6] = b.wb.x; fo[7] = b.wb.y; fo[8] = b.wb.z; fo[9] = e.w.z; fo[10] = steer_l; fo[11] = steer_r;
         fo[12] = __uint_as_float(raw_mask);
     }
-    bar_arrive(2);
+    bar_arrive<NT>(2);
     TR(TR_ARRIVE2, raw_mask);
     // The next step's launch may begin once every CTA is here (the aux warp triggers after bar.sync 2; the spacer warp and
     // the janitor CTA have exited).  Triggering at entry instead let each grid launch the next while only partly resident,
@@ -860,18 +908,18 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
     V3 wbo = rotT(R, e.w);
     const bool done = (raw_mask & (uint32_t)c.term_enable) != 0u;
     // F. auto-reset and H. interval pushes: the reset outcome, the push draws and the noise come from the aux warp
-    bar_sync(3);
+    bar_sync<NT>(3);
     if (S::fixed) {
         // as selects over both outcomes, so that a warp with resetting and pushed envs does not split.  The pushed velocities
         // are rotated whether a push fired or not: unpushed, they are the same values, so the same bits.
-        const float4* ro = reinterpret_cast<const float4*>(sh.rst[q]);
+        const float4* ro = reinterpret_cast<const float4*>(sh.rst[qs]);
         const float4 r0 = ro[0], r1 = ro[1], r2 = ro[2];
-        const float eu_r = sh.rst[q][12 + w];
+        const float eu_r = sh.rst[qs][12 + w];
         EnvState er = e;
         drift_reset_apply(DriftReset{r0.x, r0.y, r0.z, r0.w, r1.x, r1.y}, er);
         V3 vbp = vb, wbp = wbo;
         if (S::push_enable(c)) {
-            const float* pu = sh.push[q];
+            const float* pu = sh.push[qs];
             const bool hf = pu[0] != 0.0f, lf = pu[5] != 0.0f;
             e.v.x = hf ? e.v.x + pu[1] : e.v.x; e.v.y = hf ? e.v.y + pu[2] : e.v.y;
             e.w.z = hf ? e.w.z + pu[3] : e.w.z; e.w.z = lf ? e.w.z + pu[6] : e.w.z;
@@ -882,13 +930,13 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         vb = done ? V3{r1.z, r1.w, r2.x} : vbp; wbo = done ? V3{r2.y, r2.z, r2.w} : wbp;
         eu_k = done ? eu_r : eu_k;
     } else if (done) {                                                 // (sums and log: aux warp)
-        const float4* ro = reinterpret_cast<const float4*>(sh.rst[q]);
+        const float4* ro = reinterpret_cast<const float4*>(sh.rst[qs]);
         const float4 r0 = ro[0], r1 = ro[1], r2 = ro[2];
         drift_reset_apply(DriftReset{r0.x, r0.y, r0.z, r0.w, r1.x, r1.y}, e);
         vb = V3{r1.z, r1.w, r2.x}; wbo = V3{r2.y, r2.z, r2.w};
-        eu_k = sh.rst[q][12 + w];
+        eu_k = sh.rst[qs][12 + w];
     } else if (S::push_enable(c)) {
-        const float* pu = sh.push[q];
+        const float* pu = sh.push[qs];
         bool fired = false;
         if (pu[0] != 0.0f) { e.v.x = e.v.x + pu[1]; e.v.y = e.v.y + pu[2]; e.w.z = e.w.z + pu[3]; fired = true; }
         e.t_hf = pu[4];
@@ -897,20 +945,20 @@ __device__ __forceinline__ void duo_step(const wl_config& c, float4* __restrict_
         if (fired) { vb = rotT(R, e.v); wbo = rotT(R, e.w); }
     }
     const int k4 = (w < 3) ? 4 * w : 0;
-    const float zn[4] = {sh.noise[q][k4], sh.noise[q][k4 + 1], sh.noise[q][k4 + 2], sh.noise[q][k4 + 3]};
-    // the CTA's 8 observation rows are 448 contiguous bytes: staged in shared memory and written as 28 x 128-bit stores
+    const float zn[4] = {sh.noise[qs][k4], sh.noise[qs][k4 + 1], sh.noise[qs][k4 + 2], sh.noise[qs][k4 + 3]};
+    // the env warp's 8 observation rows are 448 contiguous bytes: staged in shared memory and written as 28 x 128-bit stores
     // (full sectors towards HBM, NVLink peers and -- zero-copy host transport -- PCIe, instead of 8-byte pieces)
-    float* orow0 = obs + (size_t)WL_OBS_DIM_BLIND * env0;
-    if ((FAN == 2) || (env0 + WL_DUO_ENVS <= n && (reinterpret_cast<uintptr_t>(orow0) & 15u) == 0)) {
+    float* orow0 = obs + (size_t)WL_OBS_DIM_BLIND * env8;
+    if ((FAN == 2) || (env8 + WL_DUO_ENVS <= n && (reinterpret_cast<uintptr_t>(orow0) & 15u) == 0)) {
         const float4 v = blind_obs_quad_values<S::fixed>(c, e, w, eu_k, vb, wbo, zn);
-        float* so = sh.obs + WL_OBS_DIM_BLIND * q + 4 * w;
+        float* so = sh.obs + WL_OBS_DIM_BLIND * qs + 4 * w;
         so[0] = v.x; so[1] = v.y;
         if (w < 3) { so[2] = v.z; so[3] = v.w; }
         __syncwarp();
         if (lane < (WL_DUO_ENVS * WL_OBS_DIM_BLIND) / 4)
         {
-            if (FAN) fan_store16<FAN == 2>(pf, reinterpret_cast<float4*>(orow0) + lane, reinterpret_cast<const float4*>(sh.obs)[lane]);
-            else reinterpret_cast<float4*>(orow0)[lane] = reinterpret_cast<const float4*>(sh.obs)[lane];
+            if (FAN) fan_store16<FAN == 2>(pf, reinterpret_cast<float4*>(orow0) + lane, reinterpret_cast<const float4*>(sh.obs + WL_OBS_DIM_BLIND * q0)[lane]);
+            else reinterpret_cast<float4*>(orow0)[lane] = reinterpret_cast<const float4*>(sh.obs + WL_OBS_DIM_BLIND * q0)[lane];
         }
     } else {
         if (FAN == 1) blind_obs_quad(c, e, w, eu_k, vb, wbo, zn, obs + (size_t)WL_OBS_DIM_BLIND * ii, live, pf);
@@ -930,9 +978,10 @@ wl_step_duo_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st,
     duo_step<FAN, K, false>(c, st, gl, action, obs, rew, terminated_o, truncated_o, d_log, t_arg, term_bits, pf, chained);
 }
 // The deep-chained step (FAN = 0) is an entry of its own, so that the machine code of the unchained and shallow steps, which
-// single-set rollouts run, carries none of its branches.
+// single-set rollouts run, carries none of its branches.  Launch bounds: 4 CTAs of 160 threads per SM (at most 96
+// registers: 5 warps per scheduler), 128 envs per SM against the 80 of 2-warp CTAs.
 template <uint32_t K>
-__global__ void __launch_bounds__(WL_DUO_THREADS, 4)
+__global__ void __launch_bounds__(WL_DEEP_THREADS, 4)
 wl_step_duo_deep_kernel(const __grid_constant__ wl_config c, float4* __restrict__ st, wl_globals* __restrict__ gl,
                         const float2* __restrict__ action, float* __restrict__ obs, float* __restrict__ rew,
                         uint8_t* __restrict__ terminated_o, uint8_t* __restrict__ truncated_o, float* __restrict__ d_log, uint32_t t_arg,
@@ -2247,11 +2296,10 @@ static inline int pick_block(int n) {
 }
 
 // block size of a duo-kernel launch of `grid` CTAs: with the spacer warp when every CTA is resident at once with it, else 64.
-// A deep-chained launch shares the SMs with the grids before it, so CTA slots count more than a scheduler per env warp:
-// it runs without the spacer (10 instead of 6 CTAs per SM on H100; Drift measured faster without it, DESIGN.md 6e).
+// (A deep-chained launch has CTAs of its own, WL_DEEP_THREADS: it shares the SMs with the grids before it, so CTA slots
+// count more than a scheduler per env warp, DESIGN.md 6e.)
 template <typename KF>
-static int duo_block(wl_sim* sim, KF kernel, int grid, bool deep = false) {
-    if (deep) return 64;
+static int duo_block(wl_sim* sim, KF kernel, int grid) {
     const void* kp = reinterpret_cast<const void*>(kernel);
     if (sim->duo_kernel != kp) {
         int per_sm = 0, sms = 0;
@@ -2669,8 +2717,9 @@ int wl_step(wl_sim* sim, const float* d_action, float* d_obs, float* d_rew, uint
             with_spec<SPEC_DRIFT_RWD, SPEC_DRIFT_4WD>(sim->spec, [&](auto k) {
                 specialised = k.value != 0u;
                 if (chained == WL_CHAIN_DEEP) {
-                    cta_threads = duo_block(sim, wl_step_duo_deep_kernel<k>, grid, true);
-                    launch_k(wl_step_duo_deep_kernel<k>, grid, cta_threads, 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
+                    cta_threads = WL_DEEP_THREADS;
+                    const int deep_grid = (n + WL_DEEP_ENVS - 1) / WL_DEEP_ENVS + 1;                 // + the janitor CTA
+                    launch_k(wl_step_duo_deep_kernel<k>, deep_grid, cta_threads, 0, cs, true, sim->cfg, sim->state, sim->globals, act, d_obs, d_rew, d_terminated, d_truncated, d_log, t, sim->term_bits, sim->fan);
                 } else {
                     const int shallow = chained == WL_CHAIN_SHALLOW;
                     cta_threads = duo_block(sim, wl_step_duo_kernel<0, k>, grid);
